@@ -33,17 +33,13 @@ UNIT = "images/s"
 
 
 def peaks():
-    p = dict(hbm_gbs=6650.0, bf16_tflops=1590.0, source="fallback")
-    try:
-        m = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        p = dict(hbm_gbs=float(m["hbm_gbs"]), bf16_tflops=float(m["bf16_tflops"]), bf16_tflops_sustained=float(m.get("bf16_tflops_sustained", m["bf16_tflops"])), source="measured")
-    except Exception:
-        pass
-    return p
+    """NVIDIA's data-sheet figures for the H100 SXM (700 W): HBM3 bandwidth and dense BF16 tensor rate.  A card held to a lower power
+    limit reaches less; `clocks` in the result line shows what the card ran at."""
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, source="H100 SXM data sheet")
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons while the timed region runs (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons while the timed region runs (read-only queries)."""
 
     def __init__(self, device):
         threading.Thread.__init__(self)
@@ -134,9 +130,9 @@ def cpu_baseline(image):
 
 
 DTYPES = {"f32": 0x04000, "bf16": 0x80000, "f16": 0x20000}
-MATH = {"f32": {-1: "tcgen05 kind::tf32, fp32 accumulate (TMA rounds operands to TF32); the dense layer 3xTF32", 0: "tcgen05 kind::tf32, fp32 accumulate (TMA rounds operands to TF32)",
-                1: "3xTF32: three tcgen05 kind::tf32 MMAs on (hi, lo) operand splits, fp32 accumulate", 2: "CUDA-core fp32 FFMA"},
-        "bf16": "tcgen05 kind::f16 (bf16 operands), fp32 accumulate in TMEM", "f16": "tcgen05 kind::f16 (fp16 operands), fp32 accumulate in TMEM"}
+MATH = {"f32": {-1: "wgmma tf32, fp32 accumulate (TMA rounds operands to TF32); the dense layer 3xTF32", 0: "wgmma tf32, fp32 accumulate (TMA rounds operands to TF32)",
+                1: "3xTF32: three wgmma tf32 MMAs on (hi, lo) operand splits, fp32 accumulate", 2: "CUDA-core fp32 FFMA"},
+        "bf16": "wgmma bf16 operands, fp32 accumulate in registers", "f16": "wgmma fp16 operands, fp32 accumulate in registers"}
 
 
 def to_bf16(a):
@@ -144,7 +140,34 @@ def to_bf16(a):
     return (((u + 0x7FFF + ((u >> 16) & 1)) >> 16) & 0xFFFF).astype(np.uint16)
 
 
-def run_model(args, dist, rank, world, local_rank, dtype="f32", algorithm=-1, per_op_path=""):
+def widen(a, dtype):
+    """A downloaded tensor as float32 (16-bit tensors come back as their raw 16-bit patterns or as float16)."""
+    a = np.asarray(a)
+    if a.dtype == np.uint16:
+        return (a.astype(np.uint32) << 16).view(np.float32) if dtype == "bf16" else a.view(np.float16).astype(np.float32)
+    return a.astype(np.float32)
+
+
+DUMP_SAMPLE = 1 << 22  # elements kept of each large output: 16 MB of float32
+
+
+def dump_outputs(net, directory, dtype):
+    """What the timed step hands its caller after the last timed step: the per-sample loss, and a fixed seeded sample of the updated
+    parameters and of the gradients that updated them (the same indices in every run of the same configuration).  A 16-bit model keeps its
+    fp32 batch-norm parameters and gradients in separate buffers: params_bn / grads_bn."""
+    os.makedirs(directory, exist_ok=True)
+    np.save(os.path.join(directory, "loss.npy"), widen(net.loss.download(), dtype).reshape(-1))
+    bufs = [("params", net.w_flat, dtype if dtype == "f32" else "f32"), ("grads", net.g_flat, dtype)]
+    if hasattr(net, "w_flat_b"):
+        bufs += [("params_bn", net.w_flat_b, "f32"), ("grads_bn", net.g_flat_b, "f32")]
+    for name, t, kind in bufs:
+        v = widen(t.download(), kind).reshape(-1)
+        if v.size > DUMP_SAMPLE:
+            v = v[np.sort(np.random.RandomState(0).randint(0, v.size, size=DUMP_SAMPLE))]
+        np.save(os.path.join(directory, name + ".npy"), v)
+
+
+def run_model(args, dist, rank, world, local_rank, dtype="f32", algorithm=-1, per_op_path="", dump_dir=""):
     """One measured configuration of the ResNet-50 step: returns the JSON object (rank 0 fills roofline / per_op)."""
     from ccv_b200 import nnc, resnet50
     device = local_rank
@@ -240,6 +263,8 @@ def run_model(args, dist, rank, world, local_rank, dtype="f32", algorithm=-1, pe
     sampler.start()
     ms = timed(step, args.steps)
     ms_per_step = ms / args.steps
+    if dump_dir and rank == 0:
+        dump_outputs(net, dump_dir, dtype)
 
     # end to end: every step copies its batch from pinned host memory and reads the loss back, through the same public calls
     # (CMD_DATA_TRANSFER on stream contexts).  The copy of batch k+1 runs on a second stream context while step k computes
@@ -286,7 +311,7 @@ def run_model(args, dist, rank, world, local_rank, dtype="f32", algorithm=-1, pe
                           "fp32" if dtype == "f32" else dtype + " activations / filters / gradients, fp32 master weights + batch-norm parameters", args.batch, args.image, args.image,
                           "" if dtype == "f32" else " (mixed precision)", exchange),
                       "global_batch": images_per_step, "parallelism": "dp%d" % world, "tensor_core_math": math,
-                      "cuda_graph": use_graph, "fused_pairs": n_fused, "first_step_loss": first_loss, "l2": "activations per step (>10 GB) exceed the 126 MB L2: no flush needed", "mean_loss": loss},
+                      "cuda_graph": use_graph, "fused_pairs": n_fused, "first_step_loss": first_loss, "l2": "activations per step (>10 GB) exceed the 50 MB L2: no flush needed", "mean_loss": loss},
            "e2e": {"value": images_per_step / (e2e_ms * 1e-3), "unit": UNIT, "h2d_bytes_per_step": int(host_in.nbytes + host_lab.nbytes), "d2h_bytes_per_step": int(host_loss.nbytes), "ms_per_step": e2e_ms,
                    "pipeline": "batch k+1 is copied host->device on a second stream context while step k computes (stream signals); one pinned-host copy + one loss read per step inside the timed region"},
            "gpu_launches": int(launches_per_step * (args.steps * 2 + args.warmup + 2)), "gpu_launches_per_step": int(launches_per_step), "clocks": sampler.summary()}
@@ -340,7 +365,7 @@ def run_sdpa_cfg5(args):
             fwd()
             nnc.cmd_exec(xfer, None, 0, [dev[3]], [host[3]], stream)
         res = {}
-        for name, fn, reps in (("device", fwd, 20), ("e2e", e2e, 5)):
+        for name, fn, reps in (("device", fwd, args.steps), ("e2e", e2e, args.steps)):
             for _ in range(3):
                 fn()
             e0, e1 = nnc.Event(), nnc.Event()
@@ -355,6 +380,8 @@ def run_sdpa_cfg5(args):
         bcmd.info.scaled_dot_product_attention.scale = 1.0 / np.sqrt(D)
         bcmd.info.scaled_dot_product_attention.is_causal = causal
         bcmd.info.scaled_dot_product_attention.deterministic = 1
+        if args.dump_outputs and causal == 0:
+            dump_sdpa(args.dump_outputs, dev[3], lse)
         b_ins = [dev[0], None, None, dev[0], dev[1], dev[2], None, None, None, dev[3], lse]
 
         def bwd():
@@ -364,27 +391,36 @@ def run_sdpa_cfg5(args):
         e0, e1 = nnc.Event(), nnc.Event()
         stream.wait()
         e0.record(stream)
-        for _ in range(10):
+        for _ in range(args.steps):
             bwd()
         e1.record(stream)
-        bms = e0.elapsed_ms(e1) / 10
+        bms = e0.elapsed_ms(e1) / args.steps
         bflops = 10.0 * B * H * S * S * D * (0.5 if causal else 1.0)  # the 5 GEMMs of the backward; the kernels issue 7 (S and dP twice)
         flops = 4.0 * B * H * S * S * D * (0.5 if causal else 1.0)
         byts = 4.0 * n * 2 + B * H * S * 4
         ms = res["device"]
         out["causal" if causal else "full"] = {
             "backward": {"ms": bms, "tflops": bflops / bms * 1e-9, "frac_of_bf16_peak": bflops / bms * 1e-9 / pk["bf16_tflops"], "algorithmic_flops": bflops,
-                         "note": "fused deterministic tcgen05 backward (prep + dK/dV kernel + dQ kernel), 5-GEMM flop count"},
+                         "note": "fused deterministic wgmma backward (prep + dK/dV kernel + dQ kernel), 5-GEMM flop count"},
             "ms": ms, "tflops": flops / ms * 1e-9, "frac_of_bf16_peak": flops / ms * 1e-9 / pk["bf16_tflops"], "gbs": byts / ms * 1e-6, "frac_of_hbm_peak": byts / ms * 1e-6 / pk["hbm_gbs"],
-            "algorithmic_flops": flops, "algorithmic_bytes": byts, "l2": "Q + K + V + O = 1.07 GB per launch: larger than the 126 MB L2",
+            "algorithmic_flops": flops, "algorithmic_bytes": byts, "l2": "Q + K + V + O = 1.07 GB per launch: larger than the 50 MB L2",
             "e2e": {"ms": res["e2e"], "tflops": flops / res["e2e"] * 1e-9, "h2d_bytes_per_step": int(3 * n * 2), "d2h_bytes_per_step": int(n * 2)}}
     sampler.stop_flag = True
     sampler.join()
     out["clocks"] = sampler.summary()
-    out["workload"] = "CCV_NNC_SCALED_DOT_PRODUCT_ATTENTION_FORWARD bf16 B=32 H=16 S=2048 D=128 (BASELINE.json configs[4]), tcgen05 flash-attention kernel, LSE written; `backward` = CCV_NNC_SCALED_DOT_PRODUCT_ATTENTION_BACKWARD on the same tensors"
+    out["workload"] = "CCV_NNC_SCALED_DOT_PRODUCT_ATTENTION_FORWARD bf16 B=32 H=16 S=2048 D=128 (BASELINE.json configs[4]), wgmma flash-attention kernel, LSE written; `backward` = CCV_NNC_SCALED_DOT_PRODUCT_ATTENTION_BACKWARD on the same tensors"
     for t in dev + host + grads + [lse, stream]:
         t.free()
     return out
+
+
+def dump_sdpa(directory, o, lse):
+    """The non-causal forward's output O (a fixed seeded sample of it) and its log-sum-exp, as float32."""
+    os.makedirs(directory, exist_ok=True)
+    v = widen(o.download(), "bf16").reshape(-1)
+    v = v[np.sort(np.random.RandomState(0).randint(0, v.size, size=DUMP_SAMPLE))]
+    np.save(os.path.join(directory, "sdpa_out.npy"), v)
+    np.save(os.path.join(directory, "sdpa_lse.npy"), widen(lse.download(), "f32").reshape(-1))
 
 
 def run_reference_cnnp(args):
@@ -436,6 +472,7 @@ def main():
     ap.add_argument("--no-fuse", action="store_true", help="run every reference command as its own kernel sequence (no peephole fusion)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--per-op", default="", help="write the per-command profile to this JSON file")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR", help="after the timed steps of the headline configuration, write its last step's outputs as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     if args.impl == "reference":
         return reference_arm(args)
@@ -456,7 +493,7 @@ def main():
         if rank == 0:
             r = run_sdpa_cfg5(args)
             full = r["full"]
-            print(json.dumps({"metric": "sdpa_fwd_bf16_b32_h16_s2048_d128_tflops", "value": full["tflops"], "unit": "TFLOP/s", "n_gpus": 1, "steps": 20, "warmup": 3, "ms_per_step": full["ms"], "higher_is_better": True,
+            print(json.dumps({"metric": "sdpa_fwd_bf16_b32_h16_s2048_d128_tflops", "value": full["tflops"], "unit": "TFLOP/s", "n_gpus": 1, "steps": args.steps, "warmup": 3, "ms_per_step": full["ms"], "higher_is_better": True,
                               "scaling": "weak", "vs_baseline": None, "dtype": "bf16", "data": "synthetic", "config": {"workload": r["workload"]},
                               "roofline": {"bound": "tensor", "achieved": full["tflops"], "peak": peaks()["bf16_tflops"], "unit": "TFLOP/s", "frac": full["frac_of_bf16_peak"], "traffic": None},
                               "e2e": {"value": full["e2e"]["tflops"], "unit": "TFLOP/s", "h2d_bytes_per_step": full["e2e"]["h2d_bytes_per_step"], "d2h_bytes_per_step": full["e2e"]["d2h_bytes_per_step"]},
@@ -466,7 +503,7 @@ def main():
             dist.destroy_process_group()
         return
 
-    out = run_model(args, dist, rank, world, local_rank, args.dtype, args.algorithm, args.per_op)
+    out = run_model(args, dist, rank, world, local_rank, args.dtype, args.algorithm, args.per_op, args.dump_outputs)
     if not args.no_variants:
         # the other BASELINE configurations, measured by the same code in the same process (same box, same clocks):
         #   bf16     configs[3] (ResNet-50 16-bit, batch-sharded): at N GPUs this IS configs[3]'s per-GPU shard of N x 256 images
@@ -542,10 +579,10 @@ def profile_nodes(nnc, net, graphs, stream, pk, dtype="f32", algorithm=-1):
         s["ms"] += r["ms"]
         s["flops"] += r["flops"]
         s["bytes"] += r["bytes"]
-    # tensor peak of the math the contractions run in: bf16 / fp16 = the measured cuBLAS bf16 number; TF32 = half of it;
+    # tensor peak of the math the contractions run in: bf16 / fp16 = the data-sheet dense bf16 rate; TF32 = half of it;
     # 3xTF32 = a third of the TF32 rate (three MMAs per product)
     tf32_peak = pk["bf16_tflops"] if dtype != "f32" else pk["bf16_tflops"] / 2.0 / (3.0 if algorithm == 1 else 1.0)
-    peak_note = "bf16 cuBLAS burst peak" if dtype != "f32" else ("bf16 cuBLAS burst peak / 2 (TF32 tensor rate is half the bf16 rate)" + (" / 3 (3xTF32 issues three MMAs per product)" if algorithm == 1 else ""))
+    peak_note = "dense bf16" if dtype != "f32" else ("dense bf16 / 2 (TF32 tensor rate is half the bf16 rate)" + (" / 3 (3xTF32 issues three MMAs per product)" if algorithm == 1 else ""))
     for k, s in summary.items():
         if s["flops"] > 0:
             s["tflops"] = s["flops"] / (s["ms"] * 1e-3) / 1e12
@@ -558,18 +595,8 @@ def profile_nodes(nnc, net, graphs, stream, pk, dtype="f32", algorithm=-1):
     # every contraction command against ITS OWN bound, max(flops / tensor peak, algorithmic bytes / HBM peak): the 1x1 convolutions and the
     # stem move more bytes than they have flops for (half of the 110 convolution commands of ResNet-50 at N = 256 are HBM-bound)
     bound_ms = sum(max(r["flops"] / (tf32_peak * 1e12), r["bytes"] / (pk["hbm_gbs"] * 1e9)) for r in tc) * 1e3
-    # DRAM bytes of the same launches from one ncu capture (tools/run_ncu_profiles.sh -> profiles/): all
-    # contraction launches of one step, to be read against the algorithmic operand + result bytes of those commands
-    traffic, traffic_note = None, None
-    try:
-        t = json.load(open(os.path.join(ROOT, "profiles", "r02_contraction_traffic.json")))
-        traffic, traffic_note = float(t["dram_bytes_per_step"]), "dram__bytes_read.sum + dram__bytes_write.sum over the %d contraction launches of one step (ncu, tools/run_ncu_profiles.sh -> profiles/r02_contraction_traffic.json)" % t["launches"]
-    except Exception:
-        pass
-    if dtype != "f32" or algorithm == 1:
-        traffic, traffic_note = None, None  # the committed ncu capture is of the fp32 / TF32 configuration
-    roofline = {"bound": "tensor", "kernel": "umma_* (tcgen05 GEMM / implicit-GEMM convolution kernels; all convolution + GEMM commands of one step)", "achieved": achieved, "peak": tf32_peak, "unit": "TFLOP/s",
-                "frac": achieved / tf32_peak, "traffic": traffic, "traffic_note": traffic_note, "algorithmic_bytes_per_step": sum(r["bytes"] for r in tc),
+    roofline = {"bound": "tensor", "kernel": "umma_gemm_kernel (wgmma GEMM / implicit-GEMM convolution kernel; all convolution + GEMM commands of one step)", "achieved": achieved, "peak": tf32_peak, "unit": "TFLOP/s",
+                "frac": achieved / tf32_peak, "algorithmic_bytes_per_step": sum(r["bytes"] for r in tc),
                 "peak_source": "%s %s" % (pk["source"], peak_note),
                 "launch_ms_total": tc_ms, "algorithmic_flops_per_step": tc_flops, "total_ms_all_commands": sum(r["ms"] for r in rows),
                 "per_command_bound_ms": bound_ms, "frac_of_per_command_bound": bound_ms / tc_ms if tc_ms > 0 else None,

@@ -344,7 +344,7 @@ int exec_gemm_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 	}
 	if (kind != 0)
 	{
-		// 16-bit operands: tcgen05 kind::f16, fp32 accumulate; the bias may be fp32 or in the operands' type
+		// 16-bit operands: wgmma (bf16 / fp16), fp32 accumulate; the bias may be fp32 or in the operands' type
 		const char* const bias_p = bias_t ? (const char*)bias.p : 0;
 		const bool bias32 = bias_t && is_f32(bias_t);
 		for (int i = 0; i < b.batch; i++)
@@ -584,7 +584,7 @@ bool conv_geom(const ccv_nnc_cmd_t& cmd, const ccv_nnc_hint_t& hint, const TV& a
 // [i K/g, (i+1) K/g) -- `groups` independent dense convolutions whose operands are channel SLICES of the NHWC tensors (pixel stride
 // C, not C/g) except for the filters, whose rows are contiguous per group.  When a group is wide enough to fill tensor-core tiles
 // (C/g and K/g multiples of the 16-byte vector and >= 16) each group's slices are made dense in the stream workspace (one strided
-// copy in, one out), and the dense tcgen05 kernels above do the arithmetic; narrower groups (depthwise and the like) stay on the
+// copy in, one out), and the dense wgmma kernels above do the arithmetic; narrower groups (depthwise and the like) stay on the
 // FFMA kernels, where the contraction is too short for a 64-deep MMA anyway.  PASS 0 = fprop, 1 = wgrad, 2 = dgrad.
 // returns 0 done, 1 not applicable (caller falls back), < 0 error
 template <int PASS>
@@ -673,7 +673,7 @@ int conv_forw_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 	const int kind = kind_of(inputs[0]);
 	if (kind > 0)
 	{
-		// bf16 / fp16 tensors: NHWC, one group, tcgen05 kind::f16 with fp32 accumulation; the bias is fp32 or of the tensors' type
+		// bf16 / fp16 tensors: NHWC, one group, wgmma bf16 / fp16 with fp32 accumulation; the bias is fp32 or of the tensors' type
 		if (kind_of(inputs[1]) != kind || kind_of(outputs[0]) != kind || (bias_t && ((kind_of(bias_t) != kind && !is_f32(bias_t)) || CCV_IS_TENSOR_VIEW(bias_t))))
 			return CCV_NNC_EXEC_INVALID;
 		ConvGeom g16;

@@ -150,7 +150,7 @@ static int sdpa_forw_core(SM100_EXEC_ARGS)
 	}
 	if (dt != CCV_32F)
 	{
-		// 16-bit tensors: the tcgen05 flash-attention kernel (sm100_fmha.cu) when it covers the call -- no additive mask (like the
+		// 16-bit tensors: the wgmma flash-attention kernel (sm100_fmha.cu) when it covers the call -- no additive mask (like the
 		// reference's flash-attention backend), head dimension 128; it also writes the log-sum-exp
 		float* lse = 0;
 		if (output_size > 1 && outputs[1])
@@ -269,7 +269,7 @@ int ccv_nnc_sm100_exec_sdpa_back(SM100_EXEC_ARGS)
 			return CCV_NNC_EXEC_INVALID;
 		if (dg.B != g.B || dg.H != g.H || dg.Hk != g.Hk || dg.Sq != g.Sq || dg.Sk != g.Sk || dg.D != g.D || dg.Dv != g.Dv)
 			return CCV_NNC_EXEC_INVALID;
-		// the fused tcgen05 backward (sm100_fmha_bwd.cu) when it covers the call: head dimension 128, 16-byte aligned rows.  It works
+		// the fused wgmma backward (sm100_fmha_bwd.cu) when it covers the call: head dimension 128, 16-byte aligned rows.  It works
 		// from the forward's saved output and log-sum-exp (inputs[9], inputs[10]: ...flash_attn.cu:240-241) and recomputes both itself
 		// when the caller does not pass them.
 		{

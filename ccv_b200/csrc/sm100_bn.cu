@@ -22,7 +22,7 @@ static int sms()
 		cudaGetDevice(&dev);
 		cudaDeviceGetAttribute(&g_sms_bn, cudaDevAttrMultiProcessorCount, dev);
 		if (g_sms_bn <= 0)
-			g_sms_bn = 148;
+			g_sms_bn = 132;
 	}
 	return g_sms_bn;
 }
@@ -136,7 +136,7 @@ __global__ void __launch_bounds__(256) bn_reduce_kernel(const T* __restrict__ x,
 			for (int k = 0; k < W; k++)
 				s1[k] += sh[0][t * cpb + tx][k], s2[k] += sh[1][t * cpb + tx][k];
 		// per-block partial sums; bn_finalize_partials_kernel adds the gridDim.y rows in a fixed order (no atomics: 600 same-address
-		// fp64 atomics per channel cost ~15 us per launch, profiles/r01_ncu_bn_reduce_apply.txt, and made the result run-dependent)
+		// fp64 atomics per channel made the result run-dependent)
 		float* const row = part + (size_t)blockIdx.y * 2 * C;
 #pragma unroll
 		for (int k = 0; k < W; k++)
@@ -312,7 +312,7 @@ __global__ void __launch_bounds__(1024) bn_finalize_partials_kernel(const float*
 	}
 }
 
-// Forward finalisation from the statistics a convolution epilogue produced (sm100_umma_persistent.cuh): four planes [rows][C] --
+// Forward finalisation from the statistics a convolution epilogue produced (sm100_umma_gemm.cuh): four planes [rows][C] --
 // count n_i, shift k_i, s1_i = sum(v - k_i), s2_i = sum((v - k_i)^2) -- one row per (CTA, epilogue warp quarter); rows with
 // count 0 were never touched.  Each slot is its own shifted one-pass estimate.  They are combined in double precision, in a
 // fixed order (32 row-lanes per channel, then lane by lane), in two sweeps over the (L2-resident) slots:

@@ -1,10 +1,9 @@
-// sm100_contract.cu -- host-side launchers for the tcgen05/TMA contraction kernel (sm100_umma_gemm.cuh):
+// sm100_contract.cu -- host-side launchers for the wgmma/TMA contraction kernel (sm100_umma_gemm.cuh):
 // tensor-map encoding (tile and im2col mode) and the mapping of GEMM / convolution fprop / dgrad / wgrad
 // onto its operand modes.  Reference semantics being reproduced: lib/nnc/cmd/blas/ccv_nnc_gemm_cpu_ref.c:110-448,
 // lib/nnc/cmd/convolution/ccv_nnc_conv_cpu_ref.c:13-345 (NHWC).
 #include "sm100_contract.h"
-#include "sm100_umma_persistent.cuh"
-#include "sm100_umma_wgrad.cuh"
+#include "sm100_umma_gemm.cuh"
 #include "sm100_elem.cuh"
 #include <atomic>
 #include <mutex>
@@ -56,7 +55,7 @@ static bool tma_api_init()
 }
 
 // Math mode of the launches a contraction entry point issues: 0 = one-pass TF32 (operands rounded to TF32 by the TMA unit),
-// 1 = 3xTF32 (raw fp32 operands, hi / lo split in shared memory, three MMAs per k-step; persistent kernel only).  Set by the
+// 1 = 3xTF32 (raw fp32 operands, hi / lo split in shared memory, three MMAs per k-step).  Set by the
 // entry points for the duration of the call (host thread local, like the statistics request).
 static thread_local int t_x3 = 0;
 struct X3Scope {
@@ -66,7 +65,8 @@ struct X3Scope {
 };
 static inline int operand_dtype() { return t_x3 ? (int)CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : g_tma_dtype; }
 
-// fp32 2-D row-major [rows, cols] with row pitch `ld` elements; box = {box_cols (<= 32), box_rows}
+// fp32 2-D row-major [rows, cols] with row pitch `ld` elements; box = {box_cols (<= 32), box_rows}.  K-major operand tiles are
+// 128-byte swizzled (the wgmma layout); MN-major ones land unswizzled and the kernel transposes them (sm100_umma_gemm.cuh)
 static bool make_map_2d(CUtensorMap* map, const float* ptr, long long rows, long long cols, long long ld, int box_cols, int box_rows, bool mn_major = false, int dtype = -1)
 {
 	if (dtype < 0)
@@ -77,14 +77,13 @@ static bool make_map_2d(CUtensorMap* map, const float* ptr, long long rows, long
 	cuuint64_t strides[1] = { (cuuint64_t)ld * 4 };
 	cuuint32_t box[2] = { (cuuint32_t)box_cols, (cuuint32_t)box_rows };
 	cuuint32_t estr[2] = { 1, 1 };
-	CUresult r = g_encode_tiled(map, (CUtensorMapDataType)dtype, 2, (void*)ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, mn_major ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+	CUresult r = g_encode_tiled(map, (CUtensorMapDataType)dtype, 2, (void*)ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, mn_major ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 	return r == CUDA_SUCCESS;
 }
 
 // 16-bit (bf16 / fp16) 2-D row-major [rows, cols], row pitch `ld` elements; box = {box_cols (<= 64 = one 128-byte span), box_rows}.
-// kind: 1 = bf16, 2 = fp16.  MN-major 16-bit operands use the ordinary 128-byte swizzle (64-element atoms).  swizzle64: the
-// 32 x 32 output chunks of the TMA-store epilogue (64-byte rows).
-static bool make_map_2d16(CUtensorMap* map, const void* ptr, int kind, long long rows, long long cols, long long ld, int box_cols, int box_rows, bool swizzle64 = false)
+// kind: 1 = bf16, 2 = fp16.  MN-major 16-bit operands use the same 128-byte swizzle (64-element atoms, wgmma's transposed layout).
+static bool make_map_2d16(CUtensorMap* map, const void* ptr, int kind, long long rows, long long cols, long long ld, int box_cols, int box_rows)
 {
 	if ((((uintptr_t)ptr) & 15) || ((ld * 2) & 15) || ld * 2 >= (1ll << 40))
 		return false;
@@ -93,7 +92,7 @@ static bool make_map_2d16(CUtensorMap* map, const void* ptr, int kind, long long
 	cuuint32_t box[2] = { (cuuint32_t)box_cols, (cuuint32_t)box_rows };
 	cuuint32_t estr[2] = { 1, 1 };
 	const CUresult r = g_encode_tiled(map, kind == 1 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (void*)ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-		swizzle64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+		CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 	return r == CUDA_SUCCESS;
 }
 // 16-bit NHWC tensor {C, W, H, N} in im2col mode (element strides sn, sh, sw; channel stride 1)
@@ -136,7 +135,7 @@ static bool make_map_im2col(CUtensorMap* map, const float* ptr, int N, int H, in
 	int lower[2] = { lower_w, lower_h };
 	int upper[2] = { upper_w, upper_h };
 	cuuint32_t estr[4] = { 1, (cuuint32_t)trav_w, (cuuint32_t)trav_h, 1 };
-	CUresult r = g_encode_im2col(map, (CUtensorMapDataType)dtype, 4, (void*)ptr, dims, strides, lower, upper, (cuuint32_t)channels, (cuuint32_t)pixels, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, mn_major ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+	CUresult r = g_encode_im2col(map, (CUtensorMapDataType)dtype, 4, (void*)ptr, dims, strides, lower, upper, (cuuint32_t)channels, (cuuint32_t)pixels, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, mn_major ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 	if (r != CUDA_SUCCESS)
 		return false;
 	// Same driver workaround CUTLASS applies (cute/atom/copy_traits_sm90_im2col.hpp): for tensors under 128 KiB, drivers
@@ -156,7 +155,7 @@ static int num_sms()
 		cudaGetDevice(&dev);
 		cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
 		if (g_num_sms <= 0)
-			g_num_sms = 148;
+			g_num_sms = 132;
 	}
 	return g_num_sms;
 }
@@ -290,7 +289,7 @@ static int fit_splits(int splits, int k_iters, size_t slice_bytes, const Scratch
 }
 
 // One-shot request (per host thread) for per-column output statistics from the next forward-shaped launch: set by the fused
-// convolution + batch-norm command, consumed (and cleared) by launch_umma_persistent when the launch qualifies.
+// convolution + batch-norm command, consumed (and cleared) by launch_umma when the launch qualifies.
 struct StatsRequest {
 	float* part;
 	int max_rows;
@@ -304,17 +303,44 @@ void conv_stats_request(float* part, int max_rows, int* rows_out)
 		*rows_out = 0;
 }
 
-template <int AMODE, int BMODE, int BN, int STAGES>
-static int launch_umma(cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB, const UmmaGemmParams& p, int grid_x, int grid_y)
+template <int AMODE, int BMODE, int BN, int X3 = 0, int K16 = 0, int OUT16 = 0>
+static int launch_umma(cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB, const UmmaGemmParams& p)
 {
-	using S = UmmaSmem<BN, STAGES>;
-	auto kern = umma_gemm_kernel<AMODE, BMODE, BN, STAGES>;
+	constexpr bool XF = GemmXform<AMODE, BMODE, K16, X3>::ANY;
+	constexpr int STAGES = GemmStages<BN, XF, X3>::value;
+	using S = UmmaSmem<BN, STAGES, XF, X3>;
+	auto kern = umma_gemm_kernel<AMODE, BMODE, BN, STAGES, X3, K16, OUT16>;
 	static bool configured[MAX_DEVICES];
 	if (ensure_dynamic_smem(kern, S::TOTAL, configured, "cudaFuncSetAttribute(umma_gemm_kernel)"))
 		return -1;
-	dim3 grid(grid_x, grid_y, p.grid_taps * p.splits);
-	t_stats_request.part = 0; // this kernel does not produce statistics: the requester sees rows_out == 0
-	kern<<<grid, 192, S::TOTAL, stream>>>(tmA, tmB, p);
+	const int tiles_m = (p.M + UMMA_BLOCK_M - 1) / UMMA_BLOCK_M, tiles_n = (p.N + BN - 1) / BN;
+	dim3 grid(tiles_m, tiles_n, p.grid_taps * p.splits);
+	UmmaGemmParams q = p;
+	q.stats = 0, q.stats_rows = 0;
+	if (t_stats_request.part)
+	{
+		const StatsRequest r = t_stats_request;
+		t_stats_request.part = 0;
+		// forward-shaped launches only (one statistics slot row per CTA column and 32-row quarter): each CTA walks every gridDim.x-th
+		// M tile, so the slots fit the statistics tensor and the launch still fills the SMs once
+		if (!XF && AMODE != OP_MN2D && BMODE == OP_K2D && p.splits == 1 && p.grid_taps == 1 && p.rowmap.mode == 0 && !p.accumulate && r.max_rows >= 4)
+		{
+			int gx = num_sms() / tiles_n;
+			gx = gx < 1 ? 1 : gx;
+			gx = gx < r.max_rows / 4 ? gx : r.max_rows / 4;
+			gx = gx < tiles_m ? gx : tiles_m;
+			const cudaError_t e = cudaMemsetAsync(r.part, 0, (size_t)gx * 4 * p.N * sizeof(float), stream); // the count plane
+			if (e != cudaSuccess)
+			{
+				set_last_error("memset(conv stats)", e);
+				return -1;
+			}
+			grid.x = gx;
+			q.stats = r.part, q.stats_rows = gx * 4;
+			*r.rows_out = gx * 4;
+		}
+	}
+	kern<<<grid, GEMM_THREADS, S::TOTAL, stream>>>(tmA, tmB, q);
 	count_launch();
 	cudaError_t e = cudaGetLastError();
 	if (e != cudaSuccess)
@@ -325,137 +351,12 @@ static int launch_umma(cudaStream_t stream, const CUtensorMap& tmA, const CUtens
 	return 0;
 }
 
-template <int AMODE, int BMODE, int BN, int STAGES, int EPIW, int X3 = 0, int K16 = 0, int OUT16 = 0>
-static int launch_umma_persistent(cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB, const UmmaGemmParams& p)
-{
-	using S = UmmaPersistentSmem<BN, STAGES, EPIW, X3>;
-	auto kern = umma_gemm_persistent_kernel<AMODE, BMODE, BN, STAGES, EPIW, X3, K16, OUT16>;
-	static bool configured[MAX_DEVICES];
-	if (ensure_dynamic_smem(kern, S::TOTAL, configured, "cudaFuncSetAttribute(umma_gemm_persistent_kernel)"))
-		return -1;
-	const long long tiles = (long long)((p.M + UMMA_BLOCK_M - 1) / UMMA_BLOCK_M) * ((p.N + BN - 1) / BN) * p.grid_taps * p.splits;
-	int grid = (int)(tiles < num_sms() ? tiles : num_sms());
-	// with statistics requested every tile of a CTA must cover the same output columns (the epilogue keeps its per-column sums in
-	// registers for the whole kernel): tile = blockIdx.x + i * grid and n_blk = tile % tiles_n, so grid becomes a multiple of tiles_n
-	const int tiles_n_ = (p.N + BN - 1) / BN;
-	if (t_stats_request.part && tiles_n_ > 1 && grid >= tiles_n_)
-		grid = grid / tiles_n_ * tiles_n_;
-	UmmaGemmParams q = p;
-	q.stats = 0, q.stats_rows = 0;
-	// TMA tile stores for the plain "write the tile" epilogue (dense row-major output, no split-K, no accumulate)
-	CUtensorMap tmC = tmA;
-	static int tma_store_enabled = -1;
-	if (tma_store_enabled < 0)
-	{
-		const char* e = getenv("CCV_NNC_SM100_TMA_STORE");
-		tma_store_enabled = e ? atoi(e) : 1;
-	}
-	q.tma_store = 0;
-	if (tma_store_enabled && p.splits == 1 && p.grid_taps == 1 && !p.accumulate && p.rowmap.mode == 0 && (!p.bias || (((uintptr_t)p.bias) & 15) == 0))
-	{
-		if (!OUT16 && p.N % 4 == 0 && make_map_2d(&tmC, p.out, p.M, p.N, p.rowmap.ld, 32, 32, false, (int)CU_TENSOR_MAP_DATA_TYPE_FLOAT32))
-			q.tma_store = 1;
-		if (OUT16 && p.N % 8 == 0 && (!p.bias16 || (((uintptr_t)p.bias16) & 15) == 0) && make_map_2d16(&tmC, p.out, p.out_kind, p.M, p.N, p.rowmap.ld, 32, 32, true))
-			q.tma_store = 1;
-	}
-	if (t_stats_request.part)
-	{
-		const StatsRequest r = t_stats_request;
-		t_stats_request.part = 0;
-		// forward-shaped launches only; the statistics ride on the TMA-store epilogue (one slot row per CTA and warp quarter)
-		if (q.tma_store && AMODE != OP_MN2D && BMODE == OP_K2D && p.N % 32 == 0 && grid * 4 <= r.max_rows && (tiles_n_ == 1 || grid % tiles_n_ == 0))
-		{
-			const cudaError_t e = cudaMemsetAsync(r.part, 0, (size_t)grid * 4 * p.N * sizeof(float), stream); // the count plane
-			if (e != cudaSuccess)
-			{
-				set_last_error("memset(conv stats)", e);
-				return -1;
-			}
-			q.stats = r.part, q.stats_rows = grid * 4;
-			*r.rows_out = grid * 4;
-		}
-	}
-	kern<<<grid, S::THREADS, S::TOTAL, stream>>>(tmA, tmB, tmC, q);
-	count_launch();
-	cudaError_t e = cudaGetLastError();
-	if (e != cudaSuccess)
-	{
-		set_last_error("umma_gemm_persistent_kernel launch", e);
-		return -1;
-	}
-	return 0;
-}
-
-// Kernel choice, from the measurements in profiles/r01_probe3_*.log and r01_probe4_*.log:
-//  * BN = 64 (<= 64 output columns) data gradients / transposed products and weight gradients with <= 128 columns: the
-//    one-tile-per-CTA kernel, two CTAs per SM (these are L2-bound / short tiles; two independent CTAs hide more latency
-//    than one persistent CTA); BN = 64 forward-shaped products (K-major filters) do gain from the persistent kernel
-//    (profiles/r01_probe5_wgrad_taps.log: 32 -> 64 at 112 x 112 fprop 0.635 -> 0.498 ms, dgrad 0.837 -> 1.131 ms);
-//  * otherwise the persistent kernel: long reductions (>= 12 k-iterations per tile) use 4 epilogue warps and the deepest
-//    operand pipeline (MMA-bound), short ones use 8 epilogue warps (the epilogue is then the critical path).
-// CCV_NNC_SM100_PERSISTENT=0 forces the one-tile kernel, =2 forces the persistent one, for A/B runs.
-static int persistent_mode()
-{
-	static int v = -1;
-	if (v < 0)
-	{
-		const char* e = getenv("CCV_NNC_SM100_PERSISTENT");
-		v = e ? atoi(e) : 1;
-	}
-	return v;
-}
-static bool use_persistent() { return persistent_mode() != 0; }
-
-template <int AMODE, int BMODE>
-static int launch_umma_bn(cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB, const UmmaGemmParams& p, int bn)
-{
-	if (t_x3)
-	{
-		// 2 x (A + B) per stage: BN <= 128; four epilogue warps + four split warps
-		if (bn == 64)
-			return launch_umma_persistent<AMODE, BMODE, 64, 4, 4, 1>(stream, tmA, tmB, p);
-		return launch_umma_persistent<AMODE, BMODE, 128, 3, 4, 1>(stream, tmA, tmB, p);
-	}
-	const int mode = persistent_mode();
-	const int iters_per_tile = (p.k_iters + p.splits - 1) / p.splits;
-	bool persistent = mode != 0;
-	if (mode == 1 && ((bn == 64 && !(AMODE != OP_MN2D && BMODE == OP_K2D && p.splits == 1)) || (BMODE == OP_IM2COL && bn == 128)))
-		persistent = false; // bn = 64: only forward-shaped work (K-major B, no split-K) gains from the persistent kernel (r01_probe5)
-	if (persistent)
-	{
-		bool long_k = iters_per_tile >= 12;
-		static int force_long_k = -2;
-		if (force_long_k == -2)
-		{
-			const char* e = getenv("CCV_NNC_SM100_LONGK"); // A/B switch: 1 = always 4 epilogue warps + deepest ring, 0 = always 8 + shorter ring
-			force_long_k = e ? atoi(e) : -1;
-		}
-		if (force_long_k >= 0)
-			long_k = force_long_k != 0;
-		if (bn == 64)
-			return launch_umma_persistent<AMODE, BMODE, 64, 6, 8>(stream, tmA, tmB, p);
-		if (bn == 256)
-			return long_k ? launch_umma_persistent<AMODE, BMODE, 256, 4, 4>(stream, tmA, tmB, p) : launch_umma_persistent<AMODE, BMODE, 256, 3, 8>(stream, tmA, tmB, p);
-		return long_k ? launch_umma_persistent<AMODE, BMODE, 128, 6, 4>(stream, tmA, tmB, p) : launch_umma_persistent<AMODE, BMODE, 128, 5, 8>(stream, tmA, tmB, p);
-	}
-	if (bn == 256)
-		bn = 128;
-	const int gx = (p.M + UMMA_BLOCK_M - 1) / UMMA_BLOCK_M;
-	const int gy = (p.N + bn - 1) / bn;
-	if (bn == 64)
-		return launch_umma<AMODE, BMODE, 64, 4>(stream, tmA, tmB, p, gx, gy);
-	return launch_umma<AMODE, BMODE, 128, 3>(stream, tmA, tmB, p, gx, gy);
-}
-
+// output tile width: 64 columns for narrow outputs, else 128 (wgmma m64n128 per consumer warpgroup: 64 fp32 accumulator registers)
 static int pick_bn(int N)
 {
 	const char* e = getenv("CCV_NNC_SM100_BN");
-	int bn = e ? atoi(e) : (N <= 64 ? 64 : (N <= 128 ? 128 : 256));
-	if (bn != 64 && bn != 128 && bn != 256)
-		bn = 128;
-	if (bn == 256 && (!use_persistent() || t_x3))
-		bn = 128;
-	return bn;
+	int bn = e ? atoi(e) : (N <= 64 ? 64 : 128);
+	return bn == 64 ? 64 : 128;
 }
 
 static void init_params(UmmaGemmParams& p)
@@ -463,26 +364,15 @@ static void init_params(UmmaGemmParams& p)
 	memset(&p, 0, sizeof(p));
 	p.splits = 1;
 	p.grid_taps = 1;
-	p.alpha = 1.f;
 	p.stride_h = p.stride_w = 1;
 	p.P = p.Q = 1;
-	static int lbo = -1, sbo = -1, layout = -1;
-	if (lbo < 0)
-	{
-		const char* e;
-		lbo = (e = getenv("CCV_NNC_SM100_MN_LBO")) ? atoi(e) : 4096;
-		sbo = (e = getenv("CCV_NNC_SM100_MN_SBO")) ? atoi(e) : 512;
-		layout = (e = getenv("CCV_NNC_SM100_MN_LAYOUT")) ? atoi(e) : 1;
-	}
-	p.mn_lbo = lbo, p.mn_sbo = sbo, p.mn_layout = layout;
-	p.kind16 = 0, p.out_kind = 0, p.bias16 = 0;
 }
 
 static int pick_splits(long long tiles, int k_iters, int min_iters_per_split)
 {
 	// Split-K factor against wave quantisation.  Model: `tiles * s` work items of size 1 / s run in rounds of one per SM, so the
 	// launch costs ceil(tiles * s / SMs) / s tile-times.  5 tiles -> s = 59 (295 CTAs, one wave of 2 CTAs per SM; s = 60 would
-	// spill 4 CTAs into a second wave and double the time, profiles/r01_ncu_wgrad_taps64.txt); 196 tiles (7 x 7 layers, N = 512)
+	// spill 4 CTAs into a second wave and double the time); 196 tiles (7 x 7 layers, N = 512)
 	// -> s = 3 (588 items, 3.97 rounds of thirds instead of 2 rounds of which the second is 1/3 full).  When the tiles already fill
 	// the machine a split is only taken if it buys more than 20 % (partial tiles cost a zero-fill, red.add traffic and the fused
 	// batch-norm statistics of the epilogue), never finer than `min_iters_per_split`.
@@ -558,37 +448,31 @@ static void init_params_kind(UmmaGemmParams& p, int kind)
 	init_params(p);
 	if (kind)
 	{
-		// 16-bit MN-major operands: ordinary 128-byte swizzle, 64-element atoms; boxes of 64 k-rows x 128 B; K = 16 per MMA
+		// 16-bit operands: 64 elements per 128-byte row, K = 16 per MMA
 		p.kind16 = 1;
-		p.mn_lbo = 64 * 128, p.mn_sbo = 1024, p.mn_layout = 2;
 		p.out_kind = kind;
 	}
 }
-static inline uint32_t idesc_kind(int kind, int a_mn_major, int b_mn_major, int bn)
-{
-	return umma_instr_desc(kind == 0 ? 2 : (kind == 1 ? 1 : 0), a_mn_major, b_mn_major, UMMA_BLOCK_M, bn);
-}
-// kernel choice per kind: fp32 goes through the measured table of launch_umma_bn; 16-bit always takes the persistent kernel with
-// eight epilogue warps (the MMAs are twice as fast, the epilogue is the critical path); out16 = the output tensor is 16-bit
-// (false for split-K slices, which stay fp32)
+// kernel per kind: fp32 as TF32 or 3xTF32 (t_x3); bf16 / fp16 (one kernel per element type) with a 16-bit output (out16) or fp32
+// split-K slices
 template <int AMODE, int BMODE>
 static int launch_kind(cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB, const UmmaGemmParams& p, int bn, int kind, bool out16)
 {
 	if (kind == 0)
-		return launch_umma_bn<AMODE, BMODE>(stream, tmA, tmB, p, bn);
-	if (out16)
 	{
-		if (bn == 64)
-			return launch_umma_persistent<AMODE, BMODE, 64, 6, 8, 0, 1, 1>(stream, tmA, tmB, p);
-		if (bn == 256)
-			return launch_umma_persistent<AMODE, BMODE, 256, 3, 8, 0, 1, 1>(stream, tmA, tmB, p);
-		return launch_umma_persistent<AMODE, BMODE, 128, 5, 8, 0, 1, 1>(stream, tmA, tmB, p);
+		if (t_x3)
+			return bn == 64 ? launch_umma<AMODE, BMODE, 64, 1>(stream, tmA, tmB, p) : launch_umma<AMODE, BMODE, 128, 1>(stream, tmA, tmB, p);
+		return bn == 64 ? launch_umma<AMODE, BMODE, 64>(stream, tmA, tmB, p) : launch_umma<AMODE, BMODE, 128>(stream, tmA, tmB, p);
 	}
-	if (bn == 64)
-		return launch_umma_persistent<AMODE, BMODE, 64, 6, 8, 0, 1, 0>(stream, tmA, tmB, p);
-	if (bn == 256)
-		return launch_umma_persistent<AMODE, BMODE, 256, 3, 8, 0, 1, 0>(stream, tmA, tmB, p);
-	return launch_umma_persistent<AMODE, BMODE, 128, 5, 8, 0, 1, 0>(stream, tmA, tmB, p);
+	if (kind == 1)
+	{
+		if (out16)
+			return bn == 64 ? launch_umma<AMODE, BMODE, 64, 0, 1, 1>(stream, tmA, tmB, p) : launch_umma<AMODE, BMODE, 128, 0, 1, 1>(stream, tmA, tmB, p);
+		return bn == 64 ? launch_umma<AMODE, BMODE, 64, 0, 1, 0>(stream, tmA, tmB, p) : launch_umma<AMODE, BMODE, 128, 0, 1, 0>(stream, tmA, tmB, p);
+	}
+	if (out16)
+		return bn == 64 ? launch_umma<AMODE, BMODE, 64, 0, 2, 1>(stream, tmA, tmB, p) : launch_umma<AMODE, BMODE, 128, 0, 2, 1>(stream, tmA, tmB, p);
+	return bn == 64 ? launch_umma<AMODE, BMODE, 64, 0, 2, 0>(stream, tmA, tmB, p) : launch_umma<AMODE, BMODE, 128, 0, 2, 0>(stream, tmA, tmB, p);
 }
 
 // Launch with the split factor already chosen in p.splits.  One split: straight into `out` (pitch ldo, element kind `kind`).
@@ -649,7 +533,6 @@ static int gemm_any(cudaStream_t stream, int kind, int M, int N, int K, const vo
 	p.chunks_per_tap = p.k_iters;
 	p.bias = bias, p.bias16 = bias ? 0 : bias16;
 	p.rowmap.mode = 0, p.rowmap.ld = ldc;
-	p.idesc = idesc_kind(kind, trans_a, !trans_b, bn);
 	const long long tiles = (long long)((M + 127) / 128) * ((N + bn - 1) / bn);
 	p.splits = p.bias16 ? 1 : fit_splits(pick_splits(tiles, p.k_iters, 8), p.k_iters, slice_bytes(M, N), scratch);
 	if (!trans_a && trans_b)
@@ -731,7 +614,6 @@ static int conv_fprop_any(cudaStream_t stream, int kind, const ConvGeom& g, cons
 		}
 	p.out = (float*)b, p.bias = bias, p.bias16 = bias ? 0 : bias16;
 	p.rowmap.mode = 0, p.rowmap.ld = g.K;
-	p.idesc = idesc_kind(kind, 0, 0, bn);
 	return launch_kind<OP_IM2COL, OP_K2D>(stream, tmA, tmB, p, bn, kind, kind != 0);
 }
 int conv_fprop_tf32(cudaStream_t stream, const ConvGeom& g, const float* a, const float* w, const float* bias, float* b, const Scratch& scratch, int x3)
@@ -854,7 +736,6 @@ static int conv_dgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, cons
 			p.rowmap.n_stride = (long long)g.H * g.W * g.C;
 			p.rowmap.h_stride = (long long)g.stride_h * g.W * g.C;
 			p.rowmap.w_stride = (long long)g.stride_w * g.C;
-			p.idesc = idesc_kind(kind, 0, 1, bn);
 			const int rc = launch_kind<OP_IM2COL, OP_MN2D>(stream, tmA, tmB, p, bn, kind, kind != 0);
 			if (rc)
 				return rc;
@@ -868,38 +749,6 @@ int conv_dgrad_tf32(cudaStream_t stream, const ConvGeom& g, const float* grad_b,
 int conv_dgrad_16(cudaStream_t stream, int kind, const ConvGeom& g, const void* grad_b, const void* w, void* grad_a, const Scratch& scratch)
 {
 	return kind == 1 || kind == 2 ? conv_dgrad_any(stream, kind, g, grad_b, w, grad_a, scratch, 0) : 1;
-}
-
-// Filter gradient with few filters (K <= 64): taps packed along the UMMA M dimension (sm100_umma_wgrad.cuh).
-template <int BN>
-static int launch_wgrad_taps(cudaStream_t stream, const CUtensorMap& tmX, const CUtensorMap& tmG, const WgradTapsParams& p, int tiles)
-{
-	constexpr int STAGES = 4;
-	using S = WgradTapsSmem<BN, STAGES>;
-	auto kern = umma_wgrad_taps_kernel<BN, STAGES>;
-	static bool configured[MAX_DEVICES];
-	if (ensure_dynamic_smem(kern, S::TOTAL, configured, "cudaFuncSetAttribute(umma_wgrad_taps_kernel)"))
-		return -1;
-	kern<<<dim3(tiles, p.splits), 192, S::TOTAL, stream>>>(tmX, tmG, p);
-	count_launch();
-	cudaError_t e = cudaGetLastError();
-	if (e != cudaSuccess)
-	{
-		set_last_error("umma_wgrad_taps_kernel launch", e);
-		return -1;
-	}
-	return 0;
-}
-
-static bool wgrad_taps_enabled()
-{
-	static int v = -1;
-	if (v < 0)
-	{
-		const char* e = getenv("CCV_NNC_SM100_WGRAD_TAPS");
-		v = e ? atoi(e) : 1;
-	}
-	return v != 0;
 }
 
 static int conv_wgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, const void* grad_b, const void* a, void* grad_w, int accumulate, const Scratch& scratch, int x3)
@@ -923,7 +772,6 @@ static int conv_wgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, cons
 	p.k_iters = (int)((npq + bk - 1) / bk);
 	p.chunks_per_tap = p.k_iters;
 	p.rowmap.mode = 0, p.rowmap.ld = rsc;
-	p.idesc = idesc_kind(kind, 1, 1, bn);
 	const long long tiles = (long long)((g.K + 127) / 128) * ((g.C + bn - 1) / bn) * g.R * g.S;
 	// split-K slices have the layout of dW itself ([K, RSC]); splitk_reduce adds them (and the old dW when accumulating)
 	const size_t dw_bytes = (size_t)g.K * rsc * sizeof(float);
@@ -937,35 +785,6 @@ static int conv_wgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, cons
 	}
 	if (!map_im2col(&tmB, kind, a, g.N, g.H, g.W, g.C, g.an, g.ah, g.aw, -g.pad_h0, -g.pad_w0, g.pad_h1 - (g.R - 1) * g.dil_h, g.pad_w1 - (g.S - 1) * g.dil_w, g.stride_h, g.stride_w, bk, true))
 		return 1;
-	if (kind == 0 && g.K <= 64 && g.C % 32 == 0 && g.C <= 128 && wgrad_taps_enabled() && !t_x3)
-	{
-		WgradTapsParams w;
-		memset(&w, 0, sizeof(w));
-		w.C = g.C, w.K = g.K, w.taps = g.R * g.S;
-		const int max_tpt = 128 / g.C;
-		const int tiles_m = (w.taps + max_tpt - 1) / max_tpt;
-		w.taps_per_tile = (w.taps + tiles_m - 1) / tiles_m; // balanced: 9 taps of 32 channels -> 3 + 3 + 3
-		w.k_iters = p.k_iters;
-		w.splits = fit_splits(pick_splits(tiles_m, w.k_iters, 16), w.k_iters, dw_bytes, scratch);
-		w.P = g.P, w.Q = g.Q, w.stride_h = g.stride_h, w.stride_w = g.stride_w, w.base_h = -g.pad_h0, w.base_w = -g.pad_w0;
-		for (int r = 0; r < g.R; r++)
-			for (int s = 0; s < g.S; s++)
-				w.tap_off_h[r * g.S + s] = (unsigned short)(r * g.dil_h), w.tap_off_w[r * g.S + s] = (unsigned short)(s * g.dil_w);
-		w.out = (float*)grad_w, w.rsc = rsc;
-		w.mn_lbo = p.mn_lbo, w.mn_sbo = p.mn_sbo, w.mn_layout = p.mn_layout;
-		const int wbn = g.K <= 32 ? 32 : 64;
-		w.idesc = umma_instr_desc(2, 1, 1, UMMA_BLOCK_M, wbn);
-		// one split and nothing to add to: the tile stores go straight to dW; otherwise slices + ordered combine
-		const bool direct = w.splits == 1 && !accumulate;
-		if (!direct && (!scratch.ptr || scratch.bytes < dw_bytes * (size_t)w.splits))
-			return 1;
-		w.out = direct ? (float*)grad_w : (float*)scratch.ptr;
-		w.split_out_stride = (long long)g.K * rsc;
-		const int rc = wbn == 32 ? launch_wgrad_taps<32>(stream, tmB, tmA, w, tiles_m) : launch_wgrad_taps<64>(stream, tmB, tmA, w, tiles_m);
-		if (rc || direct)
-			return rc;
-		return splitk_reduce(stream, (const float*)scratch.ptr, w.splits, w.split_out_stride, g.K, (int)rsc, rsc, (float*)grad_w, rsc, accumulate);
-	}
 	p.grid_taps = g.R * g.S;
 	p.grid_tap_out_stride = g.C;
 	p.P = g.P, p.Q = g.Q;

@@ -31,15 +31,15 @@ struct Scratch {
 constexpr size_t CONTRACT_SCRATCH_BYTES = (size_t)96 << 20;
 
 // x3 (last argument of every entry point): 0 = one-pass TF32, 1 = error-compensated 3xTF32 (fp32-grade products, a third of
-// the tensor rate; sm100_umma_persistent.cuh).
-// returns 0 on success, 1 if the shape/alignment cannot use the TMA+tcgen05 path (caller falls back to FFMA), <0 on CUDA error.
+// the tensor rate; sm100_umma_gemm.cuh).
+// returns 0 on success, 1 if the shape/alignment cannot use the TMA+wgmma path (caller falls back to FFMA), <0 on CUDA error.
 // C[M, N] (+)= op(A) * op(B) + bias; A is [M, K] (lda) or, if trans_a, [K, M]; B is [K, N] (ldb) or, if trans_b, [N, K].
 int gemm_tf32(cudaStream_t stream, int M, int N, int K, const float* a, long long lda, int trans_a, const float* b, long long ldb, int trans_b, float* c, long long ldc, const float* bias, int accumulate, const Scratch& scratch, int x3 = 0);
 int conv_fprop_tf32(cudaStream_t stream, const ConvGeom& g, const float* a, const float* w, const float* bias, float* b, const Scratch& scratch, int x3 = 0);
 int conv_dgrad_tf32(cudaStream_t stream, const ConvGeom& g, const float* grad_b, const float* w, float* grad_a, const Scratch& scratch, int x3 = 0);
 int conv_wgrad_tf32(cudaStream_t stream, const ConvGeom& g, const float* grad_b, const float* a, float* grad_w, int accumulate, const Scratch& scratch, int x3 = 0);
 
-// The same contractions on 16-bit tensors (kind 1 = bf16, 2 = fp16): tcgen05 kind::f16 with fp32 accumulation in TMEM, 16-bit
+// The same contractions on 16-bit tensors (kind 1 = bf16, 2 = fp16): wgmma bf16 / fp16 with fp32 accumulation in registers, 16-bit
 // result (rounded once, to nearest even).  Every leading dimension / channel count must be a multiple of 8 elements (16 bytes).
 // bias: fp32 (bias32) or in the tensors' 16-bit type (bias16); at most one of them.  Returns as above (1 = shape not covered).
 int gemm_16(cudaStream_t stream, int kind, int M, int N, int K, const void* a, long long lda, int trans_a, const void* b, long long ldb, int trans_b, void* c, long long ldc, const float* bias32, const void* bias16, int accumulate, const Scratch& scratch);
@@ -83,11 +83,11 @@ int sdpa_forward_f32(cudaStream_t s, const SdpaGeom& g, const float* q, const fl
 // dg carries the strides of dq / dk / dv in its q_* / k_* / v_* fields
 int sdpa_backward_f32(cudaStream_t s, const SdpaGeom& g, const float* dout, const float* q, const float* k, const float* v, float* dq, float* dk, float* dv, const SdpaGeom& dg, void* workspace);
 
-// 16-bit (bf16 / fp16) flash attention forward on tcgen05 (sm100_fmha.cu): D = Dv = 128; lse [B, H, Sq] fp32 or NULL.
+// 16-bit (bf16 / fp16) flash attention forward on wgmma (sm100_fmha.cu): D = Dv <= 128; lse [B, H, Sq] fp32 or NULL.
 // returns 0 on success, 1 when the shape is not covered, < 0 on CUDA errors
 int sdpa_forward_f16(cudaStream_t s, const SdpaGeom& g, int is_bf16, const void* q, const void* k, const void* v, void* o, float* lse);
 
-// 16-bit flash attention backward on tcgen05 (sm100_fmha_bwd.cu), deterministic: D = Dv = 128.  g carries the strides of q / k / v and, in
+// 16-bit flash attention backward on wgmma (sm100_fmha_bwd.cu), deterministic: D = Dv <= 128.  g carries the strides of q / k / v and, in
 // o_*, of dout; dg the strides of dq / dk / dv in q_* / k_* / v_*.  out (strides oo_*) / lse = the forward's saved outputs, or NULL:
 // both are then recomputed into the workspace (sdpa_backward_f16_workspace_bytes(g, 1)).  Same return convention as the forward.
 size_t sdpa_backward_f16_workspace_bytes(const SdpaGeom& g, int need_forward);

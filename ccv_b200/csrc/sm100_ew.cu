@@ -20,7 +20,7 @@ static int sms()
 		cudaGetDevice(&dev);
 		cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, dev);
 		if (g_sms <= 0)
-			g_sms = 148;
+			g_sms = 132;
 	}
 	return g_sms;
 }

@@ -31,7 +31,7 @@ int sms()
 		cudaGetDevice(&dev);
 		cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, dev);
 		if (g_sms <= 0)
-			g_sms = 148;
+			g_sms = 132;
 	}
 	return g_sms;
 }

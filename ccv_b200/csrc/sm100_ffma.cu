@@ -1,5 +1,5 @@
 // sm100_ffma.cu -- CUDA-core fp32 contractions (CCV_NNC_SM100_ALGO_FFMA): the shape-agnostic companions of the
-// tcgen05 path.  They take any stride / alignment / channel count (e.g. the 3-channel stem convolution, grouped
+// wgmma path.  They take any stride / alignment / channel count (e.g. the 3-channel stem convolution, grouped
 // convolutions, tensor views) and compute exact fp32 products, so they also serve as the on-device cross-check of
 // the tensor-core kernels.  One tiled SIMT GEMM (64 x 64 x 16, 4 x 4 register micro-tiles) is instantiated with
 // different operand "views" (functors mapping (row, k) / (k, col) to memory), which is how implicit-GEMM
@@ -190,8 +190,8 @@ int gemm_ffma(cudaStream_t stream, int M, int N, int K, const float* a, long lon
 	StridedView B = { b, b_rs, b_cs, K, N };
 	const long long tiles = (long long)((M + 63) / 64) * ((N + 63) / 64);
 	int splits = 1;
-	if (tiles < 148 && K >= 1024)
-		splits = (int)((296 + tiles - 1) / tiles);
+	if (tiles < 132 && K >= 1024)
+		splits = (int)((264 + tiles - 1) / tiles);
 	if (splits > K / 256)
 		splits = K / 256 > 0 ? K / 256 : 1;
 	return launch_ffma(stream, A, B, c, ldc, bias, M, N, K, accumulate, splits, false);

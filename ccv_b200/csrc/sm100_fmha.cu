@@ -1,22 +1,16 @@
-// sm100_fmha.cu -- SCALED_DOT_PRODUCT_ATTENTION forward for 16-bit tensors (bf16 / fp16), head dimension 128:
-// one flash-attention kernel on the tcgen05 tensor cores.  Semantics: scaled_dot_product_attention/
+// sm100_fmha.cu -- SCALED_DOT_PRODUCT_ATTENTION forward for 16-bit tensors (bf16 / fp16), head dimension <= 128:
+// one flash-attention kernel on the Hopper wgmma tensor cores.  Semantics: scaled_dot_product_attention/
 // ccv_nnc_scaled_dot_product_attention_cpu_ref.c:16-183 (O = softmax(scale * Q K^T [causal, bottom-right aligned :147]) V,
 // GQA through H / Hk :99,113), the same restrictions as the reference's flash-attention backend
 // (gpu/ccv_nnc_scaled_dot_product_attention_flash_attn.cu:13-205: 16-bit only, no additive mask, no unify-head weights).
 //
-// One CTA = 128 query rows of one (batch, head); 320 threads:
-//   warp 0    TMA producer: Q once, then K_j / V_j blocks of 128 keys through two-stage rings (4-D tensor maps over the
-//             caller's [B, S, H, D] strides, 128-byte swizzle)
-//   warp 1    tcgen05.mma issuer (kind::f16, fp32 accumulate in TMEM):
-//               S_j = Q K_j^T  -> TMEM S[j & 1]   (issued one block ahead, so it overlaps the softmax of block j - 1)
-//               O_j = P_j V_j  -> TMEM O          (P_j from shared memory, V_j as an MN-major operand)
-//   warps 2-9 softmax: two threads per query row (warps w and w + 4 share a TMEM lane quarter; each owns 64 of the 128
-//             key columns of S_j and 64 of the 128 output columns).  The two halves exchange their row max through shared
-//             memory (one named barrier per lane quarter), then exp2 / partial row sum / bf16 P_j written into the
-//             128-byte-swizzled K-major smem tile the second MMA reads; the running output lives in registers:
-//             acc = acc * alpha_j + O_j (O_j read back from TMEM), normalised by the row sum at the end.
-//             Two warps per scheduler instead of one hide the tcgen05.ld / MUFU latency of the other.
-// TMEM: S0, S1, O0, O1 = 4 x 128 columns (O_j alternates so that folding O_{j-1} into the registers overlaps P_j V_j).  smem: Q 32 KB + K 2 x 32 KB + V 2 x 32 KB + P 32 KB = 192 KB.
+// One CTA = 128 query rows of one (batch, head); 288 threads:
+//   warps 0-7  two consumer warpgroups of 64 query rows.  Per block of 128 keys: S_j = Q K_j^T (wgmma, both operands from shared
+//              memory, fp32 in registers), online softmax in registers (a row lives in the four lanes of a quad), then
+//              O += P_j V_j with P_j as 16-bit register fragments (wgmma A from registers) and V_j as an MN-major operand
+//   warp 8     TMA producer: Q once, then K_j / V_j through two-stage rings (4-D tensor maps over the caller's [B, S, H, D]
+//              strides, 128-byte swizzle, two 64-feature atoms per tile)
+// smem: Q 32 KB + K 2 x 32 KB + V 2 x 32 KB = 160 KB.
 #include "sm100_contract.h"
 #include "sm100_fmha.cuh"
 #include <string.h>
@@ -29,54 +23,41 @@ constexpr int FM_BLOCK = 128; // query rows per CTA = keys per block
 constexpr int FM_D = 128;     // head dimension (q/k and v)
 constexpr int FM_TILE_BYTES = FM_BLOCK * FM_D * 2; // 32 KB: two 128 x 64 swizzle atoms
 constexpr int FM_ATOM_BYTES = FM_BLOCK * 128;      // 16 KB
-constexpr int FM_KV_STAGES = 2;
-// P_j goes back into tensor memory (16-bit pairs over the first 32 columns of each 64-column half of S[j & 1]) and is the A operand of
-// O_j = P_j V_j from there: no shared-memory write / fence / operand fetch for P.  0 = the shared-memory P tile of round 1.
-constexpr int FM_P_IN_TMEM = 1;
+constexpr int FM_THREADS = 288;
 
 struct FmhaParams {
 	int H, Hk, Sq, Sk;
 	int D; // actual head dimension (<= 128, a multiple of 8): the tiles are always 128 wide, TMA zero-fills the rest
 	int causal;
-	int is_bf16;
 	float scale_log2; // scale * log2(e)
 	void* o;
 	long long o_b, o_s, o_h; // element strides
 	float* lse;              // [B, H, Sq] or NULL
-	uint32_t idesc_qk, idesc_pv;
-	uint32_t v_lbo, v_sbo, v_layout, v_kstep; // smem descriptor of the MN-major V operand
 };
 
 struct FmhaSmem {
 	static constexpr int Q_OFF = 0;
 	static constexpr int K_OFF = Q_OFF + FM_TILE_BYTES;
-	static constexpr int V_OFF = K_OFF + FM_KV_STAGES * FM_TILE_BYTES;
-	static constexpr int P_OFF = V_OFF + FM_KV_STAGES * FM_TILE_BYTES;
-	static constexpr int BAR_OFF = P_OFF + FM_TILE_BYTES;
-	static constexpr int XCHG_OFF = BAR_OFF + 256; // float [6][128]: row maxima per (S buffer, half), final partial row sums per half
-	static constexpr int TOTAL = XCHG_OFF + 6 * FM_BLOCK * 4 + 1024;
+	static constexpr int V_OFF = K_OFF + 2 * FM_TILE_BYTES;
+	static constexpr int BAR_OFF = V_OFF + 2 * FM_TILE_BYTES;
+	static constexpr int TOTAL = BAR_OFF + 256 + 1024;
 };
 
-template <int CL>
-__global__ void __launch_bounds__(320, 1) fmha_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV, const FmhaParams p)
+template <int BF16> // element type as a template parameter: one basic block per MMA batch
+__global__ void __launch_bounds__(FM_THREADS, 1) fmha_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV, const FmhaParams p)
 {
 	extern __shared__ uint8_t smem_raw[];
 	uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
 	uint64_t* bars = (uint64_t*)(smem + FmhaSmem::BAR_OFF);
 	uint64_t* q_full = bars;
 	uint64_t* k_full = bars + 1;  // [2]
-	uint64_t* k_empty = bars + 3; // [2]
+	uint64_t* k_empty = bars + 3; // [2] one arrival per consumer warpgroup
 	uint64_t* v_full = bars + 5;  // [2]
 	uint64_t* v_empty = bars + 7; // [2]
-	uint64_t* s_full = bars + 9;  // [2] MMA -> softmax
-	uint64_t* s_empty = bars + 11; // [2] softmax -> MMA (8 arrivals)
-	uint64_t* p_full = bars + 13; // softmax -> MMA (8 arrivals)
-	uint64_t* o_full = bars + 14; // MMA -> softmax
-	uint32_t* tmem_slot = (uint32_t*)(bars + 15);
 
 	const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 	// causal: the last query tiles see the most keys; issue them first so the tail of the launch is made of short tiles
-	const int q_tile = (CL == 1 && p.causal) ? (int)(gridDim.x - 1 - blockIdx.x) : (int)blockIdx.x;
+	const int q_tile = p.causal ? (int)(gridDim.x - 1 - blockIdx.x) : (int)blockIdx.x;
 	const int q0 = q_tile * FM_BLOCK;
 	const int h = blockIdx.y, b = blockIdx.z;
 	const int hk = h / (p.H / p.Hk);
@@ -86,315 +67,180 @@ __global__ void __launch_bounds__(320, 1) fmha_fwd_kernel(const __grid_constant_
 	if (p.causal)
 		kv_end = min(p.Sk, max(q0 + FM_BLOCK + shift, 0));
 	const int n_blk = (kv_end + FM_BLOCK - 1) / FM_BLOCK;
-	// a cluster of CL consecutive query tiles shares every K / V block: each CTA fetches 1 / CL of it and multicasts.  All
-	// CTAs must walk the same number of blocks (the cluster's last tile sees the most keys under a causal mask).
-	int n_max = n_blk;
-	uint32_t cta_rank = 0;
-	if (CL > 1)
-	{
-		cta_rank = cluster_ctarank();
-		if (p.causal)
-		{
-			const int q_last = ((int)blockIdx.x / CL * CL + CL - 1) * FM_BLOCK;
-			n_max = (min(p.Sk, max(q_last + FM_BLOCK + shift, 0)) + FM_BLOCK - 1) / FM_BLOCK;
-		}
-	}
-	const uint16_t cl_mask = (uint16_t)((1u << CL) - 1);
 
-	if (warp == 0 && lane == 0)
+	if (threadIdx.x == 0)
 	{
-		tma_prefetch_desc(&tmQ);
-		tma_prefetch_desc(&tmK);
-		tma_prefetch_desc(&tmV);
 		mbar_init(q_full, 1);
 		for (int s = 0; s < 2; s++)
 		{
-			mbar_init(&k_full[s], 1), mbar_init(&k_empty[s], CL);
-			mbar_init(&v_full[s], 1), mbar_init(&v_empty[s], CL);
-			mbar_init(&s_full[s], 1), mbar_init(&s_empty[s], 8);
+			mbar_init(&k_full[s], 1), mbar_init(&k_empty[s], 2);
+			mbar_init(&v_full[s], 1), mbar_init(&v_empty[s], 2);
 		}
-		mbar_init(p_full, 8);
-		mbar_init(o_full, 1);
 		fence_mbar_init();
 	}
-	if (warp == 1)
-	{
-		tmem_alloc(tmem_slot, 512);
-		tmem_relinquish();
-	}
-	tc_fence_before();
 	__syncthreads();
-	if (CL > 1)
-		cluster_sync_all(); // every CTA's barriers exist before any peer multicasts into them
-	tc_fence_after();
-	const uint32_t tmem_base = *tmem_slot;
-	const uint32_t tmem_o = tmem_base + 256;
 
-	if (warp == 0)
+	if (warp == 8)
 	{
-		if (n_max > 0 && elect_one())
+		if (n_blk > 0 && elect_one())
 		{
-			if (n_blk > 0)
-			{
-				mbar_expect_tx(q_full, FM_TILE_BYTES);
-				tma_load_4d(smem + FmhaSmem::Q_OFF, &tmQ, q_full, 0, h, q0, b);
-				tma_load_4d(smem + FmhaSmem::Q_OFF + FM_ATOM_BYTES, &tmQ, q_full, 64, h, q0, b);
-			}
-			for (int j = 0; j < n_max; j++)
+			tma_prefetch_desc(&tmQ);
+			tma_prefetch_desc(&tmK);
+			tma_prefetch_desc(&tmV);
+			mbar_expect_tx(q_full, FM_TILE_BYTES);
+			tma_load_4d(smem + FmhaSmem::Q_OFF, &tmQ, q_full, 0, h, q0, b);
+			tma_load_4d(smem + FmhaSmem::Q_OFF + FM_ATOM_BYTES, &tmQ, q_full, 64, h, q0, b);
+			for (int j = 0; j < n_blk; j++)
 			{
 				const int s = j & 1;
 				const uint32_t ph = (uint32_t)(j >> 1) & 1;
 				uint8_t* const sk = smem + FmhaSmem::K_OFF + s * FM_TILE_BYTES;
 				uint8_t* const sv = smem + FmhaSmem::V_OFF + s * FM_TILE_BYTES;
-				mbar_wait(&k_empty[s], ph ^ 1); // all CL consumers of this stage are done with it
+				mbar_wait(&k_empty[s], ph ^ 1);
 				mbar_expect_tx(&k_full[s], FM_TILE_BYTES);
-				if (CL == 1)
-				{
-					tma_load_4d(sk, &tmK, &k_full[s], 0, hk, j * FM_BLOCK, b);
-					tma_load_4d(sk + FM_ATOM_BYTES, &tmK, &k_full[s], 64, hk, j * FM_BLOCK, b);
-				} else // CL == 2: this CTA fetches the 64-wide d atom `rank` for both CTAs
-					tma_load_4d_multicast(sk + cta_rank * FM_ATOM_BYTES, &tmK, &k_full[s], 64 * (int)cta_rank, hk, j * FM_BLOCK, b, cl_mask);
+				tma_load_4d(sk, &tmK, &k_full[s], 0, hk, j * FM_BLOCK, b);
+				tma_load_4d(sk + FM_ATOM_BYTES, &tmK, &k_full[s], 64, hk, j * FM_BLOCK, b);
 				mbar_wait(&v_empty[s], ph ^ 1);
 				mbar_expect_tx(&v_full[s], FM_TILE_BYTES);
-				if (CL == 1)
-				{
-					tma_load_4d(sv, &tmV, &v_full[s], 0, hk, j * FM_BLOCK, b);
-					tma_load_4d(sv + FM_ATOM_BYTES, &tmV, &v_full[s], 64, hk, j * FM_BLOCK, b);
-				} else
-					tma_load_4d_multicast(sv + cta_rank * FM_ATOM_BYTES, &tmV, &v_full[s], 64 * (int)cta_rank, hk, j * FM_BLOCK, b, cl_mask);
+				tma_load_4d(sv, &tmV, &v_full[s], 0, hk, j * FM_BLOCK, b);
+				tma_load_4d(sv + FM_ATOM_BYTES, &tmV, &v_full[s], 64, hk, j * FM_BLOCK, b);
 			}
 		}
-	} else if (warp == 1) {
-		// one elected thread issues every MMA, descriptors as base + constant: operands stay in uniform registers (with a `lane == 0` test
-		// ptxas wraps each tcgen05.mma in an elect / broadcast / branch loop and rebuilds the descriptors, ~12 dependent instructions per MMA)
-		if (n_max > 0 && elect_one())
-		{
-			const uint64_t q_desc = umma_smem_desc(smem_u32(smem + FmhaSmem::Q_OFF), 16, 1024, 2);
-			const uint64_t p_desc = umma_smem_desc(smem_u32(smem + FmhaSmem::P_OFF), 16, 1024, 2);
-			const uint64_t k_desc0 = umma_smem_desc(smem_u32(smem + FmhaSmem::K_OFF), 16, 1024, 2);
-			const uint64_t v_desc0 = umma_smem_desc(smem_u32(smem + FmhaSmem::V_OFF), p.v_lbo, p.v_sbo, p.v_layout);
-			const uint32_t v_kstep16 = p.v_kstep >> 4;
-			const uint32_t idesc_qk = p.idesc_qk, idesc_pv = p.idesc_pv;
-			auto release = [&](uint64_t* bar) {
-				if (CL == 1)
-					umma_commit(bar);
-				else
-					umma_commit_multicast(bar, cl_mask); // the stage is free once every CTA of the cluster has read it
-			};
-			// S_j = Q K_j^T into S[j & 1]; blocks past this tile's causal horizon are only drained (the cluster shares the ring)
-			auto issue_qk = [&](const int j) {
-				const int s = j & 1;
-				const uint32_t ph = (uint32_t)(j >> 1) & 1;
-				// S[s] still holds block j - 2: the softmax warps have read it (shared-memory P), or P_{j-2} lives in it and the P V MMA that
-				// reads it was issued before this point -- the tensor core executes in issue order, no barrier needed (P in TMEM)
-				if (!FM_P_IN_TMEM && j < n_blk)
-					mbar_wait(&s_empty[s], ph ^ 1);
-				mbar_wait(&k_full[s], ph);
-				tc_fence_after();
-				if (j < n_blk)
-				{
-					const uint64_t k_desc = k_desc0 + (uint32_t)s * (uint32_t)(FM_TILE_BYTES >> 4);
+		return;
+	}
+
+	// ------------------------------------------------------------------ consumers: rows r0 and r0 + 8 of this thread
+	const int wg = warp >> 2;
+	const int t4 = lane & 3;
+	const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+	int kv_limit[2]; // keys [0, kv_limit) are visible to the row
 #pragma unroll
-					for (int k = 0; k < FM_D / 16; k++)
-					{
-						const uint32_t off = ((uint32_t)(k >> 2) * FM_ATOM_BYTES + (uint32_t)(k & 3) * 32) >> 4;
-						umma_f16(tmem_base + s * 128, q_desc + off, k_desc + off, idesc_qk, k > 0 ? 1u : 0u);
-					}
-				}
-				release(&k_empty[s]);
-				if (j < n_blk)
-					umma_commit(&s_full[s]);
-			};
-			if (n_blk > 0)
-				mbar_wait(q_full, 0);
-			issue_qk(0);
-			for (int j = 0; j < n_max; j++)
-			{
-				if (j + 1 < n_max)
-					issue_qk(j + 1);
-				const int s = j & 1;
-				const uint32_t ph = (uint32_t)(j >> 1) & 1;
-				if (j < n_blk)
-					mbar_wait(p_full, (uint32_t)j & 1);
-				mbar_wait(&v_full[s], ph);
-				tc_fence_after();
-				if (j < n_blk)
-				{
-					const uint64_t v_desc = v_desc0 + (uint32_t)s * (uint32_t)(FM_TILE_BYTES >> 4);
+	for (int hh = 0; hh < 2; hh++)
+		kv_limit[hh] = p.causal ? min(p.Sk, q0 + r0 + 8 * hh + shift + 1) : p.Sk;
+	float o[64], sacc[64];
 #pragma unroll
-					for (int k = 0; k < FM_BLOCK / 16; k++)
-					{
-						const uint32_t poff = ((uint32_t)(k >> 2) * FM_ATOM_BYTES + (uint32_t)(k & 3) * 32) >> 4;
-						if (FM_P_IN_TMEM) // 16 keys = 8 columns; keys [64 h, 64 h + 64) sit in columns [64 h, 64 h + 32) of S[s]
-							umma_f16_ts(tmem_o + (uint32_t)(j & 1) * 128, tmem_base + s * 128 + (uint32_t)(k >> 2) * 64 + (uint32_t)(k & 3) * 8, v_desc + k * v_kstep16, idesc_pv, k > 0 ? 1u : 0u);
-						else
-							umma_f16(tmem_o + (uint32_t)(j & 1) * 128, p_desc + poff, v_desc + k * v_kstep16, idesc_pv, k > 0 ? 1u : 0u);
-					}
-				}
-				release(&v_empty[s]);
-				if (j < n_blk)
-					umma_commit(o_full);
-			}
-		}
-	} else {
-		// ------------------------------------------------------------------ softmax / output (warps 2..9)
-		const int quarter = warp & 3;       // TMEM lanes [32 * quarter, +32) are the ones this warp may touch
-		const int half = (warp - 2) >> 2;   // key columns / output columns [64 * half, +64)
-		const int row = quarter * 32 + lane;
-		const int qi = q0 + row;
-		const uint32_t lane_sel = (uint32_t)(quarter * 32) << 16;
-		const int kv_limit = p.causal ? min(p.Sk, qi + shift + 1) : p.Sk; // keys [0, kv_limit) are visible to this row
-		float* const mx_x = (float*)(smem + FmhaSmem::XCHG_OFF); // [6][128 rows]
-		float acc[64];
+	for (int i = 0; i < 64; i++)
+		o[i] = 0.f;
+	float m[2] = { -INFINITY, -INFINITY }, l[2] = { 0.f, 0.f };
+	const uint32_t q_base = smem_u32(smem + FmhaSmem::Q_OFF) + wg * 8192;
+	if (n_blk > 0)
+		mbar_wait(q_full, 0);
+	for (int j = 0; j < n_blk; j++)
+	{
+		const int s = j & 1;
+		const uint32_t ph = (uint32_t)(j >> 1) & 1;
+		// S_j = Q K_j^T
+		mbar_wait(&k_full[s], ph);
+		const uint32_t k_base = smem_u32(smem + FmhaSmem::K_OFF + s * FM_TILE_BYTES);
 #pragma unroll
 		for (int i = 0; i < 64; i++)
-			acc[i] = 0.f;
-		float m = -INFINITY, l = 0.f, alpha_prev = 1.f;
-		uint8_t* const p_row = smem + FmhaSmem::P_OFF + half * FM_ATOM_BYTES + row * 128;
-		for (int j = 0; j < n_blk; j++)
+			sacc[i] = 0.f;
+		fence_regs(sacc);
+		wgmma_fence();
+#pragma unroll
+		for (int k = 0; k < FM_D / 16; k++)
 		{
-			const int s = j & 1;
-			mbar_wait(&s_full[s], (uint32_t)(j >> 1) & 1);
-			tc_fence_after();
-			const uint32_t ts = tmem_base + s * 128 + half * 64 + lane_sel;
-			const int kv0 = j * FM_BLOCK + half * 64;
-			const bool edge = kv0 + 64 > kv_limit; // some keys of this half block are masked for this row
-			uint32_t sr[64];
-			tmem_ld_32x32(ts, *reinterpret_cast<uint32_t(*)[32]>(&sr[0]));
-			tmem_ld_32x32(ts + 32, *reinterpret_cast<uint32_t(*)[32]>(&sr[32]));
-			tmem_ld_wait();
-			float mx = -INFINITY;
-			if (edge)
-			{
-#pragma unroll
-				for (int i = 0; i < 64; i++)
-					if (kv0 + i < kv_limit)
-						mx = fmaxf(mx, __uint_as_float(sr[i]));
-			} else {
-#pragma unroll
-				for (int i = 0; i < 64; i += 2)
-					mx = max3(mx, __uint_as_float(sr[i]), __uint_as_float(sr[i + 1]));
-			}
-			// the other half of this row lives in warp (warp +- 4): exchange the maxima
-			mx_x[(s * 2 + half) * FM_BLOCK + row] = mx;
-			asm volatile("bar.sync %0, 64;" ::"r"(1 + quarter) : "memory");
-			mx = fmaxf(mx, mx_x[(s * 2 + (half ^ 1)) * FM_BLOCK + row]);
-			const float m_new = fmaxf(m, mx * p.scale_log2);
-			const float m_use = m_new == -INFINITY ? 0.f : m_new; // a fully masked row keeps p = 0 without NaN
-			const float alpha = exp2f(m - m_use);                  // m = -inf -> 0
-			// p = exp2(s * scale_log2 - m) and the partial row sum first: the MUFU phase (16 ex2 / clk / SM = the MMA time of a
-			// whole block) runs while the tensor core is still busy with O_{j-1} = P_{j-1} V_{j-1}
-			float sum = 0.f;
-			uint32_t pk[32];
-#pragma unroll
-			for (int i = 0; i < 64; i += 2)
-			{
-				float t0, t1;
-				fma2(t0, t1, __uint_as_float(sr[i]), __uint_as_float(sr[i + 1]), p.scale_log2, p.scale_log2, -m_use, -m_use);
-				float e0 = ex2_approx(t0);
-				float e1 = ex2_approx(t1);
-				if (edge)
-				{
-					if (kv0 + i >= kv_limit)
-						e0 = 0.f;
-					if (kv0 + i + 1 >= kv_limit)
-						e1 = 0.f;
-				}
-				sum += e0 + e1;
-				pk[i >> 1] = pack2(e0, e1, p.is_bf16);
-			}
-			if (FM_P_IN_TMEM)
-			{
-				// P_j over the first 32 columns of this thread's own 64 of S[s] (which it has just read), as the K-major A operand
-				tmem_st_32x32(ts, pk);
-				tmem_st_wait();
-				tc_fence_before();
-				__syncwarp();
-				if (lane == 0)
-					mbar_arrive(p_full);
-				if (j > 0)
-				{
-					mbar_wait(o_full, (uint32_t)(j - 1) & 1); // O_{j-1} = P_{j-1} V_{j-1} is complete
-					tc_fence_after();
-				}
-			} else {
-				// o_full flips when O_{j-1} = P_{j-1} V_{j-1} is complete: the P tile may be overwritten
-				if (j > 0)
-				{
-					mbar_wait(o_full, (uint32_t)(j - 1) & 1);
-					tc_fence_after();
-				}
-				// P tile in smem (K-major, 128-byte swizzle; this half = one 64-key atom)
-#pragma unroll
-				for (int c = 0; c < 8; c++)
-					*reinterpret_cast<uint4*>(p_row + ((c ^ (row & 7)) << 4)) = make_uint4(pk[c * 4], pk[c * 4 + 1], pk[c * 4 + 2], pk[c * 4 + 3]);
-				// hand S[s] back and publish P_j to the tensor core (generic-proxy smem writes -> async proxy)
-				fence_proxy_async();
-				tc_fence_before();
-				__syncwarp();
-				if (lane == 0)
-				{
-					mbar_arrive(&s_empty[s]);
-					mbar_arrive(p_full);
-				}
-			}
-			// O_{j-1} sits in the other output buffer (O_j goes to O[j & 1]): fold it into the running output off the critical
-			// path, while the tensor core already works on P_j V_j
-			if (j > 0)
-			{
-				uint32_t r[64];
-				const uint32_t to = tmem_o + (uint32_t)((j - 1) & 1) * 128 + lane_sel + half * 64;
-				tmem_ld_32x32(to, *reinterpret_cast<uint32_t(*)[32]>(&r[0]));
-				tmem_ld_32x32(to + 32, *reinterpret_cast<uint32_t(*)[32]>(&r[32]));
-				tmem_ld_wait();
-#pragma unroll
-				for (int i = 0; i < 64; i += 2)
-					fma2(acc[i], acc[i + 1], acc[i], acc[i + 1], alpha_prev, alpha_prev, __uint_as_float(r[i]), __uint_as_float(r[i + 1]));
-				tc_fence_before();
-			}
-			l = fmaf(l, alpha, sum);
-			m = m_new;
-			alpha_prev = alpha;
+			const uint32_t off = (uint32_t)(k >> 2) * FM_ATOM_BYTES + (uint32_t)(k & 3) * 32;
+			const uint64_t dq = wgmma_desc(q_base + off, 16, 1024), dk = wgmma_desc(k_base + off, 16, 1024);
+			if constexpr (BF16 != 0)
+				wgmma_bf16_ss_n128<0, 0>(sacc, dq, dk);
+			else
+				wgmma_f16_ss_n128<0, 0>(sacc, dq, dk);
 		}
-		if (n_blk > 0)
+		wgmma_commit();
+		fence_regs(sacc);
+		wgmma_wait<0>();
+		fence_regs(sacc);
+		if ((threadIdx.x & 127) == 0)
+			mbar_arrive(&k_empty[s]);
+		// online softmax: key of accumulator i = j * 128 + 8 * (i >> 2) + 2 * t4 + (i & 1), row r0 + 8 * ((i >> 1) & 1)
+		const int kv0 = j * FM_BLOCK + 2 * t4;
+		const bool edge = j * FM_BLOCK + FM_BLOCK > min(kv_limit[0], kv_limit[1]);
+		float mx[2] = { -INFINITY, -INFINITY };
+#pragma unroll
+		for (int i = 0; i < 64; i++)
 		{
-			mbar_wait(o_full, (uint32_t)(n_blk - 1) & 1);
-			tc_fence_after();
-			uint32_t r[64];
-			const uint32_t to = tmem_o + (uint32_t)((n_blk - 1) & 1) * 128 + lane_sel + half * 64;
-			tmem_ld_32x32(to, *reinterpret_cast<uint32_t(*)[32]>(&r[0]));
-			tmem_ld_32x32(to + 32, *reinterpret_cast<uint32_t(*)[32]>(&r[32]));
-			tmem_ld_wait();
-#pragma unroll
-			for (int i = 0; i < 64; i += 2)
-				fma2(acc[i], acc[i + 1], acc[i], acc[i + 1], alpha_prev, alpha_prev, __uint_as_float(r[i]), __uint_as_float(r[i + 1]));
+			const int hh = (i >> 1) & 1;
+			if (edge && kv0 + 8 * (i >> 2) + (i & 1) >= kv_limit[hh])
+				sacc[i] = -INFINITY;
+			mx[hh] = fmaxf(mx[hh], sacc[i]);
 		}
-		// the row sum is the sum of the two halves' partial sums (same running max on both sides)
-		mx_x[(4 + half) * FM_BLOCK + row] = l;
-		asm volatile("bar.sync %0, 64;" ::"r"(1 + quarter) : "memory");
-		l += mx_x[(4 + (half ^ 1)) * FM_BLOCK + row];
-		if (qi < p.Sq)
+		float alpha[2], m_use[2];
+#pragma unroll
+		for (int hh = 0; hh < 2; hh++)
 		{
-			const float inv = l > 0.f ? 1.f / l : 0.f;
-			uint16_t* const orow = (uint16_t*)p.o + b * p.o_b + (long long)qi * p.o_s + h * p.o_h + half * 64;
-#pragma unroll
-			for (int i = 0; i < 64; i += 8)
-			{
-				const uint4 v = make_uint4(pack2(acc[i] * inv, acc[i + 1] * inv, p.is_bf16), pack2(acc[i + 2] * inv, acc[i + 3] * inv, p.is_bf16),
-					pack2(acc[i + 4] * inv, acc[i + 5] * inv, p.is_bf16), pack2(acc[i + 6] * inv, acc[i + 7] * inv, p.is_bf16));
-				if (half * 64 + i < p.D) // head dimensions below 128: the padded feature columns are not part of the tensor
-					*reinterpret_cast<uint4*>(orow + i) = v;
-			}
-			if (p.lse && half == 0)
-				p.lse[((long long)b * p.H + h) * p.Sq + qi] = l > 0.f ? (m + log2f(l)) * 0.6931471805599453f : -INFINITY;
+			mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
+			mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
+			const float m_new = fmaxf(m[hh], mx[hh] * p.scale_log2);
+			m_use[hh] = m_new == -INFINITY ? 0.f : m_new; // a fully masked row keeps p = 0 without NaN
+			alpha[hh] = exp2f(m[hh] - m_use[hh]);          // m = -inf -> 0
+			m[hh] = m_new;
 		}
+		float sum[2] = { 0.f, 0.f };
+#pragma unroll
+		for (int i = 0; i < 64; i++)
+		{
+			const int hh = (i >> 1) & 1;
+			const float e = ex2_approx(fmaf(sacc[i], p.scale_log2, -m_use[hh])); // exp2(-inf) = 0 for the masked keys
+			sacc[i] = e;
+			sum[hh] += e;
+			o[i] *= alpha[hh];
+		}
+		l[0] = fmaf(l[0], alpha[0], sum[0]), l[1] = fmaf(l[1], alpha[1], sum[1]);
+		// O += P_j V_j
+		mbar_wait(&v_full[s], ph);
+		const uint32_t v_base = smem_u32(smem + FmhaSmem::V_OFF + s * FM_TILE_BYTES);
+		// every A fragment is packed before the MMAs start: registers an in-flight wgmma reads must not be written between them
+		uint32_t pa[FM_BLOCK / 16][4];
+#pragma unroll
+		for (int kk = 0; kk < FM_BLOCK / 16; kk++)
+			acc_to_a(sacc, kk, BF16, pa[kk]);
+		fence_regs(o);
+		wgmma_fence();
+#pragma unroll
+		for (int kk = 0; kk < FM_BLOCK / 16; kk++)
+		{
+			const uint32_t (&a)[4] = pa[kk];
+			// V [128 keys x 128 d] as an MN-major B operand: two 64-wide d atoms 16 KB apart (LBO), 8-key groups 1 KB apart (SBO),
+			// one MMA consumes 16 keys = 2 KB
+			const uint64_t dv = wgmma_desc(v_base + kk * 2048, FM_ATOM_BYTES, 1024);
+			if constexpr (BF16 != 0)
+				wgmma_bf16_rs_n128<1>(o, a, dv);
+			else
+				wgmma_f16_rs_n128<1>(o, a, dv);
+		}
+		wgmma_commit();
+		fence_regs(o);
+		wgmma_wait<0>();
+		fence_regs(o);
+		if ((threadIdx.x & 127) == 0)
+			mbar_arrive(&v_empty[s]);
 	}
-	tc_fence_before();
-	__syncthreads();
-	if (CL > 1)
-		cluster_sync_all(); // no CTA leaves while a peer may still arrive on its barriers
-	if (warp == 1)
-		tmem_dealloc(tmem_base, 512);
+	// the row sum is spread over the quad's four lanes
+#pragma unroll
+	for (int hh = 0; hh < 2; hh++)
+	{
+		l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 1);
+		l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 2);
+	}
+#pragma unroll
+	for (int hh = 0; hh < 2; hh++)
+	{
+		const int qi = q0 + r0 + 8 * hh;
+		if (qi >= p.Sq)
+			continue;
+		const float inv = l[hh] > 0.f ? 1.f / l[hh] : 0.f;
+		uint16_t* const orow = (uint16_t*)p.o + b * p.o_b + (long long)qi * p.o_s + h * p.o_h;
+#pragma unroll
+		for (int jn = 0; jn < 16; jn++)
+		{
+			const int d = 8 * jn + 2 * t4;
+			if (d < p.D) // head dimensions below 128: the padded feature columns are not part of the tensor
+				*reinterpret_cast<uint32_t*>(orow + d) = pack2(o[4 * jn + 2 * hh] * inv, o[4 * jn + 2 * hh + 1] * inv, BF16);
+		}
+		if (p.lse && t4 == 0)
+			p.lse[((long long)b * p.H + h) * p.Sq + qi] = l[hh] > 0.f ? (m[hh] + log2f(l[hh])) * 0.6931471805599453f : -INFINITY;
+	}
 }
 
 } // namespace
@@ -414,18 +260,10 @@ int sdpa_forward_f16(cudaStream_t stream, const SdpaGeom& g, int is_bf16, const 
 	FmhaParams p;
 	memset(&p, 0, sizeof(p));
 	p.H = g.H, p.Hk = g.Hk, p.Sq = g.Sq, p.Sk = g.Sk, p.D = g.D;
-	p.causal = g.is_causal, p.is_bf16 = is_bf16;
+	p.causal = g.is_causal;
 	p.scale_log2 = g.scale * 1.4426950408889634f;
 	p.o = o, p.o_b = g.o_b, p.o_s = g.o_s, p.o_h = g.o_h;
 	p.lse = lse;
-	p.idesc_qk = umma_instr_desc(is_bf16 ? 1 : 0, 0, 0, FM_BLOCK, FM_BLOCK);
-	p.idesc_pv = umma_instr_desc(is_bf16 ? 1 : 0, 0, 1, FM_BLOCK, FM_D);
-	// V [128 keys x 128 d] as an MN-major B operand: two 64-wide d atoms 16 KB apart (LBO), 8-key groups 1 KB apart (SBO),
-	// one MMA consumes 16 keys = 2 KB
-	p.v_lbo = (uint32_t)env_int("CCV_NNC_SM100_FMHA_V_LBO", FM_ATOM_BYTES);
-	p.v_sbo = (uint32_t)env_int("CCV_NNC_SM100_FMHA_V_SBO", 1024);
-	p.v_layout = (uint32_t)env_int("CCV_NNC_SM100_FMHA_V_LAYOUT", 2);
-	p.v_kstep = (uint32_t)env_int("CCV_NNC_SM100_FMHA_V_KSTEP", 2048);
 	// the attribute is per device: one flag per device (a process may drive several GPUs)
 	static bool configured_on[64];
 	int dev = 0;
@@ -433,9 +271,9 @@ int sdpa_forward_f16(cudaStream_t stream, const SdpaGeom& g, int is_bf16, const 
 	bool& configured = configured_on[dev & 63];
 	if (!configured)
 	{
-		cudaError_t e = cudaFuncSetAttribute(fmha_fwd_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, FmhaSmem::TOTAL);
+		cudaError_t e = cudaFuncSetAttribute(fmha_fwd_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, FmhaSmem::TOTAL);
 		if (e == cudaSuccess)
-			e = cudaFuncSetAttribute(fmha_fwd_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, FmhaSmem::TOTAL);
+			e = cudaFuncSetAttribute(fmha_fwd_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, FmhaSmem::TOTAL);
 		if (e != cudaSuccess)
 		{
 			set_last_error("cudaFuncSetAttribute(fmha_fwd_kernel)", e);
@@ -444,26 +282,10 @@ int sdpa_forward_f16(cudaStream_t stream, const SdpaGeom& g, int is_bf16, const 
 		configured = true;
 	}
 	const int q_tiles = (g.Sq + FM_BLOCK - 1) / FM_BLOCK;
-	// CCV_NNC_SM100_FMHA_CLUSTER=2: pairs of query tiles of one (b, h) share their K / V blocks through TMA multicast (halves the
-	// L2 -> smem traffic).  Measured slightly slower than independent CTAs at configs[4] (564 vs 591 TFLOP/s): the kernel is
-	// bound by the softmax warps, not by L2, so it stays off by default
-	const int cl = (q_tiles % 2 == 0 && env_int("CCV_NNC_SM100_FMHA_CLUSTER", 1) == 2) ? 2 : 1;
-	cudaLaunchConfig_t cfg;
-	memset(&cfg, 0, sizeof(cfg));
-	cfg.gridDim = dim3(q_tiles, g.H, g.B);
-	cfg.blockDim = dim3(320, 1, 1);
-	cfg.dynamicSmemBytes = FmhaSmem::TOTAL;
-	cfg.stream = stream;
-	cudaLaunchAttribute attr[1];
-	attr[0].id = cudaLaunchAttributeClusterDimension;
-	attr[0].val.clusterDim.x = cl, attr[0].val.clusterDim.y = 1, attr[0].val.clusterDim.z = 1;
-	cfg.attrs = attr, cfg.numAttrs = 1;
-	const cudaError_t le = cl == 2 ? cudaLaunchKernelEx(&cfg, fmha_fwd_kernel<2>, tmQ, tmK, tmV, p) : cudaLaunchKernelEx(&cfg, fmha_fwd_kernel<1>, tmQ, tmK, tmV, p);
-	if (le != cudaSuccess)
-	{
-		set_last_error("fmha_fwd_kernel launch", le);
-		return -1;
-	}
+	if (is_bf16)
+		fmha_fwd_kernel<1><<<dim3(q_tiles, g.H, g.B), FM_THREADS, FmhaSmem::TOTAL, stream>>>(tmQ, tmK, tmV, p);
+	else
+		fmha_fwd_kernel<0><<<dim3(q_tiles, g.H, g.B), FM_THREADS, FmhaSmem::TOTAL, stream>>>(tmQ, tmK, tmV, p);
 	count_launch();
 	const cudaError_t e = cudaGetLastError();
 	if (e != cudaSuccess)

@@ -1,5 +1,5 @@
 // sm100_fmha.cuh -- helpers shared by the 16-bit flash-attention kernels (sm100_fmha.cu forward, sm100_fmha_bwd.cu backward):
-// 16-bit packing, the sm_100 packed fp32 instructions, and the 4-D TMA tensor map over a [B, S, H, D] tensor.
+// 16-bit packing, the 4-D TMA tensor map over a [B, S, H, D] tensor, and the register form of P / dS as a wgmma A operand.
 #pragma once
 #include "sm100_ptx.cuh"
 #include <cuda_bf16.h>
@@ -21,19 +21,12 @@ __device__ __forceinline__ uint32_t pack2(const float a, const float b, const in
 	return *reinterpret_cast<const uint32_t*>(&v);
 }
 
-// sm_100 packed / 3-input fp32 instructions: FMNMX3 halves the row-max pass, FFMA2 halves the scale-and-shift in front of the exp2
-// and the running-output update (the softmax warps are issue-limited: profiles/r01_ncu_fmha_bf16_config5.txt)
-__device__ __forceinline__ float max3(const float a, const float b, const float c)
+// the m16n8k16 A fragment of 16 key columns [16 kk, 16 kk + 16) of a wgmma accumulator (see sm100_ptx.cuh), rounded to 16 bits
+template <int R>
+__device__ __forceinline__ void acc_to_a(const float (&x)[R], const int kk, const int is_bf16, uint32_t (&a)[4])
 {
-	float d;
-	asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-	return d;
-}
-__device__ __forceinline__ void fma2(float& d0, float& d1, const float a0, const float a1, const float b0, const float b1, const float c0, const float c1)
-{
-	asm("{\n\t.reg .b64 ra, rb, rc, rd;\n\tmov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\tmov.b64 rc, {%6, %7};\n\tfma.rn.f32x2 rd, ra, rb, rc;\n\tmov.b64 {%0, %1}, rd;\n\t}"
-		: "=f"(d0), "=f"(d1)
-		: "f"(a0), "f"(a1), "f"(b0), "f"(b1), "f"(c0), "f"(c1));
+	a[0] = pack2(x[8 * kk], x[8 * kk + 1], is_bf16), a[1] = pack2(x[8 * kk + 2], x[8 * kk + 3], is_bf16);
+	a[2] = pack2(x[8 * kk + 4], x[8 * kk + 5], is_bf16), a[3] = pack2(x[8 * kk + 6], x[8 * kk + 7], is_bf16);
 }
 
 typedef CUresult (*encode_tiled_f)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -70,12 +63,6 @@ inline bool make_map_bshd(CUtensorMap* map, const void* ptr, int B, int S, int H
 	cuuint32_t box[4] = { 64, 1, (cuuint32_t)box_rows, 1 };
 	cuuint32_t estr[4] = { 1, 1, 1, 1 };
 	return encode_fn()(map, is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, (void*)ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
-inline int env_int(const char* name, int dflt)
-{
-	const char* e = getenv(name);
-	return e ? atoi(e) : dflt;
 }
 
 } // namespace

@@ -1,6 +1,6 @@
 // sm100_fmha_bwd.cu -- SCALED_DOT_PRODUCT_ATTENTION backward for 16-bit tensors (bf16 / fp16), head dimension <= 128 (multiples of 8;
 // the tiles are always 128 features wide, missing features are zero-filled by the TMA unit and never stored): a fused
-// flash-attention backward on the tcgen05 tensor cores, deterministic (no atomics, every sum in one fixed order).
+// flash-attention backward on the Hopper wgmma tensor cores, deterministic (no atomics, every sum in one fixed order).
 // Semantics: scaled_dot_product_attention/ccv_nnc_scaled_dot_product_attention_cpu_ref.c:259-479 (dq, dk, dv of
 // O = softmax(scale * Q K^T [causal, bottom-right aligned]) V, GQA gradients summed over the query heads of a key head); the reference's
 // GPU form is gpu/ccv_nnc_scaled_dot_product_attention_flash_attn.cu:221-451 (recomputation from O and the saved log-sum-exp,
@@ -14,24 +14,18 @@
 // Three launches:
 //   fmha_bwd_prep_kernel    (lse * log2 e, delta) pairs per query row, padded to whole tiles (padding rows: lse = +inf -> P = 0)
 //   fmha_bwd_kernel<0>      one CTA per 128 keys of one (batch, KEY head): K, V tiles resident in shared memory, Q_i / dO_i blocks of
-//                           64 queries streamed for every query head of the group; dV, dK accumulate in TMEM over the whole loop
+//                           64 queries streamed for every query head of the group; dV, dK accumulate in registers over the whole loop
 //   fmha_bwd_kernel<1>      one CTA per 128 queries of one (batch, query head): Q, dO resident, K_j / V_j blocks of 64 keys streamed;
-//                           dQ accumulates in TMEM
+//                           dQ accumulates in registers
 // Both recompute S and dP (7 GEMMs instead of 5) so that no gradient is ever accumulated across CTAs: that is what makes the result
 // run-to-run identical without the reference's per-split fp32 dq_accum buffers.
 //
 // One kernel body serves both (MODE 0 = dK/dV, 1 = dQ).  R1 / R2 = the resident 128-row tiles, T1 / T2 = the streamed 64-row blocks:
 //   MODE 0: R1 = K, R2 = V, T1 = Q_i, T2 = dO_i:  X = R1 T1^T = S^T,  Y = R2 T2^T = dP^T,  acc1 += P^T T2 (dV),  acc2 += dS^T T1 (dK)
 //   MODE 1: R1 = Q, R2 = dO, T1 = K_j, T2 = V_j:  X = R1 T1^T = S,    Y = R2 T2^T = dP,    acc2 += dS T1 (dQ)
-// 320 threads: warp 0 = TMA producer, warp 1 = tcgen05.mma issuer, warps 2-9 = the element-wise stage (two warps per TMEM lane
-// quarter, 32 of the 64 columns each).  X, Y from TMEM -> P, dS as bf16 / fp16 pairs written straight back into TMEM (over the
-// columns just read), where the accumulating MMAs take them as their A operand: an MMA whose two operands come from shared memory
-// is bound by the operand fetch, not by the tensor core (profiles/r02_ncu_fmha_bwd.txt).  T1 / T2 are the B operand twice --
-// K-major for X / Y, MN-major for the accumulation.  The streamed blocks sit in a ring of 4 (MODE 0) / 7 (MODE 1) stages: a stage is only free once the accumulation of its
-// block has completed, and the next X / Y is issued one block ahead, so two stages would expose the whole TMA latency every block.
-// MODE 1 also keeps its resident tiles (Q, dout) in tensor memory, so every one of its MMAs reads only the streamed block from
-// shared memory.  TMEM: X[2] 2 x 64 + Y[2] 2 x 64 + dV 128 (MODE 0) | Q 64 + dout 64 (MODE 1) + dK | dQ 128 = 512 columns.
-// smem: R 64 KB + T 4 x 32 KB = 192 KB (MODE 0), T 7 x 32 KB = 224 KB (MODE 1).
+// 384 threads: warps 0-7 = two consumer warpgroups of 64 resident rows (X, Y from shared memory; P, dS turned into 16-bit register
+// fragments that are the A operand of the accumulating MMAs, whose B operand is T1 / T2 read MN-major), warps 8-11 = the producer warpgroup (one thread issues the TMA loads; setmaxnreg moves its registers to the consumers).
+// smem: R 64 KB + T ring 4 x 32 KB = 192 KB.
 #include "sm100_contract.h"
 #include "sm100_fmha.cuh"
 #include <string.h>
@@ -47,7 +41,7 @@ constexpr int FB_R_ATOM = FB_R * 128;         // 16 KB: 128 rows x 64 features
 constexpr int FB_R_BYTES = 2 * FB_R_ATOM;     // 32 KB
 constexpr int FB_T_ATOM = FB_T * 128;         // 8 KB
 constexpr int FB_T_BYTES = 2 * FB_T_ATOM;     // 16 KB
-constexpr int FB_STAT_BYTES = FB_T * 8;       // (-lse2, -delta) per streamed query, as float4 (-l0, -l1, -d0, -d1) per query pair
+constexpr int FB_THREADS = 384;
 
 struct FmhaBwdParams {
 	int H, Hk, Sq, Sk, Sq_r;
@@ -60,21 +54,14 @@ struct FmhaBwdParams {
 	void* out2;                  // MODE 0: dK, MODE 1: dQ
 	long long o1_b, o1_s, o1_h;  // element strides
 	long long o2_b, o2_s, o2_h;
-	uint32_t idesc_xy, idesc_acc;
-	// MODE 1: the resident tiles (Q, dout) are read straight from global memory into tensor memory
-	const void* r1;
-	const void* r2;
-	long long r1_b, r1_s, r1_h, r2_b, r2_s, r2_h;
 };
 
-template <int MODE>
 struct FmhaBwdSmem {
-	static constexpr int NST = MODE == 0 ? 4 : 7; // stages of the streamed ring
-	static constexpr int R1_OFF = 0;              // MODE 0 only: MODE 1 keeps its resident tiles in tensor memory
+	static constexpr int NST = 4;                 // stages of the streamed ring
+	static constexpr int R1_OFF = 0;
 	static constexpr int R2_OFF = R1_OFF + FB_R_BYTES;
-	static constexpr int T_OFF = MODE == 0 ? R2_OFF + FB_R_BYTES : 0; // stage s: T1 at + s * 2 * FB_T_BYTES, T2 right behind it
-	static constexpr int STAT_OFF = T_OFF + NST * 2 * FB_T_BYTES;
-	static constexpr int BAR_OFF = STAT_OFF + (MODE == 0 ? NST * FB_STAT_BYTES : 0);
+	static constexpr int T_OFF = R2_OFF + FB_R_BYTES; // stage s: T1 at + s * 2 * FB_T_BYTES, T2 right behind it
+	static constexpr int BAR_OFF = T_OFF + NST * 2 * FB_T_BYTES;
 	static constexpr int TOTAL = BAR_OFF + 256 + 1024;
 	static_assert(TOTAL <= 232448, "227 KB of shared memory per CTA");
 };
@@ -129,338 +116,234 @@ __global__ void __launch_bounds__(256) fmha_bwd_prep_kernel(const uint16_t* __re
 	}
 }
 
-template <int MODE>
-__global__ void __launch_bounds__(320, 1) fmha_bwd_kernel(const __grid_constant__ CUtensorMap tmR1, const __grid_constant__ CUtensorMap tmR2, const __grid_constant__ CUtensorMap tmT1, const __grid_constant__ CUtensorMap tmT2, const FmhaBwdParams p)
+template <int MODE, int BF16> // element type as a template parameter: one basic block per MMA batch
+__global__ void __launch_bounds__(FB_THREADS, 1) fmha_bwd_kernel(const __grid_constant__ CUtensorMap tmR1, const __grid_constant__ CUtensorMap tmR2, const __grid_constant__ CUtensorMap tmT1, const __grid_constant__ CUtensorMap tmT2, const FmhaBwdParams p)
 {
-	typedef FmhaBwdSmem<MODE> L;
+	using L = FmhaBwdSmem;
 	constexpr int NST = L::NST;
 	extern __shared__ uint8_t smem_raw[];
 	uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
 	uint64_t* bars = (uint64_t*)(smem + L::BAR_OFF);
 	uint64_t* r_full = bars;
-	uint64_t* t_full = bars + 1;          // [NST] TMA -> MMA (and the element-wise warps: the stat pairs ride on the same barrier)
-	uint64_t* t_empty = t_full + NST;     // [NST] MMA (accumulation done) -> TMA
-	uint64_t* x_full = t_empty + NST;     // [2] MMA -> element-wise: X and Y of this block are in TMEM
-	uint64_t* p_full = x_full + 2;        // [2] element-wise -> MMA (8 arrivals): P / dS written back into TMEM
-	uint64_t* acc_full = p_full + 2;
-	uint32_t* tmem_slot = (uint32_t*)(acc_full + 1);
+	uint64_t* t_full = bars + 1;         // [NST]
+	uint64_t* t_empty = bars + 1 + NST;  // [NST] one arrival per consumer warpgroup
 
 	const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-	const int r0 = blockIdx.x * FB_R;
+	const int r0 = blockIdx.x * FB_R;    // first resident row (MODE 0: key, MODE 1: query)
 	const int hr = blockIdx.y, b = blockIdx.z; // MODE 0: key head, MODE 1: query head
-	const int G = p.H / p.Hk;
-	const int shift = p.Sk - p.Sq; // query i sees keys <= i + shift
-	// streamed blocks this tile needs
-	int blk0 = 0, n_blk;
+	const int group = p.H / p.Hk;
+	const int shift = p.Sk - p.Sq;       // causal: query i sees keys <= i + shift
+	// streamed blocks: MODE 0 = (query head of the group, 64-query block) from the first block a key of this tile can see;
+	// MODE 1 = 64-key blocks up to this tile's causal horizon
+	int first = 0, n_per = 0, n_total = 0;
 	if (MODE == 0)
 	{
 		const int nq = (p.Sq + FB_T - 1) / FB_T;
-		if (p.causal)
-			blk0 = min(nq, max(r0 - shift, 0) / FB_T); // queries below r0 - shift see none of this tile's keys
-		n_blk = nq - blk0;
+		first = p.causal ? min(nq, max(0, (r0 - shift) / FB_T)) : 0;
+		n_per = nq - first;
+		n_total = n_per * group;
 	} else {
 		const int kv_end = p.causal ? min(p.Sk, max(r0 + FB_R + shift, 0)) : p.Sk;
-		n_blk = (kv_end + FB_T - 1) / FB_T;
+		n_per = n_total = (kv_end + FB_T - 1) / FB_T;
 	}
-	const int n_it = MODE == 0 ? n_blk * G : n_blk;
 
-	if (warp == 0 && lane == 0)
+	if (threadIdx.x == 0)
 	{
-		tma_prefetch_desc(&tmR1);
-		tma_prefetch_desc(&tmR2);
-		tma_prefetch_desc(&tmT1);
-		tma_prefetch_desc(&tmT2);
-		mbar_init(r_full, MODE == 0 ? 1 : 8);
+		mbar_init(r_full, 1);
 		for (int s = 0; s < NST; s++)
-			mbar_init(&t_full[s], 1), mbar_init(&t_empty[s], 1);
-		for (int s = 0; s < 2; s++)
-		{
-			mbar_init(&x_full[s], 1), mbar_init(&p_full[s], 8);
-		}
-		mbar_init(acc_full, 1);
+			mbar_init(&t_full[s], 1), mbar_init(&t_empty[s], 2);
 		fence_mbar_init();
 	}
-	if (warp == 1)
-	{
-		tmem_alloc(tmem_slot, 512);
-		tmem_relinquish();
-	}
-	tc_fence_before();
 	__syncthreads();
-	tc_fence_after();
-	const uint32_t tmem_base = *tmem_slot;
-	const uint32_t tmem_x = tmem_base;        // X[s] at + 64 s
-	const uint32_t tmem_y = tmem_base + 128;  // Y[s] at + 64 s
-	const uint32_t tmem_a1 = tmem_base + 256; // dV (MODE 0)
-	const uint32_t tmem_a2 = tmem_base + 384; // dK | dQ
-	const uint32_t tmem_r1 = tmem_base + 256; // MODE 1: Q and dout as 16-bit pairs, 64 columns each
-	const uint32_t tmem_r2 = tmem_base + 320;
 
-	if (warp == 0)
+	if (warp >= 8)
 	{
-		if (n_it > 0 && elect_one())
+		// the producer warpgroup hands most of its registers to the consumers (dV and dK accumulators: 128 fp32 registers per thread)
+		asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+		if (warp == 8 && elect_one())
 		{
-			if (MODE == 0)
-			{
-				mbar_expect_tx(r_full, 2 * FB_R_BYTES);
-				tma_load_4d(smem + L::R1_OFF, &tmR1, r_full, 0, hr, r0, b);
-				tma_load_4d(smem + L::R1_OFF + FB_R_ATOM, &tmR1, r_full, 64, hr, r0, b);
-				tma_load_4d(smem + L::R2_OFF, &tmR2, r_full, 0, hr, r0, b);
-				tma_load_4d(smem + L::R2_OFF + FB_R_ATOM, &tmR2, r_full, 64, hr, r0, b);
-			}
-			int st = 0;
-			uint32_t ph = 0;
-			for (int it = 0; it < n_it; it++)
-			{
-				const int ht = MODE == 0 ? hr * G + it / n_blk : hr / G;
-				const int t0 = (MODE == 0 ? blk0 + it % n_blk : it) * FB_T;
-				uint8_t* const t1 = smem + L::T_OFF + st * 2 * FB_T_BYTES;
-				uint8_t* const t2 = t1 + FB_T_BYTES;
-				mbar_wait(&t_empty[st], ph ^ 1);
-				mbar_expect_tx(&t_full[st], 2 * FB_T_BYTES + (MODE == 0 ? FB_STAT_BYTES : 0));
-				tma_load_4d(t1, &tmT1, &t_full[st], 0, ht, t0, b);
-				tma_load_4d(t1 + FB_T_ATOM, &tmT1, &t_full[st], 64, ht, t0, b);
-				tma_load_4d(t2, &tmT2, &t_full[st], 0, ht, t0, b);
-				tma_load_4d(t2 + FB_T_ATOM, &tmT2, &t_full[st], 64, ht, t0, b);
-				if (MODE == 0)
-					bulk_load_1d(smem + L::STAT_OFF + st * FB_STAT_BYTES, p.stat + (((long long)b * p.H + ht) * p.Sq_r + t0) / 2, FB_STAT_BYTES, &t_full[st]);
-				if (++st == NST)
-					st = 0, ph ^= 1;
-			}
-		}
-	} else if (warp == 1) {
-		// One elected thread issues every MMA of the CTA.  `elect_one()` rather than `lane == 0`, and descriptors as base + constant:
-		// with a lane test ptxas cannot prove the operands uniform and wraps every tcgen05.mma in an elect / broadcast / branch loop plus the
-		// descriptor arithmetic -- about 12 dependent instructions per MMA, which made the issue rate, not the tensor core, the bound of the
-		// first version of this kernel (profiles/r02_ncu_fmha_bwd.txt).
-		if (n_it > 0 && elect_one())
-		{
-			const uint64_t r1_desc = umma_smem_desc(smem_u32(smem + L::R1_OFF), 16, 1024, 2);
-			const uint64_t r2_desc = umma_smem_desc(smem_u32(smem + L::R2_OFF), 16, 1024, 2);
-			const uint64_t t_kmajor = umma_smem_desc(smem_u32(smem + L::T_OFF), 16, 1024, 2);       // a streamed block as the K-major B operand of X / Y
-			const uint64_t t_mnmajor = umma_smem_desc(smem_u32(smem + L::T_OFF), FB_T_ATOM, 1024, 2); // and as the MN-major B operand of the accumulation
-			constexpr uint32_t STAGE16 = (2 * FB_T_BYTES) >> 4, T2_16 = FB_T_BYTES >> 4; // descriptor address units (16 bytes)
-			int xst = 0, ast = 0; // ring stage of the next X / Y block and of the next accumulation
-			uint32_t xph = 0;
-			// X = R1 T1^T, Y = R2 T2^T into buffer it & 1: both operands K-major, 8 steps of 16 features over the two 64-wide atoms
-			auto issue_xy = [&](const int it) {
-				const int s = it & 1;
-				// X[s] / Y[s] also hold P / dS of block it - 2 (below): the accumulation that reads them was issued before this point, and the
-				// tensor core executes its MMAs in issue order, so no barrier is needed before overwriting them
-				mbar_wait(&t_full[xst], xph);
-				tc_fence_after();
-				const uint64_t t1 = t_kmajor + (uint32_t)xst * STAGE16;
-				const uint64_t t2 = t1 + T2_16;
-#pragma unroll
-				for (int k = 0; k < FB_D / 16; k++)
-				{
-					const uint32_t ro = ((uint32_t)(k >> 2) * FB_R_ATOM + (uint32_t)(k & 3) * 32) >> 4;
-					const uint32_t to = ((uint32_t)(k >> 2) * FB_T_ATOM + (uint32_t)(k & 3) * 32) >> 4;
-					if (MODE == 0)
-						umma_f16(tmem_x + s * 64, r1_desc + ro, t1 + to, p.idesc_xy, k > 0 ? 1u : 0u);
-					else // the resident operand from tensor memory: 8 columns per 16 features
-						umma_f16_ts(tmem_x + s * 64, tmem_r1 + k * 8, t1 + to, p.idesc_xy, k > 0 ? 1u : 0u);
-				}
-#pragma unroll
-				for (int k = 0; k < FB_D / 16; k++)
-				{
-					const uint32_t ro = ((uint32_t)(k >> 2) * FB_R_ATOM + (uint32_t)(k & 3) * 32) >> 4;
-					const uint32_t to = ((uint32_t)(k >> 2) * FB_T_ATOM + (uint32_t)(k & 3) * 32) >> 4;
-					if (MODE == 0)
-						umma_f16(tmem_y + s * 64, r2_desc + ro, t2 + to, p.idesc_xy, k > 0 ? 1u : 0u);
-					else
-						umma_f16_ts(tmem_y + s * 64, tmem_r2 + k * 8, t2 + to, p.idesc_xy, k > 0 ? 1u : 0u);
-				}
-				umma_commit(&x_full[s]);
-				if (++xst == NST)
-					xst = 0, xph ^= 1;
-			};
-			mbar_wait(r_full, 0);
-			tc_fence_after();
-			issue_xy(0);
-			for (int it = 0; it < n_it; it++)
-			{
-				if (it + 1 < n_it)
-					issue_xy(it + 1); // one block ahead: overlaps the element-wise stage of block it
-				const int s = it & 1;
-				mbar_wait(&p_full[s], (uint32_t)(it >> 1) & 1);
-				tc_fence_after();
-				const uint64_t t1 = t_mnmajor + (uint32_t)ast * STAGE16;
-				const uint64_t t2 = t1 + T2_16;
-				// A = P / dS from tensor memory (written over the first 16 columns of each 32-column half of X[s] / Y[s]: 8 columns per
-				// 16 rows of the streamed block), B = the streamed block as an MN-major operand: two 64-wide feature atoms 8 KB apart
-				// (LBO), 8-row groups 1 KB apart (SBO), one MMA consumes 16 rows = 2 KB
-#pragma unroll
-				for (int k = 0; k < FB_T / 16; k++)
-				{
-					const uint32_t acc = (it > 0 || k > 0) ? 1u : 0u;
-					const uint32_t a_col = (uint32_t)s * 64 + (uint32_t)(k >> 1) * 32 + (uint32_t)(k & 1) * 8;
-					if (MODE == 0)
-						umma_f16_ts(tmem_a1, tmem_x + a_col, t2 + k * (2048 >> 4), p.idesc_acc, acc);
-					umma_f16_ts(tmem_a2, tmem_y + a_col, t1 + k * (2048 >> 4), p.idesc_acc, acc);
-				}
-				umma_commit(&t_empty[ast]);
-				if (it + 1 == n_it)
-					umma_commit(acc_full);
-				if (++ast == NST)
-					ast = 0;
-			}
-		}
-	} else {
-		// ------------------------------------------------------------------ element-wise stage and epilogue (warps 2..9)
-		const int quarter = warp & 3;     // TMEM lanes [32 * quarter, +32) are the ones this warp may touch
-		const int half = (warp - 2) >> 2; // columns [32 * half, +32) of a 64-wide block; [64 * half, +64) of the accumulators
-		const int set = half;
-		const int row = quarter * 32 + lane;
-		const int rr = r0 + row; // MODE 0: key index, MODE 1: query index
-		const uint32_t lane_sel = (uint32_t)(quarter * 32) << 16;
-		const int c0 = half * 32;
-		float nl = -INFINITY, nd = 0.f; // MODE 1: -lse2 and -delta of this thread's query
-		if (MODE == 1)
-		{
-			const float4 sv = p.stat[(((long long)b * p.H + hr) * p.Sq_r + rr) >> 1]; // Sq_r is a whole number of tiles
-			nl = (rr & 1) ? sv.y : sv.x, nd = (rr & 1) ? sv.w : sv.z;
-		}
-		if (MODE == 1 && n_it > 0)
-		{
-			// the resident tiles: this thread's row of Q and of dout, 64 of the 128 features each, global -> registers -> tensor memory
-			// (two 16-bit elements per column in memory order = the K-major A operand layout); rows past the end are zero
-#pragma unroll
+			tma_prefetch_desc(&tmR1);
+			tma_prefetch_desc(&tmR2);
+			tma_prefetch_desc(&tmT1);
+			tma_prefetch_desc(&tmT2);
+			mbar_expect_tx(r_full, 2 * FB_R_BYTES);
 			for (int a = 0; a < 2; a++)
 			{
-				uint32_t r[32];
-				if (rr < p.Sq)
-				{
-					const uint16_t* const src = a == 0 ? (const uint16_t*)p.r1 + b * p.r1_b + (long long)rr * p.r1_s + hr * p.r1_h + half * 64 : (const uint16_t*)p.r2 + b * p.r2_b + (long long)rr * p.r2_s + hr * p.r2_h + half * 64;
-#pragma unroll
-					for (int i = 0; i < 8; i++)
-					{
-						const uint4 v = half * 64 + i * 8 < p.D ? __ldg(reinterpret_cast<const uint4*>(src) + i) : make_uint4(0, 0, 0, 0);
-						r[i * 4] = v.x, r[i * 4 + 1] = v.y, r[i * 4 + 2] = v.z, r[i * 4 + 3] = v.w;
-					}
-				} else {
-#pragma unroll
-					for (int i = 0; i < 32; i++)
-						r[i] = 0;
-				}
-				tmem_st_32x32((a == 0 ? tmem_r1 : tmem_r2) + half * 32 + lane_sel, r);
+				tma_load_4d(smem + L::R1_OFF + a * FB_R_ATOM, &tmR1, r_full, 64 * a, hr, r0, b);
+				tma_load_4d(smem + L::R2_OFF + a * FB_R_ATOM, &tmR2, r_full, 64 * a, hr, r0, b);
 			}
-			tmem_st_wait();
-			tc_fence_before();
-			__syncwarp();
-			if (lane == 0)
-				mbar_arrive(r_full);
+			for (int n = 0; n < n_total; n++)
+			{
+				const int s = n % NST;
+				const uint32_t ph = (uint32_t)(n / NST) & 1;
+				const int row = MODE == 0 ? (first + n % n_per) * FB_T : n * FB_T;
+				const int head = MODE == 0 ? hr * group + n / n_per : hr / group; // MODE 0: query head of the group; MODE 1: the key head
+				uint8_t* const t1 = smem + L::T_OFF + s * 2 * FB_T_BYTES;
+				mbar_wait(&t_empty[s], ph ^ 1);
+				mbar_expect_tx(&t_full[s], 2 * FB_T_BYTES);
+				for (int a = 0; a < 2; a++)
+				{
+					tma_load_4d(t1 + a * FB_T_ATOM, &tmT1, &t_full[s], 64 * a, head, row, b);
+					tma_load_4d(t1 + FB_T_BYTES + a * FB_T_ATOM, &tmT2, &t_full[s], 64 * a, head, row, b);
+				}
+			}
 		}
-		int st = 0;
-		uint32_t tph = 0;
-		for (int it = 0; it < n_it; it++)
+		return;
+	}
+
+	// ------------------------------------------------------------------ consumers: resident rows rr + 8 * hh of this thread
+	asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+	const int wg = warp >> 2, t4 = lane & 3;
+	const int rr = r0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+	constexpr int is_bf16 = BF16;
+	float acc1[64], acc2[64]; // acc1: MODE 0 only
+#pragma unroll
+	for (int i = 0; i < 64; i++)
+		acc2[i] = 0.f;
+#pragma unroll
+	for (int i = 0; i < 64; i++)
+		acc1[i] = 0.f;
+	// MODE 1: the (-lse2, -delta) of the thread's two query rows, fixed for the whole loop
+	float nl[2] = { 0.f, 0.f }, nd[2] = { 0.f, 0.f };
+	if (MODE == 1)
+	{
+#pragma unroll
+		for (int hh = 0; hh < 2; hh++)
 		{
-			const int s = it & 1;
-			const uint32_t ph = (uint32_t)(it >> 1) & 1;
-			const int t0 = (MODE == 0 ? blk0 + it % n_blk : it) * FB_T;
-			// columns [cmin, cmax) of this row are visible
-			int cmin = 0, cmax = FB_T;
-			if (MODE == 0)
-			{
-				if (p.causal)
-					cmin = rr - shift - t0; // key rr is seen by queries >= rr - shift
-			} else
-				cmax = (p.causal ? min(p.Sk, rr + shift + 1) : p.Sk) - t0;
-			const bool edge = cmin > c0 || cmax < c0 + 32;
-			mbar_wait(&x_full[s], ph);
-			if (MODE == 0)
-				mbar_wait(&t_full[st], tph); // the stat pairs of this block (the MMA warp has observed this phase already)
-			tc_fence_after();
-			uint32_t xr[32], yr[32];
-			tmem_ld_32x32(tmem_x + s * 64 + c0 + lane_sel, xr);
-			tmem_ld_32x32(tmem_y + s * 64 + c0 + lane_sel, yr);
-			tmem_ld_wait();
-			const float4* const sp = (const float4*)(smem + L::STAT_OFF + st * FB_STAT_BYTES) + (c0 >> 1);
-			uint32_t pk[16], dk[16];
-#pragma unroll
-			for (int i = 0; i < 32; i += 2)
-			{
-				float l0 = nl, l1 = nl, d0 = nd, d1 = nd;
-				if (MODE == 0)
-				{
-					const float4 sv = sp[i >> 1]; // (-l, -l', -d, -d') of two queries, the same address for the whole warp
-					l0 = sv.x, l1 = sv.y, d0 = sv.z, d1 = sv.w;
-				}
-				float t0f, t1f, u0, u1, g0, g1;
-				fma2(t0f, t1f, __uint_as_float(xr[i]), __uint_as_float(xr[i + 1]), p.scale_log2, p.scale_log2, l0, l1);
-				float e0 = ex2_approx(t0f);
-				float e1 = ex2_approx(t1f);
-				if (edge)
-				{
-					if (c0 + i < cmin || c0 + i >= cmax)
-						e0 = 0.f;
-					if (c0 + i + 1 < cmin || c0 + i + 1 >= cmax)
-						e1 = 0.f;
-				}
-				fma2(u0, u1, __uint_as_float(yr[i]), __uint_as_float(yr[i + 1]), 1.f, 1.f, d0, d1);
-				fma2(g0, g1, e0, e1, u0, u1, 0.f, 0.f);
-				if (MODE == 0)
-					pk[i >> 1] = pack2(e0, e1, p.is_bf16);
-				dk[i >> 1] = pack2(g0, g1, p.is_bf16);
-			}
-			// P / dS go back into tensor memory as the A operand of the accumulating MMAs (16-bit pairs per column, K-major): over the first
-			// 16 columns of this thread's own 32 of X[s] / Y[s], which it has just read -- no shared-memory round trip
-			if (MODE == 0)
-				tmem_st_32x16(tmem_x + s * 64 + c0 + lane_sel, pk);
-			tmem_st_32x16(tmem_y + s * 64 + c0 + lane_sel, dk);
-			tmem_st_wait();
-			tc_fence_before();
-			__syncwarp();
-			if (lane == 0)
-				mbar_arrive(&p_full[s]);
-			if (++st == NST)
-				st = 0, tph ^= 1;
-		}
-		// epilogue: the accumulators -> 16-bit gradients (this thread: one row, 64 of the 128 features)
-		if (n_it > 0)
-		{
-			mbar_wait(acc_full, 0);
-			tc_fence_after();
-		}
-		const int limit = MODE == 0 ? p.Sk : p.Sq;
-#pragma unroll
-		for (int a = MODE == 0 ? 0 : 1; a < 2; a++)
-		{
-			uint32_t r[64];
-			if (n_it > 0)
-			{
-				const uint32_t ta = (a == 0 ? tmem_a1 : tmem_a2) + lane_sel + set * 64;
-				tmem_ld_32x32(ta, *reinterpret_cast<uint32_t(*)[32]>(&r[0]));
-				tmem_ld_32x32(ta + 32, *reinterpret_cast<uint32_t(*)[32]>(&r[32]));
-				tmem_ld_wait();
-			} else {
-#pragma unroll
-				for (int i = 0; i < 64; i++)
-					r[i] = 0;
-			}
-			if (rr < limit)
-			{
-				const float f = a == 0 ? 1.f : p.scale;
-				uint16_t* const orow = a == 0 ? (uint16_t*)p.out1 + b * p.o1_b + (long long)rr * p.o1_s + hr * p.o1_h + set * 64 : (uint16_t*)p.out2 + b * p.o2_b + (long long)rr * p.o2_s + hr * p.o2_h + set * 64;
-#pragma unroll
-				for (int i = 0; i < 64; i += 8)
-				{
-					const uint4 v = make_uint4(pack2(__uint_as_float(r[i]) * f, __uint_as_float(r[i + 1]) * f, p.is_bf16), pack2(__uint_as_float(r[i + 2]) * f, __uint_as_float(r[i + 3]) * f, p.is_bf16),
-						pack2(__uint_as_float(r[i + 4]) * f, __uint_as_float(r[i + 5]) * f, p.is_bf16), pack2(__uint_as_float(r[i + 6]) * f, __uint_as_float(r[i + 7]) * f, p.is_bf16));
-					if (set * 64 + i < p.D)
-						*reinterpret_cast<uint4*>(orow + i) = v;
-				}
-			}
+			const int q = rr + 8 * hh;
+			const float4 st = p.stat[(((long long)b * p.H + hr) * p.Sq_r + q) >> 1];
+			nl[hh] = (q & 1) ? st.y : st.x;
+			nd[hh] = (q & 1) ? st.w : st.z;
 		}
 	}
-	tc_fence_before();
-	__syncthreads();
-	if (warp == 1)
-		tmem_dealloc(tmem_base, 512);
+	const uint32_t r1_base = smem_u32(smem + L::R1_OFF) + wg * 8192, r2_base = smem_u32(smem + L::R2_OFF) + wg * 8192;
+	mbar_wait(r_full, 0);
+	for (int n = 0; n < n_total; n++)
+	{
+		const int s = n % NST;
+		const uint32_t ph = (uint32_t)(n / NST) & 1;
+		const int c0 = MODE == 0 ? (first + n % n_per) * FB_T : n * FB_T; // first streamed row (MODE 0: query, MODE 1: key)
+		const int hq = MODE == 0 ? hr * group + n / n_per : hr;
+		mbar_wait(&t_full[s], ph);
+		const uint32_t t1_base = smem_u32(smem + L::T_OFF + s * 2 * FB_T_BYTES), t2_base = t1_base + FB_T_BYTES;
+		float x[32], y[32];
+#pragma unroll
+		for (int i = 0; i < 32; i++)
+			x[i] = y[i] = 0.f;
+		fence_regs(x);
+		fence_regs(y);
+		wgmma_fence();
+#pragma unroll
+		for (int k = 0; k < FB_D / 16; k++)
+		{
+			const uint32_t roff = (uint32_t)(k >> 2) * FB_R_ATOM + (uint32_t)(k & 3) * 32, toff = (uint32_t)(k >> 2) * FB_T_ATOM + (uint32_t)(k & 3) * 32;
+			if constexpr (BF16 != 0)
+			{
+				wgmma_bf16_ss_n64<0, 0>(x, wgmma_desc(r1_base + roff, 16, 1024), wgmma_desc(t1_base + toff, 16, 1024));
+				wgmma_bf16_ss_n64<0, 0>(y, wgmma_desc(r2_base + roff, 16, 1024), wgmma_desc(t2_base + toff, 16, 1024));
+			} else {
+				wgmma_f16_ss_n64<0, 0>(x, wgmma_desc(r1_base + roff, 16, 1024), wgmma_desc(t1_base + toff, 16, 1024));
+				wgmma_f16_ss_n64<0, 0>(y, wgmma_desc(r2_base + roff, 16, 1024), wgmma_desc(t2_base + toff, 16, 1024));
+			}
+		}
+		wgmma_commit();
+		fence_regs(x);
+		fence_regs(y);
+		wgmma_wait<0>();
+		fence_regs(x);
+		fence_regs(y);
+		// accumulator i: resident row rr + 8 * ((i >> 1) & 1), streamed column c0 + 8 * (i >> 2) + 2 * t4 + (i & 1).
+		// P = exp2(scale_log2 * X - lse2) (0 where the causal mask hides the pair, or the key is past Sk), dS = P (Y - delta)
+#pragma unroll
+		for (int jn = 0; jn < 8; jn++)
+		{
+			const int c = c0 + 8 * jn + 2 * t4;
+			float cl[2], cd[2];
+			if (MODE == 0)
+			{
+				const float4 st = p.stat[(((long long)b * p.H + hq) * p.Sq_r + c) >> 1];
+				cl[0] = st.x, cl[1] = st.y, cd[0] = st.z, cd[1] = st.w;
+			}
+#pragma unroll
+			for (int e = 0; e < 4; e++)
+			{
+				const int i = 4 * jn + e, hh = e >> 1, col = c + (e & 1);
+				const int row = rr + 8 * hh;
+				const float lse2 = MODE == 0 ? cl[e & 1] : nl[hh];
+				const float delta = MODE == 0 ? cd[e & 1] : nd[hh];
+				const int key = MODE == 0 ? row : col, query = MODE == 0 ? col : row;
+				const bool visible = key < p.Sk && (!p.causal || key <= query + shift);
+				const float pv = visible ? ex2_approx(fmaf(x[i], p.scale_log2, lse2)) : 0.f;
+				x[i] = pv;
+				y[i] = pv * (y[i] + delta);
+			}
+		}
+		// every A fragment is packed before the MMAs start: registers an in-flight wgmma reads must not be written between them
+		uint32_t fp[FB_T / 16][4], fds[FB_T / 16][4];
+#pragma unroll
+		for (int kk = 0; kk < FB_T / 16; kk++)
+		{
+			acc_to_a(y, kk, is_bf16, fds[kk]);
+			if constexpr (MODE == 0)
+				acc_to_a(x, kk, is_bf16, fp[kk]);
+		}
+		fence_regs(acc2);
+		if constexpr (MODE == 0)
+			fence_regs(acc1);
+		wgmma_fence();
+#pragma unroll
+		for (int kk = 0; kk < FB_T / 16; kk++)
+		{
+			// T1 / T2 [64 streamed rows x 128 d] as MN-major B operands: d atoms 8 KB apart (LBO), 8-row groups 1 KB apart, 16 rows = 2 KB per MMA
+			const uint64_t d1 = wgmma_desc(t1_base + kk * 2048, FB_T_ATOM, 1024), d2 = wgmma_desc(t2_base + kk * 2048, FB_T_ATOM, 1024);
+			const uint32_t (&ap)[4] = fp[kk], (&ads)[4] = fds[kk];
+			if constexpr (BF16 != 0)
+			{
+				if constexpr (MODE == 0)
+					wgmma_bf16_rs_n128<1>(acc1, ap, d2);
+				wgmma_bf16_rs_n128<1>(acc2, ads, d1);
+			} else {
+				if constexpr (MODE == 0)
+					wgmma_f16_rs_n128<1>(acc1, ap, d2);
+				wgmma_f16_rs_n128<1>(acc2, ads, d1);
+			}
+		}
+		wgmma_commit();
+		fence_regs(acc2);
+		if constexpr (MODE == 0)
+			fence_regs(acc1);
+		wgmma_wait<0>();
+		fence_regs(acc2);
+		if constexpr (MODE == 0)
+			fence_regs(acc1);
+		if ((threadIdx.x & 127) == 0)
+			mbar_arrive(&t_empty[s]);
+	}
+	// epilogue: MODE 0 writes dV (acc1) and scale * dK (acc2) for keys < Sk; MODE 1 scale * dQ for queries < Sq
+#pragma unroll
+	for (int hh = 0; hh < 2; hh++)
+	{
+		const int row = rr + 8 * hh;
+		if (row >= (MODE == 0 ? p.Sk : p.Sq))
+			continue;
+		uint16_t* const o2 = (uint16_t*)p.out2 + b * p.o2_b + (long long)row * p.o2_s + hr * p.o2_h;
+		uint16_t* const o1 = MODE == 0 ? (uint16_t*)p.out1 + b * p.o1_b + (long long)row * p.o1_s + hr * p.o1_h : 0;
+#pragma unroll
+		for (int jn = 0; jn < 16; jn++)
+		{
+			const int d = 8 * jn + 2 * t4;
+			if (d >= p.D)
+				continue;
+			const int i = 4 * jn + 2 * hh;
+			*reinterpret_cast<uint32_t*>(o2 + d) = pack2(acc2[i] * p.scale, acc2[i + 1] * p.scale, is_bf16);
+			if (MODE == 0)
+				*reinterpret_cast<uint32_t*>(o1 + d) = pack2(acc1[i], acc1[i + 1], is_bf16);
+		}
+	}
 }
 
-template <int MODE>
-int launch_bwd(cudaStream_t stream, const CUtensorMap& r1, const CUtensorMap& r2, const CUtensorMap& t1, const CUtensorMap& t2, const FmhaBwdParams& p, int tiles, int heads, int B)
+template <int MODE, int BF16>
+int launch_bwd_t(cudaStream_t stream, const CUtensorMap& r1, const CUtensorMap& r2, const CUtensorMap& t1, const CUtensorMap& t2, const FmhaBwdParams& p, int tiles, int heads, int B)
 {
 	static bool configured_on[64]; // the attribute is per device
 	int dev = 0;
@@ -468,7 +351,7 @@ int launch_bwd(cudaStream_t stream, const CUtensorMap& r1, const CUtensorMap& r2
 	bool& configured = configured_on[dev & 63];
 	if (!configured)
 	{
-		const cudaError_t e = cudaFuncSetAttribute(fmha_bwd_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, FmhaBwdSmem<MODE>::TOTAL);
+		const cudaError_t e = cudaFuncSetAttribute(fmha_bwd_kernel<MODE, BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, FmhaBwdSmem::TOTAL);
 		if (e != cudaSuccess)
 		{
 			set_last_error("cudaFuncSetAttribute(fmha_bwd_kernel)", e);
@@ -476,7 +359,7 @@ int launch_bwd(cudaStream_t stream, const CUtensorMap& r1, const CUtensorMap& r2
 		}
 		configured = true;
 	}
-	fmha_bwd_kernel<MODE><<<dim3(tiles, heads, B), 320, FmhaBwdSmem<MODE>::TOTAL, stream>>>(r1, r2, t1, t2, p);
+	fmha_bwd_kernel<MODE, BF16><<<dim3(tiles, heads, B), FB_THREADS, FmhaBwdSmem::TOTAL, stream>>>(r1, r2, t1, t2, p);
 	count_launch();
 	const cudaError_t e = cudaGetLastError();
 	if (e != cudaSuccess)
@@ -485,6 +368,12 @@ int launch_bwd(cudaStream_t stream, const CUtensorMap& r1, const CUtensorMap& r2
 		return -1;
 	}
 	return 0;
+}
+
+template <int MODE>
+int launch_bwd(cudaStream_t stream, const CUtensorMap& r1, const CUtensorMap& r2, const CUtensorMap& t1, const CUtensorMap& t2, const FmhaBwdParams& p, int tiles, int heads, int B)
+{
+	return p.is_bf16 ? launch_bwd_t<MODE, 1>(stream, r1, r2, t1, t2, p, tiles, heads, B) : launch_bwd_t<MODE, 0>(stream, r1, r2, t1, t2, p, tiles, heads, B);
 }
 
 } // namespace
@@ -546,8 +435,6 @@ int sdpa_backward_f16(cudaStream_t stream, const SdpaGeom& g, const SdpaGeom& dg
 	p.causal = g.is_causal, p.is_bf16 = is_bf16;
 	p.scale = g.scale, p.scale_log2 = g.scale * 1.4426950408889634f;
 	p.stat = (const float4*)stat;
-	p.idesc_xy = umma_instr_desc(is_bf16 ? 1 : 0, 0, 0, FB_R, FB_T);
-	p.idesc_acc = umma_instr_desc(is_bf16 ? 1 : 0, 0, 1, FB_R, FB_D);
 	// dK, dV: one CTA per 128 keys of a (batch, key head)
 	p.out1 = dv, p.o1_b = dg.v_b, p.o1_s = dg.v_s, p.o1_h = dg.v_h;
 	p.out2 = dk, p.o2_b = dg.k_b, p.o2_s = dg.k_s, p.o2_h = dg.k_h;
@@ -557,8 +444,6 @@ int sdpa_backward_f16(cudaStream_t stream, const SdpaGeom& g, const SdpaGeom& dg
 	// dQ: one CTA per 128 queries of a (batch, query head)
 	p.out1 = 0;
 	p.out2 = dq, p.o2_b = dg.q_b, p.o2_s = dg.q_s, p.o2_h = dg.q_h;
-	p.r1 = q, p.r1_b = g.q_b, p.r1_s = g.q_s, p.r1_h = g.q_h;
-	p.r2 = dout, p.r2_b = g.o_b, p.r2_s = g.o_s, p.r2_h = g.o_h;
 	return launch_bwd<1>(stream, tmQr, tmGr, tmKt, tmVt, p, (g.Sq + FB_R - 1) / FB_R, g.H, g.B);
 }
 

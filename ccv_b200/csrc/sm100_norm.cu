@@ -236,8 +236,8 @@ int upsample_fwd_f32(cudaStream_t s, const float* a, float* b, int N, int H, int
 	float rh, rw;
 	ratios(H, W, OH, OW, align_corners, rh, rw);
 	size_t blocks = (total + 255) / 256;
-	if (blocks > 148 * 16)
-		blocks = 148 * 16;
+	if (blocks > 132 * 16)
+		blocks = 132 * 16;
 	upsample_kernel<0><<<(unsigned)blocks, 256, 0, s>>>(a, b, N, H, W, C, OH, OW, type, align_corners, nchw, rh, rw);
 	return check("upsample_fwd");
 }
@@ -251,8 +251,8 @@ int upsample_bwd_f32(cudaStream_t s, const float* g, float* h, int N, int H, int
 	float rh, rw;
 	ratios(H, W, OH, OW, align_corners, rh, rw);
 	size_t blocks = (total + 255) / 256;
-	if (blocks > 148 * 16)
-		blocks = 148 * 16;
+	if (blocks > 132 * 16)
+		blocks = 132 * 16;
 	upsample_kernel<1><<<(unsigned)blocks, 256, 0, s>>>(g, h, N, H, W, C, OH, OW, type, align_corners, nchw, rh, rw);
 	return check("upsample_bwd");
 }
@@ -433,8 +433,8 @@ int group_norm_fwd_f32(cudaStream_t s, const GroupNormGeom& g, const float* x, c
 	gn_stats_kernel<<<(unsigned)slots, 512, 0, s>>>(g, x, saved_mean, saved_inv_std, epsilon);
 	count_launch();
 	long long blocks = (total + 255) / 256;
-	if (blocks > 148 * 16)
-		blocks = 148 * 16;
+	if (blocks > 132 * 16)
+		blocks = 132 * 16;
 	gn_apply_kernel<<<(unsigned)blocks, 256, 0, s>>>(g, x, scale, bias, saved_mean, saved_inv_std, y, total);
 	return check("group_norm_fwd");
 }
@@ -452,8 +452,8 @@ int group_norm_bwd_f32(cudaStream_t s, const GroupNormGeom& g, const float* grad
 		gn_bwd_stats_kernel<<<(unsigned)slots, 512, 0, s>>>(g, grad, x, scale, saved_mean, saved_inv_std, sums);
 		count_launch();
 		long long blocks = (total + 255) / 256;
-		if (blocks > 148 * 16)
-			blocks = 148 * 16;
+		if (blocks > 132 * 16)
+			blocks = 132 * 16;
 		gn_bwd_apply_kernel<<<(unsigned)blocks, 256, 0, s>>>(g, grad, x, scale, saved_mean, saved_inv_std, sums, h, total, (float)slots / (float)total);
 		count_launch();
 	}

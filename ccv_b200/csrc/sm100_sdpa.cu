@@ -1,10 +1,10 @@
 // sm100_sdpa.cu -- SCALED_DOT_PRODUCT_ATTENTION forward / backward, composed per (batch, head) from the tensor-core GEMM
-// (tcgen05 TF32) and two row kernels (masked / causal softmax, softmax gradient), i.e. the same decomposition the
+// (wgmma TF32) and two row kernels (masked / causal softmax, softmax gradient), i.e. the same decomposition the
 // reference's own unit test checks the fused op against (test/unit/nnc/attention.tests.c:14-468).  The score matrix of
 // one (batch, head) lives in the stream workspace.  Semantics: scaled_dot_product_attention/
 // ccv_nnc_scaled_dot_product_attention_cpu_ref.c:16-257 (forward), :259-479 (backward); causal masks are aligned to
 // the bottom-right (x_end = max(x - Sq + Sk + 1, 0), :147); GQA maps query head h to kv head h / (Hq / Hk).
-// A single-kernel tcgen05 flash-attention (S and O in TMEM, online softmax) is the round-2 replacement for this path.
+// 16-bit tensors take the single-kernel flash attention of sm100_fmha.cu instead.
 #include "sm100_contract.h"
 #include "sm100_ew.h"
 #include <float.h>

@@ -1,31 +1,38 @@
-// sm100_umma_gemm.cuh -- the one tensor-core contraction kernel of the backend.
+// sm100_umma_gemm.cuh -- the one tensor-core contraction kernel of the backend (Hopper wgmma).
 //
-//   D[M, N] (+)= A[M, Kdim] * B[Kdim, N]        fp32 in HBM, TF32 tcgen05.mma, fp32 accumulators in TMEM
+//   D[M, N] (+)= A[M, Kdim] * B[Kdim, N]        fp32 accumulators in registers
 //
 // GEMM fwd/bwd, convolution fprop / dgrad / wgrad (implicit GEMM, NHWC) are all this kernel with a different way of
-// bringing the A and B tiles into shared memory (OperandMode).  Data path per CTA (one 128 x BN output tile,
-// optional split-K along gridDim.z):
+// bringing the A and B tiles into shared memory (OperandMode).  One CTA computes one 128 x BN output tile (optional split-K
+// and filter taps along gridDim.z) with 288 threads:
 //
-//   warp 0   TMA producer: cp.async.bulk.tensor (tile mode or im2col mode) -> 128B-swizzled smem stages, mbarrier tx
-//   warp 1   TMEM allocator + single-thread tcgen05.mma issuer (UMMA 128 x BN x 8, kind::tf32), tcgen05.commit
-//   warp 2-5 epilogue: tcgen05.ld 32x32b -> registers -> (+bias, +C) -> 128-bit global stores (split-K: into this split's scratch slice)
+//   warps 0-7  two consumer warpgroups, 64 output rows each: wgmma.mma_async from 128-byte-swizzled K-major tiles (16-bit MN-major
+//              tiles through the descriptor's transpose bit), then the epilogue straight from the accumulator registers
+//              (+bias, +C, 16-bit rounding; split-K: into this split's scratch slice)
+//   warp 8     TMA producer: cp.async.bulk.tensor (tile mode or im2col mode) into a ring of STAGES stages, mbarrier tx counts
 //
-// Two CTAs are resident per SM (3 stages x 32 KB at BN = 128), so one CTA's epilogue overlaps the other's main loop.
+// fp32 operands run as TF32 (kind 0; the TMA unit rounds them to TF32 on the way in) or as 3xTF32 (X3).  wgmma reads TF32 operands
+// K-major only, so the fp32 kernels whose operands arrive MN-major, and the 3xTF32 kernels, pass every stage through a transform
+// step first: the consumers copy the staged tiles into one of two K-major operand slots (transposing MN-major tiles, splitting
+// 3xTF32 operands into hi / lo) and release the stage to the producer before the MMAs run.
 #pragma once
 #include "sm100_ptx.cuh"
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 
 namespace sm100 {
 
 enum OperandMode {
-	OP_K2D = 0,    // K-major 2-D tensor [rows, K]: one box {32 k, rows} per stage
-	OP_MN2D = 1,   // MN-major 2-D tensor [K, rows]: rows/32 boxes {32 mn, BLOCK_K k} per stage
+	OP_K2D = 0,    // K-major 2-D tensor [rows, K]: one box {one 128-byte span of k, rows} per stage
+	OP_MN2D = 1,   // MN-major 2-D tensor [K, rows]: boxes {BK mn, BK k} per stage
 	OP_IM2COL = 2, // NHWC tensor through im2col-mode TMA.  As A: pixels are rows (K-major, channels = K).
 	               //                                       As B: pixels are K   (MN-major, channels = N).
 };
 
 constexpr int UMMA_BLOCK_M = 128;
-constexpr int UMMA_BLOCK_K = 32; // fp32 elements per stage along K = one 128-byte swizzle span
+constexpr int UMMA_BLOCK_K = 32; // fp32 elements per stage along K = one 128-byte span
 constexpr int UMMA_MAX_TAPS = 64;
+constexpr int GEMM_THREADS = 288;
 
 struct UmmaRowMap {
 	// output row m -> element offset.  mode 0: m * ld.  mode 1: m = (n, i, j) over a (Pc x Qc) grid per image:
@@ -37,7 +44,7 @@ struct UmmaRowMap {
 
 struct UmmaGemmParams {
 	int M, N;
-	int k_iters;        // BLOCK_K iterations over the whole reduction (all taps x chunks)
+	int k_iters;        // BK iterations over the whole reduction (all taps x chunks)
 	int chunks_per_tap; // k-iteration it -> tap = it / chunks_per_tap, chunk = it % chunks_per_tap
 	int splits;         // split-K factor; gridDim.z = grid_taps * splits.  Split s writes its partial tile to out + s * split_out_stride
 	                    // (a scratch slice per split, plain stores); splitk_reduce_kernel then adds the slices in a fixed order, so the
@@ -55,88 +62,149 @@ struct UmmaGemmParams {
 	float* out;
 	const float* bias;
 	int accumulate; // 1: D += existing output (CCV_NNC_ACCUMULATE_OUTPUT)
-	float alpha;    // scales the product (1 for the reference's commands)
 	UmmaRowMap rowmap;
-	// optional per-column statistics of the output (batch-norm forward fused into the producing convolution; persistent kernel,
-	// TMA-store epilogue only).  Four planes of stats_rows x N floats: count, shift k, sum(v - k), sum((v - k)^2).  Row
-	// blockIdx.x * 4 + quarter belongs to one epilogue warp quarter of one CTA and every (row, column) slot to exactly one thread,
-	// which updates it with plain loads / stores tile after tile: no atomics, a fixed summation order, and a per-slot shift (the
-	// first value seen) that keeps the one-pass variance well conditioned.  The count plane must be zero on entry.
+	// optional per-column statistics of the output (batch-norm forward fused into the producing convolution; kernels without the
+	// transform step only).  Four planes of stats_rows x N floats: count, shift k, sum(v - k), sum((v - k)^2).  Row blockIdx.x * 4 + quarter
+	// belongs to one 32-row quarter of the tiles of one CTA column (gridDim.x CTAs walk the M tiles, blockIdx.x + i * gridDim.x), and every
+	// (row, column) slot to one thread, which merges the per-warp shifted sums of each tile into it in a fixed order: no atomics, and the
+	// shift (the first value seen) keeps the one-pass variance well conditioned.  The count plane must be zero on entry.
 	float* stats;
 	int stats_rows;
-	int tma_store; // persistent kernel: the epilogue writes 32 x 32 chunks with TMA tile stores through the output tensor map
-	// Operand / output format of the PERSISTENT kernel (the one-tile and taps kernels are fp32-only and ignore these).  Operand
-	// tiles are always 128-byte-span swizzled rows, so a stage holds bk = 128 / sizeof(element) elements along K: 32 fp32
-	// (kind::tf32, 4 MMAs of K = 8) or 64 bf16 / fp16 (kind::f16, 4 MMAs of K = 16); all byte sizes are the same.
-	int kind16;            // 0: fp32 operands through kind::tf32; 1: 16-bit operands through kind::f16 (idesc names bf16 / fp16); the
-	                       // kernel itself is compiled per operand size (template K16), this records which one the host chose
-	int out_kind;          // OUT16 kernels: 1 = bf16, 2 = fp16 output elements (0: fp32 output)
-	const void* bias16;    // OUT16 kernels: bias in the output's 16-bit type (p.bias, fp32, wins when both are given)
-	uint32_t idesc;
-	// smem descriptor fields for MN-major operands (layout SWIZZLE_128B_BASE32B: 128 B of MN x 4 k-rows per atom)
-	uint32_t mn_lbo, mn_sbo, mn_layout;
+	int kind16;         // 0: fp32 operands (TF32 / 3xTF32); 1: 16-bit operands (the kernel is compiled per operand size, template K16)
+	int out_kind;       // 16-bit operands: 1 = bf16, 2 = fp16 (also the output element type of OUT16 kernels)
+	const void* bias16; // OUT16 kernels: bias in the output's 16-bit type (p.bias, fp32, wins when both are given)
 };
 
-template <int BN, int STAGES>
-struct UmmaSmem {
-	static constexpr int A_BYTES = UMMA_BLOCK_M * UMMA_BLOCK_K * 4;
-	static constexpr int B_BYTES = BN * UMMA_BLOCK_K * 4;
-	static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-	static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;
-	static constexpr int TOTAL = BAR_OFFSET + 256 + 1024; // barriers + slack for the 1024-byte alignment
-};
-
-template <int AMODE, int BMODE, int BN, int STAGES>
-__global__ void __launch_bounds__(192, 1) umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const UmmaGemmParams p)
+// 16-bit output helpers: kind 1 = bf16, 2 = fp16, round to nearest even
+__device__ __forceinline__ uint32_t pack16x2(const float a, const float b, const int kind)
 {
-	using S = UmmaSmem<BN, STAGES>;
+	if (kind == 1)
+	{
+		const __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
+		return *reinterpret_cast<const uint32_t*>(&v);
+	}
+	const __half2 v = __floats2half2_rn(a, b);
+	return *reinterpret_cast<const uint32_t*>(&v);
+}
+__device__ __forceinline__ float cvt16(const uint16_t x, const int kind)
+{
+	return kind == 1 ? __uint_as_float((uint32_t)x << 16) : __half2float(__ushort_as_half(x));
+}
+
+// X3 = 1 selects the error-compensated "3xTF32" form (CCV_NNC_SM100_ALGO_3XTF32): the operands arrive as raw fp32 (tensor map data type
+// FLOAT32, no rounding); the transform step splits every element into hi = x with the low 13 mantissa bits cleared (exactly representable
+// in TF32) and lo = x - hi (exact in fp32), and three MMAs per k-step -- lo*hi + hi*lo + hi*hi (lo*lo ~ 2^-22 is dropped) -- accumulate
+// into the same fp32 registers.  The product then carries ~2^-21 relative error per term instead of TF32's 2^-11: fp32-grade results
+// (the reference's fp32 GEMM is CUBLAS_COMPUTE_32F, lib/nnc/gpu/ccv_nnc_compat.cu:786-803) at a third of the tensor rate.
+template <int AMODE, int BMODE, int K16, int X3>
+struct GemmXform {
+	static constexpr bool A_T = !K16 && AMODE == OP_MN2D; // fp32 MN-major A: transposed into the K-major slot
+	static constexpr bool B_T = !K16 && BMODE != OP_K2D;  // fp32 MN-major B (2-D or im2col)
+	static constexpr bool ANY = A_T || B_T || X3;
+};
+
+template <int BN, int STAGES, bool XF, int X3>
+struct UmmaSmem {
+	static constexpr int A_BYTES = UMMA_BLOCK_M * 128;
+	static constexpr int B_BYTES = BN * 128;
+	static constexpr int RAW_BYTES = A_BYTES + B_BYTES;            // one TMA stage
+	static constexpr int SLOT_BYTES = RAW_BYTES * (X3 ? 2 : 1);     // one K-major operand slot: [A hi][B hi] ([A lo][B lo])
+	static constexpr int SLOT_OFFSET = STAGES * RAW_BYTES;
+	static constexpr int STATS_OFFSET = SLOT_OFFSET + (XF ? 2 * SLOT_BYTES : 0);
+	static constexpr int STATS_BYTES = XF ? 0 : 4 * BN * 4 * 4 + 2 * 4 * BN * 3 * 4; // running (n, k, s1, s2) per slot + per-warp partials
+	static constexpr int BAR_OFFSET = STATS_OFFSET + STATS_BYTES;
+	static constexpr int TOTAL = BAR_OFFSET + 256 + 1024;           // barriers + slack for the 1024-byte alignment
+};
+
+// stages per kernel: as deep as 227 KB of shared memory allows with the transform slots
+template <int BN, bool XF, int X3>
+struct GemmStages {
+	static constexpr int value = X3 ? (BN == 128 ? 3 : 4) : (XF ? 4 : (BN == 128 ? 5 : 6));
+};
+
+// one staged fp32 operand tile (rows x 32 k) -> K-major 128-byte-swizzled slot (16-byte chunk c of row r at chunk c ^ (r & 7)).
+// MN-major input (T): 32-wide MN boxes of 32 k-rows of 128 B, no swizzle; K-major input: already in the slot layout.
+template <bool T, int X3>
+__device__ __forceinline__ void xform_tile(const float* __restrict__ raw, float* __restrict__ hi, float* __restrict__ lo, const int rows, const int tid)
+{
+	for (int idx = tid; idx < rows * 8; idx += 256)
+	{
+		float4 x;
+		int dst;
+		if (T)
+		{
+			const int mn = idx % rows, c = idx / rows;
+			const float* const src = raw + (mn >> 5) * 1024 + (c * 4) * 32 + (mn & 31);
+			x = make_float4(src[0], src[32], src[64], src[96]);
+			dst = mn * 32 + ((c ^ (mn & 7)) << 2);
+		} else {
+			x = reinterpret_cast<const float4*>(raw)[idx];
+			dst = idx * 4;
+		}
+		if (X3)
+		{
+			float4 h, l;
+			h.x = __uint_as_float(__float_as_uint(x.x) & 0xffffe000u), h.y = __uint_as_float(__float_as_uint(x.y) & 0xffffe000u);
+			h.z = __uint_as_float(__float_as_uint(x.z) & 0xffffe000u), h.w = __uint_as_float(__float_as_uint(x.w) & 0xffffe000u);
+			// x - hi is exact; an infinity keeps lo = 0 so that inf stays inf instead of turning into inf - inf
+			l.x = fabsf(x.x) < __int_as_float(0x7f800000) ? x.x - h.x : 0.f, l.y = fabsf(x.y) < __int_as_float(0x7f800000) ? x.y - h.y : 0.f;
+			l.z = fabsf(x.z) < __int_as_float(0x7f800000) ? x.z - h.z : 0.f, l.w = fabsf(x.w) < __int_as_float(0x7f800000) ? x.w - h.w : 0.f;
+			*reinterpret_cast<float4*>(hi + dst) = h;
+			*reinterpret_cast<float4*>(lo + dst) = l;
+		} else
+			*reinterpret_cast<float4*>(hi + dst) = x;
+	}
+}
+
+// K16 = 1 / 2: bf16 / fp16 operands (p.out_kind holds the same kind), 64 elements per 128-byte row, K = 16 per MMA; K16 = 0: fp32
+// operands (32 per row, K = 8 per MMA).  The element type is a template parameter so that every wgmma of a k-step sits in one basic
+// block (a runtime type branch makes ptxas fence each MMA on its own).  OUT16 = 1: the output tensor (and an optional 16-bit bias) is bf16 / fp16 (p.out_kind).
+template <int AMODE, int BMODE, int BN, int STAGES, int X3 = 0, int K16 = 0, int OUT16 = 0>
+__global__ void __launch_bounds__(GEMM_THREADS, 1) umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const UmmaGemmParams p)
+{
+	using XF = GemmXform<AMODE, BMODE, K16, X3>;
+	using S = UmmaSmem<BN, STAGES, XF::ANY, X3>;
 	extern __shared__ uint8_t smem_raw[];
 	uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
 	uint64_t* full_bar = (uint64_t*)(smem + S::BAR_OFFSET);
 	uint64_t* empty_bar = full_bar + STAGES;
-	uint64_t* tmem_full_bar = empty_bar + STAGES;
-	uint32_t* tmem_slot = (uint32_t*)(tmem_full_bar + 1);
 
+	constexpr int BK = K16 ? 64 : 32;          // K elements per stage = MN elements per MN-major box: one 128-byte span
+	constexpr int MN_BOX_BYTES = BK * 128;     // an MN-major box: BK k-rows of 128 bytes
 	const int warp = threadIdx.x >> 5;
 	const int lane = threadIdx.x & 31;
-	const int m0 = blockIdx.x * UMMA_BLOCK_M;
+	const int tiles_m = (p.M + UMMA_BLOCK_M - 1) / UMMA_BLOCK_M; // M tiles blockIdx.x, blockIdx.x + gridDim.x, ... (one unless statistics)
 	const int n0 = blockIdx.y * BN;
 	const int split = blockIdx.z % p.splits;
 	const int gtap = blockIdx.z / p.splits;
-	// this CTA's slice of the reduction
 	const int per = (p.k_iters + p.splits - 1) / p.splits;
 	const int it_begin = split * per;
 	const int it_end = min(p.k_iters, it_begin + per);
-	const int n_it = it_end - it_begin;
+	const int n_it = max(it_end - it_begin, 0);
 
-	if (warp == 0 && lane == 0)
+	if (threadIdx.x == 0)
 	{
-		tma_prefetch_desc(&tmA);
-		tma_prefetch_desc(&tmB);
 		for (int s = 0; s < STAGES; s++)
 		{
 			mbar_init(&full_bar[s], 1);
-			mbar_init(&empty_bar[s], 1);
+			mbar_init(&empty_bar[s], XF::ANY ? 1 : 2); // transform: one arrival after the consumers' barrier; else one per warpgroup
 		}
-		mbar_init(tmem_full_bar, 1);
 		fence_mbar_init();
 	}
-	if (warp == 1)
-	{
-		tmem_alloc(tmem_slot, BN);
-		tmem_relinquish();
-	}
-	tc_fence_before();
 	__syncthreads();
-	tc_fence_after();
-	const uint32_t tmem_base = *tmem_slot;
 
-	if (warp == 0)
+	if (warp == 8)
 	{
 		// ------------------------------------------------------------------ TMA producer
-		if (n_it > 0 && elect_one())
+		if (elect_one())
 		{
-			// im2col base coordinates of this tile's first row (A side); fixed for the whole loop
+			tma_prefetch_desc(&tmA);
+			tma_prefetch_desc(&tmB);
+			int stage = 0;
+			uint32_t phase = 0;
+			for (int mt = blockIdx.x; mt < tiles_m; mt += gridDim.x)
+			{
+			const int m0 = mt * UMMA_BLOCK_M;
 			int a_w = 0, a_h = 0, a_n = 0;
 			if (AMODE == OP_IM2COL)
 			{
@@ -146,152 +214,292 @@ __global__ void __launch_bounds__(192, 1) umma_gemm_kernel(const __grid_constant
 				a_h = (t % p.P) * p.stride_h + p.base_h;
 				a_n = t / p.P;
 			}
-			int stage = 0;
-			uint32_t phase = 0;
 			for (int it = it_begin; it < it_end; it++)
 			{
 				const int tap = it / p.chunks_per_tap;
 				const int chunk = it - tap * p.chunks_per_tap;
 				mbar_wait(&empty_bar[stage], phase ^ 1);
-				uint8_t* sA = smem + stage * S::STAGE_BYTES;
+				uint8_t* sA = smem + stage * S::RAW_BYTES;
 				uint8_t* sB = sA + S::A_BYTES;
-				mbar_expect_tx(&full_bar[stage], S::STAGE_BYTES);
+				mbar_expect_tx(&full_bar[stage], S::RAW_BYTES);
 				if (AMODE == OP_K2D)
-					tma_load_2d(sA, &tmA, &full_bar[stage], chunk * UMMA_BLOCK_K, m0);
+					tma_load_2d(sA, &tmA, &full_bar[stage], chunk * BK, m0);
 				else if (AMODE == OP_MN2D) {
 #pragma unroll
-					for (int j = 0; j < UMMA_BLOCK_M / 32; j++)
-						tma_load_2d(sA + j * 4096, &tmA, &full_bar[stage], m0 + 32 * j, it * UMMA_BLOCK_K);
+					for (int j = 0; j < UMMA_BLOCK_M / BK; j++)
+						tma_load_2d(sA + j * MN_BOX_BYTES, &tmA, &full_bar[stage], m0 + BK * j, it * BK);
 				} else
-					tma_load_im2col_4d(sA, &tmA, &full_bar[stage], chunk * UMMA_BLOCK_K, a_w, a_h, a_n, p.tap_off_w[tap], p.tap_off_h[tap]);
+					tma_load_im2col_4d(sA, &tmA, &full_bar[stage], chunk * BK, a_w, a_h, a_n, p.tap_off_w[tap], p.tap_off_h[tap]);
 				if (BMODE == OP_K2D)
-					tma_load_2d(sB, &tmB, &full_bar[stage], p.tap_b_col[tap] + chunk * UMMA_BLOCK_K, n0);
+					tma_load_2d(sB, &tmB, &full_bar[stage], p.tap_b_col[tap] + chunk * BK, n0);
 				else if (BMODE == OP_MN2D) {
 #pragma unroll
-					for (int j = 0; j < BN / 32; j++)
-						tma_load_2d(sB + j * 4096, &tmB, &full_bar[stage], p.tap_b_col[tap] + n0 + 32 * j, chunk * UMMA_BLOCK_K);
+					for (int j = 0; j < BN / BK; j++)
+						tma_load_2d(sB + j * MN_BOX_BYTES, &tmB, &full_bar[stage], p.tap_b_col[tap] + n0 + BK * j, chunk * BK);
 				} else {
-					// pixels are the reduction: this iteration covers base pixels [it * 32, it * 32 + 32)
-					const int pix = it * UMMA_BLOCK_K;
+					// pixels are the reduction: this iteration covers base pixels [it * BK, it * BK + BK)
+					const int pix = it * BK;
 					const int q = pix % p.Q;
 					const int t = pix / p.Q;
 					const int b_w = q * p.stride_w + p.base_w;
 					const int b_h = (t % p.P) * p.stride_h + p.base_h;
 					const int b_n = t / p.P;
 #pragma unroll
-					for (int j = 0; j < BN / 32; j++)
-						tma_load_im2col_4d(sB + j * 4096, &tmB, &full_bar[stage], n0 + 32 * j, b_w, b_h, b_n, p.tap_off_w[gtap], p.tap_off_h[gtap]);
+					for (int j = 0; j < BN / BK; j++)
+						tma_load_im2col_4d(sB + j * MN_BOX_BYTES, &tmB, &full_bar[stage], n0 + BK * j, b_w, b_h, b_n, p.tap_off_w[gtap], p.tap_off_h[gtap]);
 				}
 				if (++stage == STAGES) { stage = 0; phase ^= 1; }
 			}
-		}
-	} else if (warp == 1) {
-		// ------------------------------------------------------------------ MMA issuer: one elected thread, operands in uniform registers
-		// (sm100_umma_persistent.cuh explains why not `lane == 0`)
-		if (n_it > 0 && elect_one())
-		{
-			const uint32_t smem_base = smem_u32(smem);
-			// K-major (SWIZZLE_128B): 8 fp32 = 32 bytes along the swizzled row per MMA; SBO = 8 rows x 128 B.
-			// MN-major tf32 (SWIZZLE_128B_BASE32B is the only legal layout): 8 k-rows x 128 B = 1024 bytes per MMA;
-			// LBO = stride between 32-wide MN groups, SBO = stride between 4-row k atoms.  The start-address field counts 16-byte units.
-			const uint64_t a_desc0 = (AMODE == OP_MN2D) ? umma_smem_desc(smem_base, p.mn_lbo, p.mn_sbo, p.mn_layout) : umma_smem_desc(smem_base, 16, 1024, 2);
-			const uint64_t b_desc0 = (BMODE == OP_K2D) ? umma_smem_desc(smem_base + S::A_BYTES, 16, 1024, 2) : umma_smem_desc(smem_base + S::A_BYTES, p.mn_lbo, p.mn_sbo, p.mn_layout);
-			constexpr uint32_t A_STEP = (AMODE == OP_MN2D ? 1024 : 32) >> 4, B_STEP = (BMODE == OP_K2D ? 32 : 1024) >> 4;
-			const uint32_t idesc = p.idesc;
-			int stage = 0;
-			uint32_t phase = 0;
-			for (int it = 0; it < n_it; it++)
-			{
-				mbar_wait(&full_bar[stage], phase);
-				tc_fence_after();
-				const uint64_t da0 = a_desc0 + (uint32_t)stage * (uint32_t)(S::STAGE_BYTES >> 4);
-				const uint64_t db0 = b_desc0 + (uint32_t)stage * (uint32_t)(S::STAGE_BYTES >> 4);
-#pragma unroll
-				for (int k = 0; k < UMMA_BLOCK_K / 8; k++)
-					umma_tf32(tmem_base, da0 + k * A_STEP, db0 + k * B_STEP, idesc, (it > 0 || k > 0) ? 1u : 0u);
-				umma_commit(&empty_bar[stage]); // frees the smem stage once these MMAs have read it
-				if (it == n_it - 1)
-					umma_commit(tmem_full_bar);
-				if (++stage == STAGES) { stage = 0; phase ^= 1; }
 			}
 		}
-	} else {
-		// ------------------------------------------------------------------ epilogue (warps 2..5)
-		const int quarter = warp & 3; // TMEM lanes [32 * quarter, +32) are the ones this warp may read
-		const int row = m0 + quarter * 32 + lane;
-		if (n_it > 0)
+		return;
+	}
+
+	// ------------------------------------------------------------------ consumers (warps 0..7)
+	const int wg = warp >> 2; // output rows [64 * wg, +64) of the tile
+	float acc[BN / 2];
+	constexpr bool A_MN16 = K16 && AMODE == OP_MN2D, B_MN16 = K16 && BMODE != OP_K2D;
+	constexpr uint32_t A_STEP = A_MN16 ? 2048 : 32, B_STEP = B_MN16 ? 2048 : 32; // bytes per MMA step along K
+	int stage = 0;
+	uint32_t phase = 0;
+	int prev_stage = 0;
+	int gi = 0; // k-iterations of all tiles so far: the operand slot parity
+	float* const st_run = reinterpret_cast<float*>(smem + S::STATS_OFFSET); // [4 quarters][BN] x (n, k, s1, s2)
+	float* const st_part = st_run + 4 * BN * 4;                                // [2 warps of a quarter][4 quarters][BN] x (k, s1, s2)
+	const bool stats = !XF::ANY && p.stats != 0;
+	if (stats)
+		for (int i = threadIdx.x; i < 4 * BN; i += 256)
+			st_run[i * 4] = 0.f;
+	for (int mt = blockIdx.x; mt < tiles_m; mt += gridDim.x)
+	{
+	const int m0 = mt * UMMA_BLOCK_M;
+#pragma unroll
+	for (int i = 0; i < BN / 2; i++)
+		acc[i] = 0.f;
+	for (int it = 0; it < n_it; it++, gi++)
+	{
+		mbar_wait(&full_bar[stage], phase);
+		uint8_t* op = smem + stage * S::RAW_BYTES;
+		if (XF::ANY)
 		{
-			mbar_wait(tmem_full_bar, 0);
-			tc_fence_after();
+			// every consumer has retired the MMAs that read slot (it & 1) two iterations ago (wgmma_wait<1> below)
+			named_bar_sync(1, 256);
+			op = smem + S::SLOT_OFFSET + (gi & 1) * S::SLOT_BYTES;
+			const float* const raw = reinterpret_cast<const float*>(smem + stage * S::RAW_BYTES);
+			float* const hi = reinterpret_cast<float*>(op);
+			float* const lo = reinterpret_cast<float*>(op + S::RAW_BYTES);
+			xform_tile<XF::A_T, X3>(raw, hi, lo, UMMA_BLOCK_M, threadIdx.x);
+			xform_tile<XF::B_T, X3>(raw + S::A_BYTES / 4, hi + S::A_BYTES / 4, lo + S::A_BYTES / 4, BN, threadIdx.x);
+			fence_proxy_async(); // the tensor core reads shared memory through the async proxy
+			named_bar_sync(1, 256);
+			if (threadIdx.x == 0)
+				mbar_arrive(&empty_bar[stage]); // the raw stage has been consumed
 		}
-		long long row_off;
+		const uint32_t base = smem_u32(op);
+		const uint64_t da0 = wgmma_desc(base + wg * 8192, 16, 1024);
+		const uint64_t db0 = wgmma_desc(base + S::A_BYTES, 8192, 1024);
+		fence_regs(acc);
+		wgmma_fence();
+#pragma unroll
+		for (int k = 0; k < 4; k++)
+		{
+			const uint64_t da = da0 + ((k * A_STEP) >> 4), db = db0 + ((k * B_STEP) >> 4);
+			if constexpr (K16 != 0)
+			{
+				if constexpr (K16 == 1)
+				{
+					if constexpr (BN == 128)
+						wgmma_bf16_ss_n128<A_MN16, B_MN16>(*reinterpret_cast<float(*)[64]>(acc), da, db);
+					else
+						wgmma_bf16_ss_n64<A_MN16, B_MN16>(*reinterpret_cast<float(*)[32]>(acc), da, db);
+				} else {
+					if constexpr (BN == 128)
+						wgmma_f16_ss_n128<A_MN16, B_MN16>(*reinterpret_cast<float(*)[64]>(acc), da, db);
+					else
+						wgmma_f16_ss_n64<A_MN16, B_MN16>(*reinterpret_cast<float(*)[32]>(acc), da, db);
+				}
+			} else {
+				constexpr uint32_t LO = (uint32_t)(S::RAW_BYTES >> 4);
+				if constexpr (BN == 128)
+				{
+					float (&d)[64] = *reinterpret_cast<float(*)[64]>(acc);
+					if (X3)
+					{
+						// small terms first, then hi * hi
+						wgmma_tf32_ss_n128(d, da + LO, db);
+						wgmma_tf32_ss_n128(d, da, db + LO);
+					}
+					wgmma_tf32_ss_n128(d, da, db);
+				} else {
+					float (&d)[32] = *reinterpret_cast<float(*)[32]>(acc);
+					if (X3)
+					{
+						wgmma_tf32_ss_n64(d, da + LO, db);
+						wgmma_tf32_ss_n64(d, da, db + LO);
+					}
+					wgmma_tf32_ss_n64(d, da, db);
+				}
+			}
+		}
+		wgmma_commit();
+		fence_regs(acc);
+		wgmma_wait<1>(); // the MMAs of iteration it - 1 are complete
+		if (!XF::ANY && it > 0 && (threadIdx.x & 127) == 0)
+			mbar_arrive(&empty_bar[prev_stage]);
+		prev_stage = stage;
+		if (++stage == STAGES) { stage = 0; phase ^= 1; }
+	}
+	wgmma_wait<0>();
+	fence_regs(acc);
+	if (!XF::ANY && n_it > 0 && (threadIdx.x & 127) == 0)
+		mbar_arrive(&empty_bar[prev_stage]); // the last stage of this tile
+
+	// ------------------------------------------------------------------ epilogue: accumulator i -> (row, column), see sm100_ptx.cuh
+	constexpr int OSZ = OUT16 ? 2 : 4;
+	const bool add_bias = split == 0;
+	const float* const bias = p.bias;
+	const uint16_t* const bias16 = OUT16 && !p.bias ? reinterpret_cast<const uint16_t*>(p.bias16) : 0;
+	char* orow[2];
+#pragma unroll
+	for (int h = 0; h < 2; h++)
+	{
+		const int row = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+		long long off;
 		if (p.rowmap.mode == 0)
-			row_off = (long long)row * p.rowmap.ld;
+			off = (long long)row * p.rowmap.ld;
 		else {
 			const int pq = p.rowmap.Pc * p.rowmap.Qc;
 			const int n = row / pq;
 			const int rem = row - n * pq;
-			const int i = rem / p.rowmap.Qc;
-			const int j = rem - i * p.rowmap.Qc;
-			row_off = n * p.rowmap.n_stride + i * p.rowmap.h_stride + j * p.rowmap.w_stride;
+			const int ii = rem / p.rowmap.Qc;
+			const int jj = rem - ii * p.rowmap.Qc;
+			off = n * p.rowmap.n_stride + ii * p.rowmap.h_stride + jj * p.rowmap.w_stride;
 		}
-		float* const orow = p.out + row_off + (long long)gtap * p.grid_tap_out_stride + (long long)split * p.split_out_stride;
-		const bool row_ok = row < p.M;
-		const bool vec_ok = ((((uintptr_t)orow) & 15) == 0);
-		const bool add_bias = p.bias != 0 && split == 0;
-#pragma unroll 1
-		for (int c = 0; c < BN / 32; c++)
+		orow[h] = row < p.M ? reinterpret_cast<char*>(p.out) + (off + (long long)gtap * p.grid_tap_out_stride + (long long)split * p.split_out_stride) * OSZ : 0;
+	}
+	const int N = p.N;
+	const bool accumulate = p.accumulate != 0;
+#pragma unroll
+	for (int j = 0; j < BN / 8; j++)
+	{
+		const int col = n0 + 8 * j + 2 * (lane & 3);
+		if (col >= N)
+			continue;
+		const bool two = col + 1 < N;
+		float b0 = 0.f, b1 = 0.f;
+		if (add_bias && bias)
+			b0 = __ldg(bias + col), b1 = two ? __ldg(bias + col + 1) : 0.f;
+		else if (add_bias && bias16)
+			b0 = cvt16(__ldg(bias16 + col), p.out_kind), b1 = two ? cvt16(__ldg(bias16 + col + 1), p.out_kind) : 0.f;
+#pragma unroll
+		for (int h = 0; h < 2; h++)
 		{
-			uint32_t r[32];
-			if (n_it > 0)
-			{
-				tmem_ld_32x32(tmem_base + ((uint32_t)(quarter * 32) << 16) + c * 32, r);
-				tmem_ld_wait();
-			} else {
-#pragma unroll
-				for (int i = 0; i < 32; i++)
-					r[i] = 0;
-			}
-			const int col0 = n0 + c * 32;
-			if (!row_ok || col0 >= p.N)
+			if (!orow[h])
 				continue;
-			float v[32];
-#pragma unroll
-			for (int i = 0; i < 32; i++)
-				v[i] = __uint_as_float(r[i]) * p.alpha;
-			if (add_bias)
+			float v0 = acc[4 * j + 2 * h] + b0, v1 = acc[4 * j + 2 * h + 1] + b1;
+			if (!OUT16)
 			{
-#pragma unroll
-				for (int i = 0; i < 32; i++)
-					if (col0 + i < p.N)
-						v[i] += __ldg(p.bias + col0 + i);
-			}
-			float* const o = orow + col0;
-			if (col0 + 32 <= p.N && vec_ok)
-			{
-				if (p.accumulate)
+				float* const o = reinterpret_cast<float*>(orow[h]) + col;
+				if (two && ((((uintptr_t)o) & 7) == 0))
 				{
-#pragma unroll
-					for (int i = 0; i < 32; i += 4)
+					if (accumulate)
 					{
-						const float4 e = *reinterpret_cast<const float4*>(o + i);
-						v[i] += e.x, v[i + 1] += e.y, v[i + 2] += e.z, v[i + 3] += e.w;
+						const float2 e = *reinterpret_cast<const float2*>(o);
+						v0 += e.x, v1 += e.y;
 					}
+					*reinterpret_cast<float2*>(o) = make_float2(v0, v1);
+				} else {
+					o[0] = accumulate ? o[0] + v0 : v0;
+					if (two)
+						o[1] = accumulate ? o[1] + v1 : v1;
 				}
-#pragma unroll
-				for (int i = 0; i < 32; i += 4)
-					*reinterpret_cast<float4*>(o + i) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
 			} else {
-				for (int i = 0; i < 32; i++)
-					if (col0 + i < p.N)
-						o[i] = p.accumulate ? o[i] + v[i] : v[i];
+				uint16_t* const o = reinterpret_cast<uint16_t*>(orow[h]) + col;
+				if (two && ((((uintptr_t)o) & 3) == 0))
+				{
+					if (accumulate)
+					{
+						const uint32_t e = *reinterpret_cast<const uint32_t*>(o);
+						v0 += cvt16((uint16_t)(e & 0xffffu), p.out_kind), v1 += cvt16((uint16_t)(e >> 16), p.out_kind);
+					}
+					*reinterpret_cast<uint32_t*>(o) = pack16x2(v0, v1, p.out_kind);
+				} else {
+					o[0] = (uint16_t)(pack16x2(accumulate ? cvt16(o[0], p.out_kind) + v0 : v0, 0.f, p.out_kind) & 0xffffu);
+					if (two)
+						o[1] = (uint16_t)(pack16x2(accumulate ? cvt16(o[1], p.out_kind) + v1 : v1, 0.f, p.out_kind) & 0xffffu);
+				}
 			}
 		}
 	}
-	tc_fence_before();
-	__syncthreads();
-	if (warp == 1)
-		tmem_dealloc(tmem_base, BN);
+	if (stats)
+	{
+		// per warp: shifted sums of its 16 rows (as stored: after the bias and the 16-bit rounding) per column, shift = the warp's first
+		// row; lanes 0..3 leave them in st_part for the slot owners
+		const int quarter = wg * 2 + ((warp & 3) >> 1), half = warp & 1;
+		const int row0 = m0 + wg * 64 + (warp & 3) * 16;
+		const int valid = max(0, min(16, p.M - row0));
+		const bool r1_ok = (lane >> 2) + 8 < valid, r0_ok = (lane >> 2) < valid;
+		float* const part = st_part + ((half * 4 + quarter) * BN) * 3;
+#pragma unroll
+		for (int j = 0; j < BN / 8; j++)
+#pragma unroll
+			for (int e = 0; e < 2; e++)
+			{
+				const int c = n0 + 8 * j + 2 * (lane & 3) + e;
+				float v0 = acc[4 * j + e] + (bias && c < p.N ? __ldg(bias + c) : (bias16 && c < p.N ? cvt16(__ldg(bias16 + c), p.out_kind) : 0.f));
+				float v1 = acc[4 * j + 2 + e] + (bias && c < p.N ? __ldg(bias + c) : (bias16 && c < p.N ? cvt16(__ldg(bias16 + c), p.out_kind) : 0.f));
+				if (OUT16)
+					v0 = cvt16((uint16_t)(pack16x2(v0, 0.f, p.out_kind) & 0xffffu), p.out_kind), v1 = cvt16((uint16_t)(pack16x2(v1, 0.f, p.out_kind) & 0xffffu), p.out_kind);
+				const float k = __shfl_sync(0xffffffffu, v0, lane & 3);
+				const float d0 = r0_ok ? v0 - k : 0.f, d1 = r1_ok ? v1 - k : 0.f;
+				float s1 = d0 + d1, s2 = fmaf(d0, d0, d1 * d1);
+#pragma unroll
+				for (int m = 4; m <= 16; m <<= 1)
+					s1 += __shfl_xor_sync(0xffffffffu, s1, m), s2 += __shfl_xor_sync(0xffffffffu, s2, m);
+				if (lane < 4)
+				{
+					float* const q = part + (8 * j + 2 * lane + e) * 3;
+					q[0] = k, q[1] = s1, q[2] = s2;
+				}
+			}
+		named_bar_sync(1, 256);
+		// slot owners: (quarter, column) -> merge the two warps' sums, shifted to the slot's own k (exact algebra: d' = d + (k_w - k))
+		for (int i = threadIdx.x; i < 4 * BN; i += 256)
+		{
+			const int q = i / BN, c = i - q * BN;
+			float* const run = st_run + i * 4;
+#pragma unroll
+			for (int h = 0; h < 2; h++)
+			{
+				const float nw = (float)max(0, min(16, p.M - (m0 + q * 32 + h * 16)));
+				if (nw <= 0.f)
+					continue;
+				const float* const w = st_part + ((h * 4 + q) * BN + c) * 3;
+				if (run[0] == 0.f)
+					run[1] = w[0], run[2] = 0.f, run[3] = 0.f;
+				const float dk = w[0] - run[1];
+				run[3] += w[2] + 2.f * dk * w[1] + nw * dk * dk;
+				run[2] += w[1] + nw * dk;
+				run[0] += nw;
+			}
+		}
+		named_bar_sync(1, 256);
+	}
+	}
+	if (stats)
+	{
+		const size_t plane = (size_t)p.stats_rows * p.N;
+		for (int i = threadIdx.x; i < 4 * BN; i += 256)
+		{
+			const int q = i / BN, c = n0 + i - q * BN;
+			const float* const run = st_run + i * 4;
+			if (c < p.N && run[0] > 0.f)
+			{
+				float* const slot = p.stats + ((size_t)blockIdx.x * 4 + q) * p.N + c;
+				slot[0] = run[0], slot[plane] = run[1], slot[2 * plane] = run[2], slot[3 * plane] = run[3];
+			}
+		}
+	}
 }
 
 } // namespace sm100

@@ -448,7 +448,7 @@ enum {
 
 /* algorithm selectors of this backend for the contraction commands (cmd.algorithm; -1 = backend default) */
 enum {
-	CCV_NNC_SM100_ALGO_TF32 = 0,   /* one tcgen05 kind::tf32 pass, fp32 accumulate in TMEM */
+	CCV_NNC_SM100_ALGO_TF32 = 0,   /* one wgmma tf32 pass, fp32 accumulate */
 	CCV_NNC_SM100_ALGO_3XTF32 = 1, /* error-compensated: three tf32 passes on (hi, lo) splits */
 	CCV_NNC_SM100_ALGO_FFMA = 2,   /* CUDA-core fp32 FMA (exact fp32 products; any shape / stride) */
 	CCV_NNC_SM100_ALGO_COUNT = 3,

@@ -8,7 +8,7 @@ sys.path.insert(0, ROOT)
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (select with -m gpu on a machine with an H100)")
     config.addinivalue_line("markers", "ref: needs oracle/_ref/libccv_ref.so (the compiled reference)")
 
 

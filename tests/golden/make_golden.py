@@ -2,12 +2,15 @@
 (oracle/_ref/libccv_ref.so).  Run in the build container (needs /root/reference built through `make -C oracle`):
 
     python tests/golden/make_golden.py
+    python tests/golden/make_golden.py registry <reference>/lib/nnc/cmd/ccv_nnc_cmd.inc
 
 Two kinds of fixtures:
   literal_*   inputs + expected outputs typed from the reference's unit tests (test/unit/nnc/gemm.tests.c etc.); these
               pin the oracle itself.
   cpuref_*    seeded inputs + the outputs CCV_NNC_BACKEND_CPU_REF produced for them here; these travel to the GPU box
               so parity can be checked even without the compiled reference.
+  reference_cmd_registry.json   the registry tables of the reference's generated ccv_nnc_cmd.inc: command and backend ids, both
+              perfect hashes, and every (command, backend, command slot, backend slot) registration call.
 """
 import os
 import sys
@@ -66,7 +69,20 @@ def cpuref_cases():
     return cases
 
 
-if __name__ == "__main__":
+def reference_registry(inc):
+    sys.path.insert(0, os.path.join(ROOT, "tools"))
+    import gen_backend_ph as g
+    cmds, backends, top, cases, btop, bcases = g.parse_inc(inc)
+    return {"source": "lib/nnc/cmd/ccv_nnc_cmd.inc of the reference", "commands": cmds, "backends": backends,
+            "cmd_ph": {"top": list(top), "cases": {str(i): list(p) for i, p in sorted(cases.items())}},
+            "backend_ph": {"top": list(btop), "cases": {str(i): list(p) for i, p in sorted(bcases.items())}},
+            "calls": g.registration_calls(open(inc).read())}
+
+
+if __name__ == "__main__" and sys.argv[1:2] == ["registry"]:
+    import json
+    json.dump(reference_registry(sys.argv[2]), open(os.path.join(OUT, "reference_cmd_registry.json"), "w"), indent=0)
+elif __name__ == "__main__":
     np.savez(os.path.join(OUT, "literal_gemm.npz"), **literal_gemm())
     for name, d in cpuref_cases().items():
         np.savez(os.path.join(OUT, "cpuref_%s.npz" % name), **d)

@@ -180,7 +180,7 @@ def test_two_rank_allreduce_and_data_parallel_step(gpu, tmp_path):
 
 def test_one_process_two_devices_convolution_and_allreduce(gpu, ref):
     """The reference's own shape (comm/gpu/ccv_nnc_comm_gpu_nccl.cu:12-58, test/int/nnc/nccl.tests.c:13-44): ONE process drives
-    several devices.  A tcgen05 convolution (dynamic shared memory attribute, stream workspace, tensor maps) runs on device 1
+    several devices.  A tensor-core convolution (dynamic shared memory attribute, stream workspace, tensor maps) runs on device 1
     through a stream context of device 1 while device 0 is current, and is checked against CPU_REF; then one
     COMM_ALLREDUCE command sums a tensor per device, its per-device streams found through neighbour discovery."""
     from tests.util import assert_close, ref_exec, seeded

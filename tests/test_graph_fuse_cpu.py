@@ -95,6 +95,7 @@ def test_comm_plumbing_without_a_device():
 def test_gradient_buckets_cover_the_flat_buffer_and_follow_their_producers():
     """ccv_b200/resnet50.py backward_with_exchange (host logic, oracle-side tensors): the allreduce nodes partition the flat
     gradient buffer, and each sits behind the last backward node that writes into its bucket."""
+    import pytest
     from oracle import ref, ref_factory
     if not ref.available():
         pytest.skip("oracle/_ref/libccv_ref.so not built")

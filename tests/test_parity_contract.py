@@ -2,7 +2,7 @@
 CCV_NNC_BACKEND_CPU_REF on the same seeded inputs, through the C ABI.
 
 Tolerance: BASELINE.json north_star -- <= 1e-3 relative for fp32, applied to max|diff| / max|ref| (tests/util.rel_err).
-Algorithms: CCV_NNC_SM100_ALGO_TF32 (one tcgen05 kind::tf32 pass, TMA rounds the operands to TF32: the convolution default,
+Algorithms: CCV_NNC_SM100_ALGO_TF32 (one wgmma tf32 pass, TMA rounds the operands to TF32: the convolution default,
 as the reference's cuDNN path runs CUDNN_TENSOR_OP_MATH) is held to 1e-3; CCV_NNC_SM100_ALGO_3XTF32 (error-compensated, three
 MMAs on hi / lo splits: the GEMM default, as the reference's cuBLAS path computes in CUBLAS_COMPUTE_32F) to 2e-5;
 CCV_NNC_SM100_ALGO_FFMA (CUDA-core fp32) to 1e-5.  The full-size BASELINE configs (GEMM 1024^3, convolution N=64 C=64 56x56

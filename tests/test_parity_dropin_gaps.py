@@ -148,7 +148,7 @@ def test_sgd_with_16bit_parameters(gpu, ref, nesterov):
 
 @pytest.mark.parametrize("half", [False, True])
 def test_grouped_convolution_on_tensor_cores(gpu, ref, half):
-    """groups = 2 with 32-wide groups: each group's channel slices are made dense and run on the tcgen05 kernels (forward, filter and
+    """groups = 2 with 32-wide groups: each group's channel slices are made dense and run on the wgmma kernels (forward, filter and
     data gradients); CPU_REF's grouped NHWC path is the oracle (convolution/ccv_nnc_conv_cpu_ref.c:47-65).  Half precision: oracle on
     the rounded inputs (there is no 16-bit FFMA fallback, so this also proves the tensor-core path took it)."""
     nnc = gpu

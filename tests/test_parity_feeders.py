@@ -277,6 +277,9 @@ def test_convolution_epilogue_statistics_feed_the_batch_norm(gpu, ref, N, H, C, 
     assert kinds == ([6, 1] if relu else [6, 7]), kinds
     assert g.run(stream) == 0
     stream.wait()
+    # the convolution's epilogue produced the statistics (rows in use > 0): the batch norm did not fall back to its own reduction pass
+    stats_ptr = g.nodes()[0][3][1]
+    assert stats_ptr and abi.Tensor.from_address(stats_ptr).sig > 0
     assert_close(ty.download(), y, 1e-3, "convolution output")
     assert_close(tsm.download(), sm, 1e-3, "saved mean"), assert_close(tsis.download(), sis, 1e-3, "saved inv_std")
     assert_close(tmean.download(), mean, 1e-3, "running mean"), assert_close(tvar.download(), var, 1e-3, "running var")

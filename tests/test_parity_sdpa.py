@@ -194,7 +194,7 @@ BWD16 = [
 
 @pytest.mark.parametrize("B,Sq,Sk,Hq,Hk,causal,dtype,saved,D", BWD16)
 def test_attention_16bit_backward_fused(gpu, ref, B, Sq, Sk, Hq, Hk, causal, dtype, saved, D):
-    """bf16 / fp16 SDPA backward, D <= 128: the fused deterministic tcgen05 kernels (sm100_fmha_bwd.cu) against CPU_REF's fp32 backward
+    """bf16 / fp16 SDPA backward, D <= 128: the fused deterministic wgmma kernels (sm100_fmha_bwd.cu) against CPU_REF's fp32 backward
     (…attention_cpu_ref.c:259-479) on the rounded operands; 1e-2 of max|ref| (P and dS are rounded to 16 bits on the way, like the
     reference's flash-attention backward).  Covers GQA (dk / dv summed over the query heads), causal with Sq != Sk (bottom-right
     aligned, Sq > Sk leaves fully masked rows), ragged tiles, with and without the forward's saved output / log-sum-exp, and that two
@@ -247,7 +247,7 @@ def test_attention_16bit_backward_fused(gpu, ref, B, Sq, Sk, Hq, Hk, causal, dty
 @pytest.mark.parametrize("D,masked,causal", [(40, 0, 0), (64, 0, 1), (96, 0, 0), (160, 0, 0), (224, 0, 1), (128, 1, 0)])
 def test_attention_16bit_forward_other_head_dims_and_masks(gpu, ref, D, masked, causal):
     """Head dimensions the reference trials (40, 64, 160, 224: test/int/nnc/cublas.tests.c:2752-2833) and additive masks on bf16
-    tensors.  D <= 128 without a mask runs on the tcgen05 flash kernel (one launch: the tiles stay 128 features wide, the TMA unit
+    tensors.  D <= 128 without a mask runs on the wgmma flash kernel (one launch: the tiles stay 128 features wide, the TMA unit
     zero-fills the rest); D > 128 and masks take the functional form (widen -> fp32 path -> narrow) instead of returning NO_KERNEL.
     Against CPU_REF on the bf16-rounded operands, 1e-2 of max|ref|."""
     nnc = gpu

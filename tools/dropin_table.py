@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """Merge the reports of integration/run_reference_tests.py (a full run, then retries of what failed after fixes) into one table of the
-reference's own test cases on the drop-in build: profiles/<name>.json and profiles/<name>.md.
+reference's own test cases on the drop-in build: <name>.json and <name>.md.
 
-  python tools/dropin_table.py profiles/r02_dropin_reference_tests gpurun_out/run_full.json [gpurun_out/retry1.json ...]"""
+  python tools/dropin_table.py <name> run_full.json [retry1.json ...]"""
 import json
 import sys
 

@@ -20,10 +20,14 @@ Then it emits, for the 8-backend set, the files a ccv maintainer would regenerat
 and ccv_b200/csrc/nnc_registry_generated.inc, which the stand-alone host (nnc_host.cu) compiles: the same two hash functions,
 so that its init_map[cmd].backends[8] / ccv_nnc_cmd_find_backend walk the slots exactly as lib/nnc/ccv_nnc_cmd.c:307-328 does.
 
-  python tools/gen_backend_ph.py [--reference /root/reference] [--check-only]
+  python tools/gen_backend_ph.py [--registry FILE] [--check-only]
+
+FILE is the reference's lib/nnc/cmd/ccv_nnc_cmd.inc, or (the default) tests/golden/reference_cmd_registry.json: the same tables
+extracted from it by tests/golden/make_golden.py, so that the checks run without the reference tree.
 """
 import argparse
 import hashlib
+import json
 import os
 import re
 import sys
@@ -80,6 +84,13 @@ def perfect_hashing(keys, hashval):
 
 
 def parse_inc(path):
+    """(commands, backends, command-hash top level, its buckets, backend-hash top level, its buckets) of a generated ccv_nnc_cmd.inc, or
+    of the JSON fixture holding the same tables."""
+    if path.endswith(".json"):
+        t = json.load(open(path))
+        cases = {int(i): tuple(p) for i, p in t["cmd_ph"]["cases"].items()}
+        bcases = {int(i): tuple(p) for i, p in t["backend_ph"]["cases"].items()}
+        return [tuple(c) for c in t["commands"]], [tuple(b) for b in t["backends"]], tuple(t["cmd_ph"]["top"]), cases, tuple(t["backend_ph"]["top"]), bcases
     text = open(path).read()
     cmds = re.findall(r'\{\.name = "(CCV_NNC_[A-Z0-9_]+)", \.cmd = (0x[0-9a-f]+)\}', text)
     backends = re.findall(r'\{\.name = "(CCV_NNC_BACKEND_[A-Z0-9_]+)", \.backend = (0x[0-9a-f]+)\}', text)
@@ -94,6 +105,14 @@ def parse_inc(path):
     for cm in re.finditer(r"case (\d+):(?:\s*default:)?\s*return \(\(backend >> (\d+)\) % (\d+)\) \+ (\d+);", b.group(3)):
         bcases[int(cm.group(1))] = (int(cm.group(2)), int(cm.group(3)), int(cm.group(4)))
     return [(n, int(v, 16)) for n, v in cmds], [(n, int(v, 16)) for n, v in backends], top, cases, btop, bcases
+
+
+REGISTER_CALL = re.compile(r"_register_command_(CCV_NNC_[A-Z0-9_]+?)_backend_(CCV_NNC_BACKEND_[A-Z0-9_]+)\(&\(init_map\[(\d+)\]\.backends\[(\d+)\]\)\);")
+
+
+def registration_calls(text):
+    """(command, backend, command slot, backend slot) of every registration call in a generated ccv_nnc_cmd.inc."""
+    return [(c, b, int(i), int(j)) for c, b, i, j in REGISTER_CALL.findall(text)]
 
 
 def c_switch(fn, arg, top, params, pair):
@@ -116,11 +135,10 @@ def c_switch(fn, arg, top, params, pair):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--reference", default="/root/reference")
+    ap.add_argument("--registry", default=os.path.join(ROOT, "tests", "golden", "reference_cmd_registry.json"))
     ap.add_argument("--check-only", action="store_true")
     args = ap.parse_args()
-    inc = os.path.join(args.reference, "lib/nnc/cmd/ccv_nnc_cmd.inc")
-    cmds, backends, top, cases, btop, bcases = parse_inc(inc)
+    cmds, backends, top, cases, btop, bcases = parse_inc(args.registry)
     assert len(cmds) % 2 == 0 and all(sha_id(n[:-len("_FORWARD")]) & ~1 == v for n, v in cmds if n.endswith("_FORWARD")), "command ids are not SHA-256 prefixes"  # build-cmd.rb:292
     assert all(sha_id(n) == v for n, v in backends), "backend ids are not SHA-256 prefixes"
 
