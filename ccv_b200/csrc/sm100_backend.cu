@@ -607,11 +607,13 @@ int conv_grouped_tc(ccv_nnc_stream_context_t* const stream_context, const int ki
 	gg.bw = Kg, gg.bh = (long long)g.Q * Kg, gg.bn = (long long)g.P * g.Q * Kg;
 	const size_t nx = (size_t)g.N * g.H * g.W * Cg, ny = (size_t)g.N * g.P * g.Q * Kg;
 	const size_t xb = (nx * es + 255) & ~(size_t)255, yb = (ny * es + 255) & ~(size_t)255;
-	unsigned char* const ws = (unsigned char*)ccv_nnc_stream_context_get_workspace(stream_context, CONTRACT_SCRATCH_BYTES + xb + yb, CCV_TENSOR_GPU_MEMORY);
+	// [contraction workspace | one group's activations | its results]: the fp32 data gradient's workspace, else the split-K scratch
+	const size_t inner = PASS == 2 && kind == 0 ? conv_dgrad_workspace_bytes(gg) : CONTRACT_SCRATCH_BYTES;
+	unsigned char* const ws = (unsigned char*)ccv_nnc_stream_context_get_workspace(stream_context, inner + xb + yb, CCV_TENSOR_GPU_MEMORY);
 	if (!ws)
 		return 1;
 	const Scratch scratch = scratch_at(ws, CONTRACT_SCRATCH_BYTES);
-	unsigned char* const xg = ws + CONTRACT_SCRATCH_BYTES;
+	unsigned char* const xg = ws + inner;
 	unsigned char* const yg = xg + xb;
 	cudaStream_t s = stream_of(stream_context);
 	const int xd[4] = { g.N, g.H, g.W, Cg }, xs_t[4] = { (int)g.an, (int)g.ah, (int)g.aw, 1 }, xs_d[4] = { g.H * g.W * Cg, g.W * Cg, Cg, 1 };
@@ -653,7 +655,7 @@ int conv_grouped_tc(ccv_nnc_stream_context_t* const stream_context, const int ki
 			if (copy_strided(s, res_i, ys_t, yg, ys_d, yd, (int)es))
 				return -1;
 			if (kind == 0)
-				rc = conv_dgrad_tf32(s, gg, (const float*)yg, (const float*)w_i, (float*)xg, scratch, x3);
+				rc = conv_dgrad_tf32(s, gg, (const float*)yg, (const float*)w_i, (float*)xg, ws, x3);
 			else
 				rc = conv_dgrad_16(s, kind, gg, yg, w_i, xg, scratch);
 			if (rc)
@@ -861,7 +863,12 @@ int conv_back_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 			return CCV_NNC_EXEC_INVALID;
 		int rc = 1;
 		if (groups == 1 && algo != CCV_NNC_SM100_ALGO_FFMA)
-			rc = conv_dgrad_tf32(s, gh, gb, w_t->data.f32, h_t->data.f32, scratch_of(stream_context), x3);
+		{
+			void* const ws = ccv_nnc_stream_context_get_workspace(stream_context, conv_dgrad_workspace_bytes(gh), CCV_TENSOR_GPU_MEMORY);
+			if (!ws)
+				return CCV_NNC_EXEC_OOM;
+			rc = conv_dgrad_tf32(s, gh, gb, w_t->data.f32, h_t->data.f32, ws, x3);
+		}
 		if (groups > 1 && algo != CCV_NNC_SM100_ALGO_FFMA)
 			rc = conv_grouped_tc<2>(stream_context, 0, gh, groups, x3, 0, 0, w_t->data.f32, 0, 0, gb, h_t->data.f32);
 		if (rc < 0)
@@ -915,12 +922,15 @@ bool stage_plan(ccv_nnc_tensor_t* const t, Staged& st)
 // upper bound of what the NHWC command requests from the workspace for this geometry
 size_t conv_inner_workspace(const ConvGeom& g, const int kind, const int groups)
 {
-	size_t need = CONTRACT_SCRATCH_BYTES;
+	// the fp32 data gradient asks for its own workspace, which includes the split-K scratch
+	size_t need = kind == 0 ? conv_dgrad_workspace_bytes(g) : CONTRACT_SCRATCH_BYTES;
 	if (groups > 1 && g.C % groups == 0 && g.K % groups == 0)
 	{
-		// conv_grouped_tc: split-K scratch + one group's dense activations and results
-		const size_t es = kind_size(kind), nx = (size_t)g.N * g.H * g.W * (g.C / groups), ny = (size_t)g.N * g.P * g.Q * (g.K / groups);
-		need += ((nx * es + 255) & ~(size_t)255) + ((ny * es + 255) & ~(size_t)255);
+		// conv_grouped_tc: contraction workspace of one group + its dense activations and results
+		ConvGeom gg = g;
+		gg.C /= groups, gg.K /= groups;
+		const size_t es = kind_size(kind), nx = (size_t)g.N * g.H * g.W * gg.C, ny = (size_t)g.N * g.P * g.Q * gg.K;
+		need = (kind == 0 ? conv_dgrad_workspace_bytes(gg) : CONTRACT_SCRATCH_BYTES) + ((nx * es + 255) & ~(size_t)255) + ((ny * es + 255) & ~(size_t)255);
 	}
 	if (g.C % (kind == 0 ? 4 : 8) != 0)
 		need = std::max(need, kind == 0 ? conv_im2col_workspace_bytes(g) : conv_im2col_workspace_bytes(g, kind));

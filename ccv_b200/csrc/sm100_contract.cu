@@ -5,6 +5,7 @@
 #include "sm100_contract.h"
 #include "sm100_umma_gemm.cuh"
 #include "sm100_elem.cuh"
+#include "sm100_ew.h"
 #include <atomic>
 #include <mutex>
 #include <stdio.h>
@@ -340,6 +341,18 @@ static int launch_umma(cudaStream_t stream, const CUtensorMap& tmA, const CUtens
 			*r.rows_out = gx * 4;
 		}
 	}
+	const long long sms = num_sms(), columns = (long long)grid.y * grid.z, ctas = tiles_m * columns;
+	if (!q.stats && p.splits == 1 && p.grid_taps == 1 && ctas > sms)
+	{
+		// more tiles than one wave of one CTA per SM: gx CTAs per column walk the M tiles, so the producer loads the next tile while the
+		// consumers store this one.  Taken only when it costs no more rounds of tiles than one tile per CTA does.  Not for split-K or
+		// per-tap launches (the weight gradients): their few M tiles share one large B slice per column, which side-by-side CTAs read
+		// from L2 once and walking CTAs read again from HBM (walked, ResNet-50's 1x1 weight gradients ran 12-19 % slower on an H100)
+		long long gx = sms / columns;
+		gx = gx < 1 ? 1 : (gx > tiles_m ? tiles_m : gx);
+		if ((gx * columns + sms - 1) / sms * ((tiles_m + gx - 1) / gx) <= (ctas + sms - 1) / sms)
+			grid.x = (unsigned)gx;
+	}
 	kern<<<grid, GEMM_THREADS, S::TOTAL, stream>>>(tmA, tmB, q);
 	count_launch();
 	cudaError_t e = cudaGetLastError();
@@ -454,16 +467,10 @@ static void init_params_kind(UmmaGemmParams& p, int kind)
 	}
 }
 // kernel per kind: fp32 as TF32 or 3xTF32 (t_x3); bf16 / fp16 (one kernel per element type) with a 16-bit output (out16) or fp32
-// split-K slices
+// split-K slices.  launch_kind16 covers the 16-bit kinds only, for operand modes that fp32 operands never take.
 template <int AMODE, int BMODE>
-static int launch_kind(cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB, const UmmaGemmParams& p, int bn, int kind, bool out16)
+static int launch_kind16(cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB, const UmmaGemmParams& p, int bn, int kind, bool out16)
 {
-	if (kind == 0)
-	{
-		if (t_x3)
-			return bn == 64 ? launch_umma<AMODE, BMODE, 64, 1>(stream, tmA, tmB, p) : launch_umma<AMODE, BMODE, 128, 1>(stream, tmA, tmB, p);
-		return bn == 64 ? launch_umma<AMODE, BMODE, 64>(stream, tmA, tmB, p) : launch_umma<AMODE, BMODE, 128>(stream, tmA, tmB, p);
-	}
 	if (kind == 1)
 	{
 		if (out16)
@@ -473,6 +480,17 @@ static int launch_kind(cudaStream_t stream, const CUtensorMap& tmA, const CUtens
 	if (out16)
 		return bn == 64 ? launch_umma<AMODE, BMODE, 64, 0, 2, 1>(stream, tmA, tmB, p) : launch_umma<AMODE, BMODE, 128, 0, 2, 1>(stream, tmA, tmB, p);
 	return bn == 64 ? launch_umma<AMODE, BMODE, 64, 0, 2, 0>(stream, tmA, tmB, p) : launch_umma<AMODE, BMODE, 128, 0, 2, 0>(stream, tmA, tmB, p);
+}
+template <int AMODE, int BMODE>
+static int launch_kind(cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB, const UmmaGemmParams& p, int bn, int kind, bool out16)
+{
+	if (kind == 0)
+	{
+		if (t_x3)
+			return bn == 64 ? launch_umma<AMODE, BMODE, 64, 1>(stream, tmA, tmB, p) : launch_umma<AMODE, BMODE, 128, 1>(stream, tmA, tmB, p);
+		return bn == 64 ? launch_umma<AMODE, BMODE, 64>(stream, tmA, tmB, p) : launch_umma<AMODE, BMODE, 128>(stream, tmA, tmB, p);
+	}
+	return launch_kind16<AMODE, BMODE>(stream, tmA, tmB, p, bn, kind, out16);
 }
 
 // Launch with the split factor already chosen in p.splits.  One split: straight into `out` (pitch ldo, element kind `kind`).
@@ -625,18 +643,42 @@ int conv_fprop_16(cudaStream_t stream, int kind, const ConvGeom& g, const void* 
 	return kind == 1 || kind == 2 ? conv_fprop_any(stream, kind, g, a, w, bias32, bias16, b, scratch, 0) : 1;
 }
 
-static int conv_dgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, const void* grad_b, const void* w, void* grad_a, const Scratch& scratch, int x3)
+// The data gradient reads the filters w[K, R*S*C] as its B operand with k = the output channel.  wgmma reads TF32 operands K-major
+// only, so fp32 filters are first copied to wt[R*S*C, K] ([tap][c][k], the head of the workspace) and taken as a K-major B: the
+// kernel runs without the transform step, and its products see the same TF32-rounded values in the same k order.  16-bit filters
+// are read in place as an MN-major B (the wgmma descriptor transposes 16-bit tiles).
+static size_t dgrad_filter_copy_bytes(const ConvGeom& g)
+{
+	return ((size_t)g.K * g.R * g.S * g.C * sizeof(float) + 511) & ~(size_t)511;
+}
+size_t conv_dgrad_workspace_bytes(const ConvGeom& g)
+{
+	return dgrad_filter_copy_bytes(g) + CONTRACT_SCRATCH_BYTES;
+}
+
+// wt: room for the fp32 filter copy (kind 0; NULL for 16-bit kinds)
+static int conv_dgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, const void* grad_b, const void* w, float* wt, void* grad_a, const Scratch& scratch, int x3)
 {
 	const X3Scope math(kind == 0 ? x3 : 0);
-	if (!tma_api_init() || !conv_shape_consistent(g) || !conv_out_contiguous(g) || !conv_in_contiguous(g) || g.C % kind_align(kind) || g.K % kind_align(kind))
+	const long long rsc = (long long)g.R * g.S * g.C;
+	if (!tma_api_init() || !conv_shape_consistent(g) || !conv_out_contiguous(g) || !conv_in_contiguous(g) || g.C % kind_align(kind) || g.K % kind_align(kind) || g.K * rsc > 0x7fffffffll)
 		return 1;
+	if (kind == 0)
+	{
+		const int dim[4] = { 1, 1, g.K, (int)rsc }, w_stride[4] = { 0, 0, (int)rsc, 1 }, wt_stride[4] = { 0, 0, 1, g.K };
+		if (copy_strided(stream, w, w_stride, wt, wt_stride, dim, 4))
+			return -1;
+	}
 	if (conv_is_pointwise(g)) // dA[NHW, C] = dB[NHW, K] x W[K, C]
+	{
+		if (kind == 0)
+			return gemm_any(stream, kind, g.N * g.H * g.W, g.C, g.K, grad_b, g.K, 0, wt, g.K, 1, grad_a, g.C, 0, 0, 0, scratch, x3);
 		return gemm_any(stream, kind, g.N * g.H * g.W, g.C, g.K, grad_b, g.K, 0, w, g.C, 0, grad_a, g.C, 0, 0, 0, scratch, x3);
+	}
 	const int bn = pick_bn(g.C), bk = kind_bk(kind);
 	const size_t esz = kind_esz(kind);
-	const long long rsc = (long long)g.R * g.S * g.C;
 	CUtensorMap tmB;
-	if (!map_2d(&tmB, kind, w, g.K, rsc, rsc, bk, true))
+	if (kind == 0 ? !map_2d(&tmB, kind, wt, rsc, g.K, g.K, bn, false) : !map_2d(&tmB, kind, w, g.K, rsc, rsc, bk, true))
 		return 1;
 	// Decompose by output-pixel residue class (ah, aw) modulo the stride: within a class, pixel h = i * stride + ah
 	// receives from filter row r iff (ah + pad - r * dil) % stride == 0, reading grad_b row i + (ah + pad - r * dil) / stride.
@@ -728,7 +770,7 @@ static int conv_dgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, cons
 					const int t = i * cp.ntaps_w + j;
 					p.tap_off_h[t] = (unsigned short)(cp.e_h[i] - lo_h);
 					p.tap_off_w[t] = (unsigned short)(cp.e_w[j] - lo_w);
-					p.tap_b_col[t] = (cp.r_h[i] * g.S + cp.s_w[j]) * g.C;
+					(kind == 0 ? p.tap_b_row : p.tap_b_col)[t] = (cp.r_h[i] * g.S + cp.s_w[j]) * g.C;
 				}
 			p.out = (float*)((char*)grad_a + ((long long)ah * g.W + aw) * g.C * esz);
 			p.rowmap.mode = 1;
@@ -736,19 +778,20 @@ static int conv_dgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, cons
 			p.rowmap.n_stride = (long long)g.H * g.W * g.C;
 			p.rowmap.h_stride = (long long)g.stride_h * g.W * g.C;
 			p.rowmap.w_stride = (long long)g.stride_w * g.C;
-			const int rc = launch_kind<OP_IM2COL, OP_MN2D>(stream, tmA, tmB, p, bn, kind, kind != 0);
+			const int rc = kind == 0 ? launch_kind<OP_IM2COL, OP_K2D>(stream, tmA, tmB, p, bn, kind, false) : launch_kind16<OP_IM2COL, OP_MN2D>(stream, tmA, tmB, p, bn, kind, true);
 			if (rc)
 				return rc;
 		}
 	return 0;
 }
-int conv_dgrad_tf32(cudaStream_t stream, const ConvGeom& g, const float* grad_b, const float* w, float* grad_a, const Scratch& scratch, int x3)
+int conv_dgrad_tf32(cudaStream_t stream, const ConvGeom& g, const float* grad_b, const float* w, float* grad_a, void* workspace, int x3)
 {
-	return conv_dgrad_any(stream, 0, g, grad_b, w, grad_a, scratch, x3);
+	const Scratch scratch = { (char*)workspace + dgrad_filter_copy_bytes(g), CONTRACT_SCRATCH_BYTES };
+	return conv_dgrad_any(stream, 0, g, grad_b, w, (float*)workspace, grad_a, scratch, x3);
 }
 int conv_dgrad_16(cudaStream_t stream, int kind, const ConvGeom& g, const void* grad_b, const void* w, void* grad_a, const Scratch& scratch)
 {
-	return kind == 1 || kind == 2 ? conv_dgrad_any(stream, kind, g, grad_b, w, grad_a, scratch, 0) : 1;
+	return kind == 1 || kind == 2 ? conv_dgrad_any(stream, kind, g, grad_b, w, 0, grad_a, scratch, 0) : 1;
 }
 
 static int conv_wgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, const void* grad_b, const void* a, void* grad_w, int accumulate, const Scratch& scratch, int x3)

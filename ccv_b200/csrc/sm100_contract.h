@@ -36,7 +36,9 @@ constexpr size_t CONTRACT_SCRATCH_BYTES = (size_t)96 << 20;
 // C[M, N] (+)= op(A) * op(B) + bias; A is [M, K] (lda) or, if trans_a, [K, M]; B is [K, N] (ldb) or, if trans_b, [N, K].
 int gemm_tf32(cudaStream_t stream, int M, int N, int K, const float* a, long long lda, int trans_a, const float* b, long long ldb, int trans_b, float* c, long long ldc, const float* bias, int accumulate, const Scratch& scratch, int x3 = 0);
 int conv_fprop_tf32(cudaStream_t stream, const ConvGeom& g, const float* a, const float* w, const float* bias, float* b, const Scratch& scratch, int x3 = 0);
-int conv_dgrad_tf32(cudaStream_t stream, const ConvGeom& g, const float* grad_b, const float* w, float* grad_a, const Scratch& scratch, int x3 = 0);
+// the fp32 data gradient works in a workspace of conv_dgrad_workspace_bytes(g) (which includes CONTRACT_SCRATCH_BYTES for split-K slices)
+size_t conv_dgrad_workspace_bytes(const ConvGeom& g);
+int conv_dgrad_tf32(cudaStream_t stream, const ConvGeom& g, const float* grad_b, const float* w, float* grad_a, void* workspace, int x3 = 0);
 int conv_wgrad_tf32(cudaStream_t stream, const ConvGeom& g, const float* grad_b, const float* a, float* grad_w, int accumulate, const Scratch& scratch, int x3 = 0);
 
 // The same contractions on 16-bit tensors (kind 1 = bf16, 2 = fp16): wgmma bf16 / fp16 with fp32 accumulation in registers, 16-bit

@@ -58,6 +58,7 @@ struct UmmaGemmParams {
 	int base_h, base_w;
 	unsigned short tap_off_h[UMMA_MAX_TAPS], tap_off_w[UMMA_MAX_TAPS];
 	int tap_b_col[UMMA_MAX_TAPS]; // B's column (or row-block) origin for this tap
+	int tap_b_row[UMMA_MAX_TAPS]; // K-major B: row origin for this tap (the data gradient's filter copy [tap][c][k])
 	// epilogue
 	float* out;
 	const float* bias;
@@ -173,7 +174,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) umma_gemm_kernel(const __grid
 	constexpr int MN_BOX_BYTES = BK * 128;     // an MN-major box: BK k-rows of 128 bytes
 	const int warp = threadIdx.x >> 5;
 	const int lane = threadIdx.x & 31;
-	const int tiles_m = (p.M + UMMA_BLOCK_M - 1) / UMMA_BLOCK_M; // M tiles blockIdx.x, blockIdx.x + gridDim.x, ... (one unless statistics)
+	const int tiles_m = (p.M + UMMA_BLOCK_M - 1) / UMMA_BLOCK_M; // M tiles blockIdx.x, blockIdx.x + gridDim.x, ... (launch_umma picks gridDim.x)
 	const int n0 = blockIdx.y * BN;
 	const int split = blockIdx.z % p.splits;
 	const int gtap = blockIdx.z / p.splits;
@@ -231,7 +232,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) umma_gemm_kernel(const __grid
 				} else
 					tma_load_im2col_4d(sA, &tmA, &full_bar[stage], chunk * BK, a_w, a_h, a_n, p.tap_off_w[tap], p.tap_off_h[tap]);
 				if (BMODE == OP_K2D)
-					tma_load_2d(sB, &tmB, &full_bar[stage], p.tap_b_col[tap] + chunk * BK, n0);
+					tma_load_2d(sB, &tmB, &full_bar[stage], p.tap_b_col[tap] + chunk * BK, p.tap_b_row[tap] + n0);
 				else if (BMODE == OP_MN2D) {
 #pragma unroll
 					for (int j = 0; j < BN / BK; j++)
