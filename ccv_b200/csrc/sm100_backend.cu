@@ -239,7 +239,7 @@ int gemm_dispatch(cudaStream_t s, const Scratch& scratch, const int algorithm, c
 				return rc;
 		}
 	}
-	return gemm_ffma(s, M, N, K, a, a_rs, a_cs, b, b_rs, b_cs, c, c_rs, bias, accumulate);
+	return gemm_ffma(s, M, N, K, a, a_rs, a_cs, b, b_rs, b_cs, c, c_rs, bias, accumulate, scratch);
 }
 
 // the same for 16-bit tensors (kind 1 = bf16, 2 = fp16): tensor-core path only (unit stride along one axis of every operand)
@@ -852,7 +852,7 @@ int conv_back_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 		if (rc < 0)
 			return CCV_NNC_EXEC_INVALID;
 		if (rc > 0)
-			RC(conv_wgrad_ffma(s, g, groups, gb, a, dw_t->data.f32, accumulate));
+			RC(conv_wgrad_ffma(s, g, groups, gb, a, dw_t->data.f32, accumulate, scratch_of(stream_context)));
 	}
 	if (h_t)
 	{

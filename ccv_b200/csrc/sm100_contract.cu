@@ -241,7 +241,7 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(const float* __restr
 		}
 	}
 }
-static int splitk_reduce(cudaStream_t stream, const float* part, int splits, long long split_stride, int rows, int cols, long long ldp, float* out, long long ldo, int accumulate, int out_kind = 0)
+int splitk_reduce(cudaStream_t stream, const float* part, int splits, long long split_stride, int rows, int cols, long long ldp, float* out, long long ldo, int accumulate, int out_kind)
 {
 	if (out_kind)
 	{

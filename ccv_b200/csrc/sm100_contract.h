@@ -65,11 +65,14 @@ int conv_wgrad_im2col_tf32(cudaStream_t stream, const ConvGeom& g, const float* 
 int conv_fprop_im2col_16(cudaStream_t stream, int kind, const ConvGeom& g, const void* a, const void* w, const float* bias32, const void* bias16, void* b, void* workspace);
 int conv_wgrad_im2col_16(cudaStream_t stream, int kind, const ConvGeom& g, const void* grad_b, const void* a, void* grad_w, int accumulate, void* workspace);
 
-// CUDA-core fp32 versions of the same contractions: any stride/alignment, groups, exact fp32 products.
-int gemm_ffma(cudaStream_t stream, int M, int N, int K, const float* a, long long a_rs, long long a_cs, const float* b, long long b_rs, long long b_cs, float* c, long long ldc, const float* bias, int accumulate);
+// CUDA-core fp32 versions of the same contractions: any stride/alignment, groups, exact fp32 products.  Long reductions over few
+// output tiles split K into slices of `scratch` (none given: no split), combined in split order like the tensor-core path.
+int gemm_ffma(cudaStream_t stream, int M, int N, int K, const float* a, long long a_rs, long long a_cs, const float* b, long long b_rs, long long b_cs, float* c, long long ldc, const float* bias, int accumulate, const Scratch& scratch = Scratch());
 int conv_fprop_ffma(cudaStream_t stream, const ConvGeom& g, int groups, const float* a, const float* w, const float* bias, float* b);
 int conv_dgrad_ffma(cudaStream_t stream, const ConvGeom& g, int groups, const float* grad_b, const float* w, float* grad_a);
-int conv_wgrad_ffma(cudaStream_t stream, const ConvGeom& g, int groups, const float* grad_b, const float* a, float* grad_w, int accumulate);
+int conv_wgrad_ffma(cudaStream_t stream, const ConvGeom& g, int groups, const float* grad_b, const float* a, float* grad_w, int accumulate, const Scratch& scratch = Scratch());
+// out[r, c] = (accumulate ? out[r, c] : 0) + part[0][r, c] + part[1][r, c] + ... (fp32 slices [rows, cols] of pitch ldp, split_stride apart)
+int splitk_reduce(cudaStream_t stream, const float* part, int splits, long long split_stride, int rows, int cols, long long ldp, float* out, long long ldo, int accumulate, int out_kind = 0);
 
 // scaled dot product attention (sm100_sdpa.cu): element strides of q [B, Sq, H, D], k / v [B, Sk, Hk, D | Dv], o [B, Sq, H, Dv]
 struct SdpaGeom {

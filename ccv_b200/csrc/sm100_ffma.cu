@@ -86,8 +86,9 @@ struct Im2colCols {
 };
 
 template <class AV, class BV>
-__global__ void __launch_bounds__(256) ffma_gemm_kernel(const AV A, const BV B, float* __restrict__ C, const long long ldc, const float* __restrict__ bias, const int M, const int N, const int K, const int k_per_split, const int accumulate, const int atomic)
+__global__ void __launch_bounds__(256) ffma_gemm_kernel(const AV A, const BV B, float* __restrict__ C, const long long ldc, const float* __restrict__ bias, const int M, const int N, const int K, const int k_per_split, const int accumulate, const long long split_stride)
 {
+	C += blockIdx.z * split_stride;
 	__shared__ float As[16][64 + 4];
 	__shared__ float Bs[16][64 + 4];
 	const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
@@ -144,36 +145,35 @@ __global__ void __launch_bounds__(256) ffma_gemm_kernel(const AV A, const BV B, 
 			if (bias && blockIdx.z == 0)
 				v += bias[n];
 			float* o = C + m * ldc + n;
-			if (atomic)
-				atomicAdd(o, v);
-			else
-				*o = accumulate ? *o + v : v;
+			*o = accumulate ? *o + v : v;
 		}
 	}
 }
 
+// splits > 1: each split writes its partial products to its own fp32 slice [M, ldp] of the scratch, and splitk_reduce adds the
+// slices into C in split order (bit-identical from run to run, unlike atomic adds); as many splits as the scratch holds
 template <class AV, class BV>
-static int launch_ffma(cudaStream_t stream, const AV& A, const BV& B, float* C, long long ldc, const float* bias, int M, int N, int K, int accumulate, int splits, bool c_rows_contiguous_zero)
+static int launch_ffma(cudaStream_t stream, const AV& A, const BV& B, float* C, long long ldc, const float* bias, int M, int N, int K, int accumulate, int splits, const Scratch& scratch)
 {
 	if (M <= 0 || N <= 0)
 		return 0;
+	const long long ldp = ((long long)N + 3) & ~3ll;
+	const size_t slice = (size_t)M * ldp * sizeof(float);
+	if (splits > 1 && (long long)splits > (long long)((scratch.ptr ? scratch.bytes : 0) / slice))
+		splits = (int)((scratch.ptr ? scratch.bytes : 0) / slice);
 	int k_per = K;
 	if (splits > 1)
 	{
 		k_per = ((K + splits - 1) / splits + 15) / 16 * 16;
 		splits = (K + k_per - 1) / k_per;
 	}
-	if (splits > 1 && !accumulate)
-	{
-		cudaError_t e = cudaMemset2DAsync(C, ldc * 4, 0, (size_t)N * 4, M, stream);
-		if (e != cudaSuccess)
-		{
-			set_last_error("memset(ffma split-K)", e);
-			return -1;
-		}
-	}
-	dim3 grid((N + 63) / 64, (M + 63) / 64, splits < 1 ? 1 : splits);
-	ffma_gemm_kernel<AV, BV><<<grid, 256, 0, stream>>>(A, B, C, ldc, bias, M, N, K, k_per, accumulate, splits > 1);
+	if (splits < 1)
+		splits = 1;
+	dim3 grid((N + 63) / 64, (M + 63) / 64, splits);
+	if (splits > 1)
+		ffma_gemm_kernel<AV, BV><<<grid, 256, 0, stream>>>(A, B, (float*)scratch.ptr, ldp, bias, M, N, K, k_per, 0, (long long)M * ldp);
+	else
+		ffma_gemm_kernel<AV, BV><<<grid, 256, 0, stream>>>(A, B, C, ldc, bias, M, N, K, k_per, accumulate, 0);
 	count_launch();
 	cudaError_t e = cudaGetLastError();
 	if (e != cudaSuccess)
@@ -181,10 +181,10 @@ static int launch_ffma(cudaStream_t stream, const AV& A, const BV& B, float* C, 
 		set_last_error("ffma_gemm_kernel launch", e);
 		return -1;
 	}
-	return 0;
+	return splits > 1 ? splitk_reduce(stream, (const float*)scratch.ptr, splits, (long long)M * ldp, M, N, ldp, C, ldc, accumulate) : 0;
 }
 
-int gemm_ffma(cudaStream_t stream, int M, int N, int K, const float* a, long long a_rs, long long a_cs, const float* b, long long b_rs, long long b_cs, float* c, long long ldc, const float* bias, int accumulate)
+int gemm_ffma(cudaStream_t stream, int M, int N, int K, const float* a, long long a_rs, long long a_cs, const float* b, long long b_rs, long long b_cs, float* c, long long ldc, const float* bias, int accumulate, const Scratch& scratch)
 {
 	StridedView A = { a, a_rs, a_cs, M, K };
 	StridedView B = { b, b_rs, b_cs, K, N };
@@ -194,7 +194,7 @@ int gemm_ffma(cudaStream_t stream, int M, int N, int K, const float* a, long lon
 		splits = (int)((264 + tiles - 1) / tiles);
 	if (splits > K / 256)
 		splits = K / 256 > 0 ? K / 256 : 1;
-	return launch_ffma(stream, A, B, c, ldc, bias, M, N, K, accumulate, splits, false);
+	return launch_ffma(stream, A, B, c, ldc, bias, M, N, K, accumulate, splits, scratch);
 }
 
 static Im2colRows im2col_view(const ConvGeom& g, int groups, const float* a, int group)
@@ -217,7 +217,7 @@ int conv_fprop_ffma(cudaStream_t stream, const ConvGeom& g, int groups, const fl
 		Im2colRows A = im2col_view(g, groups, a, gr);
 		// w[K, R, S, Cg]: B(k, n) = w[(gr * Kg + n), k]
 		StridedView B = { w + (long long)gr * Kg * g.R * g.S * Cg, 1, (long long)g.R * g.S * Cg, g.R * g.S * Cg, Kg };
-		const int rc = launch_ffma(stream, A, B, b + gr * Kg, g.bw, bias ? bias + gr * Kg : 0, g.N * g.P * g.Q, Kg, g.R * g.S * Cg, 0, 1, false);
+		const int rc = launch_ffma(stream, A, B, b + gr * Kg, g.bw, bias ? bias + gr * Kg : 0, g.N * g.P * g.Q, Kg, g.R * g.S * Cg, 0, 1, Scratch());
 		if (rc)
 			return rc;
 	}
@@ -237,14 +237,14 @@ int conv_dgrad_ffma(cudaStream_t stream, const ConvGeom& g, int groups, const fl
 		A.sh = g.stride_h, A.sw = g.stride_w, A.ph = g.pad_h0, A.pw = g.pad_w0, A.dh = g.dil_h, A.dw = g.dil_w;
 		A.gn = g.bn, A.gh = g.bh, A.gw = g.bw;
 		DgradFilter B = { w + (long long)gr * Kg * g.R * g.S * Cg, Kg, g.R, g.S, Cg };
-		const int rc = launch_ffma(stream, A, B, grad_a + gr * Cg, g.aw, 0, g.N * g.H * g.W, Cg, g.R * g.S * Kg, 0, 1, false);
+		const int rc = launch_ffma(stream, A, B, grad_a + gr * Cg, g.aw, 0, g.N * g.H * g.W, Cg, g.R * g.S * Kg, 0, 1, Scratch());
 		if (rc)
 			return rc;
 	}
 	return 0;
 }
 
-int conv_wgrad_ffma(cudaStream_t stream, const ConvGeom& g, int groups, const float* grad_b, const float* a, float* grad_w, int accumulate)
+int conv_wgrad_ffma(cudaStream_t stream, const ConvGeom& g, int groups, const float* grad_b, const float* a, float* grad_w, int accumulate, const Scratch& scratch)
 {
 	const int Cg = g.C / groups, Kg = g.K / groups;
 	const int npq = g.N * g.P * g.Q;
@@ -260,7 +260,7 @@ int conv_wgrad_ffma(cudaStream_t stream, const ConvGeom& g, int groups, const fl
 		int splits = (int)((592 + tiles - 1) / tiles);
 		if (splits > npq / 512)
 			splits = npq / 512 > 0 ? npq / 512 : 1;
-		const int rc = launch_ffma(stream, A, B, grad_w + (long long)gr * Kg * rsc, rsc, 0, Kg, rsc, npq, accumulate, splits, true);
+		const int rc = launch_ffma(stream, A, B, grad_w + (long long)gr * Kg * rsc, rsc, 0, Kg, rsc, npq, accumulate, splits, scratch);
 		if (rc)
 			return rc;
 	}
