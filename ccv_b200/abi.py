@@ -26,7 +26,7 @@ CCV_NNC_GEMM_32F, CCV_NNC_GEMM_32TF, CCV_NNC_GEMM_16F = 0x1, 0x2, 0x4  # lib/nnc
 # commands (lib/nnc/cmd/ccv_nnc_cmd.h)
 CMD_IDS = dict(
     ADD=0x58fb3664, AVERAGE_POOL=0x51267ab8, BATCH_NORM=0x5419819c, CATEGORICAL_CROSSENTROPY=0x1eb327a2,
-    COMM_ALLREDUCE=0x75c8d340, CONVOLUTION=0x254d05f4, DATATYPE_CONVERSION=0xd873e38c, DATA_TRANSFER=0x12d21e1a,
+    COMM_ALLREDUCE=0x75c8d340, CONVOLUTION=0x254d05f4, CONVOLUTION_TRANSPOSE=0xd691f78e, DATATYPE_CONVERSION=0xd873e38c, DATA_TRANSFER=0x12d21e1a,
     EWSUM=0xe21a2c4c, FORMAT_TRANSFORM=0xe4a2b192, GEMM=0x7e87d00c, GROUP_NORM=0x17deb074, LAYER_NORM=0xbed3c264, MAX_POOL=0x7bec9360,
     MUL=0x24721a46, RELU=0xc51eaa80, RMSNORM=0x6889e9d0, SCALAR_MUL=0x8b4d86aa,
     SCALED_DOT_PRODUCT_ATTENTION=0x284ed926, SET=0x2b070804, SGD=0xe650ad26, SOFTMAX=0xc969a252,
@@ -60,6 +60,10 @@ class _Size(C.Structure):
 
 class _Convolution(C.Structure):
     _fields_ = [("count", C.c_int), ("groups", C.c_int), ("dilation", C.c_int * MAX_DIM_ALLOC)]
+
+
+class _ConvolutionTranspose(C.Structure):
+    _fields_ = [("count", C.c_int), ("groups", C.c_int), ("dilation", C.c_int * MAX_DIM_ALLOC), ("output_padding", C.c_int)]
 
 
 class _Pool(C.Structure):
@@ -132,7 +136,7 @@ class _Dropout(C.Structure):
 
 
 class _CmdUnion(C.Union):
-    _fields_ = [("convolution", _Convolution), ("pool", _Pool), ("bnorm", _Bnorm), ("lnorm", _Lnorm), ("gnorm", _Gnorm), ("rmsnorm", _Rmsnorm),
+    _fields_ = [("convolution", _Convolution), ("convolution_transpose", _ConvolutionTranspose), ("pool", _Pool), ("bnorm", _Bnorm), ("lnorm", _Lnorm), ("gnorm", _Gnorm), ("rmsnorm", _Rmsnorm),
                 ("sgd", _Sgd), ("adam", _Adam), ("gelu", _Gelu), ("blas", _Blas), ("label_smoothing", _LabelSmoothing), ("reduce", _Reduce), ("transpose", _Transpose),
                 ("upsample", _Upsample), ("clamp", _Clamp), ("leaky_relu", _LeakyRelu), ("dropout", _Dropout), ("scaled_dot_product_attention", _Sdpa), ("userdata", C.c_void_p)]
 

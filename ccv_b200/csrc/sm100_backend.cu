@@ -651,13 +651,15 @@ int conv_grouped_tc(ccv_nnc_stream_context_t* const stream_context, const int ki
 			if (rc)
 				return i == 0 ? rc : -1;
 		} else {
-			// h_i = dgrad(g_i, w_i)
+			// h_i = dgrad(g_i, w_i) (+ bias_i: the forward of a transposed convolution, whose outputs are the C side)
 			if (copy_strided(s, res_i, ys_t, yg, ys_d, yd, (int)es))
 				return -1;
+			const float* const bias32_i = bias32 ? bias32 + (size_t)i * Cg : 0;
+			const void* const bias16_i = bias16 ? (const unsigned char*)bias16 + (size_t)i * Cg * 2 : 0;
 			if (kind == 0)
-				rc = conv_dgrad_tf32(s, gg, (const float*)yg, (const float*)w_i, (float*)xg, ws, x3);
+				rc = conv_dgrad_tf32(s, gg, (const float*)yg, (const float*)w_i, bias32_i, (float*)xg, ws, x3);
 			else
-				rc = conv_dgrad_16(s, kind, gg, yg, w_i, xg, scratch);
+				rc = conv_dgrad_16(s, kind, gg, yg, w_i, bias32_i, bias16_i, xg, scratch);
 			if (rc)
 				return i == 0 ? rc : -1;
 			if (copy_strided(s, xg, xs_d, (unsigned char*)out + (size_t)i * Cg * es, xs_t, xd, (int)es))
@@ -665,6 +667,65 @@ int conv_grouped_tc(ccv_nnc_stream_context_t* const stream_context, const int ki
 		}
 	}
 	return 0;
+}
+
+// h = dgrad(gb, w) (+ bias[C]) on the geometry gh, returns a CCV_NNC_EXEC_* status: the data gradient of CONVOLUTION_BACKWARD (no
+// bias) and the forward of CONVOLUTION_TRANSPOSE (bias32 fp32, or bias16 of the tensors' 16-bit type).  fp32: tensor cores for one
+// group, per-group dense launches for wide groups, FFMA for narrow groups, unaligned channels and ALGO_FFMA.  16-bit: tensor cores
+// (wide groups only when grouped); shapes they cannot take (3-channel pixels) run in the functional form -- widen g, w and the bias,
+// fp32 FFMA data gradient + bias, one rounding on the way back.
+// workspace of the 16-bit functional form below: fp32 copies of g, w, h and the bias, 256-byte aligned
+size_t dgrad16_fallback_bytes(const ConvGeom& gh)
+{
+	return ((size_t)gh.N * gh.P * gh.Q * gh.K + (size_t)gh.K * gh.R * gh.S * gh.C + (size_t)gh.N * gh.H * gh.W * gh.C + gh.C) * sizeof(float) + 1280;
+}
+int dgrad_nhwc(ccv_nnc_stream_context_t* const stream_context, const int kind, const int algo, const int groups, const ConvGeom& gh, const void* const gb, const void* const w, const float* const bias32, const void* const bias16, void* const h)
+{
+	cudaStream_t s = stream_of(stream_context);
+	if (kind > 0)
+	{
+		if (groups > 1)
+			return conv_grouped_tc<2>(stream_context, kind, gh, groups, 0, 0, 0, w, bias32, bias16, gb, h) == 0 ? CCV_NNC_EXEC_SUCCESS : CCV_NNC_EXEC_INVALID;
+		const int rc = conv_dgrad_16(s, kind, gh, gb, w, bias32, bias16, h, scratch_of(stream_context));
+		if (rc < 0)
+			return CCV_NNC_EXEC_INVALID;
+		if (rc > 0)
+		{
+			// (the image gradient of a stem, test/int/nnc/cudnn.tests.c:499-577; the RGB head of a transposed convolution)  Dense tensors only.
+			const size_t ng = (size_t)gh.N * gh.P * gh.Q * gh.K, nw = (size_t)gh.K * gh.R * gh.S * gh.C, nh = (size_t)gh.N * gh.H * gh.W * gh.C, nb = bias16 ? gh.C : 0;
+			if (gh.bw != gh.K || gh.bh != (long long)gh.Q * gh.K || gh.bn != (long long)gh.P * gh.Q * gh.K || gh.aw != gh.C || gh.ah != (long long)gh.W * gh.C || gh.an != (long long)gh.H * gh.W * gh.C || ng > 0x7fffffffull || nh > 0x7fffffffull)
+				return CCV_NNC_EXEC_INVALID;
+			float* const g32 = (float*)ccv_nnc_stream_context_get_workspace(stream_context, dgrad16_fallback_bytes(gh), CCV_TENSOR_GPU_MEMORY);
+			if (!g32)
+				return CCV_NNC_EXEC_OOM;
+			float* const w32 = (float*)(((uintptr_t)(g32 + ng) + 255) & ~(uintptr_t)255);
+			float* const h32 = (float*)(((uintptr_t)(w32 + nw) + 255) & ~(uintptr_t)255);
+			float* const b32 = (float*)(((uintptr_t)(h32 + nh) + 255) & ~(uintptr_t)255);
+			RC(widen_matrix(s, gb, kind, (long long)ng, 1, g32, 1, (int)ng));
+			RC(widen_matrix(s, w, kind, (long long)nw, 1, w32, 1, (int)nw));
+			if (nb)
+				RC(widen_matrix(s, bias16, kind, (long long)nb, 1, b32, 1, (int)nb));
+			RC(conv_dgrad_ffma(s, gh, 1, g32, w32, nb ? b32 : bias32, h32));
+			RC(narrow_matrix(s, h32, h, kind, (long long)nh, 1, 1, (int)nh, 0));
+		}
+		return CCV_NNC_EXEC_SUCCESS;
+	}
+	const int x3 = algo == CCV_NNC_SM100_ALGO_3XTF32;
+	int rc = 1;
+	if (groups == 1 && algo != CCV_NNC_SM100_ALGO_FFMA)
+	{
+		void* const ws = ccv_nnc_stream_context_get_workspace(stream_context, conv_dgrad_workspace_bytes(gh), CCV_TENSOR_GPU_MEMORY);
+		if (!ws)
+			return CCV_NNC_EXEC_OOM;
+		rc = conv_dgrad_tf32(s, gh, (const float*)gb, (const float*)w, bias32, (float*)h, ws, x3);
+	}
+	if (groups > 1 && algo != CCV_NNC_SM100_ALGO_FFMA)
+		rc = conv_grouped_tc<2>(stream_context, 0, gh, groups, x3, 0, 0, w, bias32, 0, gb, h);
+	if (rc < 0)
+		return CCV_NNC_EXEC_INVALID;
+	if (rc > 0)
+		RC(conv_dgrad_ffma(s, gh, groups, (const float*)gb, (const float*)w, bias32, (float*)h));
+	return CCV_NNC_EXEC_SUCCESS;
 }
 
 int conv_forw_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
@@ -788,32 +849,7 @@ int conv_back_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 			ConvGeom gh16;
 			if (!w_t || !conv_geom(cmd, hint, view_of(h_t), view_of(w_t), view_of(inputs[0]), gh16))
 				return CCV_NNC_EXEC_INVALID;
-			if (groups16 > 1)
-			{
-				if (conv_grouped_tc<2>(stream_context, kind, gh16, groups16, 0, 0, 0, w_t->data.u8, 0, 0, inputs[0]->data.u8, h_t->data.u8))
-					return CCV_NNC_EXEC_INVALID;
-			} else {
-				const int rc = conv_dgrad_16(s16, kind, gh16, inputs[0]->data.u8, w_t->data.u8, h_t->data.u8, scratch_of(stream_context));
-				if (rc < 0)
-					return CCV_NNC_EXEC_INVALID;
-				if (rc > 0)
-				{
-					// shapes the tensor-core path cannot take (3-channel pixels: the image gradient of a stem, test/int/nnc/cudnn.tests.c:499-577):
-					// functional form -- widen g and w, fp32 FFMA data gradient, one rounding on the way back.  Dense tensors only.
-					const size_t ng = (size_t)gh16.N * gh16.P * gh16.Q * gh16.K, nw = (size_t)gh16.K * gh16.R * gh16.S * gh16.C, nh = (size_t)gh16.N * gh16.H * gh16.W * gh16.C;
-					if (gh16.bw != gh16.K || gh16.bh != (long long)gh16.Q * gh16.K || gh16.bn != (long long)gh16.P * gh16.Q * gh16.K || gh16.aw != gh16.C || gh16.ah != (long long)gh16.W * gh16.C || gh16.an != (long long)gh16.H * gh16.W * gh16.C || ng > 0x7fffffffull || nh > 0x7fffffffull)
-						return CCV_NNC_EXEC_INVALID;
-					float* const g32 = (float*)ccv_nnc_stream_context_get_workspace(stream_context, (ng + nw + nh) * sizeof(float) + 1024, CCV_TENSOR_GPU_MEMORY);
-					if (!g32)
-						return CCV_NNC_EXEC_OOM;
-					float* const w32 = (float*)(((uintptr_t)(g32 + ng) + 255) & ~(uintptr_t)255);
-					float* const h32 = (float*)(((uintptr_t)(w32 + nw) + 255) & ~(uintptr_t)255);
-					RC(widen_matrix(s16, inputs[0]->data.u8, kind, (long long)ng, 1, g32, 1, (int)ng));
-					RC(widen_matrix(s16, w_t->data.u8, kind, (long long)nw, 1, w32, 1, (int)nw));
-					RC(conv_dgrad_ffma(s16, gh16, 1, g32, w32, h32));
-					RC(narrow_matrix(s16, h32, h_t->data.u8, kind, (long long)nh, 1, 1, (int)nh, 0));
-				}
-			}
+			return dgrad_nhwc(stream_context, kind, CCV_NNC_SM100_ALGO_TF32, groups16, gh16, inputs[0]->data.u8, w_t->data.u8, 0, 0, h_t->data.u8);
 		}
 		return CCV_NNC_EXEC_SUCCESS;
 	}
@@ -861,20 +897,7 @@ int conv_back_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 		ConvGeom gh;
 		if (!conv_geom(cmd, hint, view_of(h_t), view_of(w_t), view_of(inputs[0]), gh))
 			return CCV_NNC_EXEC_INVALID;
-		int rc = 1;
-		if (groups == 1 && algo != CCV_NNC_SM100_ALGO_FFMA)
-		{
-			void* const ws = ccv_nnc_stream_context_get_workspace(stream_context, conv_dgrad_workspace_bytes(gh), CCV_TENSOR_GPU_MEMORY);
-			if (!ws)
-				return CCV_NNC_EXEC_OOM;
-			rc = conv_dgrad_tf32(s, gh, gb, w_t->data.f32, h_t->data.f32, ws, x3);
-		}
-		if (groups > 1 && algo != CCV_NNC_SM100_ALGO_FFMA)
-			rc = conv_grouped_tc<2>(stream_context, 0, gh, groups, x3, 0, 0, w_t->data.f32, 0, 0, gb, h_t->data.f32);
-		if (rc < 0)
-			return CCV_NNC_EXEC_INVALID;
-		if (rc > 0)
-			RC(conv_dgrad_ffma(s, gh, groups, gb, w_t->data.f32, h_t->data.f32));
+		return dgrad_nhwc(stream_context, 0, algo, groups, gh, gb, w_t->data.f32, 0, 0, h_t->data.f32);
 	}
 	return CCV_NNC_EXEC_SUCCESS;
 }
@@ -1030,7 +1053,12 @@ size_t conv_staged_inner(const ccv_nnc_cmd_t& cmd, const ccv_nnc_hint_t& hint, c
 	ConvGeom g;
 	if (!act || !filt || !res || kind_of(act) < 0 || !conv_geom(cmd, hint, view_of(act), view_of(filt), view_of(res), g))
 		return (size_t)-1;
-	return conv_inner_workspace(g, kind_of(act), cmd.info.convolution.groups > 1 ? cmd.info.convolution.groups : 1);
+	const int kind = kind_of(act), groups = cmd.info.convolution.groups > 1 ? cmd.info.convolution.groups : 1;
+	size_t need = conv_inner_workspace(g, kind, groups);
+	// a 16-bit data gradient the tensor cores decline runs in the functional form (dgrad_nhwc)
+	if (BACKWARD && output_size > 0 && out[0] && kind > 0 && groups == 1 && conv_dgrad_may_decline(g, kind))
+		need = std::max(need, (dgrad16_fallback_bytes(g) + 255) & ~(size_t)255);
+	return need;
 }
 template <int BACKWARD>
 int conv_staged(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
@@ -1061,6 +1089,148 @@ int exec_conv_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 	if (any_nchw(inputs, input_size, outputs, output_size))
 		return conv_staged<1>(cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
 	return conv_back_nhwc(cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
+}
+
+// ================================================================================================ CONVOLUTION_TRANSPOSE
+// convolution/ccv_nnc_conv_transpose_cpu_ref.c:13-197.  y = T(a) is the data gradient of the "mirrored" convolution, the one that
+// maps y's extent onto a's: y plays its input (C = Cout = count), a its output (K = Cin), and w[Cin, R, S, Cout / groups] has its
+// filter layout [K, R, S, C / groups]; the hint means what it means for that convolution (CPU_REF walks the same clipped windows).
+// Pixels of y that no tap reaches hold the bias.  The backward (which the reference leaves undefined) is the mirrored convolution's
+// forward for da = conv(g, w), its weight gradient with the activations swapped for dw = wgrad(grad = a, x = g), and the column sum
+// of g for dbias: the same launches as CONVOLUTION_FORWARD / _BACKWARD, bit for bit.
+// The mirrored CONVOLUTION command: count = Cin (convolution_transpose.count is Cout; groups and dilation sit at the same offsets)
+bool conv_mirror(const ccv_nnc_cmd_t& cmd, const TV& w, const uint32_t mirror_id, ccv_nnc_cmd_t& mirror)
+{
+	const int groups = cmd.info.convolution_transpose.groups > 0 ? cmd.info.convolution_transpose.groups : 1;
+	if (w.nd != 4 || w.dim[3] * groups != cmd.info.convolution_transpose.count)
+		return false;
+	mirror = cmd;
+	mirror.cmd = mirror_id;
+	mirror.info.convolution.count = w.dim[0];
+	return true;
+}
+// geometry of the mirrored convolution from (big = y or its gradient, w, small = a or its gradient)
+bool conv_transpose_geom(const ccv_nnc_cmd_t& cmd, const ccv_nnc_hint_t& hint, const TV& big, const TV& w, const TV& small, ConvGeom& g)
+{
+	ccv_nnc_cmd_t mirror;
+	return conv_mirror(cmd, w, CCV_NNC_CONVOLUTION_BACKWARD, mirror) && conv_geom(mirror, hint, big, w, small, g);
+}
+
+// inputs (a, w, bias?), output y (always overwritten)
+int conv_transpose_forw_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
+{
+	if (input_size < 2 || output_size < 1 || !inputs[0] || !inputs[1] || !outputs[0])
+		return CCV_NNC_EXEC_INVALID;
+	const ccv_nnc_tensor_t* const bias_t = input_size > 2 ? inputs[2] : 0;
+	const int kind = kind_of(inputs[0]);
+	if (kind < 0 || kind_of(inputs[1]) != kind || kind_of(outputs[0]) != kind || (bias_t && ((kind_of(bias_t) != kind && !is_f32(bias_t)) || CCV_IS_TENSOR_VIEW(bias_t))))
+		return CCV_NNC_EXEC_INVALID;
+	ConvGeom g;
+	if (!conv_transpose_geom(cmd, hint, view_of(outputs[0]), view_of(inputs[1]), view_of(inputs[0]), g) || (bias_t && bias_t->info.dim[0] != g.C))
+		return CCV_NNC_EXEC_INVALID;
+	const int groups = cmd.info.convolution_transpose.groups > 0 ? cmd.info.convolution_transpose.groups : 1;
+	const float* const bias32 = bias_t && is_f32(bias_t) ? bias_t->data.f32 : 0;
+	const void* const bias16 = bias_t && !is_f32(bias_t) ? (const void*)bias_t->data.u8 : 0;
+	return dgrad_nhwc(stream_context, kind, conv_algorithm(cmd), groups, g, inputs[0]->data.u8, inputs[1]->data.u8, bias32, bias16, outputs[0]->data.u8);
+}
+
+// inputs (g, a, w), outputs (da, dw, dbias), any output may be NULL; dw / dbias honour CCV_NNC_ACCUMULATE_OUTPUT, da is overwritten
+int conv_transpose_back_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
+{
+	ccv_nnc_tensor_t* const g_t = input_size > 0 ? inputs[0] : 0;
+	ccv_nnc_tensor_t* const a_t = input_size > 1 ? inputs[1] : 0;
+	ccv_nnc_tensor_t* const w_t = input_size > 2 ? inputs[2] : 0;
+	ccv_nnc_tensor_t* const da_t = output_size > 0 ? outputs[0] : 0;
+	ccv_nnc_tensor_t* const dw_t = output_size > 1 ? outputs[1] : 0;
+	ccv_nnc_tensor_t* const dbias_t = output_size > 2 ? outputs[2] : 0;
+	const ccv_nnc_tensor_t* const filt = dw_t ? dw_t : w_t;
+	const ccv_nnc_tensor_t* const small = a_t ? a_t : da_t;
+	const int kind = g_t ? kind_of(g_t) : -1;
+	if (kind < 0 || !filt || !small || (dw_t && !a_t) || (da_t && !w_t))
+		return CCV_NNC_EXEC_INVALID;
+	ConvGeom g, gchk;
+	if (!conv_transpose_geom(cmd, hint, view_of(g_t), view_of(filt), view_of(small), g))
+		return CCV_NNC_EXEC_INVALID;
+	// every operand is checked before the first launch: a refused call leaves the outputs as they were
+	const int groups = cmd.info.convolution_transpose.groups > 0 ? cmd.info.convolution_transpose.groups : 1;
+	if ((a_t && kind_of(a_t) != kind) || (w_t && kind_of(w_t) != kind) || (da_t && kind_of(da_t) != kind) || (dw_t && kind_of(dw_t) != kind))
+		return CCV_NNC_EXEC_INVALID;
+	if ((dw_t && !conv_transpose_geom(cmd, hint, view_of(g_t), view_of(dw_t), view_of(a_t), gchk)) || (da_t && !conv_transpose_geom(cmd, hint, view_of(g_t), view_of(w_t), view_of(da_t), gchk)))
+		return CCV_NNC_EXEC_INVALID;
+	// 16-bit forwards and weight gradients run on the tensor cores only: Cin a multiple of 8, grouped ones with wide groups
+	if (kind > 0 && (da_t || dw_t) && (g.K % 8 || (groups > 1 && (g.C / groups % 8 || g.K / groups % 8 || g.C / groups < 16 || g.K / groups < 16))))
+		return CCV_NNC_EXEC_INVALID;
+	const int db_kind = dbias_t ? kind_of(dbias_t) : 0;
+	if (dbias_t && (db_kind < 0 || (kind == 0 && db_kind != 0) || dbias_t->info.dim[0] != g.C || g.ah != (long long)g.W * g.aw || g.an != (long long)g.H * g.ah))
+		return CCV_NNC_EXEC_INVALID;
+	if (da_t)
+	{
+		// da = conv(g, w), the mirrored convolution's forward
+		ccv_nnc_cmd_t mirror;
+		conv_mirror(cmd, view_of(w_t), CCV_NNC_CONVOLUTION_FORWARD, mirror);
+		ccv_nnc_tensor_t* const in[2] = { g_t, w_t };
+		ccv_nnc_tensor_t* const out[1] = { da_t };
+		const int rc = conv_forw_nhwc(mirror, hint, 0, in, 2, out, 1, stream_context);
+		if (rc != CCV_NNC_EXEC_SUCCESS)
+			return rc;
+	}
+	if (dw_t)
+	{
+		// dw (+)= wgrad(grad = a, x = g) of the mirrored convolution
+		ccv_nnc_cmd_t mirror;
+		conv_mirror(cmd, view_of(dw_t), CCV_NNC_CONVOLUTION_BACKWARD, mirror);
+		ccv_nnc_tensor_t* const in[3] = { a_t, g_t, 0 };
+		ccv_nnc_tensor_t* const out[2] = { 0, dw_t };
+		const int rc = conv_back_nhwc(mirror, hint, flags, in, 3, out, 2, stream_context);
+		if (rc != CCV_NNC_EXEC_SUCCESS)
+			return rc;
+	}
+	if (dbias_t)
+	{
+		// dbias[c] (+)= sum over the pixels of g, which are the mirrored convolution's input pixels
+		const int accumulate = (flags & CCV_NNC_ACCUMULATE_OUTPUT) ? 1 : 0;
+		cudaStream_t s = stream_of(stream_context);
+		void* const ws = ccv_nnc_stream_context_get_workspace(stream_context, colsum_workspace_bytes(g.C), CCV_TENSOR_GPU_MEMORY);
+		if (kind == 0)
+			RC(colsum_f32(s, g_t->data.f32, (size_t)g.N * g.H * g.W, g.C, g.aw, dbias_t->data.f32, accumulate, ws));
+		else
+			RC(colsum_any(s, kind, g_t->data.u8, (size_t)g.N * g.H * g.W, g.C, g.aw, dbias_t->data.u8, db_kind, accumulate, ws));
+	}
+	return CCV_NNC_EXEC_SUCCESS;
+}
+
+// NCHW: staged like the convolution (filters [Cin, Cout / groups, R, S] become [Cin, R, S, Cout / groups]).  The bound covers every
+// path above on the mirrored geometry: its data gradient, forward and weight gradient, the 16-bit functional form whenever the
+// tensor cores may decline the data gradient, and the column sum over Cout.
+template <int BACKWARD>
+size_t conv_transpose_staged_inner(const ccv_nnc_cmd_t& cmd, const ccv_nnc_hint_t& hint, ccv_nnc_tensor_t* const* const in, const int input_size, ccv_nnc_tensor_t* const* const out, const int output_size)
+{
+	ccv_nnc_tensor_t* const big = BACKWARD ? in[0] : out[0];
+	ccv_nnc_tensor_t* const filt = BACKWARD ? (output_size > 1 && out[1] ? out[1] : (input_size > 2 ? in[2] : 0)) : in[1];
+	ccv_nnc_tensor_t* const small = BACKWARD ? (input_size > 1 && in[1] ? in[1] : out[0]) : in[0];
+	ConvGeom g;
+	const int kind = big ? kind_of(big) : -1;
+	if (kind < 0 || !filt || !small || !conv_transpose_geom(cmd, hint, view_of(big), view_of(filt), view_of(small), g))
+		return (size_t)-1;
+	const int groups = cmd.info.convolution_transpose.groups > 1 ? cmd.info.convolution_transpose.groups : 1;
+	size_t need = std::max(conv_inner_workspace(g, kind, groups), colsum_workspace_bytes(g.C));
+	if (!BACKWARD && kind > 0 && groups == 1 && conv_dgrad_may_decline(g, kind))
+		need = std::max(need, dgrad16_fallback_bytes(g));
+	return (need + 255) & ~(size_t)255;
+}
+
+int exec_conv_transpose_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
+{
+	if (any_nchw(inputs, input_size, outputs, output_size))
+		return nchw_staged(conv_transpose_forw_nhwc, conv_transpose_staged_inner<0>, 0, cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
+	return conv_transpose_forw_nhwc(cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
+}
+
+int exec_conv_transpose_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
+{
+	if (any_nchw(inputs, input_size, outputs, output_size))
+		return nchw_staged(conv_transpose_back_nhwc, conv_transpose_staged_inner<1>, 1, cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
+	return conv_transpose_back_nhwc(cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
 }
 
 
@@ -2292,6 +2462,8 @@ REGISTER_SM100(CCV_NNC_GEMM_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV
 REGISTER_SM100(CCV_NNC_GEMM_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, CCV_NNC_SM100_ALGO_COUNT, exec_gemm_nd4<exec_gemm_back>); registry->autotune = autotune_contraction<exec_gemm_nd4<exec_gemm_back> >; }
 REGISTER_SM100(CCV_NNC_CONVOLUTION_FORWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF, CCV_NNC_SM100_ALGO_COUNT, exec_conv_forw); registry->autotune = autotune_contraction<exec_conv_forw>; }
 REGISTER_SM100(CCV_NNC_CONVOLUTION_BACKWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF, CCV_NNC_SM100_ALGO_COUNT, exec_conv_back); registry->autotune = autotune_contraction<exec_conv_back>; }
+REGISTER_SM100(CCV_NNC_CONVOLUTION_TRANSPOSE_FORWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF, CCV_NNC_SM100_ALGO_COUNT, exec_conv_transpose_forw); registry->autotune = autotune_contraction<exec_conv_transpose_forw>; }
+REGISTER_SM100(CCV_NNC_CONVOLUTION_TRANSPOSE_BACKWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF, CCV_NNC_SM100_ALGO_COUNT, exec_conv_transpose_back); registry->autotune = autotune_contraction<exec_conv_transpose_back>; }
 REGISTER_SM100(CCV_NNC_SCALED_DOT_PRODUCT_ATTENTION_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, ccv_nnc_sm100_exec_sdpa_forw); }
 REGISTER_SM100(CCV_NNC_SCALED_DOT_PRODUCT_ATTENTION_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, ccv_nnc_sm100_exec_sdpa_back); }
 REGISTER_SM100(CCV_NNC_SOFTMAX_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_via_f32<exec_softmax_forw>); }

@@ -656,9 +656,37 @@ size_t conv_dgrad_workspace_bytes(const ConvGeom& g)
 	return dgrad_filter_copy_bytes(g) + CONTRACT_SCRATCH_BYTES;
 }
 
-// wt: room for the fp32 filter copy (kind 0; NULL for 16-bit kinds)
-static int conv_dgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, const void* grad_b, const void* w, float* wt, void* grad_a, const Scratch& scratch, int x3)
+// out[m, c] = bias[c] over a dense [rows, C] tensor of element kind `kind` (fp32 bias32, or bias16 in the output's 16-bit type): the
+// value of the pixels of a biased data gradient that no filter tap reaches, rounded like the epilogue rounds 0 + bias
+__global__ void __launch_bounds__(256) bias_fill_kernel(void* __restrict__ out, const float* __restrict__ bias32, const uint16_t* __restrict__ bias16, const int kind, const int C, const long long total)
 {
+	for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x)
+	{
+		const int c = (int)(i % C);
+		const float v = bias32 ? bias32[c] : cvt16(bias16[c], kind);
+		if (kind == 0)
+			reinterpret_cast<float*>(out)[i] = v;
+		else
+			reinterpret_cast<uint16_t*>(out)[i] = (uint16_t)(pack16x2(v, 0.f, kind) & 0xffffu);
+	}
+}
+
+bool conv_dgrad_may_decline(const ConvGeom& g, int kind)
+{
+	if (g.R * g.S > UMMA_MAX_TAPS || g.C % kind_align(kind) || g.K % kind_align(kind) || g.C % 4 || g.K % 4 || (long long)g.K * g.R * g.S * g.C > 0x7fffffffll || !conv_out_contiguous(g) || !conv_in_contiguous(g))
+		return true;
+	// a class's im2col box starts at lo = min over its taps of (a + pad0 - r * dil) / stride and ends at Hc - P + lo: both lie within
+	// +-(2 * span + 3) below, so the box limits of [-128, 127] hold whenever span <= 62
+	const int span_h = abs(g.pad_h0) + abs(g.pad_h1) + (g.R - 1) * g.dil_h + g.stride_h, span_w = abs(g.pad_w0) + abs(g.pad_w1) + (g.S - 1) * g.dil_w + g.stride_w;
+	return span_h > 62 || span_w > 62;
+}
+
+// wt: room for the fp32 filter copy (kind 0; NULL for 16-bit kinds).  bias (fp32) / bias16 (16-bit kinds): added in the epilogue of
+// every launch, and broadcast into the pixels of tap-less residue classes
+static int conv_dgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, const void* grad_b, const void* w, const float* bias, const void* bias16, float* wt, void* grad_a, const Scratch& scratch, int x3)
+{
+	if (bias)
+		bias16 = 0;
 	const X3Scope math(kind == 0 ? x3 : 0);
 	const long long rsc = (long long)g.R * g.S * g.C;
 	if (!tma_api_init() || !conv_shape_consistent(g) || !conv_out_contiguous(g) || !conv_in_contiguous(g) || g.C % kind_align(kind) || g.K % kind_align(kind) || g.K * rsc > 0x7fffffffll)
@@ -672,8 +700,8 @@ static int conv_dgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, cons
 	if (conv_is_pointwise(g)) // dA[NHW, C] = dB[NHW, K] x W[K, C]
 	{
 		if (kind == 0)
-			return gemm_any(stream, kind, g.N * g.H * g.W, g.C, g.K, grad_b, g.K, 0, wt, g.K, 1, grad_a, g.C, 0, 0, 0, scratch, x3);
-		return gemm_any(stream, kind, g.N * g.H * g.W, g.C, g.K, grad_b, g.K, 0, w, g.C, 0, grad_a, g.C, 0, 0, 0, scratch, x3);
+			return gemm_any(stream, kind, g.N * g.H * g.W, g.C, g.K, grad_b, g.K, 0, wt, g.K, 1, grad_a, g.C, bias, 0, 0, scratch, x3);
+		return gemm_any(stream, kind, g.N * g.H * g.W, g.C, g.K, grad_b, g.K, 0, w, g.C, 0, grad_a, g.C, bias, bias16, 0, scratch, x3);
 	}
 	const int bn = pick_bn(g.C), bk = kind_bk(kind);
 	const size_t esz = kind_esz(kind);
@@ -713,8 +741,21 @@ static int conv_dgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, cons
 				continue;
 			}
 		}
-	if (need_zero)
+	if (need_zero && (bias || bias16))
 	{
+		const long long total = (long long)g.N * g.H * g.W * g.C;
+		long long blocks = (total + 255) / 256;
+		if (blocks > (long long)num_sms() * 8)
+			blocks = (long long)num_sms() * 8;
+		bias_fill_kernel<<<(unsigned)blocks, 256, 0, stream>>>(grad_a, bias, (const uint16_t*)bias16, kind, g.C, total);
+		count_launch();
+		const cudaError_t e = cudaGetLastError();
+		if (e != cudaSuccess)
+		{
+			set_last_error("bias_fill_kernel", e);
+			return -1;
+		}
+	} else if (need_zero) {
 		cudaError_t e = cudaMemsetAsync(grad_a, 0, (size_t)g.N * g.H * g.W * g.C * esz, stream);
 		if (e != cudaSuccess)
 		{
@@ -773,6 +814,7 @@ static int conv_dgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, cons
 					(kind == 0 ? p.tap_b_row : p.tap_b_col)[t] = (cp.r_h[i] * g.S + cp.s_w[j]) * g.C;
 				}
 			p.out = (float*)((char*)grad_a + ((long long)ah * g.W + aw) * g.C * esz);
+			p.bias = bias, p.bias16 = bias16;
 			p.rowmap.mode = 1;
 			p.rowmap.Pc = Hc, p.rowmap.Qc = Wc;
 			p.rowmap.n_stride = (long long)g.H * g.W * g.C;
@@ -784,14 +826,14 @@ static int conv_dgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, cons
 		}
 	return 0;
 }
-int conv_dgrad_tf32(cudaStream_t stream, const ConvGeom& g, const float* grad_b, const float* w, float* grad_a, void* workspace, int x3)
+int conv_dgrad_tf32(cudaStream_t stream, const ConvGeom& g, const float* grad_b, const float* w, const float* bias, float* grad_a, void* workspace, int x3)
 {
 	const Scratch scratch = { (char*)workspace + dgrad_filter_copy_bytes(g), CONTRACT_SCRATCH_BYTES };
-	return conv_dgrad_any(stream, 0, g, grad_b, w, (float*)workspace, grad_a, scratch, x3);
+	return conv_dgrad_any(stream, 0, g, grad_b, w, bias, 0, (float*)workspace, grad_a, scratch, x3);
 }
-int conv_dgrad_16(cudaStream_t stream, int kind, const ConvGeom& g, const void* grad_b, const void* w, void* grad_a, const Scratch& scratch)
+int conv_dgrad_16(cudaStream_t stream, int kind, const ConvGeom& g, const void* grad_b, const void* w, const float* bias32, const void* bias16, void* grad_a, const Scratch& scratch)
 {
-	return kind == 1 || kind == 2 ? conv_dgrad_any(stream, kind, g, grad_b, w, 0, grad_a, scratch, 0) : 1;
+	return kind == 1 || kind == 2 ? conv_dgrad_any(stream, kind, g, grad_b, w, bias32, bias16, 0, grad_a, scratch, 0) : 1;
 }
 
 static int conv_wgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, const void* grad_b, const void* a, void* grad_w, int accumulate, const Scratch& scratch, int x3)

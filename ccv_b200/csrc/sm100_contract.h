@@ -36,9 +36,11 @@ constexpr size_t CONTRACT_SCRATCH_BYTES = (size_t)96 << 20;
 // C[M, N] (+)= op(A) * op(B) + bias; A is [M, K] (lda) or, if trans_a, [K, M]; B is [K, N] (ldb) or, if trans_b, [N, K].
 int gemm_tf32(cudaStream_t stream, int M, int N, int K, const float* a, long long lda, int trans_a, const float* b, long long ldb, int trans_b, float* c, long long ldc, const float* bias, int accumulate, const Scratch& scratch, int x3 = 0);
 int conv_fprop_tf32(cudaStream_t stream, const ConvGeom& g, const float* a, const float* w, const float* bias, float* b, const Scratch& scratch, int x3 = 0);
-// the fp32 data gradient works in a workspace of conv_dgrad_workspace_bytes(g) (which includes CONTRACT_SCRATCH_BYTES for split-K slices)
+// the fp32 data gradient works in a workspace of conv_dgrad_workspace_bytes(g) (which includes CONTRACT_SCRATCH_BYTES for split-K slices).
+// bias[C] (NULL: none) is added to every pixel of grad_a, also to those no filter tap reaches: that makes the data gradient the
+// forward of a transposed convolution (CONVOLUTION_TRANSPOSE_FORWARD).
 size_t conv_dgrad_workspace_bytes(const ConvGeom& g);
-int conv_dgrad_tf32(cudaStream_t stream, const ConvGeom& g, const float* grad_b, const float* w, float* grad_a, void* workspace, int x3 = 0);
+int conv_dgrad_tf32(cudaStream_t stream, const ConvGeom& g, const float* grad_b, const float* w, const float* bias, float* grad_a, void* workspace, int x3 = 0);
 int conv_wgrad_tf32(cudaStream_t stream, const ConvGeom& g, const float* grad_b, const float* a, float* grad_w, int accumulate, const Scratch& scratch, int x3 = 0);
 
 // The same contractions on 16-bit tensors (kind 1 = bf16, 2 = fp16): wgmma bf16 / fp16 with fp32 accumulation in registers, 16-bit
@@ -46,7 +48,10 @@ int conv_wgrad_tf32(cudaStream_t stream, const ConvGeom& g, const float* grad_b,
 // bias: fp32 (bias32) or in the tensors' 16-bit type (bias16); at most one of them.  Returns as above (1 = shape not covered).
 int gemm_16(cudaStream_t stream, int kind, int M, int N, int K, const void* a, long long lda, int trans_a, const void* b, long long ldb, int trans_b, void* c, long long ldc, const float* bias32, const void* bias16, int accumulate, const Scratch& scratch);
 int conv_fprop_16(cudaStream_t stream, int kind, const ConvGeom& g, const void* a, const void* w, const float* bias32, const void* bias16, void* b, const Scratch& scratch);
-int conv_dgrad_16(cudaStream_t stream, int kind, const ConvGeom& g, const void* grad_b, const void* w, void* grad_a, const Scratch& scratch);
+int conv_dgrad_16(cudaStream_t stream, int kind, const ConvGeom& g, const void* grad_b, const void* w, const float* bias32, const void* bias16, void* grad_a, const Scratch& scratch);
+// true when conv_dgrad_tf32 / conv_dgrad_16 may return 1 for this geometry and element kind on shape grounds (a superset of the shape
+// tests they make; operand pointers aside): callers that reserve the workspace of their fallback ahead of the call count it in then
+bool conv_dgrad_may_decline(const ConvGeom& g, int kind);
 int conv_wgrad_16(cudaStream_t stream, int kind, const ConvGeom& g, const void* grad_b, const void* a, void* grad_w, int accumulate, const Scratch& scratch);
 
 // Ask the NEXT conv_fprop_tf32 / gemm_tf32 launch of this host thread to also produce per-column statistics of its output
@@ -69,7 +74,7 @@ int conv_wgrad_im2col_16(cudaStream_t stream, int kind, const ConvGeom& g, const
 // output tiles split K into slices of `scratch` (none given: no split), combined in split order like the tensor-core path.
 int gemm_ffma(cudaStream_t stream, int M, int N, int K, const float* a, long long a_rs, long long a_cs, const float* b, long long b_rs, long long b_cs, float* c, long long ldc, const float* bias, int accumulate, const Scratch& scratch = Scratch());
 int conv_fprop_ffma(cudaStream_t stream, const ConvGeom& g, int groups, const float* a, const float* w, const float* bias, float* b);
-int conv_dgrad_ffma(cudaStream_t stream, const ConvGeom& g, int groups, const float* grad_b, const float* w, float* grad_a);
+int conv_dgrad_ffma(cudaStream_t stream, const ConvGeom& g, int groups, const float* grad_b, const float* w, const float* bias, float* grad_a);
 int conv_wgrad_ffma(cudaStream_t stream, const ConvGeom& g, int groups, const float* grad_b, const float* a, float* grad_w, int accumulate, const Scratch& scratch = Scratch());
 // out[r, c] = (accumulate ? out[r, c] : 0) + part[0][r, c] + part[1][r, c] + ... (fp32 slices [rows, cols] of pitch ldp, split_stride apart)
 int splitk_reduce(cudaStream_t stream, const float* part, int splits, long long split_stride, int rows, int cols, long long ldp, float* out, long long ldo, int accumulate, int out_kind = 0);

@@ -224,7 +224,8 @@ int conv_fprop_ffma(cudaStream_t stream, const ConvGeom& g, int groups, const fl
 	return 0;
 }
 
-int conv_dgrad_ffma(cudaStream_t stream, const ConvGeom& g, int groups, const float* grad_b, const float* w, float* grad_a)
+// every pixel of grad_a is a row of the GEMM (pixels no tap reaches are 0 + bias)
+int conv_dgrad_ffma(cudaStream_t stream, const ConvGeom& g, int groups, const float* grad_b, const float* w, const float* bias, float* grad_a)
 {
 	const int Cg = g.C / groups, Kg = g.K / groups;
 	if (g.ah != (long long)g.W * g.aw || g.an != (long long)g.H * g.ah)
@@ -237,7 +238,7 @@ int conv_dgrad_ffma(cudaStream_t stream, const ConvGeom& g, int groups, const fl
 		A.sh = g.stride_h, A.sw = g.stride_w, A.ph = g.pad_h0, A.pw = g.pad_w0, A.dh = g.dil_h, A.dw = g.dil_w;
 		A.gn = g.bn, A.gh = g.bh, A.gw = g.bw;
 		DgradFilter B = { w + (long long)gr * Kg * g.R * g.S * Cg, Kg, g.R, g.S, Cg };
-		const int rc = launch_ffma(stream, A, B, grad_a + gr * Cg, g.aw, 0, g.N * g.H * g.W, Cg, g.R * g.S * Kg, 0, 1, Scratch());
+		const int rc = launch_ffma(stream, A, B, grad_a + gr * Cg, g.aw, bias ? bias + gr * Cg : 0, g.N * g.H * g.W, Cg, g.R * g.S * Kg, 0, 1, Scratch());
 		if (rc)
 			return rc;
 	}

@@ -416,6 +416,23 @@ def CMD_CONVOLUTION_BACKWARD(groups, count, kh, kw_, channels, dilation=(1, 1), 
     return c
 
 
+def CMD_CONVOLUTION_TRANSPOSE_FORWARD(groups, count, output_padding, kh, kw_, channels, dilation=(1, 1), **kw):
+    """Argument order of the reference macro (cmd/convolution/ccv_nnc_convolution.c:119): count = output channels."""
+    info = abi.CmdParam()
+    _size(info, (kh, kw_, channels))
+    info.convolution_transpose.count = count
+    info.convolution_transpose.groups = groups
+    info.convolution_transpose.dilation[0], info.convolution_transpose.dilation[1] = dilation
+    info.convolution_transpose.output_padding = output_padding
+    return Command(abi.CCV_NNC_CONVOLUTION_TRANSPOSE_FORWARD, info, **kw)
+
+
+def CMD_CONVOLUTION_TRANSPOSE_BACKWARD(groups, count, output_padding, kh, kw_, channels, dilation=(1, 1), **kw):
+    c = CMD_CONVOLUTION_TRANSPOSE_FORWARD(groups, count, output_padding, kh, kw_, channels, dilation, **kw)
+    c.cmd = abi.CCV_NNC_CONVOLUTION_TRANSPOSE_BACKWARD
+    return c
+
+
 def CMD_BATCH_NORM_FORWARD(epsilon, is_test, momentum, axes=(0, 1, 2), **kw):
     info = abi.CmdParam()
     _size(info, (1, 1, 1))

@@ -180,6 +180,12 @@ typedef struct {
 			int dilation[CCV_NNC_MAX_DIM_ALLOC];
 		} convolution;
 		struct {
+			int count;
+			int groups;
+			int dilation[CCV_NNC_MAX_DIM_ALLOC];
+			int output_padding; /* only the output extent (ccv_nnc_hint_tensor_auto) depends on it */
+		} convolution_transpose;
+		struct {
 			int reserved;
 		} pool;
 		struct {
@@ -346,6 +352,8 @@ enum {
 	CCV_NNC_COMM_ALLREDUCE_BACKWARD = 0x75c8d341,
 	CCV_NNC_CONVOLUTION_FORWARD = 0x254d05f4,
 	CCV_NNC_CONVOLUTION_BACKWARD = 0x254d05f5,
+	CCV_NNC_CONVOLUTION_TRANSPOSE_FORWARD = 0xd691f78e,
+	CCV_NNC_CONVOLUTION_TRANSPOSE_BACKWARD = 0xd691f78f,
 	CCV_NNC_DATATYPE_CONVERSION_FORWARD = 0xd873e38c,
 	CCV_NNC_DATATYPE_CONVERSION_BACKWARD = 0xd873e38d,
 	CCV_NNC_DATA_TRANSFER_FORWARD = 0x12d21e1a,
@@ -463,6 +471,7 @@ enum {
 #define CCV_NNC_SM100_COMMANDS(X) \
 	X(CCV_NNC_GEMM_FORWARD) X(CCV_NNC_GEMM_BACKWARD) \
 	X(CCV_NNC_CONVOLUTION_FORWARD) X(CCV_NNC_CONVOLUTION_BACKWARD) \
+	X(CCV_NNC_CONVOLUTION_TRANSPOSE_FORWARD) X(CCV_NNC_CONVOLUTION_TRANSPOSE_BACKWARD) \
 	X(CCV_NNC_SCALED_DOT_PRODUCT_ATTENTION_FORWARD) X(CCV_NNC_SCALED_DOT_PRODUCT_ATTENTION_BACKWARD) \
 	X(CCV_NNC_SOFTMAX_FORWARD) X(CCV_NNC_SOFTMAX_BACKWARD) \
 	X(CCV_NNC_BATCH_NORM_FORWARD) X(CCV_NNC_BATCH_NORM_BACKWARD) \
