@@ -258,13 +258,9 @@ int ccv_nnc_sm100_exec_sdpa_back(SM100_EXEC_ARGS)
 	if (dt != CCV_32F)
 	{
 		// 16-bit backward.  Outside the fused kernel's shapes (below) the functional form: widen g, q, k, v to fp32 in the stream
-		// workspace, run the fp32 composed backward (TF32 tensor-core GEMMs per (b, h)), narrow dq, dk, dv back.
-		for (int i : { 0, 3, 4, 5 })
-			if (CCV_IS_TENSOR_VIEW(inputs[i]))
-				return CCV_NNC_EXEC_INVALID;
-		for (int i = 0; i < 3; i++)
-			if (CCV_IS_TENSOR_VIEW(outputs[i]))
-				return CCV_NNC_EXEC_INVALID;
+		// workspace, run the fp32 composed backward (TF32 tensor-core GEMMs per (b, h)), narrow dq, dk, dv back.  The fused kernels
+		// take every operand through its strides, so views (a slice of a packed QKV tensor, pitched gradients) reach them; only the
+		// functional form, which widens whole tensors, refuses views.
 		if (!sdpa_geom(cmd, inputs[3], inputs[4], inputs[5], inputs[0], g) || !sdpa_geom(cmd, outputs[0], outputs[1], outputs[2], inputs[0], dg))
 			return CCV_NNC_EXEC_INVALID;
 		if (dg.B != g.B || dg.H != g.H || dg.Hk != g.Hk || dg.Sq != g.Sq || dg.Sk != g.Sk || dg.D != g.D || dg.Dv != g.Dv)
@@ -295,6 +291,12 @@ int ccv_nnc_sm100_exec_sdpa_back(SM100_EXEC_ARGS)
 			if (rc == 0)
 				return CCV_NNC_EXEC_SUCCESS;
 		}
+		for (int i : { 0, 3, 4, 5 })
+			if (CCV_IS_TENSOR_VIEW(inputs[i]))
+				return CCV_NNC_EXEC_INVALID;
+		for (int i = 0; i < 3; i++)
+			if (CCV_IS_TENSOR_VIEW(outputs[i]))
+				return CCV_NNC_EXEC_INVALID;
 		const size_t nq = count_of(inputs[3]), nk = count_of(inputs[4]), nv = count_of(inputs[5]), no = count_of(inputs[0]);
 		const size_t floats = no + 2 * nq + 2 * nk + 2 * nv;
 		const size_t ws_bytes = floats * sizeof(float) + 256 + sdpa_workspace_bytes(g.Sq, g.Sk, 1);

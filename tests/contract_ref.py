@@ -55,6 +55,7 @@ def to_bits16(x, out):
         return x.astype(np.float16).view(np.uint16)
     m, e = np.frexp(x)
     r = np.ldexp(np.rint(m * 256.0), e - 8)  # 8 significant bits, ties to even
+    r = np.where(np.abs(x) < 2.0 ** -126, np.rint(x * 2.0 ** 133) * 2.0 ** -133, r)  # subnormals: multiples of 2^-133
     return (r.astype(np.float32).view(np.uint32) >> 16).astype(np.uint16)
 
 

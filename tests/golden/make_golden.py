@@ -3,6 +3,7 @@
 
     python tests/golden/make_golden.py
     python tests/golden/make_golden.py registry <reference>/lib/nnc/cmd/ccv_nnc_cmd.inc
+    python tests/golden/make_golden.py sdpa          # cpuref_sdpa.npz only
 
 Two kinds of fixtures:
   literal_*   inputs + expected outputs typed from the reference's unit tests (test/unit/nnc/gemm.tests.c etc.); these
@@ -69,6 +70,32 @@ def cpuref_cases():
     return cases
 
 
+def cpuref_sdpa():
+    """SCALED_DOT_PRODUCT_ATTENTION forward and backward of CPU_REF on the seeded calls of tests/attention_ref.PINS (GQA, causal with
+    Sq < Sk and Sq > Sk, Dv != D, 3-d tensors, every mask shape): inputs and outputs, keys prefixed "<case>_"."""
+    from ccv_b200 import abi
+    from tests import attention_ref as ar
+    out = {}
+    for i in range(len(ar.PINS)):
+        d = ar.pin_inputs(i)
+        q, k, v, do, mask = d["q"], d["k"], d["v"], d["do"], d["mask"]
+        fwd = nnc._simple(abi.CCV_NNC_SCALED_DOT_PRODUCT_ATTENTION_FORWARD)
+        fwd.info.scaled_dot_product_attention.scale, fwd.info.scaled_dot_product_attention.is_causal = d["scale"], d["causal"]
+        o = np.zeros(q.shape[:-1] + v.shape[-1:], np.float32)
+        assert ref.run(fwd, None, 0, [q, k, v] + ([mask] if mask is not None else []), [o]) == 0
+        rec = dict(q=q, k=k, v=v, o=o)
+        if mask is not None:
+            rec["mask"] = mask
+        if d["backward"]:
+            bwd = nnc._simple(abi.CCV_NNC_SCALED_DOT_PRODUCT_ATTENTION_BACKWARD)
+            bwd.info.scaled_dot_product_attention.scale, bwd.info.scaled_dot_product_attention.is_causal = d["scale"], d["causal"]
+            dq, dk, dv = np.zeros_like(q), np.zeros_like(k), np.zeros_like(v)
+            assert ref.run(bwd, None, 0, [do, None, None, q, k, v], [dq, dk, dv]) == 0
+            rec.update(do=do, dq=dq, dk=dk, dv=dv)
+        out.update(("%d_%s" % (i, name), a) for name, a in rec.items())
+    return out
+
+
 def reference_registry(inc):
     sys.path.insert(0, os.path.join(ROOT, "tools"))
     import gen_backend_ph as g
@@ -82,8 +109,11 @@ def reference_registry(inc):
 if __name__ == "__main__" and sys.argv[1:2] == ["registry"]:
     import json
     json.dump(reference_registry(sys.argv[2]), open(os.path.join(OUT, "reference_cmd_registry.json"), "w"), indent=0)
+elif __name__ == "__main__" and sys.argv[1:2] == ["sdpa"]:
+    np.savez(os.path.join(OUT, "cpuref_sdpa.npz"), **cpuref_sdpa())
 elif __name__ == "__main__":
     np.savez(os.path.join(OUT, "literal_gemm.npz"), **literal_gemm())
     for name, d in cpuref_cases().items():
         np.savez(os.path.join(OUT, "cpuref_%s.npz" % name), **d)
+    np.savez(os.path.join(OUT, "cpuref_sdpa.npz"), **cpuref_sdpa())
     print("wrote", sorted(os.listdir(OUT)))
