@@ -271,14 +271,59 @@ ccv_nnc_hint_t ccv_nnc_hint_auto(const ccv_nnc_cmd_param_t cmd, const ccv_nnc_te
 	return hint;
 }
 
-size_t ccv_nnc_tensor_data_size(const ccv_nnc_tensor_param_t params)
+size_t ccv_nnc_tensor_data_size_without_padding(const ccv_nnc_tensor_param_t params)
 {
 	size_t count = 1;
 	int i;
 	for (i = 0; i < CCV_NNC_MAX_DIM_ALLOC && params.dim[i] > 0; i++)
 		count *= (size_t)params.dim[i];
-	const size_t size = count * datatype_size(params.datatype);
-	return (size + 63) & ~(size_t)63;
+	// lib/nnc/ccv_nnc_easy.h:221-235: a palettized tensor holds one palette per block of `reserved` elements plus the packed indices
+	if (CCV_GET_DATA_TYPE(params.datatype) == CCV_QX)
+	{
+		const int qbits = (params.datatype >> 8) & 0xf;
+		if (!sm100::palettize_params_ok(qbits, params.reserved))
+			return 0;
+		return sm100::palettize_data_bytes(count, qbits, params.reserved, datatype_size((params.datatype & 0xff) << 12));
+	}
+	return count * datatype_size(params.datatype);
+}
+
+size_t ccv_nnc_tensor_data_size(const ccv_nnc_tensor_param_t params)
+{
+	return (ccv_nnc_tensor_data_size_without_padding(params) + 63) & ~(size_t)63;
+}
+
+ccv_nnc_tensor_param_t ccv_nnc_tensor_palettize(const ccv_nnc_tensor_param_t params, const int qbits, const int number_in_blocks)
+{
+	ccv_nnc_tensor_param_t new_params = params;
+	new_params.datatype = ((params.datatype >> 12) & 0xff) | CCV_QX | ((qbits << 8) & 0xf00);
+	new_params.reserved = number_in_blocks;
+	return new_params;
+}
+
+// lib/nnc/ccv_nnc_palettize.c:958-972.  GPU memory only: this host has no CPU kernels.  `output` receives output_length elements of
+// `datatype` (CCV_16F, CCV_32F or CCV_64F), enqueued on the calling thread's default stream like every stream-less command.  Invalid
+// parameters (qbits outside 4..8, a block size whose index bytes are not whole, another datatype) leave the output untouched.
+void ccv_nnc_depalettize(const void* input, const int datatype, const int memory_type, const size_t input_length, const int qbits, const int number_in_blocks, void* output, const size_t output_length)
+{
+	if (memory_type != CCV_TENSOR_GPU_MEMORY)
+	{
+		sm100::set_last_error("ccv_nnc_depalettize: only GPU memory is supported", cudaErrorInvalidValue);
+		return;
+	}
+	ccv_nnc_sm100_depalettize(input, datatype, input_length, qbits, number_in_blocks, output, output_length, 0);
+}
+
+int ccv_nnc_sm100_depalettize(const void* input, const int datatype, const size_t input_length, const int qbits, const int number_in_blocks, void* output, const size_t output_length, ccv_nnc_stream_context_t* const stream_context)
+{
+	const int dt = CCV_GET_DATA_TYPE(datatype);
+	if (!sm100::palettize_params_ok(qbits, number_in_blocks) || (dt != CCV_16F && dt != CCV_32F && dt != CCV_64F) ||
+		input_length < sm100::palettize_data_bytes(output_length, qbits, number_in_blocks, datatype_size(dt)))
+	{
+		sm100::set_last_error("ccv_nnc_depalettize: invalid parameters", cudaErrorInvalidValue);
+		return -1;
+	}
+	return sm100::depalettize((cudaStream_t)ccv_nnc_stream_context_get_stream(stream_context), input, dt, qbits, number_in_blocks, output, output_length) ? -1 : 0;
 }
 
 ccv_nnc_tensor_t* ccv_nnc_tensor_new(const void* const ptr, const ccv_nnc_tensor_param_t params, const int flags)

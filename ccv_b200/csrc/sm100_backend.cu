@@ -2283,6 +2283,242 @@ int exec_pool_any(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int 
 	return F(cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
 }
 
+// ================================================================================================ palettized (CCV_QX) operands
+// lib/nnc/cmd/blas/gpu/ccv_nnc_gemm_gpu_cublas.cu:291-334, convolution/gpu/ccv_nnc_conv_gpu_cudnn.cu:79,328,
+// convolution/gpu/ccv_nnc_conv_transpose_gpu_cudnn.cu:72,127: a weight operand may be a palettized tensor.  It is decoded into the
+// workspace and the command runs on the decoded tensor, so the result is the dense command's, bit for bit.  The workspace is one
+// request [what the dense command asks for | decoded operands]: the dense command's own requests then never grow (and move) it.
+inline bool is_qx(const ccv_nnc_tensor_t* const t) { return t && CCV_GET_DATA_TYPE(t->info.datatype) == CCV_QX; }
+inline int qx_palette(const ccv_nnc_tensor_t* const t) { return (t->info.datatype & 0xff) << 12; }
+inline int qx_bits(const ccv_nnc_tensor_t* const t) { return (t->info.datatype >> 8) & 0xf; }
+
+bool any_qx(ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size)
+{
+	for (int i = 0; i < input_size; i++)
+		if (is_qx(inputs[i]))
+			return true;
+	for (int i = 0; i < output_size; i++)
+		if (is_qx(outputs[i]))
+			return true;
+	return false;
+}
+
+// what nchw_staged(exec, inner_of, ...) asks the workspace for, or (size_t)-1 when it would refuse the operands
+size_t nchw_staged_request(const staged_inner_f inner_of, const ccv_nnc_cmd_t& cmd, const ccv_nnc_hint_t& hint, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size)
+{
+	if (input_size > 3 || output_size > 3)
+		return (size_t)-1;
+	Staged st[6];
+	ccv_nnc_tensor_t* in[3] = { 0, 0, 0 };
+	ccv_nnc_tensor_t* out[3] = { 0, 0, 0 };
+	int n = 0;
+	size_t staging = 0;
+	for (int i = 0; i < input_size; i++)
+	{
+		in[i] = inputs[i];
+		if (is_nchw(inputs[i]))
+		{
+			if (!stage_plan(inputs[i], st[n]))
+				return (size_t)-1;
+			staging += st[n].bytes, in[i] = &st[n].shadow, n++;
+		}
+	}
+	for (int i = 0; i < output_size; i++)
+	{
+		out[i] = outputs[i];
+		if (is_nchw(outputs[i]))
+		{
+			if (!stage_plan(outputs[i], st[n]))
+				return (size_t)-1;
+			staging += st[n].bytes, out[i] = &st[n].shadow, n++;
+		}
+	}
+	const size_t inner = inner_of(cmd, hint, in, input_size, out, output_size);
+	return inner == (size_t)-1 ? inner : inner + staging;
+}
+
+// `exec` = the dense command, `inner_of` = the most it asks the workspace for (on the decoded operands), `qx_inputs` = bit i set when
+// inputs[i] may be palettized.  Refused (outputs untouched): a palettized output or other operand, qbits outside 4..8, a block size
+// whose index bytes are not whole, a view, a palette that is not fp16 / fp32 or not the type of the command's other tensors.
+typedef size_t (*qx_inner_f)(const ccv_nnc_cmd_t& cmd, const ccv_nnc_hint_t& hint, ccv_nnc_tensor_t* const* in, int input_size, ccv_nnc_tensor_t* const* out, int output_size);
+int exec_depalettized(const ccv_nnc_cmd_exec_f exec, const qx_inner_f inner_of, const unsigned qx_inputs, const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
+{
+	enum { MAXT = 8 };
+	if (input_size > MAXT)
+		return CCV_NNC_EXEC_INVALID;
+	int dense = 0;
+	for (int i = 0; i < output_size && !dense; i++)
+		if (outputs[i])
+		{
+			if (is_qx(outputs[i]))
+				return CCV_NNC_EXEC_INVALID;
+			dense = CCV_GET_DATA_TYPE(outputs[i]->info.datatype);
+		}
+	for (int i = 0; i < input_size && !dense; i++)
+		if (inputs[i] && !is_qx(inputs[i]))
+			dense = CCV_GET_DATA_TYPE(inputs[i]->info.datatype);
+	ccv_nnc_tensor_t shadow[MAXT];
+	ccv_nnc_tensor_t* in[MAXT];
+	size_t off[MAXT], decoded = 0;
+	for (int i = 0; i < input_size; i++)
+	{
+		in[i] = inputs[i];
+		if (!is_qx(inputs[i]))
+			continue;
+		const int pal = qx_palette(inputs[i]);
+		if (!(qx_inputs & (1u << i)) || CCV_IS_TENSOR_VIEW(inputs[i]) || !palettize_params_ok(qx_bits(inputs[i]), inputs[i]->info.reserved) || (pal != CCV_16F && pal != CCV_32F) || pal != dense)
+			return CCV_NNC_EXEC_INVALID;
+		memcpy(&shadow[i], inputs[i], sizeof(ccv_nnc_tensor_t));
+		shadow[i].info.datatype = pal;
+		shadow[i].info.reserved = 0;
+		shadow[i].type = (shadow[i].type & ~0xFF000) | pal;
+		shadow[i].data_size = 0;
+		off[i] = decoded;
+		decoded += (view_of(inputs[i]).count * dtype_size(pal) + 255) & ~(size_t)255;
+		in[i] = &shadow[i];
+	}
+	const size_t inner = inner_of(cmd, hint, in, input_size, outputs, output_size);
+	if (inner == (size_t)-1)
+		return CCV_NNC_EXEC_INVALID;
+	unsigned char* const ws = (unsigned char*)ccv_nnc_stream_context_get_workspace(stream_context, inner + decoded, CCV_TENSOR_GPU_MEMORY);
+	if (!ws)
+		return CCV_NNC_EXEC_OOM;
+	cudaStream_t s = stream_of(stream_context);
+	for (int i = 0; i < input_size; i++)
+		if (is_qx(inputs[i]))
+		{
+			shadow[i].data.u8 = ws + inner + off[i];
+			RC(depalettize(s, inputs[i]->data.u8, qx_palette(inputs[i]), qx_bits(inputs[i]), inputs[i]->info.reserved, shadow[i].data.u8, view_of(inputs[i]).count));
+		}
+	const int rc = exec(cmd, hint, flags, in, input_size, outputs, output_size, stream_context);
+	if (rc != CCV_NNC_EXEC_SUCCESS)
+		return rc;
+	if (ccv_nnc_stream_context_get_workspace(stream_context, 1, CCV_TENSOR_GPU_MEMORY) != (void*)ws)
+	{
+		set_last_error("palettized operands: workspace moved under the decoded tensors", cudaErrorInvalidValue);
+		return CCV_NNC_EXEC_INVALID;
+	}
+	return CCV_NNC_EXEC_SUCCESS;
+}
+
+// GEMM: the contraction scratch, and the column sum of the bias gradient
+size_t gemm_qx_inner(const ccv_nnc_cmd_t&, const ccv_nnc_hint_t&, ccv_nnc_tensor_t* const* const in, const int input_size, ccv_nnc_tensor_t* const*, int)
+{
+	const TV g = view_of(in[0]);
+	return (std::max(CONTRACT_SCRATCH_BYTES, colsum_workspace_bytes(g.nd > 0 ? g.dim[g.nd - 1] : 1)) + 255) & ~(size_t)255;
+}
+template <staged_inner_f INNER>
+size_t conv_qx_inner(const ccv_nnc_cmd_t& cmd, const ccv_nnc_hint_t& hint, ccv_nnc_tensor_t* const* const in, const int input_size, ccv_nnc_tensor_t* const* const out, const int output_size)
+{
+	if (any_nchw(in, input_size, out, output_size))
+		return nchw_staged_request(INNER, cmd, hint, in, input_size, out, output_size);
+	return INNER(cmd, hint, in, input_size, out, output_size);
+}
+
+// The few-row dense layer on a palettized weight, without decoding it: c[M, N] = a[M, K] w[N, K]^T (+ bias), a / c fp16, w with fp16
+// palettes and no batch axis, M = every row of a up to PALETTIZED_GEMM_M_MAX.  Returns false when the call is not of that form.
+bool gemm_fused_qx_plan(const ccv_nnc_cmd_t& cmd, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, int& M, int& N, int& K)
+{
+	if (input_size < 2 || output_size < 1 || !inputs[0] || !is_qx(inputs[1]) || !outputs[0] || is_qx(inputs[0]) || CCV_IS_TENSOR_VIEW(inputs[1]))
+		return false;
+	const ccv_nnc_tensor_t* const bias_t = input_size > 2 ? inputs[2] : 0;
+	if (CCV_GET_DATA_TYPE(inputs[0]->info.datatype) != CCV_16F || CCV_GET_DATA_TYPE(outputs[0]->info.datatype) != CCV_16F || qx_palette(inputs[1]) != CCV_16F ||
+		!palettize_params_ok(qx_bits(inputs[1]), inputs[1]->info.reserved))
+		return false;
+	const int* const ta = cmd.info.blas.transpose_a;
+	const int* const tb = cmd.info.blas.transpose_b;
+	const TV a = view_of(inputs[0]), w = view_of(inputs[1]), c = view_of(outputs[0]);
+	if (w.nd != 2 || tb[0] == tb[1] || ta[0] != ta[1] || a.nd < 1 || a.nd > 3 || c.nd != a.nd || !a.contiguous || !c.contiguous)
+		return false;
+	K = w.dim[1], N = w.dim[0];
+	if (a.dim[a.nd - 1] != K || c.dim[c.nd - 1] != N)
+		return false;
+	const size_t rows = a.count / K;
+	if (rows < 1 || rows > (size_t)PALETTIZED_GEMM_M_MAX || c.count / N != rows)
+		return false;
+	if (bias_t)
+	{
+		const TV b = view_of(bias_t);
+		if (b.nd != 1 || b.dim[0] != N || is_qx(bias_t) || (CCV_GET_DATA_TYPE(bias_t->info.datatype) != CCV_16F && CCV_GET_DATA_TYPE(bias_t->info.datatype) != CCV_32F))
+			return false;
+	}
+	M = (int)rows;
+	return true;
+}
+
+int exec_gemm_forw_any(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
+{
+	if (!any_qx(inputs, input_size, outputs, output_size))
+		return exec_gemm_nd4<exec_gemm_forw>(cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
+	int M, N, K;
+	if (gemm_fused_qx_plan(cmd, inputs, input_size, outputs, output_size, M, N, K))
+	{
+		const ccv_nnc_tensor_t* const bias_t = input_size > 2 ? inputs[2] : 0;
+		const bool b32 = bias_t && is_f32(bias_t);
+		RC(gemm_palettized_f16(stream_of(stream_context), M, N, K, inputs[0]->data.u8, K, inputs[1]->data.u8, qx_bits(inputs[1]), inputs[1]->info.reserved, outputs[0]->data.u8, N,
+			b32 ? bias_t->data.f32 : 0, bias_t && !b32 ? (const void*)bias_t->data.u8 : 0));
+		return CCV_NNC_EXEC_SUCCESS;
+	}
+	return exec_depalettized(exec_gemm_nd4<exec_gemm_forw>, gemm_qx_inner, 0x3, cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
+}
+
+int exec_gemm_back_any(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
+{
+	if (!any_qx(inputs, input_size, outputs, output_size))
+		return exec_gemm_nd4<exec_gemm_back>(cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
+	// inputs (g, a, w): a is palettized only for dw, w only for h
+	const unsigned mask = (output_size > 1 && outputs[1] ? 0x2u : 0u) | (output_size > 0 && outputs[0] ? 0x4u : 0u);
+	return exec_depalettized(exec_gemm_nd4<exec_gemm_back>, gemm_qx_inner, mask, cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
+}
+
+// convolutions: the filters, inputs[1] of the forwards and inputs[2] of the backwards when the data gradient (outputs[0]) is asked for
+template <ccv_nnc_cmd_exec_f EXEC, staged_inner_f INNER, int BACKWARD>
+int exec_conv_any(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
+{
+	if (!any_qx(inputs, input_size, outputs, output_size))
+		return EXEC(cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
+	const unsigned mask = BACKWARD ? (output_size > 0 && outputs[0] ? 0x4u : 0u) : 0x2u;
+	return exec_depalettized(EXEC, conv_qx_inner<INNER>, mask, cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
+}
+
+// util/gpu/ccv_nnc_util_gpu_ref.cu:22-24: a palettized tensor moves as its bytes; both sides carry the same datatype word and block size
+int exec_data_transfer_any(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
+{
+	if (!any_qx(inputs, input_size, outputs, output_size))
+		return exec_data_transfer(cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
+	const int n = input_size < output_size ? input_size : output_size;
+	for (int i = 0; i < n; i++)
+		if (inputs[i] && outputs[i] && (is_qx(inputs[i]) || is_qx(outputs[i])))
+		{
+			const ccv_nnc_tensor_t* const a = inputs[i];
+			const ccv_nnc_tensor_t* const b = outputs[i];
+			if (a->info.datatype != b->info.datatype || a->info.reserved != b->info.reserved || CCV_IS_TENSOR_VIEW(a) || CCV_IS_TENSOR_VIEW(b) || view_of(a).count != view_of(b).count ||
+				!palettize_params_ok(qx_bits(a), a->info.reserved))
+				return CCV_NNC_EXEC_INVALID;
+		}
+	cudaStream_t s = stream_of(stream_context);
+	for (int i = 0; i < n; i++)
+	{
+		if (!inputs[i] || !outputs[i] || inputs[i] == outputs[i])
+			continue;
+		if (!is_qx(inputs[i]))
+		{
+			RC(copy_tensor(s, inputs[i], outputs[i]));
+			continue;
+		}
+		const size_t bytes = palettize_data_bytes(view_of(inputs[i]).count, qx_bits(inputs[i]), inputs[i]->info.reserved, dtype_size(qx_palette(inputs[i])));
+		const cudaError_t e = cudaMemcpyAsync(outputs[i]->data.u8, inputs[i]->data.u8, bytes, cudaMemcpyDefault, s);
+		if (e != cudaSuccess)
+		{
+			set_last_error("data transfer (palettized)", e);
+			return CCV_NNC_EXEC_INVALID;
+		}
+	}
+	if (!stream_context && cudaStreamSynchronize(s) != cudaSuccess)
+		return CCV_NNC_EXEC_INVALID;
+	return CCV_NNC_EXEC_SUCCESS;
+}
+
 void fill(ccv_nnc_cmd_backend_registry_t* const registry, const int formats, const int datatypes, const int algorithms, const ccv_nnc_cmd_exec_f exec)
 {
 	registry->tensor_formats = formats;
@@ -2458,13 +2694,13 @@ int exec_via_f32_rt(ccv_nnc_cmd_exec_f f32, const ccv_nnc_cmd_t cmd, const ccv_n
 
 #define REGISTER_SM100(cmd) extern "C" void _register_command_ ## cmd ## _backend_CCV_NNC_BACKEND_GPU_SM100(ccv_nnc_cmd_backend_registry_t* const registry)
 
-REGISTER_SM100(CCV_NNC_GEMM_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, CCV_NNC_SM100_ALGO_COUNT, exec_gemm_nd4<exec_gemm_forw>); registry->autotune = autotune_contraction<exec_gemm_nd4<exec_gemm_forw> >; }
-REGISTER_SM100(CCV_NNC_GEMM_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, CCV_NNC_SM100_ALGO_COUNT, exec_gemm_nd4<exec_gemm_back>); registry->autotune = autotune_contraction<exec_gemm_nd4<exec_gemm_back> >; }
-REGISTER_SM100(CCV_NNC_CONVOLUTION_FORWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF, CCV_NNC_SM100_ALGO_COUNT, exec_conv_forw); registry->autotune = autotune_contraction<exec_conv_forw>; }
-REGISTER_SM100(CCV_NNC_CONVOLUTION_BACKWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF, CCV_NNC_SM100_ALGO_COUNT, exec_conv_back); registry->autotune = autotune_contraction<exec_conv_back>; }
-REGISTER_SM100(CCV_NNC_CONVOLUTION_TRANSPOSE_FORWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF, CCV_NNC_SM100_ALGO_COUNT, exec_conv_transpose_forw); registry->autotune = autotune_contraction<exec_conv_transpose_forw>; }
-REGISTER_SM100(CCV_NNC_CONVOLUTION_TRANSPOSE_BACKWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF, CCV_NNC_SM100_ALGO_COUNT, exec_conv_transpose_back); registry->autotune = autotune_contraction<exec_conv_transpose_back>; }
-REGISTER_SM100(CCV_NNC_SCALED_DOT_PRODUCT_ATTENTION_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, ccv_nnc_sm100_exec_sdpa_forw); }
+REGISTER_SM100(CCV_NNC_GEMM_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_gemm_forw_any); registry->autotune = autotune_contraction<exec_gemm_forw_any>; }
+REGISTER_SM100(CCV_NNC_GEMM_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_gemm_back_any); registry->autotune = autotune_contraction<exec_gemm_back_any>; }
+REGISTER_SM100(CCV_NNC_CONVOLUTION_FORWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_conv_any<exec_conv_forw, conv_staged_inner<0>, 0>); registry->autotune = autotune_contraction<exec_conv_any<exec_conv_forw, conv_staged_inner<0>, 0> >; }
+REGISTER_SM100(CCV_NNC_CONVOLUTION_BACKWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_conv_any<exec_conv_back, conv_staged_inner<1>, 1>); registry->autotune = autotune_contraction<exec_conv_any<exec_conv_back, conv_staged_inner<1>, 1> >; }
+REGISTER_SM100(CCV_NNC_CONVOLUTION_TRANSPOSE_FORWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_conv_any<exec_conv_transpose_forw, conv_transpose_staged_inner<0>, 0>); registry->autotune = autotune_contraction<exec_conv_any<exec_conv_transpose_forw, conv_transpose_staged_inner<0>, 0> >; }
+REGISTER_SM100(CCV_NNC_CONVOLUTION_TRANSPOSE_BACKWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_conv_any<exec_conv_transpose_back, conv_transpose_staged_inner<1>, 1>); registry->autotune = autotune_contraction<exec_conv_any<exec_conv_transpose_back, conv_transpose_staged_inner<1>, 1> >; }
+REGISTER_SM100(CCV_NNC_SCALED_DOT_PRODUCT_ATTENTION_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, 1, ccv_nnc_sm100_exec_sdpa_forw); }
 REGISTER_SM100(CCV_NNC_SCALED_DOT_PRODUCT_ATTENTION_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, ccv_nnc_sm100_exec_sdpa_back); }
 REGISTER_SM100(CCV_NNC_SOFTMAX_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_via_f32<exec_softmax_forw>); }
 REGISTER_SM100(CCV_NNC_SOFTMAX_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_via_f32<exec_softmax_back>); }
@@ -2494,8 +2730,8 @@ REGISTER_SM100(CCV_NNC_UPSAMPLE_FORWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC
 REGISTER_SM100(CCV_NNC_UPSAMPLE_BACKWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF, 1, exec_via_f32<ccv_nnc_sm100_exec_upsample_back>); }
 REGISTER_SM100(CCV_NNC_SET_FORWARD) { fill(registry, ALL_FORMATS, CCV_64F | CCV_32F | CCV_16F | CCV_16BF | CCV_32S, 1, exec_set_forw); }
 REGISTER_SM100(CCV_NNC_SET_BACKWARD) { fill(registry, ALL_FORMATS, CCV_64F | CCV_32F | CCV_16F | CCV_16BF | CCV_32S, 1, exec_set_forw); }
-REGISTER_SM100(CCV_NNC_DATA_TRANSFER_FORWARD) { fill(registry, ALL_FORMATS, CCV_64F | CCV_32F | CCV_16F | CCV_16BF | CCV_32S | CCV_8U, 1, exec_data_transfer); registry->tensor_memory = CCV_TENSOR_CPU_MEMORY | CCV_TENSOR_GPU_MEMORY; }
-REGISTER_SM100(CCV_NNC_DATA_TRANSFER_BACKWARD) { fill(registry, ALL_FORMATS, CCV_64F | CCV_32F | CCV_16F | CCV_16BF | CCV_32S | CCV_8U, 1, exec_data_transfer); registry->tensor_memory = CCV_TENSOR_CPU_MEMORY | CCV_TENSOR_GPU_MEMORY; }
+REGISTER_SM100(CCV_NNC_DATA_TRANSFER_FORWARD) { fill(registry, ALL_FORMATS, CCV_64F | CCV_32F | CCV_16F | CCV_16BF | CCV_32S | CCV_8U | CCV_QX, 1, exec_data_transfer_any); registry->tensor_memory = CCV_TENSOR_CPU_MEMORY | CCV_TENSOR_GPU_MEMORY; }
+REGISTER_SM100(CCV_NNC_DATA_TRANSFER_BACKWARD) { fill(registry, ALL_FORMATS, CCV_64F | CCV_32F | CCV_16F | CCV_16BF | CCV_32S | CCV_8U | CCV_QX, 1, exec_data_transfer_any); registry->tensor_memory = CCV_TENSOR_CPU_MEMORY | CCV_TENSOR_GPU_MEMORY; }
 REGISTER_SM100(CCV_NNC_FORMAT_TRANSFORM_FORWARD) { fill(registry, ALL_FORMATS, CCV_64F | CCV_32F | CCV_32S | CCV_16F | CCV_16BF | CCV_8U, 1, exec_format_transform); }
 REGISTER_SM100(CCV_NNC_FORMAT_TRANSFORM_BACKWARD) { fill(registry, ALL_FORMATS, CCV_64F | CCV_32F | CCV_32S | CCV_16F | CCV_16BF | CCV_8U, 1, exec_format_transform); }
 REGISTER_SM100(CCV_NNC_TRANSPOSE_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_transpose); }

@@ -220,7 +220,20 @@ int ccv_nnc_sm100_exec_sdpa_forw(SM100_EXEC_ARGS)
 	const int c_nd = nd_of(c), d_nd = nd_of(d);
 	if (CCV_IS_TENSOR_VIEW(c) || CCV_IS_TENSOR_VIEW(d) || CCV_IS_TENSOR_VIEW(w) || (c_nd != 3 && c_nd != 4) || d_nd != 3 || nd_of(w) != 2)
 		return CCV_NNC_EXEC_INVALID;
-	if (CCV_GET_DATA_TYPE(c->info.datatype) != dt || CCV_GET_DATA_TYPE(d->info.datatype) != dt || CCV_GET_DATA_TYPE(w->info.datatype) != dt)
+	// the weights may be palettized (attention/gpu/ccv_nnc_scaled_dot_product_attention_flash_attn.cu registers CCV_QX), with a
+	// palette of the activations' type; no other operand may be
+	const bool w_qx = CCV_GET_DATA_TYPE(w->info.datatype) == CCV_QX;
+	const int w_dt = w_qx ? (w->info.datatype & 0xff) << 12 : CCV_GET_DATA_TYPE(w->info.datatype);
+	const int w_q = (w->info.datatype >> 8) & 0xf;
+	if (w_qx && ((dt != CCV_16F && dt != CCV_32F) || !palettize_params_ok(w_q, w->info.reserved)))
+		return CCV_NNC_EXEC_INVALID;
+	for (int i = 0; i < input_size; i++)
+		if (i != 4 && inputs[i] && CCV_GET_DATA_TYPE(inputs[i]->info.datatype) == CCV_QX)
+			return CCV_NNC_EXEC_INVALID;
+	for (int i = 0; i < output_size; i++)
+		if (outputs[i] && CCV_GET_DATA_TYPE(outputs[i]->info.datatype) == CCV_QX)
+			return CCV_NNC_EXEC_INVALID;
+	if (CCV_GET_DATA_TYPE(c->info.datatype) != dt || CCV_GET_DATA_TYPE(d->info.datatype) != dt || w_dt != dt)
 		return CCV_NNC_EXEC_INVALID;
 	const int B = c->info.dim[0], S = c->info.dim[1];
 	const long long hd = c_nd == 4 ? (long long)c->info.dim[2] * c->info.dim[3] : c->info.dim[2];
@@ -241,7 +254,18 @@ int ccv_nnc_sm100_exec_sdpa_forw(SM100_EXEC_ARGS)
 	if (st != CCV_NNC_EXEC_SUCCESS)
 		return st;
 	const int kind = dt == CCV_32F ? 0 : (dt == CCV_16BF ? 1 : 2);
-	if (backend_gemm_nt_bias(stream_context, kind, B * S, (int)hd, (int)hd, c->data.u8, w->data.u8, d->data.u8, bias ? bias->data.u8 : 0, bias_f32))
+	const void* w_data = w->data.u8;
+	if (w_qx)
+	{
+		// one workspace request [the projection's contraction scratch | decoded weights]: the projection's own request does not move it
+		unsigned char* const ws = (unsigned char*)ccv_nnc_stream_context_get_workspace(stream_context, CONTRACT_SCRATCH_BYTES + (size_t)hd * hd * (dt == CCV_32F ? 4 : 2), CCV_TENSOR_GPU_MEMORY);
+		if (!ws)
+			return CCV_NNC_EXEC_OOM;
+		if (depalettize(stream_of(stream_context), w->data.u8, dt, w_q, w->info.reserved, ws + CONTRACT_SCRATCH_BYTES, (size_t)hd * hd))
+			return CCV_NNC_EXEC_INVALID;
+		w_data = ws + CONTRACT_SCRATCH_BYTES;
+	}
+	if (backend_gemm_nt_bias(stream_context, kind, B * S, (int)hd, (int)hd, c->data.u8, w_data, d->data.u8, bias ? bias->data.u8 : 0, bias_f32))
 		return CCV_NNC_EXEC_INVALID;
 	return CCV_NNC_EXEC_SUCCESS;
 }

@@ -109,6 +109,19 @@ int sdpa_backward_f16(cudaStream_t s, const SdpaGeom& g, const SdpaGeom& dg, int
 // commands that end in a dense projection (the attention "unify head" output).  Returns 0, or non-zero like the GEMM launchers.
 int backend_gemm_nt_bias(void* stream_context, int kind, int M, int N, int K, const void* a, const void* w, void* c, const void* bias, int bias_is_f32);
 
+// palettized (CCV_QX) tensors (sm100_palettize.cu).  qbits 4..8; nib (elements per palette block) must make the block stride
+// nib * qbits / 8 a whole number of bytes.  palette_datatype is CCV_16F, CCV_32F or CCV_64F; out holds `count` decoded elements.
+bool palettize_params_ok(int qbits, int nib);
+size_t palettize_data_bytes(size_t count, int qbits, int nib, size_t palette_elem);
+// returns 0, 1 when the parameters are refused, < 0 on CUDA errors
+int depalettize(cudaStream_t stream, const void* in, int palette_datatype, int qbits, int nib, void* out, size_t count);
+// c[M, N] (ldc) = a[M, K] (lda) w[N, K]^T (+ bias[N], fp32 or fp16) with fp16 a / c and w palettized with fp16 palettes, packed
+// [N, K]; M <= PALETTIZED_GEMM_M_MAX.  Decodes w in registers, fp32 accumulation in a fixed order, no workspace.  Returns as above.
+// The bound is measured (tools/bench_palettize.py, DESIGN.md §7.3): on an H100 the kernel beats decode + dense GEMM on every benchmark
+// shape at one row only; from 4 rows on it loses on some of them.
+constexpr int PALETTIZED_GEMM_M_MAX = 1;
+int gemm_palettized_f16(cudaStream_t stream, int M, int N, int K, const void* a, long long lda, const void* wq, int qbits, int nib, void* c, long long ldc, const float* bias32, const void* bias16);
+
 // bookkeeping shared by every launcher in the backend
 void count_launch(int n = 1);
 unsigned long long launch_count();

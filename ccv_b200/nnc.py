@@ -90,6 +90,16 @@ def lib():
         l.ccv_nnc_sm100_comm_init_rank.argtypes = [vp, sz, i32, i32]
         l.ccv_nnc_sm100_comm_rank.restype = i32
         l.ccv_nnc_sm100_comm_world.restype = i32
+        l.ccv_nnc_tensor_palettize.restype = abi.TensorParam
+        l.ccv_nnc_tensor_palettize.argtypes = [abi.TensorParam, i32, i32]
+        l.ccv_nnc_tensor_data_size.restype = sz
+        l.ccv_nnc_tensor_data_size.argtypes = [abi.TensorParam]
+        l.ccv_nnc_tensor_data_size_without_padding.restype = sz
+        l.ccv_nnc_tensor_data_size_without_padding.argtypes = [abi.TensorParam]
+        l.ccv_nnc_depalettize.restype = None
+        l.ccv_nnc_depalettize.argtypes = [vp, i32, i32, sz, i32, i32, vp, sz]
+        l.ccv_nnc_sm100_depalettize.restype = i32
+        l.ccv_nnc_sm100_depalettize.argtypes = [vp, i32, sz, i32, i32, vp, sz, vp]
         _lib = l
     return _lib
 
@@ -131,7 +141,13 @@ class Tensor(object):
         return n
 
     @property
+    def is_palettized(self):
+        return (self.params.datatype & 0xFF000) == abi.CCV_QX
+
+    @property
     def nbytes(self):
+        if self.is_palettized:
+            return lib().ccv_nnc_tensor_data_size_without_padding(self.params)
         return self.count * abi.DTYPE_SIZE[self.params.datatype & 0xFF000]
 
     @property
@@ -148,8 +164,13 @@ class Tensor(object):
 
     # --- staging helpers (blocking copies; tests and benchmark set-up only) -------------------------------
     def upload(self, array, stream=None):
-        a = np.ascontiguousarray(array, dtype=NP_DTYPE[self.params.datatype & 0xFF000])
-        assert a.size == self.count, (a.shape, self.dims)
+        """A palettized tensor takes its packed bytes (a uint8 array of nbytes, tests/palette_ref.py makes them)."""
+        if self.is_palettized:
+            a = np.ascontiguousarray(array, dtype=np.uint8).reshape(-1)
+            assert a.size == self.nbytes, (a.size, self.nbytes)
+        else:
+            a = np.ascontiguousarray(array, dtype=NP_DTYPE[self.params.datatype & 0xFF000])
+            assert a.size == self.count, (a.shape, self.dims)
         if self.on_gpu:
             rc = lib().ccv_nnc_sm100_memcpy_h2d(self.data_ptr, a.ctypes.data, a.nbytes, stream.ptr if stream else None)
             if rc != 0:
@@ -159,7 +180,10 @@ class Tensor(object):
         return self
 
     def download(self, stream=None):
-        out = np.empty(self.dims, dtype=NP_DTYPE[self.params.datatype & 0xFF000])
+        if self.is_palettized:
+            out = np.empty(self.nbytes, dtype=np.uint8)
+        else:
+            out = np.empty(self.dims, dtype=NP_DTYPE[self.params.datatype & 0xFF000])
         if self.on_gpu:
             rc = lib().ccv_nnc_sm100_memcpy_d2h(out.ctypes.data, self.data_ptr, out.nbytes, stream.ptr if stream else None)
             if rc != 0:
@@ -183,6 +207,33 @@ def gpu_tensor(dims, fmt=abi.CCV_TENSOR_FORMAT_NHWC, datatype=abi.CCV_32F, devic
 
 def cpu_tensor(dims, fmt=abi.CCV_TENSOR_FORMAT_NHWC, datatype=abi.CCV_32F):
     return tensor_new(abi.tensor_param(abi.CCV_TENSOR_CPU_MEMORY, fmt, datatype, dims))
+
+
+def palettize_param(params, qbits, number_in_blocks):
+    """ccv_nnc_tensor_palettize (lib/nnc/ccv_nnc_easy.h:210-217): the parameters of a palettized copy of a CCV_16F / CCV_32F /
+    CCV_64F tensor, qbits 4..8, `number_in_blocks` elements per palette."""
+    return lib().ccv_nnc_tensor_palettize(params, qbits, number_in_blocks)
+
+
+def gpu_palettized_tensor(dims, datatype, qbits, number_in_blocks, fmt=abi.CCV_TENSOR_FORMAT_NHWC, device=0):
+    """A GPU tensor holding a palettized copy of a `datatype` tensor of `dims`; fill it with Tensor.upload(packed bytes)."""
+    return tensor_new(palettize_param(abi.tensor_param(abi.CCV_TENSOR_GPU_MEMORY, fmt, datatype, dims, device), qbits, number_in_blocks))
+
+
+def cpu_palettized_tensor(dims, datatype, qbits, number_in_blocks, fmt=abi.CCV_TENSOR_FORMAT_NHWC):
+    return tensor_new(palettize_param(abi.tensor_param(abi.CCV_TENSOR_CPU_MEMORY, fmt, datatype, dims), qbits, number_in_blocks))
+
+
+def tensor_data_size(params):
+    """ccv_nnc_tensor_data_size: the bytes ccv_nnc_tensor_new allocates for `params` (64-byte padded)."""
+    return lib().ccv_nnc_tensor_data_size(params)
+
+
+def depalettize(src, dst, stream=None):
+    """ccv_nnc_depalettize on GPU memory (ccv_nnc_sm100_depalettize on `stream`): decode palettized tensor `src` into the dense
+    tensor `dst` of its palette type.  Returns 0, or -1 when the parameters are refused."""
+    p = src.params
+    return lib().ccv_nnc_sm100_depalettize(src.data_ptr, (p.datatype & 0xff) << 12, src.nbytes, (p.datatype >> 8) & 0xf, p.reserved, dst.data_ptr, src.count, stream.ptr if stream else None)
 
 
 def tensor_view_new(tensor, dims, ofs, stride):

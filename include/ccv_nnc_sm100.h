@@ -540,6 +540,14 @@ ccv_nnc_tensor_view_t* ccv_nnc_tensor_view_new(const ccv_nnc_tensor_t* const ten
 void ccv_nnc_tensor_view_free(ccv_nnc_tensor_view_t* const tensor_view);
 int ccv_nnc_tensor_pin_memory(ccv_nnc_tensor_t* const tensor);
 size_t ccv_nnc_tensor_data_size(const ccv_nnc_tensor_param_t params);
+size_t ccv_nnc_tensor_data_size_without_padding(const ccv_nnc_tensor_param_t params);
+/* lib/nnc/ccv_nnc_easy.h:210-217 (an inline function there): the parameters of a palettized (CCV_QX) copy of a CCV_16F / CCV_32F / CCV_64F
+ * tensor: the datatype word carries qbits (4..8) and the palette type, `reserved` the number of elements that share one palette */
+ccv_nnc_tensor_param_t ccv_nnc_tensor_palettize(const ccv_nnc_tensor_param_t params, const int qbits, const int number_in_blocks);
+/* lib/nnc/ccv_nnc.h:916: decode output_length elements of `datatype` (CCV_16F, CCV_32F or CCV_64F) from a palettized buffer of
+ * input_length bytes.  This library decodes GPU memory only (memory_type CCV_TENSOR_GPU_MEMORY), on the calling thread's default
+ * stream; invalid parameters leave the output untouched and set ccv_nnc_sm100_last_error(). */
+void ccv_nnc_depalettize(const void* input, const int datatype, const int memory_type, const size_t input_length, const int qbits, const int number_in_blocks, void* output, const size_t output_length);
 
 /* lib/nnc/ccv_nnc.h:940-1100 */
 ccv_nnc_stream_context_t* ccv_nnc_stream_context_new(const int type);
@@ -580,6 +588,9 @@ void* ccv_nnc_sm100_event_new(void);
 int ccv_nnc_sm100_event_record(void* const event, ccv_nnc_stream_context_t* const stream_context);
 float ccv_nnc_sm100_event_elapsed_ms(void* const begin, void* const end);
 void ccv_nnc_sm100_event_free(void* const event);
+/* ccv_nnc_depalettize of GPU memory on a stream context's stream (NULL: the calling thread's default stream); 0, or -1 when the
+ * parameters are refused (the output is then untouched) or the launch failed */
+int ccv_nnc_sm100_depalettize(const void* input, const int datatype, const size_t input_length, const int qbits, const int number_in_blocks, void* output, const size_t output_length, ccv_nnc_stream_context_t* const stream_context);
 /* number of kernels this backend has launched since process start (bench.py's gpu_launches) */
 uint64_t ccv_nnc_sm100_launch_count(void);
 /* last CUDA error string seen by the backend (empty if none) */
