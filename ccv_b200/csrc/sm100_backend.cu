@@ -90,8 +90,8 @@ inline cudaStream_t stream_of(ccv_nnc_stream_context_t* const stream_context)
 	return (cudaStream_t)ccv_nnc_stream_context_get_stream(stream_context);
 }
 
-// split-K scratch of one command: the stream workspace (grow-only, one buffer per stream: lib/nnc/gpu/ccv_nnc_compat.cu:438-471).
-// A command that also stages tensors in the workspace asks for both at once and passes the tail (scratch_at).
+// split-K scratch of a command that no staging layer wraps: the stream workspace (grow-only, one buffer per stream:
+// lib/nnc/gpu/ccv_nnc_compat.cu:438-471).  The wrapped commands carve it out of their one workspace request (scratch_at).
 inline Scratch scratch_of(ccv_nnc_stream_context_t* const stream_context)
 {
 	void* const p = ccv_nnc_stream_context_get_workspace(stream_context, CONTRACT_SCRATCH_BYTES, CCV_TENSOR_GPU_MEMORY);
@@ -296,6 +296,25 @@ int gemm_dispatch16(cudaStream_t s, const Scratch& scratch, const int kind, cons
 	return narrow_matrix(s, c32, c, kind, c_rs, c_cs, M, N, accumulate) ? -1 : 0;
 }
 
+// Workspace function of a command that a staging layer may wrap: the exact size of the one workspace request the command makes for
+// these operands (0: none), or (size_t)-1 when it refuses them.  The command asks for that size before its first launch and hands
+// slices of it to the helpers under it, which never ask themselves.
+typedef size_t (*staged_inner_f)(const ccv_nnc_cmd_t& cmd, const ccv_nnc_hint_t& hint, ccv_nnc_tensor_t* const* in, int input_size, ccv_nnc_tensor_t* const* out, int output_size);
+size_t no_workspace(const ccv_nnc_cmd_t&, const ccv_nnc_hint_t&, ccv_nnc_tensor_t* const*, int, ccv_nnc_tensor_t* const*, int) { return 0; }
+
+// GEMM: the contraction scratch; the backward's column sum of the bias gradient shares it
+size_t gemm_forw_workspace(const ccv_nnc_cmd_t&, const ccv_nnc_hint_t&, ccv_nnc_tensor_t* const*, int, ccv_nnc_tensor_t* const*, int) { return CONTRACT_SCRATCH_BYTES; }
+size_t gemm_back_workspace(const ccv_nnc_cmd_t&, const ccv_nnc_hint_t&, ccv_nnc_tensor_t* const* const in, const int input_size, ccv_nnc_tensor_t* const* const out, const int output_size)
+{
+	size_t need = (output_size > 0 && out[0]) || (output_size > 1 && out[1]) ? CONTRACT_SCRATCH_BYTES : 0;
+	if (output_size > 2 && out[2] && input_size > 0 && in[0])
+	{
+		const TV g = view_of(in[0]);
+		need = std::max(need, colsum_workspace_bytes(g.nd > 0 ? g.dim[g.nd - 1] : 1));
+	}
+	return need;
+}
+
 // blas/ccv_nnc_gemm_cpu_ref.c:110-184
 int exec_gemm_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
 {
@@ -331,7 +350,10 @@ int exec_gemm_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 			bias.batch_inc = 0;
 	}
 	cudaStream_t s = stream_of(stream_context);
-	const Scratch scratch = scratch_of(stream_context);
+	void* const ws = ccv_nnc_stream_context_get_workspace(stream_context, gemm_forw_workspace(cmd, hint, inputs, input_size, outputs, output_size), CCV_TENSOR_GPU_MEMORY);
+	if (!ws)
+		return CCV_NNC_EXEC_OOM;
+	const Scratch scratch = scratch_at(ws, CONTRACT_SCRATCH_BYTES);
 	if (matrix_bias)
 	{
 		for (int i = 0; i < b.batch; i++)
@@ -370,6 +392,11 @@ int exec_gemm_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 		return CCV_NNC_EXEC_INVALID;
 	const size_t esz = kind_size(kind);
 	cudaStream_t s = stream_of(stream_context);
+	const size_t ws_bytes = gemm_back_workspace(cmd, hint, inputs, input_size, outputs, output_size);
+	void* const ws = ws_bytes ? ccv_nnc_stream_context_get_workspace(stream_context, ws_bytes, CCV_TENSOR_GPU_MEMORY) : 0;
+	if (ws_bytes && !ws)
+		return CCV_NNC_EXEC_OOM;
+	const Scratch scratch = scratch_at(ws, CONTRACT_SCRATCH_BYTES);
 	ccv_nnc_tensor_t* const dbias_t = output_size > 2 ? outputs[2] : 0;
 	ccv_nnc_tensor_t* const dw_t = output_size > 1 ? outputs[1] : 0;
 	ccv_nnc_tensor_t* const h_t = outputs[0];
@@ -384,7 +411,7 @@ int exec_gemm_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 		if (db_kind < 0)
 			return CCV_NNC_EXEC_INVALID;
 		for (int i = 0; i < g.batch; i++)
-			RC(colsum_any(s, kind, (const char*)g.p + (size_t)i * g.batch_inc * esz, g.rows, g.cols, g.rs, (char*)db.p + (db.batch == 1 ? 0 : (size_t)i * db.batch_inc * kind_size(db_kind)), db_kind, accumulate || (db.batch == 1 && i > 0), ccv_nnc_stream_context_get_workspace(stream_context, colsum_workspace_bytes(g.cols), CCV_TENSOR_GPU_MEMORY)));
+			RC(colsum_any(s, kind, (const char*)g.p + (size_t)i * g.batch_inc * esz, g.rows, g.cols, g.rs, (char*)db.p + (db.batch == 1 ? 0 : (size_t)i * db.batch_inc * kind_size(db_kind)), db_kind, accumulate || (db.batch == 1 && i > 0), ws));
 	}
 	if (dw_t)
 	{
@@ -401,10 +428,10 @@ int exec_gemm_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 		if (kind != 0)
 		{
 			for (int i = 0; i < g.batch; i++)
-				RC(gemm_dispatch16(s, scratch_of(stream_context), kind, dw.rows, dw.cols, g.rows, (const char*)a.p + (size_t)i * a.batch_inc * 2, a.cs, a.rs, (const char*)g.p + (size_t)i * g.batch_inc * 2, g.rs, g.cs, (char*)dw.p + (dw.batch == 1 ? 0 : (size_t)i * dw.batch_inc * 2), dw.rs, dw.cs, 0, 0, accumulate || (dw.batch == 1 && i > 0)));
+				RC(gemm_dispatch16(s, scratch, kind, dw.rows, dw.cols, g.rows, (const char*)a.p + (size_t)i * a.batch_inc * 2, a.cs, a.rs, (const char*)g.p + (size_t)i * g.batch_inc * 2, g.rs, g.cs, (char*)dw.p + (dw.batch == 1 ? 0 : (size_t)i * dw.batch_inc * 2), dw.rs, dw.cs, 0, 0, accumulate || (dw.batch == 1 && i > 0)));
 		} else
 		for (int i = 0; i < g.batch; i++)
-			RC(gemm_dispatch(s, scratch_of(stream_context), gemm_algorithm(cmd), dw.rows, dw.cols, g.rows, a.p + i * a.batch_inc, a.cs, a.rs, g.p + i * g.batch_inc, g.rs, g.cs, dw.p + (dw.batch == 1 ? 0 : i * dw.batch_inc), dw.rs, dw.cs, 0, accumulate || (dw.batch == 1 && i > 0)));
+			RC(gemm_dispatch(s, scratch, gemm_algorithm(cmd), dw.rows, dw.cols, g.rows, a.p + i * a.batch_inc, a.cs, a.rs, g.p + i * g.batch_inc, g.rs, g.cs, dw.p + (dw.batch == 1 ? 0 : i * dw.batch_inc), dw.rs, dw.cs, 0, accumulate || (dw.batch == 1 && i > 0)));
 	}
 	if (h_t)
 	{
@@ -421,10 +448,10 @@ int exec_gemm_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 		if (kind != 0)
 		{
 			for (int i = 0; i < g.batch; i++)
-				RC(gemm_dispatch16(s, scratch_of(stream_context), kind, h.rows, h.cols, g.cols, (const char*)g.p + (size_t)i * g.batch_inc * 2, g.rs, g.cs, (const char*)w.p + (size_t)i * w.batch_inc * 2, w.cs, w.rs, (char*)h.p + (h.batch == 1 ? 0 : (size_t)i * h.batch_inc * 2), h.rs, h.cs, 0, 0, accumulate || (h.batch == 1 && i > 0)));
+				RC(gemm_dispatch16(s, scratch, kind, h.rows, h.cols, g.cols, (const char*)g.p + (size_t)i * g.batch_inc * 2, g.rs, g.cs, (const char*)w.p + (size_t)i * w.batch_inc * 2, w.cs, w.rs, (char*)h.p + (h.batch == 1 ? 0 : (size_t)i * h.batch_inc * 2), h.rs, h.cs, 0, 0, accumulate || (h.batch == 1 && i > 0)));
 		} else
 		for (int i = 0; i < g.batch; i++)
-			RC(gemm_dispatch(s, scratch_of(stream_context), gemm_algorithm(cmd), h.rows, h.cols, g.cols, g.p + i * g.batch_inc, g.rs, g.cs, w.p + i * w.batch_inc, w.cs, w.rs, h.p + (h.batch == 1 ? 0 : i * h.batch_inc), h.rs, h.cs, 0, accumulate || (h.batch == 1 && i > 0)));
+			RC(gemm_dispatch(s, scratch, gemm_algorithm(cmd), h.rows, h.cols, g.cols, g.p + i * g.batch_inc, g.rs, g.cs, w.p + i * w.batch_inc, w.cs, w.rs, h.p + (h.batch == 1 ? 0 : i * h.batch_inc), h.rs, h.cs, 0, accumulate || (h.batch == 1 && i > 0)));
 	}
 	return CCV_NNC_EXEC_SUCCESS;
 }
@@ -586,36 +613,49 @@ bool conv_geom(const ccv_nnc_cmd_t& cmd, const ccv_nnc_hint_t& hint, const TV& a
 // (C/g and K/g multiples of the 16-byte vector and >= 16) each group's slices are made dense in the stream workspace (one strided
 // copy in, one out), and the dense wgmma kernels above do the arithmetic; narrower groups (depthwise and the like) stay on the
 // FFMA kernels, where the contraction is too short for a 64-deep MMA anyway.  PASS 0 = fprop, 1 = wgrad, 2 = dgrad.
-// returns 0 done, 1 not applicable (caller falls back), < 0 error
-template <int PASS>
-int conv_grouped_tc(ccv_nnc_stream_context_t* const stream_context, const int kind, const ConvGeom& g, const int groups, const int x3, const int accumulate,
-	const void* const act, const void* const filt, const float* const bias32, const void* const bias16, const void* const res, void* const out)
+// The workspace of one pass is [contraction workspace | one group's dense activations | its results]; false when the groups are too
+// narrow or unaligned for it (the caller falls back).
+struct GroupPlan {
+	ConvGeom gg; // one group as a dense convolution
+	size_t inner, xb, yb;
+};
+bool group_plan(const ConvGeom& g, const int kind, const int groups, const int pass, GroupPlan& p)
 {
 	const int align = kind == 0 ? 4 : 8;
 	const size_t es = kind_size(kind);
 	if (groups <= 1 || g.C % groups || g.K % groups)
-		return 1;
+		return false;
 	const int Cg = g.C / groups, Kg = g.K / groups;
 	if (Cg % align || Kg % align || Cg < 16 || Kg < 16)
-		return 1;
+		return false;
 	const long long lim = 0x7fffffffll;
 	if ((long long)g.N * g.an > lim || (long long)g.N * g.bn > lim)
-		return 1; // copy_strided walks int strides
-	ConvGeom gg = g;
+		return false; // copy_strided walks int strides
+	ConvGeom& gg = p.gg;
+	gg = g;
 	gg.C = Cg, gg.K = Kg;
 	gg.aw = Cg, gg.ah = (long long)g.W * Cg, gg.an = (long long)g.H * g.W * Cg;
 	gg.bw = Kg, gg.bh = (long long)g.Q * Kg, gg.bn = (long long)g.P * g.Q * Kg;
 	const size_t nx = (size_t)g.N * g.H * g.W * Cg, ny = (size_t)g.N * g.P * g.Q * Kg;
-	const size_t xb = (nx * es + 255) & ~(size_t)255, yb = (ny * es + 255) & ~(size_t)255;
-	// [contraction workspace | one group's activations | its results]: the fp32 data gradient's workspace, else the split-K scratch
-	const size_t inner = PASS == 2 && kind == 0 ? conv_dgrad_workspace_bytes(gg) : CONTRACT_SCRATCH_BYTES;
-	unsigned char* const ws = (unsigned char*)ccv_nnc_stream_context_get_workspace(stream_context, inner + xb + yb, CCV_TENSOR_GPU_MEMORY);
-	if (!ws)
+	p.xb = (nx * es + 255) & ~(size_t)255, p.yb = (ny * es + 255) & ~(size_t)255;
+	// the fp32 data gradient's workspace, else the split-K scratch
+	p.inner = pass == 2 && kind == 0 ? conv_dgrad_workspace_bytes(gg) : CONTRACT_SCRATCH_BYTES;
+	return true;
+}
+// returns 0 done, 1 not applicable (caller falls back), < 0 error; ws holds the group plan's bytes
+template <int PASS>
+int conv_grouped_tc(cudaStream_t s, unsigned char* const ws, const int kind, const ConvGeom& g, const int groups, const int x3, const int accumulate,
+	const void* const act, const void* const filt, const float* const bias32, const void* const bias16, const void* const res, void* const out)
+{
+	GroupPlan p;
+	if (!group_plan(g, kind, groups, PASS, p))
 		return 1;
+	const ConvGeom& gg = p.gg;
+	const int Cg = gg.C, Kg = gg.K;
+	const size_t es = kind_size(kind);
 	const Scratch scratch = scratch_at(ws, CONTRACT_SCRATCH_BYTES);
-	unsigned char* const xg = ws + inner;
-	unsigned char* const yg = xg + xb;
-	cudaStream_t s = stream_of(stream_context);
+	unsigned char* const xg = ws + p.inner;
+	unsigned char* const yg = xg + p.xb;
 	const int xd[4] = { g.N, g.H, g.W, Cg }, xs_t[4] = { (int)g.an, (int)g.ah, (int)g.aw, 1 }, xs_d[4] = { g.H * g.W * Cg, g.W * Cg, Cg, 1 };
 	const int yd[4] = { g.N, g.P, g.Q, Kg }, ys_t[4] = { (int)g.bn, (int)g.bh, (int)g.bw, 1 }, ys_d[4] = { g.P * g.Q * Kg, g.Q * Kg, Kg, 1 };
 	const size_t wstep = (size_t)Kg * g.R * g.S * Cg * es;
@@ -679,14 +719,14 @@ size_t dgrad16_fallback_bytes(const ConvGeom& gh)
 {
 	return ((size_t)gh.N * gh.P * gh.Q * gh.K + (size_t)gh.K * gh.R * gh.S * gh.C + (size_t)gh.N * gh.H * gh.W * gh.C + gh.C) * sizeof(float) + 1280;
 }
-int dgrad_nhwc(ccv_nnc_stream_context_t* const stream_context, const int kind, const int algo, const int groups, const ConvGeom& gh, const void* const gb, const void* const w, const float* const bias32, const void* const bias16, void* const h)
+// ws holds conv_workspace(gh, kind, groups, algo, CONV_DGRAD)
+int dgrad_nhwc(cudaStream_t s, unsigned char* const ws, const int kind, const int algo, const int groups, const ConvGeom& gh, const void* const gb, const void* const w, const float* const bias32, const void* const bias16, void* const h)
 {
-	cudaStream_t s = stream_of(stream_context);
 	if (kind > 0)
 	{
 		if (groups > 1)
-			return conv_grouped_tc<2>(stream_context, kind, gh, groups, 0, 0, 0, w, bias32, bias16, gb, h) == 0 ? CCV_NNC_EXEC_SUCCESS : CCV_NNC_EXEC_INVALID;
-		const int rc = conv_dgrad_16(s, kind, gh, gb, w, bias32, bias16, h, scratch_of(stream_context));
+			return conv_grouped_tc<2>(s, ws, kind, gh, groups, 0, 0, 0, w, bias32, bias16, gb, h) == 0 ? CCV_NNC_EXEC_SUCCESS : CCV_NNC_EXEC_INVALID;
+		const int rc = conv_dgrad_16(s, kind, gh, gb, w, bias32, bias16, h, scratch_at(ws, CONTRACT_SCRATCH_BYTES));
 		if (rc < 0)
 			return CCV_NNC_EXEC_INVALID;
 		if (rc > 0)
@@ -695,9 +735,7 @@ int dgrad_nhwc(ccv_nnc_stream_context_t* const stream_context, const int kind, c
 			const size_t ng = (size_t)gh.N * gh.P * gh.Q * gh.K, nw = (size_t)gh.K * gh.R * gh.S * gh.C, nh = (size_t)gh.N * gh.H * gh.W * gh.C, nb = bias16 ? gh.C : 0;
 			if (gh.bw != gh.K || gh.bh != (long long)gh.Q * gh.K || gh.bn != (long long)gh.P * gh.Q * gh.K || gh.aw != gh.C || gh.ah != (long long)gh.W * gh.C || gh.an != (long long)gh.H * gh.W * gh.C || ng > 0x7fffffffull || nh > 0x7fffffffull)
 				return CCV_NNC_EXEC_INVALID;
-			float* const g32 = (float*)ccv_nnc_stream_context_get_workspace(stream_context, dgrad16_fallback_bytes(gh), CCV_TENSOR_GPU_MEMORY);
-			if (!g32)
-				return CCV_NNC_EXEC_OOM;
+			float* const g32 = (float*)ws;
 			float* const w32 = (float*)(((uintptr_t)(g32 + ng) + 255) & ~(uintptr_t)255);
 			float* const h32 = (float*)(((uintptr_t)(w32 + nw) + 255) & ~(uintptr_t)255);
 			float* const b32 = (float*)(((uintptr_t)(h32 + nh) + 255) & ~(uintptr_t)255);
@@ -713,14 +751,9 @@ int dgrad_nhwc(ccv_nnc_stream_context_t* const stream_context, const int kind, c
 	const int x3 = algo == CCV_NNC_SM100_ALGO_3XTF32;
 	int rc = 1;
 	if (groups == 1 && algo != CCV_NNC_SM100_ALGO_FFMA)
-	{
-		void* const ws = ccv_nnc_stream_context_get_workspace(stream_context, conv_dgrad_workspace_bytes(gh), CCV_TENSOR_GPU_MEMORY);
-		if (!ws)
-			return CCV_NNC_EXEC_OOM;
 		rc = conv_dgrad_tf32(s, gh, (const float*)gb, (const float*)w, bias32, (float*)h, ws, x3);
-	}
 	if (groups > 1 && algo != CCV_NNC_SM100_ALGO_FFMA)
-		rc = conv_grouped_tc<2>(stream_context, 0, gh, groups, x3, 0, 0, w, bias32, 0, gb, h);
+		rc = conv_grouped_tc<2>(s, ws, 0, gh, groups, x3, 0, 0, w, bias32, 0, gb, h);
 	if (rc < 0)
 		return CCV_NNC_EXEC_INVALID;
 	if (rc > 0)
@@ -728,10 +761,73 @@ int dgrad_nhwc(ccv_nnc_stream_context_t* const stream_context, const int kind, c
 	return CCV_NNC_EXEC_SUCCESS;
 }
 
+// The workspace of the products `which` of a convolution on g: the most any path the shapes permit uses -- the split-K scratch or
+// the fp32 data gradient's workspace, the grouped [contraction | group activations | group results], im2col for unaligned channels,
+// the 16-bit functional data gradient where the tensor cores may decline.  The FFMA kernels use none, except the weight gradient's
+// split-K scratch.
+enum { CONV_FPROP = 1, CONV_WGRAD = 2, CONV_DGRAD = 4 };
+size_t conv_workspace(const ConvGeom& g, const int kind, const int groups, const int algo, const unsigned which)
+{
+	size_t need = 0;
+	GroupPlan gp;
+	for (int pass = 0; pass < 3; pass++)
+	{
+		if (!(which & (1u << pass)))
+			continue;
+		if (kind == 0 && algo == CCV_NNC_SM100_ALGO_FFMA)
+			need = std::max(need, pass == 1 ? CONTRACT_SCRATCH_BYTES : 0);
+		else if (groups > 1)
+			need = std::max(need, group_plan(g, kind, groups, pass, gp) ? gp.inner + gp.xb + gp.yb : kind == 0 && pass == 1 ? CONTRACT_SCRATCH_BYTES : 0);
+		else {
+			need = std::max(need, pass == 2 && kind == 0 ? conv_dgrad_workspace_bytes(g) : CONTRACT_SCRATCH_BYTES);
+			if (pass < 2 && g.C % (kind == 0 ? 4 : 8) != 0)
+				need = std::max(need, conv_im2col_workspace_bytes(g, kind));
+			if (pass == 2 && kind > 0 && conv_dgrad_may_decline(g, kind))
+				need = std::max(need, dgrad16_fallback_bytes(g));
+		}
+	}
+	return need;
+}
+inline int conv_groups(const ccv_nnc_cmd_t& cmd) { return cmd.info.convolution.groups > 0 ? cmd.info.convolution.groups : 1; }
+
+size_t conv_forw_workspace(const ccv_nnc_cmd_t& cmd, const ccv_nnc_hint_t& hint, ccv_nnc_tensor_t* const* const in, const int input_size, ccv_nnc_tensor_t* const* const out, const int output_size)
+{
+	ConvGeom g;
+	if (input_size < 2 || output_size < 1 || !in[0] || !in[1] || !out[0] || kind_of(in[0]) < 0 || !conv_geom(cmd, hint, view_of(in[0]), view_of(in[1]), view_of(out[0]), g))
+		return (size_t)-1;
+	return conv_workspace(g, kind_of(in[0]), conv_groups(cmd), conv_algorithm(cmd), CONV_FPROP);
+}
+
+// inputs (g, a, w), outputs (h, dw, dbias): the weight gradient and the column sum on the geometry of a, the data gradient on h's
+size_t conv_back_workspace(const ccv_nnc_cmd_t& cmd, const ccv_nnc_hint_t& hint, ccv_nnc_tensor_t* const* const in, const int input_size, ccv_nnc_tensor_t* const* const out, const int output_size)
+{
+	if (input_size < 2 || output_size < 1 || !in[0] || !in[1])
+		return (size_t)-1;
+	ccv_nnc_tensor_t* const h_t = out[0];
+	ccv_nnc_tensor_t* const dw_t = output_size > 1 ? out[1] : 0;
+	ccv_nnc_tensor_t* const w_t = input_size > 2 ? in[2] : 0;
+	ccv_nnc_tensor_t* const filt = dw_t ? dw_t : w_t;
+	const int kind = kind_of(in[0]), groups = conv_groups(cmd), algo = conv_algorithm(cmd);
+	ConvGeom g, gh;
+	if (!filt || kind < 0 || !conv_geom(cmd, hint, view_of(in[1]), view_of(filt), view_of(in[0]), g))
+		return (size_t)-1;
+	size_t need = conv_workspace(g, kind, groups, algo, dw_t ? CONV_WGRAD : 0);
+	if (output_size > 2 && out[2])
+		need = std::max(need, colsum_workspace_bytes(g.K));
+	if (h_t && w_t && conv_geom(cmd, hint, view_of(h_t), view_of(w_t), view_of(in[0]), gh))
+		need = std::max(need, conv_workspace(gh, kind, groups, algo, CONV_DGRAD));
+	return need;
+}
+
 int conv_forw_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
 {
-	if (input_size < 2 || output_size < 1 || !inputs[0] || !inputs[1] || !outputs[0])
+	const size_t ws_bytes = conv_forw_workspace(cmd, hint, inputs, input_size, outputs, output_size);
+	if (ws_bytes == (size_t)-1)
 		return CCV_NNC_EXEC_INVALID;
+	unsigned char* const ws = ws_bytes ? (unsigned char*)ccv_nnc_stream_context_get_workspace(stream_context, ws_bytes, CCV_TENSOR_GPU_MEMORY) : 0;
+	if (ws_bytes && !ws)
+		return CCV_NNC_EXEC_OOM;
+	const Scratch scratch = scratch_at(ws, CONTRACT_SCRATCH_BYTES);
 	const ccv_nnc_tensor_t* const bias_t = input_size > 2 ? inputs[2] : 0;
 	const int kind = kind_of(inputs[0]);
 	if (kind > 0)
@@ -746,15 +842,10 @@ int conv_forw_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 		const float* const bias32 = bias_t && is_f32(bias_t) ? bias_t->data.f32 : 0;
 		const void* const bias16 = bias_t && !is_f32(bias_t) ? (const void*)bias_t->data.u8 : 0;
 		if (cmd.info.convolution.groups > 1) // wide groups only: there is no 16-bit FFMA kernel to fall back to
-			return conv_grouped_tc<0>(stream_context, kind, g16, cmd.info.convolution.groups, 0, 0, inputs[0]->data.u8, inputs[1]->data.u8, bias32, bias16, 0, outputs[0]->data.u8) == 0 ? CCV_NNC_EXEC_SUCCESS : CCV_NNC_EXEC_INVALID;
-		int rc = conv_fprop_16(s16, kind, g16, inputs[0]->data.u8, inputs[1]->data.u8, bias32, bias16, outputs[0]->data.u8, scratch_of(stream_context));
-		if (rc > 0 && g16.C % 8 != 0)
-		{
-			// pixels that TMA cannot address (the 3-channel stem): explicit im2col + tensor-core GEMM
-			void* const ws = ccv_nnc_stream_context_get_workspace(stream_context, conv_im2col_workspace_bytes(g16, kind), CCV_TENSOR_GPU_MEMORY);
-			if (ws)
-				rc = conv_fprop_im2col_16(s16, kind, g16, inputs[0]->data.u8, inputs[1]->data.u8, bias32, bias16, outputs[0]->data.u8, ws);
-		}
+			return conv_grouped_tc<0>(s16, ws, kind, g16, cmd.info.convolution.groups, 0, 0, inputs[0]->data.u8, inputs[1]->data.u8, bias32, bias16, 0, outputs[0]->data.u8) == 0 ? CCV_NNC_EXEC_SUCCESS : CCV_NNC_EXEC_INVALID;
+		int rc = conv_fprop_16(s16, kind, g16, inputs[0]->data.u8, inputs[1]->data.u8, bias32, bias16, outputs[0]->data.u8, scratch);
+		if (rc > 0 && g16.C % 8 != 0) // pixels that TMA cannot address (the 3-channel stem): explicit im2col + tensor-core GEMM
+			rc = conv_fprop_im2col_16(s16, kind, g16, inputs[0]->data.u8, inputs[1]->data.u8, bias32, bias16, outputs[0]->data.u8, ws);
 		return rc == 0 ? CCV_NNC_EXEC_SUCCESS : CCV_NNC_EXEC_INVALID;
 	}
 	if (!is_f32(inputs[0]) || !is_f32(inputs[1]) || !is_f32(outputs[0]) || (bias_t && (!is_f32(bias_t) || CCV_IS_TENSOR_VIEW(bias_t))))
@@ -774,14 +865,9 @@ int conv_forw_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 		return CCV_NNC_EXEC_INVALID;
 	if (groups == 1 && algo != CCV_NNC_SM100_ALGO_FFMA)
 	{
-		int rc = conv_fprop_tf32(s, g, a, w, bias, b, scratch_of(stream_context), x3);
-		if (rc > 0 && g.C % 4 != 0)
-		{
-			// TMA cannot address 12-byte pixels (the 3-channel stem): explicit im2col + tensor-core GEMM
-			void* const ws = ccv_nnc_stream_context_get_workspace(stream_context, conv_im2col_workspace_bytes(g), CCV_TENSOR_GPU_MEMORY);
-			if (ws)
-				rc = conv_fprop_im2col_tf32(s, g, a, w, bias, b, ws, x3);
-		}
+		int rc = conv_fprop_tf32(s, g, a, w, bias, b, scratch, x3);
+		if (rc > 0 && g.C % 4 != 0) // TMA cannot address 12-byte pixels (the 3-channel stem): explicit im2col + tensor-core GEMM
+			rc = conv_fprop_im2col_tf32(s, g, a, w, bias, b, ws, x3);
 		if (rc == 0)
 			return CCV_NNC_EXEC_SUCCESS;
 		if (rc < 0)
@@ -789,7 +875,7 @@ int conv_forw_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 	}
 	if (groups > 1 && algo != CCV_NNC_SM100_ALGO_FFMA)
 	{
-		const int rc = conv_grouped_tc<0>(stream_context, 0, g, groups, x3, 0, a, w, bias, 0, 0, b);
+		const int rc = conv_grouped_tc<0>(s, ws, 0, g, groups, x3, 0, a, w, bias, 0, 0, b);
 		if (rc == 0)
 			return CCV_NNC_EXEC_SUCCESS;
 		if (rc < 0)
@@ -803,8 +889,13 @@ int conv_forw_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 // CCV_NNC_ACCUMULATE_OUTPUT, h is always overwritten (:286)
 int conv_back_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
 {
-	if (input_size < 2 || output_size < 1 || !inputs[0] || !inputs[1])
+	const size_t ws_bytes = conv_back_workspace(cmd, hint, inputs, input_size, outputs, output_size);
+	if (ws_bytes == (size_t)-1)
 		return CCV_NNC_EXEC_INVALID;
+	unsigned char* const ws = ws_bytes ? (unsigned char*)ccv_nnc_stream_context_get_workspace(stream_context, ws_bytes, CCV_TENSOR_GPU_MEMORY) : 0;
+	if (ws_bytes && !ws)
+		return CCV_NNC_EXEC_OOM;
+	const Scratch scratch = scratch_at(ws, CONTRACT_SCRATCH_BYTES);
 	ccv_nnc_tensor_t* const h_t = outputs[0];
 	ccv_nnc_tensor_t* const dw_t = output_size > 1 ? outputs[1] : 0;
 	ccv_nnc_tensor_t* const dbias_t = output_size > 2 ? outputs[2] : 0;
@@ -827,20 +918,16 @@ int conv_back_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 			const int db_kind = kind_of(dbias_t);
 			if (db_kind < 0 || dbias_t->info.dim[0] != g16.K || g16.bh != (long long)g16.Q * g16.bw || g16.bn != (long long)g16.P * g16.bh)
 				return CCV_NNC_EXEC_INVALID;
-			RC(colsum_any(s16, kind, inputs[0]->data.u8, (size_t)g16.N * g16.P * g16.Q, g16.K, g16.bw, dbias_t->data.u8, db_kind, acc16, ccv_nnc_stream_context_get_workspace(stream_context, colsum_workspace_bytes(g16.K), CCV_TENSOR_GPU_MEMORY)));
+			RC(colsum_any(s16, kind, inputs[0]->data.u8, (size_t)g16.N * g16.P * g16.Q, g16.K, g16.bw, dbias_t->data.u8, db_kind, acc16, ws));
 		}
 		if (dw_t && groups16 > 1)
 		{
-			if (conv_grouped_tc<1>(stream_context, kind, g16, groups16, 0, acc16, inputs[1]->data.u8, 0, 0, 0, inputs[0]->data.u8, dw_t->data.u8))
+			if (conv_grouped_tc<1>(s16, ws, kind, g16, groups16, 0, acc16, inputs[1]->data.u8, 0, 0, 0, inputs[0]->data.u8, dw_t->data.u8))
 				return CCV_NNC_EXEC_INVALID;
 		} else if (dw_t) {
-			int rc = conv_wgrad_16(s16, kind, g16, inputs[0]->data.u8, inputs[1]->data.u8, dw_t->data.u8, acc16, scratch_of(stream_context));
+			int rc = conv_wgrad_16(s16, kind, g16, inputs[0]->data.u8, inputs[1]->data.u8, dw_t->data.u8, acc16, scratch);
 			if (rc > 0 && g16.C % 8 != 0)
-			{
-				void* const ws = ccv_nnc_stream_context_get_workspace(stream_context, conv_im2col_workspace_bytes(g16, kind), CCV_TENSOR_GPU_MEMORY);
-				if (ws)
-					rc = conv_wgrad_im2col_16(s16, kind, g16, inputs[0]->data.u8, inputs[1]->data.u8, dw_t->data.u8, acc16, ws);
-			}
+				rc = conv_wgrad_im2col_16(s16, kind, g16, inputs[0]->data.u8, inputs[1]->data.u8, dw_t->data.u8, acc16, ws);
 			if (rc)
 				return CCV_NNC_EXEC_INVALID;
 		}
@@ -849,7 +936,7 @@ int conv_back_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 			ConvGeom gh16;
 			if (!w_t || !conv_geom(cmd, hint, view_of(h_t), view_of(w_t), view_of(inputs[0]), gh16))
 				return CCV_NNC_EXEC_INVALID;
-			return dgrad_nhwc(stream_context, kind, CCV_NNC_SM100_ALGO_TF32, groups16, gh16, inputs[0]->data.u8, w_t->data.u8, 0, 0, h_t->data.u8);
+			return dgrad_nhwc(s16, ws, kind, CCV_NNC_SM100_ALGO_TF32, groups16, gh16, inputs[0]->data.u8, w_t->data.u8, 0, 0, h_t->data.u8);
 		}
 		return CCV_NNC_EXEC_SUCCESS;
 	}
@@ -868,27 +955,23 @@ int conv_back_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 	{
 		if (dbias_t->info.dim[0] != g.K || g.bh != (long long)g.Q * g.bw || g.bn != (long long)g.P * g.bh)
 			return CCV_NNC_EXEC_INVALID;
-		RC(colsum_f32(s, gb, (size_t)g.N * g.P * g.Q, g.K, g.bw, dbias_t->data.f32, accumulate, ccv_nnc_stream_context_get_workspace(stream_context, colsum_workspace_bytes(g.K), CCV_TENSOR_GPU_MEMORY)));
+		RC(colsum_f32(s, gb, (size_t)g.N * g.P * g.Q, g.K, g.bw, dbias_t->data.f32, accumulate, ws));
 	}
 	if (dw_t)
 	{
 		int rc = 1;
 		if (groups == 1 && algo != CCV_NNC_SM100_ALGO_FFMA)
 		{
-			rc = conv_wgrad_tf32(s, g, gb, a, dw_t->data.f32, accumulate, scratch_of(stream_context), x3);
+			rc = conv_wgrad_tf32(s, g, gb, a, dw_t->data.f32, accumulate, scratch, x3);
 			if (rc > 0 && g.C % 4 != 0)
-			{
-				void* const ws = ccv_nnc_stream_context_get_workspace(stream_context, conv_im2col_workspace_bytes(g), CCV_TENSOR_GPU_MEMORY);
-				if (ws)
-					rc = conv_wgrad_im2col_tf32(s, g, gb, a, dw_t->data.f32, accumulate, ws, x3);
-			}
+				rc = conv_wgrad_im2col_tf32(s, g, gb, a, dw_t->data.f32, accumulate, ws, x3);
 		}
 		if (groups > 1 && algo != CCV_NNC_SM100_ALGO_FFMA)
-			rc = conv_grouped_tc<1>(stream_context, 0, g, groups, x3, accumulate, a, 0, 0, 0, gb, dw_t->data.f32);
+			rc = conv_grouped_tc<1>(s, ws, 0, g, groups, x3, accumulate, a, 0, 0, 0, gb, dw_t->data.f32);
 		if (rc < 0)
 			return CCV_NNC_EXEC_INVALID;
 		if (rc > 0)
-			RC(conv_wgrad_ffma(s, g, groups, gb, a, dw_t->data.f32, accumulate, scratch_of(stream_context)));
+			RC(conv_wgrad_ffma(s, g, groups, gb, a, dw_t->data.f32, accumulate, scratch));
 	}
 	if (h_t)
 	{
@@ -897,198 +980,222 @@ int conv_back_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 		ConvGeom gh;
 		if (!conv_geom(cmd, hint, view_of(h_t), view_of(w_t), view_of(inputs[0]), gh))
 			return CCV_NNC_EXEC_INVALID;
-		return dgrad_nhwc(stream_context, 0, algo, groups, gh, gb, w_t->data.f32, 0, 0, h_t->data.f32);
+		return dgrad_nhwc(s, ws, 0, algo, groups, gh, gb, w_t->data.f32, 0, 0, h_t->data.f32);
 	}
 	return CCV_NNC_EXEC_SUCCESS;
 }
 
-// ------------------------------------------------------------------------------------------------ NCHW / mixed formats
-// The kernels are NHWC.  The reference's GPU convolution takes any mix of formats -- its tests run NHWC activations against NCHW
-// filters and all-NCHW forward and backward (convolution/gpu/ccv_nnc_conv_gpu_cudnn.cu:204-357; test/int/nnc/cudnn.tests.c:24-85,
-// 87-140, 417-497) -- so every NCHW operand is re-laid out into the stream workspace (one strided copy each way), the NHWC
-// command runs on shadow tensors, and NCHW results are copied back.  The workspace is one grow-only buffer per stream: this
-// layer asks for [inner | staging] in ONE request, `inner` being the most the NHWC command will ask for, so that the nested
-// requests (smaller) return the same base and never move the staged tensors.
-struct Staged {
-	ccv_nnc_tensor_t shadow;
-	ccv_nnc_tensor_t* orig;
-	int d[4], src[4], dst[4]; // index space N, H, W, C with the NCHW and the NHWC strides
-	size_t bytes;
-	int elem;
-};
+// ------------------------------------------------------------------------------------------------ staged operands
+// Some operands reach a command in a form its kernels do not take.  The command then runs in its dense form on shadow copies in
+// the stream workspace, and results are copied back:
+//   - STAGE_NCHW: the convolution, transposed convolution and pooling kernels are NHWC.  The reference's GPU convolution takes any
+//     mix of formats -- its tests run NHWC activations against NCHW filters and all-NCHW forward and backward
+//     (convolution/gpu/ccv_nnc_conv_gpu_cudnn.cu:204-357; test/int/nnc/cudnn.tests.c:24-85, 87-140, 417-497), and so do its pools
+//     (pool/gpu/ccv_nnc_max_pool_gpu_cudnn.cu; test/int/nnc/cudnn.tests.c:2772-2870) -- so every NCHW operand is re-laid out (one
+//     strided copy each way).  Outputs that accumulate are staged in as well.
+//   - STAGE_F32: the commands with fp32 kernels only take bf16 / fp16 tensors in their functional form (widen every 16-bit tensor,
+//     round every 16-bit result once, to nearest even).  Aliased 16-bit tensors share one shadow.
+//   - STAGE_QX: a palettized weight (CCV_QX) is decoded, so the result is the dense command's, bit for bit.
+// The workspace is one grow-only buffer per stream, and growing it frees the old one.  So the layer makes one request,
+// [inner | staging], `inner` being the wrapped command's workspace function on the shadows: the command's own request is then
+// the same size or smaller and returns the same base.  Layers compose (a palettized filter of an NCHW convolution): a layer's own
+// workspace function is inner(shadows) + staging.
+enum { STAGE_NCHW, STAGE_F32, STAGE_QX };
 
 inline bool is_nchw(const ccv_nnc_tensor_t* const t) { return t && t->info.format == CCV_TENSOR_FORMAT_NCHW && tensor_nd(t->info.dim) >= 3; }
-
-bool stage_plan(ccv_nnc_tensor_t* const t, Staged& st)
+inline bool is_qx(const ccv_nnc_tensor_t* const t) { return t && CCV_GET_DATA_TYPE(t->info.datatype) == CCV_QX; }
+inline int qx_palette(const ccv_nnc_tensor_t* const t) { return (t->info.datatype & 0xff) << 12; }
+inline int qx_bits(const ccv_nnc_tensor_t* const t) { return (t->info.datatype >> 8) & 0xf; }
+// a palettized operand the decoder takes, with a palette of the command's dense type: not a view, qbits 4..8, whole index bytes per
+// block, fp16 / fp32 palettes
+bool qx_ok(const ccv_nnc_tensor_t* const t, const int dense)
 {
+	const int pal = qx_palette(t);
+	return !CCV_IS_TENSOR_VIEW(t) && palettize_params_ok(qx_bits(t), t->info.reserved) && (pal == CCV_16F || pal == CCV_32F) && pal == dense;
+}
+inline int qx_decode(cudaStream_t s, const ccv_nnc_tensor_t* const t, void* const out)
+{
+	return depalettize(s, t->data.u8, qx_palette(t), qx_bits(t), t->info.reserved, out, view_of(t).count);
+}
+
+struct Shadow {
+	ccv_nnc_tensor_t t; // what the wrapped command sees
+	ccv_nnc_tensor_t* orig;
+	size_t bytes;
+	int in, out; // filled before the command runs / copied back after it
+	int d[4], src[4], dst[4], elem; // STAGE_NCHW: index space N, H, W, C with the NCHW and the NHWC strides
+};
+struct StagePlan {
+	enum { MAXT = 16 };
+	Shadow sh[2 * MAXT];
+	int n;
+	size_t staging;
+	ccv_nnc_tensor_t* in[MAXT];
+	ccv_nnc_tensor_t* out[MAXT];
+};
+
+inline bool is_staged(const int transform, const ccv_nnc_tensor_t* const t)
+{
+	return t && (transform == STAGE_NCHW ? is_nchw(t) : transform == STAGE_F32 ? kind_of(t) > 0 : is_qx(t));
+}
+
+// the shadow of one operand, t itself when the transform leaves it alone, NULL when the call is refused
+ccv_nnc_tensor_t* stage_operand(StagePlan& p, const int transform, ccv_nnc_tensor_t* const t, const int is_out, const int stage_in, const int dense)
+{
+	if (!is_staged(transform, t))
+		return t;
+	if (transform == STAGE_F32)
+		for (int j = 0; j < p.n; j++)
+			if (p.sh[j].orig == t || p.sh[j].orig->data.u8 == t->data.u8)
+			{
+				p.sh[j].out |= is_out;
+				return &p.sh[j].t;
+			}
 	const TV v = view_of(t);
-	const size_t elem = dtype_size(t->info.datatype);
-	if (!v.contiguous || (v.nd != 3 && v.nd != 4) || elem == 0)
+	Shadow& x = p.sh[p.n];
+	memcpy(&x.t, t, sizeof(ccv_nnc_tensor_t));
+	x.t.type &= ~CCV_TENSOR_VIEW;
+	x.orig = t, x.in = stage_in, x.out = is_out;
+	size_t elem;
+	if (transform == STAGE_NCHW)
+	{
+		elem = dtype_size(t->info.datatype);
+		if (!v.contiguous || (v.nd != 3 && v.nd != 4) || elem == 0)
+			return 0;
+		const int N = v.nd == 4 ? v.dim[0] : 1, C = v.dim[v.nd - 3], H = v.dim[v.nd - 2], W = v.dim[v.nd - 1];
+		const int d[4] = { N, H, W, C }, src[4] = { C * H * W, W, 1, H * W }, dst[4] = { H * W * C, W * C, C, 1 };
+		memcpy(x.d, d, sizeof(d)), memcpy(x.src, src, sizeof(src)), memcpy(x.dst, dst, sizeof(dst));
+		x.elem = (int)elem;
+		x.t.info.format = CCV_TENSOR_FORMAT_NHWC;
+		memset(x.t.info.dim, 0, sizeof(x.t.info.dim));
+		if (v.nd == 4)
+			x.t.info.dim[0] = N, x.t.info.dim[1] = H, x.t.info.dim[2] = W, x.t.info.dim[3] = C;
+		else
+			x.t.info.dim[0] = H, x.t.info.dim[1] = W, x.t.info.dim[2] = C;
+	} else if (transform == STAGE_F32) {
+		if (!v.contiguous || v.count > 0x7fffffffull)
+			return 0;
+		elem = sizeof(float);
+		x.t.info.datatype = CCV_32F;
+		x.in = 1; // an output may be read by the command too (in-place forms)
+	} else {
+		if (is_out || !qx_ok(t, dense))
+			return 0;
+		const int pal = qx_palette(t);
+		elem = dtype_size(pal);
+		x.t.info.datatype = pal;
+		x.t.info.reserved = 0;
+		x.t.type = (x.t.type & ~0xFF000) | pal;
+		x.t.data_size = 0;
+	}
+	x.bytes = (v.count * elem + 255) & ~(size_t)255;
+	p.staging += x.bytes;
+	p.n++;
+	return &x.t;
+}
+
+// `select`: STAGE_NCHW, non-zero when outputs[1..] accumulate under CCV_NNC_ACCUMULATE_OUTPUT; STAGE_QX, bit i set when inputs[i]
+// may be palettized.  false: the call is refused (outputs untouched).  p.n == 0: nothing to stage, the command runs on the
+// caller's operands, whatever their number.
+bool stage_plan(const int transform, const unsigned select, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, StagePlan& p)
+{
+	p.n = 0, p.staging = 0;
+	bool any = false;
+	for (int i = 0; i < input_size; i++)
+		any = any || is_staged(transform, inputs[i]);
+	for (int i = 0; i < output_size; i++)
+		any = any || is_staged(transform, outputs[i]);
+	if (!any)
+		return true;
+	if (input_size > StagePlan::MAXT || output_size > StagePlan::MAXT || (transform == STAGE_NCHW && (input_size > 3 || output_size > 3)))
 		return false;
-	const int N = v.nd == 4 ? v.dim[0] : 1, C = v.dim[v.nd - 3], H = v.dim[v.nd - 2], W = v.dim[v.nd - 1];
-	const int d[4] = { N, H, W, C }, src[4] = { C * H * W, W, 1, H * W }, dst[4] = { H * W * C, W * C, C, 1 };
-	memcpy(st.d, d, sizeof(d)), memcpy(st.src, src, sizeof(src)), memcpy(st.dst, dst, sizeof(dst));
-	st.orig = t;
-	st.elem = (int)elem;
-	st.bytes = (v.count * elem + 255) & ~(size_t)255;
-	memcpy(&st.shadow, t, sizeof(ccv_nnc_tensor_t));
-	st.shadow.type &= ~CCV_TENSOR_VIEW;
-	st.shadow.info.format = CCV_TENSOR_FORMAT_NHWC;
-	memset(st.shadow.info.dim, 0, sizeof(st.shadow.info.dim));
-	if (v.nd == 4)
-		st.shadow.info.dim[0] = N, st.shadow.info.dim[1] = H, st.shadow.info.dim[2] = W, st.shadow.info.dim[3] = C;
-	else
-		st.shadow.info.dim[0] = H, st.shadow.info.dim[1] = W, st.shadow.info.dim[2] = C;
+	int dense = 0; // the type of the command's other tensors, which a palette must have
+	for (int i = 0; i < output_size && !dense; i++)
+		if (outputs[i])
+			dense = CCV_GET_DATA_TYPE(outputs[i]->info.datatype);
+	for (int i = 0; i < input_size && !dense; i++)
+		if (inputs[i] && !is_qx(inputs[i]))
+			dense = CCV_GET_DATA_TYPE(inputs[i]->info.datatype);
+	for (int i = 0; i < input_size; i++)
+		if ((transform == STAGE_QX && is_qx(inputs[i]) && !(select & (1u << i))) || (!(p.in[i] = stage_operand(p, transform, inputs[i], 0, 1, dense)) && inputs[i]))
+			return false;
+	const int accumulating = transform == STAGE_NCHW && select && (flags & CCV_NNC_ACCUMULATE_OUTPUT);
+	for (int i = 0; i < output_size; i++)
+		if (!(p.out[i] = stage_operand(p, transform, outputs[i], 1, accumulating && i > 0, dense)) && outputs[i])
+			return false;
 	return true;
 }
 
-// upper bound of what the NHWC command requests from the workspace for this geometry
-size_t conv_inner_workspace(const ConvGeom& g, const int kind, const int groups)
+// one operand into its shadow, or (!in) the shadow's result back
+int stage(cudaStream_t s, const int transform, const Shadow& x, const int in)
 {
-	// the fp32 data gradient asks for its own workspace, which includes the split-K scratch
-	size_t need = kind == 0 ? conv_dgrad_workspace_bytes(g) : CONTRACT_SCRATCH_BYTES;
-	if (groups > 1 && g.C % groups == 0 && g.K % groups == 0)
-	{
-		// conv_grouped_tc: contraction workspace of one group + its dense activations and results
-		ConvGeom gg = g;
-		gg.C /= groups, gg.K /= groups;
-		const size_t es = kind_size(kind), nx = (size_t)g.N * g.H * g.W * gg.C, ny = (size_t)g.N * g.P * g.Q * gg.K;
-		need = (kind == 0 ? conv_dgrad_workspace_bytes(gg) : CONTRACT_SCRATCH_BYTES) + ((nx * es + 255) & ~(size_t)255) + ((ny * es + 255) & ~(size_t)255);
-	}
-	if (g.C % (kind == 0 ? 4 : 8) != 0)
-		need = std::max(need, kind == 0 ? conv_im2col_workspace_bytes(g) : conv_im2col_workspace_bytes(g, kind));
-	need = std::max(need, colsum_workspace_bytes(g.K));
-	return (need + 255) & ~(size_t)255;
+	const ccv_nnc_tensor_t* const t = x.orig;
+	const size_t n = view_of(t).count;
+	if (transform == STAGE_NCHW)
+		return in ? copy_strided(s, t->data.u8, x.src, x.t.data.u8, x.dst, x.d, x.elem) : copy_strided(s, x.t.data.u8, x.dst, t->data.u8, x.src, x.d, x.elem);
+	if (transform == STAGE_F32)
+		return in ? widen_matrix(s, t->data.u8, kind_of(t), (long long)n, 1, x.t.data.f32, 1, (int)n) : narrow_matrix(s, x.t.data.f32, t->data.u8, kind_of(t), (long long)n, 1, 1, (int)n, 0);
+	return qx_decode(s, t, x.t.data.u8);
 }
 
-// `exec` = the NHWC command, `inner_of` = the most it requests from the workspace given the shadow tensor lists; `accumulating`
-// = outputs[1..] may be read before they are written (CCV_NNC_ACCUMULATE_OUTPUT), so they are staged in as well
-typedef size_t (*staged_inner_f)(const ccv_nnc_cmd_t& cmd, const ccv_nnc_hint_t& hint, ccv_nnc_tensor_t* const* in, int input_size, ccv_nnc_tensor_t* const* out, int output_size);
-int nchw_staged(const ccv_nnc_cmd_exec_f exec, const staged_inner_f inner_of, const int accumulating, const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
+// `exec` runs on the shadows, `inner_of` is its workspace function
+int staged(const int transform, const unsigned select, const ccv_nnc_cmd_exec_f exec, const staged_inner_f inner_of, const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
 {
-	enum { MAXT = 6 };
-	if (input_size > 3 || output_size > 3)
+	StagePlan p;
+	if (!stage_plan(transform, select, flags, inputs, input_size, outputs, output_size, p))
 		return CCV_NNC_EXEC_INVALID;
-	Staged st[MAXT];
-	ccv_nnc_tensor_t* in[3] = { 0, 0, 0 };
-	ccv_nnc_tensor_t* out[3] = { 0, 0, 0 };
-	int n = 0, slot_in[3] = { -1, -1, -1 }, slot_out[3] = { -1, -1, -1 };
-	size_t staging = 0;
-	for (int i = 0; i < input_size; i++)
-	{
-		in[i] = inputs[i];
-		if (is_nchw(inputs[i]))
-		{
-			if (!stage_plan(inputs[i], st[n]))
-				return CCV_NNC_EXEC_INVALID;
-			staging += st[n].bytes, slot_in[i] = n++;
-		}
-	}
-	for (int i = 0; i < output_size; i++)
-	{
-		out[i] = outputs[i];
-		if (is_nchw(outputs[i]))
-		{
-			if (!stage_plan(outputs[i], st[n]))
-				return CCV_NNC_EXEC_INVALID;
-			staging += st[n].bytes, slot_out[i] = n++;
-		}
-	}
-	for (int i = 0; i < 3; i++)
-	{
-		if (slot_in[i] >= 0)
-			in[i] = &st[slot_in[i]].shadow;
-		if (slot_out[i] >= 0)
-			out[i] = &st[slot_out[i]].shadow;
-	}
-	const size_t inner = inner_of(cmd, hint, in, input_size, out, output_size);
+	if (!p.n)
+		return exec(cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
+	const size_t inner = inner_of(cmd, hint, p.in, input_size, p.out, output_size);
 	if (inner == (size_t)-1)
 		return CCV_NNC_EXEC_INVALID;
-	unsigned char* const ws = (unsigned char*)ccv_nnc_stream_context_get_workspace(stream_context, inner + staging, CCV_TENSOR_GPU_MEMORY);
+	const size_t at = (inner + 255) & ~(size_t)255;
+	unsigned char* const ws = (unsigned char*)ccv_nnc_stream_context_get_workspace(stream_context, at + p.staging, CCV_TENSOR_GPU_MEMORY);
 	if (!ws)
 		return CCV_NNC_EXEC_OOM;
 	cudaStream_t s = stream_of(stream_context);
-	unsigned char* p = ws + inner;
-	for (int i = 0; i < n; i++)
-		st[i].shadow.data.u8 = p, p += st[i].bytes;
-	// operands in; outputs that accumulate come in too
-	for (int i = 0; i < 3; i++)
-		if (slot_in[i] >= 0)
-		{
-			const Staged& t = st[slot_in[i]];
-			RC(copy_strided(s, t.orig->data.u8, t.src, t.shadow.data.u8, t.dst, t.d, t.elem));
-		}
-	if (accumulating && (flags & CCV_NNC_ACCUMULATE_OUTPUT))
-		for (int i = 1; i < 3; i++)
-			if (slot_out[i] >= 0)
-			{
-				const Staged& t = st[slot_out[i]];
-				RC(copy_strided(s, t.orig->data.u8, t.src, t.shadow.data.u8, t.dst, t.d, t.elem));
-			}
-	const int rc = exec(cmd, hint, flags, in, input_size, out, output_size, stream_context);
+	unsigned char* q = ws + at;
+	for (int j = 0; j < p.n; j++)
+		p.sh[j].t.data.u8 = q, q += p.sh[j].bytes;
+	for (int j = 0; j < p.n; j++)
+		if (p.sh[j].in)
+			RC(stage(s, transform, p.sh[j], 1));
+	const int rc = exec(cmd, hint, flags, p.in, input_size, p.out, output_size, stream_context);
 	if (rc != CCV_NNC_EXEC_SUCCESS)
 		return rc;
 	if (ccv_nnc_stream_context_get_workspace(stream_context, 1, CCV_TENSOR_GPU_MEMORY) != (void*)ws)
 	{
-		// the NHWC command asked for more than `inner`: the workspace moved and the staged tensors with it (a bound above is wrong)
-		set_last_error("staged convolution / pooling: workspace moved under the staged tensors", cudaErrorInvalidValue);
+		// the wrapped command asked for more than its workspace function said: the staged tensors moved with the workspace
+		set_last_error("staged operands: the workspace moved under them", cudaErrorInvalidValue);
 		return CCV_NNC_EXEC_INVALID;
 	}
-	for (int i = 0; i < 3; i++)
-		if (slot_out[i] >= 0)
-		{
-			const Staged& t = st[slot_out[i]];
-			RC(copy_strided(s, t.shadow.data.u8, t.dst, t.orig->data.u8, t.src, t.d, t.elem));
-		}
+	for (int j = 0; j < p.n; j++)
+		if (p.sh[j].out)
+			RC(stage(s, transform, p.sh[j], 0));
 	return CCV_NNC_EXEC_SUCCESS;
 }
 
-template <int BACKWARD>
-size_t conv_staged_inner(const ccv_nnc_cmd_t& cmd, const ccv_nnc_hint_t& hint, ccv_nnc_tensor_t* const* const in, const int input_size, ccv_nnc_tensor_t* const* const out, const int output_size)
+size_t staged_workspace(const int transform, const unsigned select, const staged_inner_f inner_of, const ccv_nnc_cmd_t& cmd, const ccv_nnc_hint_t& hint, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size)
 {
-	// geometry on the shadows: activations, filter, output of the forward convolution
-	ccv_nnc_tensor_t* const act = BACKWARD ? in[1] : in[0];
-	ccv_nnc_tensor_t* const filt = BACKWARD ? (output_size > 1 && out[1] ? out[1] : (input_size > 2 ? in[2] : 0)) : in[1];
-	ccv_nnc_tensor_t* const res = BACKWARD ? in[0] : out[0];
-	ConvGeom g;
-	if (!act || !filt || !res || kind_of(act) < 0 || !conv_geom(cmd, hint, view_of(act), view_of(filt), view_of(res), g))
+	StagePlan p;
+	if (!stage_plan(transform, select, 0, inputs, input_size, outputs, output_size, p))
 		return (size_t)-1;
-	const int kind = kind_of(act), groups = cmd.info.convolution.groups > 1 ? cmd.info.convolution.groups : 1;
-	size_t need = conv_inner_workspace(g, kind, groups);
-	// a 16-bit data gradient the tensor cores decline runs in the functional form (dgrad_nhwc)
-	if (BACKWARD && output_size > 0 && out[0] && kind > 0 && groups == 1 && conv_dgrad_may_decline(g, kind))
-		need = std::max(need, (dgrad16_fallback_bytes(g) + 255) & ~(size_t)255);
-	return need;
-}
-template <int BACKWARD>
-int conv_staged(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
-{
-	return nchw_staged(BACKWARD ? conv_back_nhwc : conv_forw_nhwc, conv_staged_inner<BACKWARD>, BACKWARD, cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
+	if (!p.n)
+		return inner_of(cmd, hint, inputs, input_size, outputs, output_size);
+	const size_t inner = inner_of(cmd, hint, p.in, input_size, p.out, output_size);
+	return inner == (size_t)-1 ? inner : ((inner + 255) & ~(size_t)255) + p.staging;
 }
 
-inline bool any_nchw(ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size)
+// the NHWC command EXEC (workspace function WS) on any mix of formats; ACCUMULATING: outputs[1..] may be read before written
+template <ccv_nnc_cmd_exec_f EXEC, staged_inner_f WS, int ACCUMULATING>
+int exec_nchw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
 {
-	for (int i = 0; i < input_size; i++)
-		if (is_nchw(inputs[i]))
-			return true;
-	for (int i = 0; i < output_size; i++)
-		if (is_nchw(outputs[i]))
-			return true;
-	return false;
+	return staged(STAGE_NCHW, ACCUMULATING, EXEC, WS, cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
 }
-
-int exec_conv_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
+template <staged_inner_f WS>
+size_t nchw_workspace(const ccv_nnc_cmd_t& cmd, const ccv_nnc_hint_t& hint, ccv_nnc_tensor_t* const* const in, const int input_size, ccv_nnc_tensor_t* const* const out, const int output_size)
 {
-	if (any_nchw(inputs, input_size, outputs, output_size))
-		return conv_staged<0>(cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
-	return conv_forw_nhwc(cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
-}
-
-int exec_conv_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
-{
-	if (any_nchw(inputs, input_size, outputs, output_size))
-		return conv_staged<1>(cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
-	return conv_back_nhwc(cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
+	return staged_workspace(STAGE_NCHW, 0, WS, cmd, hint, in, input_size, out, output_size);
 }
 
 // ================================================================================================ CONVOLUTION_TRANSPOSE
@@ -1116,6 +1223,36 @@ bool conv_transpose_geom(const ccv_nnc_cmd_t& cmd, const ccv_nnc_hint_t& hint, c
 	return conv_mirror(cmd, w, CCV_NNC_CONVOLUTION_BACKWARD, mirror) && conv_geom(mirror, hint, big, w, small, g);
 }
 
+// workspace functions: the mirrored convolution's data gradient; for the backward its forward (da), weight gradient (dw) and the
+// column sum over Cout (dbias)
+size_t conv_transpose_forw_workspace(const ccv_nnc_cmd_t& cmd, const ccv_nnc_hint_t& hint, ccv_nnc_tensor_t* const* const in, const int input_size, ccv_nnc_tensor_t* const* const out, const int output_size)
+{
+	ConvGeom g;
+	if (input_size < 2 || output_size < 1 || !in[0] || !in[1] || !out[0] || kind_of(in[0]) < 0 || !conv_transpose_geom(cmd, hint, view_of(out[0]), view_of(in[1]), view_of(in[0]), g))
+		return (size_t)-1;
+	return conv_workspace(g, kind_of(in[0]), conv_groups(cmd), conv_algorithm(cmd), CONV_DGRAD);
+}
+size_t conv_transpose_back_workspace(const ccv_nnc_cmd_t& cmd, const ccv_nnc_hint_t& hint, ccv_nnc_tensor_t* const* const in, const int input_size, ccv_nnc_tensor_t* const* const out, const int output_size)
+{
+	ccv_nnc_tensor_t* const g_t = input_size > 0 ? in[0] : 0;
+	ccv_nnc_tensor_t* const a_t = input_size > 1 ? in[1] : 0;
+	ccv_nnc_tensor_t* const w_t = input_size > 2 ? in[2] : 0;
+	ccv_nnc_tensor_t* const da_t = output_size > 0 ? out[0] : 0;
+	ccv_nnc_tensor_t* const dw_t = output_size > 1 ? out[1] : 0;
+	ccv_nnc_tensor_t* const filt = dw_t ? dw_t : w_t;
+	ccv_nnc_tensor_t* const small = a_t ? a_t : da_t;
+	const int kind = g_t ? kind_of(g_t) : -1, groups = conv_groups(cmd), algo = conv_algorithm(cmd);
+	ConvGeom g;
+	if (kind < 0 || !filt || !small || !conv_transpose_geom(cmd, hint, view_of(g_t), view_of(filt), view_of(small), g))
+		return (size_t)-1;
+	size_t need = output_size > 2 && out[2] ? colsum_workspace_bytes(g.C) : 0;
+	if (da_t && w_t && conv_transpose_geom(cmd, hint, view_of(g_t), view_of(w_t), view_of(da_t), g))
+		need = std::max(need, conv_workspace(g, kind, groups, algo, CONV_FPROP));
+	if (dw_t && a_t && conv_transpose_geom(cmd, hint, view_of(g_t), view_of(dw_t), view_of(a_t), g))
+		need = std::max(need, conv_workspace(g, kind, groups, algo, CONV_WGRAD));
+	return need;
+}
+
 // inputs (a, w, bias?), output y (always overwritten)
 int conv_transpose_forw_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
 {
@@ -1128,10 +1265,13 @@ int conv_transpose_forw_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint,
 	ConvGeom g;
 	if (!conv_transpose_geom(cmd, hint, view_of(outputs[0]), view_of(inputs[1]), view_of(inputs[0]), g) || (bias_t && bias_t->info.dim[0] != g.C))
 		return CCV_NNC_EXEC_INVALID;
-	const int groups = cmd.info.convolution_transpose.groups > 0 ? cmd.info.convolution_transpose.groups : 1;
+	const size_t ws_bytes = conv_transpose_forw_workspace(cmd, hint, inputs, input_size, outputs, output_size);
+	unsigned char* const ws = ws_bytes ? (unsigned char*)ccv_nnc_stream_context_get_workspace(stream_context, ws_bytes, CCV_TENSOR_GPU_MEMORY) : 0;
+	if (ws_bytes && !ws)
+		return CCV_NNC_EXEC_OOM;
 	const float* const bias32 = bias_t && is_f32(bias_t) ? bias_t->data.f32 : 0;
 	const void* const bias16 = bias_t && !is_f32(bias_t) ? (const void*)bias_t->data.u8 : 0;
-	return dgrad_nhwc(stream_context, kind, conv_algorithm(cmd), groups, g, inputs[0]->data.u8, inputs[1]->data.u8, bias32, bias16, outputs[0]->data.u8);
+	return dgrad_nhwc(stream_of(stream_context), ws, kind, conv_algorithm(cmd), conv_groups(cmd), g, inputs[0]->data.u8, inputs[1]->data.u8, bias32, bias16, outputs[0]->data.u8);
 }
 
 // inputs (g, a, w), outputs (da, dw, dbias), any output may be NULL; dw / dbias honour CCV_NNC_ACCUMULATE_OUTPUT, da is overwritten
@@ -1152,7 +1292,7 @@ int conv_transpose_back_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint,
 	if (!conv_transpose_geom(cmd, hint, view_of(g_t), view_of(filt), view_of(small), g))
 		return CCV_NNC_EXEC_INVALID;
 	// every operand is checked before the first launch: a refused call leaves the outputs as they were
-	const int groups = cmd.info.convolution_transpose.groups > 0 ? cmd.info.convolution_transpose.groups : 1;
+	const int groups = conv_groups(cmd);
 	if ((a_t && kind_of(a_t) != kind) || (w_t && kind_of(w_t) != kind) || (da_t && kind_of(da_t) != kind) || (dw_t && kind_of(dw_t) != kind))
 		return CCV_NNC_EXEC_INVALID;
 	if ((dw_t && !conv_transpose_geom(cmd, hint, view_of(g_t), view_of(dw_t), view_of(a_t), gchk)) || (da_t && !conv_transpose_geom(cmd, hint, view_of(g_t), view_of(w_t), view_of(da_t), gchk)))
@@ -1163,6 +1303,11 @@ int conv_transpose_back_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint,
 	const int db_kind = dbias_t ? kind_of(dbias_t) : 0;
 	if (dbias_t && (db_kind < 0 || (kind == 0 && db_kind != 0) || dbias_t->info.dim[0] != g.C || g.ah != (long long)g.W * g.aw || g.an != (long long)g.H * g.ah))
 		return CCV_NNC_EXEC_INVALID;
+	// one request for the whole call: the mirrored commands below then get the same buffer
+	const size_t ws_bytes = conv_transpose_back_workspace(cmd, hint, inputs, input_size, outputs, output_size);
+	void* const ws = ws_bytes ? ccv_nnc_stream_context_get_workspace(stream_context, ws_bytes, CCV_TENSOR_GPU_MEMORY) : 0;
+	if (ws_bytes && !ws)
+		return CCV_NNC_EXEC_OOM;
 	if (da_t)
 	{
 		// da = conv(g, w), the mirrored convolution's forward
@@ -1190,7 +1335,6 @@ int conv_transpose_back_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint,
 		// dbias[c] (+)= sum over the pixels of g, which are the mirrored convolution's input pixels
 		const int accumulate = (flags & CCV_NNC_ACCUMULATE_OUTPUT) ? 1 : 0;
 		cudaStream_t s = stream_of(stream_context);
-		void* const ws = ccv_nnc_stream_context_get_workspace(stream_context, colsum_workspace_bytes(g.C), CCV_TENSOR_GPU_MEMORY);
 		if (kind == 0)
 			RC(colsum_f32(s, g_t->data.f32, (size_t)g.N * g.H * g.W, g.C, g.aw, dbias_t->data.f32, accumulate, ws));
 		else
@@ -1198,41 +1342,6 @@ int conv_transpose_back_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint,
 	}
 	return CCV_NNC_EXEC_SUCCESS;
 }
-
-// NCHW: staged like the convolution (filters [Cin, Cout / groups, R, S] become [Cin, R, S, Cout / groups]).  The bound covers every
-// path above on the mirrored geometry: its data gradient, forward and weight gradient, the 16-bit functional form whenever the
-// tensor cores may decline the data gradient, and the column sum over Cout.
-template <int BACKWARD>
-size_t conv_transpose_staged_inner(const ccv_nnc_cmd_t& cmd, const ccv_nnc_hint_t& hint, ccv_nnc_tensor_t* const* const in, const int input_size, ccv_nnc_tensor_t* const* const out, const int output_size)
-{
-	ccv_nnc_tensor_t* const big = BACKWARD ? in[0] : out[0];
-	ccv_nnc_tensor_t* const filt = BACKWARD ? (output_size > 1 && out[1] ? out[1] : (input_size > 2 ? in[2] : 0)) : in[1];
-	ccv_nnc_tensor_t* const small = BACKWARD ? (input_size > 1 && in[1] ? in[1] : out[0]) : in[0];
-	ConvGeom g;
-	const int kind = big ? kind_of(big) : -1;
-	if (kind < 0 || !filt || !small || !conv_transpose_geom(cmd, hint, view_of(big), view_of(filt), view_of(small), g))
-		return (size_t)-1;
-	const int groups = cmd.info.convolution_transpose.groups > 1 ? cmd.info.convolution_transpose.groups : 1;
-	size_t need = std::max(conv_inner_workspace(g, kind, groups), colsum_workspace_bytes(g.C));
-	if (!BACKWARD && kind > 0 && groups == 1 && conv_dgrad_may_decline(g, kind))
-		need = std::max(need, dgrad16_fallback_bytes(g));
-	return (need + 255) & ~(size_t)255;
-}
-
-int exec_conv_transpose_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
-{
-	if (any_nchw(inputs, input_size, outputs, output_size))
-		return nchw_staged(conv_transpose_forw_nhwc, conv_transpose_staged_inner<0>, 0, cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
-	return conv_transpose_forw_nhwc(cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
-}
-
-int exec_conv_transpose_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
-{
-	if (any_nchw(inputs, input_size, outputs, output_size))
-		return nchw_staged(conv_transpose_back_nhwc, conv_transpose_staged_inner<1>, 1, cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
-	return conv_transpose_back_nhwc(cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
-}
-
 
 // ================================================================================================ BATCH NORM
 // norm/ccv_nnc_batch_norm_cpu_ref.c:16-250.  Supported reduction shapes: per-channel statistics of an NHWC
@@ -1619,64 +1728,91 @@ int exec_mul_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int 
 }
 
 // blas/ccv_nnc_mul_cpu_ref.c:192-330: d(p a b)/da = p g b, d/db = p g a, each summed over the axes along which that operand was
-// broadcast (g == NULL reads as ones).  Same shapes: one fused pass; otherwise the product is formed over the full index space in
-// the stream workspace and reduced onto the operand's shape in a fixed order.
-int exec_mul_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
+// broadcast (g == NULL reads as ones).  Same shapes: one fused pass; otherwise the product is formed over the full index space fd
+// -- the gradient's shape, or (no gradient) the broadcast of the two operands -- in the stream workspace and reduced onto the
+// operand's shape in a fixed order.  mul_back_plan returns that space's element count for outputs[i], 0 for the fused pass,
+// (size_t)-1 when refused.
+size_t mul_back_plan(ccv_nnc_tensor_t* const* const inputs, ccv_nnc_tensor_t* const* const outputs, const int i, int fd[4], int fs[4], int od[4], int xs[4], int gs[4])
+{
+	const ccv_nnc_tensor_t* const other = inputs[2 - i]; // ha needs b (inputs[2]), hb needs a (inputs[1])
+	if (!other || !is_f32(other) || !is_f32(outputs[i]) || (inputs[0] && !is_f32(inputs[0])))
+		return (size_t)-1;
+	const TV o = view_of(outputs[i]), x = view_of(other);
+	if (!o.contiguous || o.nd > 4 || x.nd > 4)
+		return (size_t)-1;
+	int os[4], xd[4], gd[4] = { 1, 1, 1, 1 };
+	dims4(o, od, os);
+	if (x.contiguous && same_shape(o, x) && (!inputs[0] || (view_of(inputs[0]).contiguous && same_shape(view_of(inputs[0]), o))))
+	{
+		memcpy(fs, os, sizeof(os));
+		return 0;
+	}
+	dims4(x, xd, xs);
+	memset(gs, 0, 4 * sizeof(int));
+	if (inputs[0])
+	{
+		const TV g = view_of(inputs[0]);
+		if (g.nd > 4)
+			return (size_t)-1;
+		dims4(g, gd, gs);
+	}
+	size_t fcount = 1;
+	for (int k = 0; k < 4; k++)
+	{
+		fd[k] = std::max(std::max(od[k], xd[k]), gd[k]);
+		if ((od[k] != fd[k] && od[k] != 1) || (xd[k] != fd[k] && xd[k] != 1) || (gd[k] != fd[k] && gd[k] != 1))
+			return (size_t)-1;
+		if (xd[k] == 1)
+			xs[k] = 0;
+		if (gd[k] == 1)
+			gs[k] = 0;
+		fcount *= (size_t)fd[k];
+	}
+	for (int k = 3, packed = 1; k >= 0; k--)
+		fs[k] = packed, packed *= fd[k];
+	return fcount;
+}
+// the largest full index space of the two gradients, in fp32
+size_t mul_back_workspace(const ccv_nnc_cmd_t&, const ccv_nnc_hint_t&, ccv_nnc_tensor_t* const* const in, const int input_size, ccv_nnc_tensor_t* const* const out, const int output_size)
 {
 	if (input_size < 3)
+		return (size_t)-1;
+	size_t need = 0;
+	int fd[4], fs[4], od[4], xs[4], gs[4];
+	for (int i = 0; i < 2 && i < output_size; i++)
+		if (out[i])
+		{
+			const size_t n = mul_back_plan(in, out, i, fd, fs, od, xs, gs);
+			if (n == (size_t)-1)
+				return n;
+			need = std::max(need, n * sizeof(float));
+		}
+	return need;
+}
+int exec_mul_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
+{
+	const size_t ws_bytes = mul_back_workspace(cmd, hint, inputs, input_size, outputs, output_size);
+	if (ws_bytes == (size_t)-1)
 		return CCV_NNC_EXEC_INVALID;
+	float* const t = ws_bytes ? (float*)ccv_nnc_stream_context_get_workspace(stream_context, ws_bytes, CCV_TENSOR_GPU_MEMORY) : 0;
+	if (ws_bytes && !t)
+		return CCV_NNC_EXEC_OOM;
 	cudaStream_t s = stream_of(stream_context);
 	const float p = cmd.info.blas.a[0];
 	for (int i = 0; i < 2 && i < output_size; i++)
 	{
 		if (!outputs[i])
 			continue;
-		const ccv_nnc_tensor_t* const other = inputs[2 - i]; // ha needs b (inputs[2]), hb needs a (inputs[1])
-		if (!other || !is_f32(other) || !is_f32(outputs[i]) || (inputs[0] && !is_f32(inputs[0])))
-			return CCV_NNC_EXEC_INVALID;
-		const TV o = view_of(outputs[i]), x = view_of(other);
-		if (!o.contiguous || o.nd > 4 || x.nd > 4)
-			return CCV_NNC_EXEC_INVALID;
-		if (x.contiguous && same_shape(o, x) && (!inputs[0] || (view_of(inputs[0]).contiguous && same_shape(view_of(inputs[0]), o))))
+		const ccv_nnc_tensor_t* const other = inputs[2 - i];
+		int fd[4], fs[4], od[4], xs[4], gs[4];
+		if (!mul_back_plan(inputs, outputs, i, fd, fs, od, xs, gs))
 		{
 			if (!inputs[0])
-				RC(ew_axpby_f32(s, p, other->data.f32, 0.f, 0, outputs[i]->data.f32, o.count));
-			else {
-				int d[4], st[4];
-				dims4(o, d, st);
-				RC(ew_mul_bcast_f32(s, p, inputs[0]->data.f32, st, other->data.f32, st, outputs[i]->data.f32, st, d));
-			}
+				RC(ew_axpby_f32(s, p, other->data.f32, 0.f, 0, outputs[i]->data.f32, view_of(outputs[i]).count));
+			else
+				RC(ew_mul_bcast_f32(s, p, inputs[0]->data.f32, fs, other->data.f32, fs, outputs[i]->data.f32, fs, od));
 			continue;
 		}
-		// the full index space: the gradient's shape, or (no gradient) the broadcast of the two operands
-		int fd[4], od[4], os[4], xd[4], xs[4], gd[4] = { 1, 1, 1, 1 }, gs[4] = { 0, 0, 0, 0 };
-		dims4(o, od, os);
-		dims4(x, xd, xs);
-		if (inputs[0])
-		{
-			const TV g = view_of(inputs[0]);
-			if (g.nd > 4)
-				return CCV_NNC_EXEC_INVALID;
-			dims4(g, gd, gs);
-		}
-		size_t fcount = 1;
-		for (int k = 0; k < 4; k++)
-		{
-			fd[k] = std::max(std::max(od[k], xd[k]), gd[k]);
-			if ((od[k] != fd[k] && od[k] != 1) || (xd[k] != fd[k] && xd[k] != 1) || (gd[k] != fd[k] && gd[k] != 1))
-				return CCV_NNC_EXEC_INVALID;
-			if (xd[k] == 1)
-				xs[k] = 0;
-			if (gd[k] == 1)
-				gs[k] = 0;
-			fcount *= (size_t)fd[k];
-		}
-		float* const t = (float*)ccv_nnc_stream_context_get_workspace(stream_context, fcount * sizeof(float), CCV_TENSOR_GPU_MEMORY);
-		if (!t)
-			return CCV_NNC_EXEC_OOM;
-		int fs[4];
-		for (int k = 3, packed = 1; k >= 0; k--)
-			fs[k] = packed, packed *= fd[k];
 		if (inputs[0])
 			RC(ew_mul_bcast_f32(s, p, inputs[0]->data.f32, gs, other->data.f32, xs, t, fs, fd));
 		else
@@ -2156,9 +2292,8 @@ int exec_datatype_conversion(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint,
 // ================================================================================================ 16-bit tensors on fp32-only commands
 // The commands below have fp32 kernels only; the reference's GPU backends register them for CCV_16F as well (e.g.
 // softmax/gpu/ccv_nnc_softmax_gpu_cudnn.cu, blas/gpu/ccv_nnc_add_gpu_cudnn.cu) and its half-precision tests run them
-// (test/int/nnc/cudnn.tests.c:3504-3678, 4151-4323, 4363-4735).  For bf16 / fp16 tensors the command runs in its functional form:
-// every 16-bit operand is widened into the stream workspace, the fp32 command runs on shadow tensors, every 16-bit result is
-// rounded once (to nearest even) on the way back.  One workspace request [inner | staging], as in conv_staged.
+// (test/int/nnc/cudnn.tests.c:3504-3678, 4151-4323, 4363-4735).  For bf16 / fp16 tensors the command runs in its functional form
+// (STAGE_F32).
 inline uint16_t f32_to_16(const float v, const int kind)
 {
 	uint32_t u;
@@ -2184,83 +2319,10 @@ inline uint16_t f32_to_16(const float v, const int kind)
 	return (uint16_t)(sign | (r + (rem > 0x1000u || (rem == 0x1000u && (r & 1)))));
 }
 
-int via_f32(const ccv_nnc_cmd_exec_f F32, const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
-{
-	enum { MAXT = 16 };
-	bool any16 = false;
-	for (int i = 0; i < input_size; i++)
-		any16 = any16 || (inputs[i] && kind_of(inputs[i]) > 0);
-	for (int i = 0; i < output_size; i++)
-		any16 = any16 || (outputs[i] && kind_of(outputs[i]) > 0);
-	if (!any16)
-		return F32(cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
-	if (input_size > MAXT || output_size > MAXT)
-		return CCV_NNC_EXEC_INVALID;
-	struct Shadow { ccv_nnc_tensor_t t; ccv_nnc_tensor_t* orig; size_t n; int kind; int is_out; } sh[2 * MAXT];
-	ccv_nnc_tensor_t* in[MAXT];
-	ccv_nnc_tensor_t* out[MAXT];
-	int n = 0;
-	size_t staging = 0;
-	const auto shadow_of = [&](ccv_nnc_tensor_t* const t, const int is_out) -> ccv_nnc_tensor_t* {
-		if (!t || kind_of(t) <= 0)
-			return t;
-		for (int j = 0; j < n; j++)
-			if (sh[j].orig == t || sh[j].orig->data.u8 == t->data.u8)
-			{
-				sh[j].is_out |= is_out;
-				return &sh[j].t;
-			}
-		const TV v = view_of(t);
-		if (!v.contiguous || v.count > 0x7fffffffull)
-			return 0;
-		Shadow& x = sh[n++];
-		memcpy(&x.t, t, sizeof(ccv_nnc_tensor_t));
-		x.t.type &= ~CCV_TENSOR_VIEW;
-		x.t.info.datatype = CCV_32F;
-		x.orig = t, x.n = v.count, x.kind = kind_of(t), x.is_out = is_out;
-		staging += (v.count * sizeof(float) + 255) & ~(size_t)255;
-		return &x.t;
-	};
-	for (int i = 0; i < input_size; i++)
-		if (!(in[i] = shadow_of(inputs[i], 0)) && inputs[i])
-			return CCV_NNC_EXEC_INVALID;
-	for (int i = 0; i < output_size; i++)
-		if (!(out[i] = shadow_of(outputs[i], 1)) && outputs[i])
-			return CCV_NNC_EXEC_INVALID;
-	// what the fp32 command itself may ask the workspace for: partial rows, or (MUL backward with broadcasting) one temporary of
-	// the full index space, which is the size of its largest operand
-	size_t largest = 0;
-	for (int j = 0; j < n; j++)
-		largest = std::max(largest, (sh[j].n * sizeof(float) + 255) & ~(size_t)255);
-	const size_t inner = ((size_t)4 << 20) + largest;
-	unsigned char* const ws = (unsigned char*)ccv_nnc_stream_context_get_workspace(stream_context, inner + staging, CCV_TENSOR_GPU_MEMORY);
-	if (!ws)
-		return CCV_NNC_EXEC_OOM;
-	cudaStream_t s = stream_of(stream_context);
-	unsigned char* p = ws + inner;
-	for (int j = 0; j < n; j++)
-	{
-		sh[j].t.data.u8 = p, p += (sh[j].n * sizeof(float) + 255) & ~(size_t)255;
-		// every shadow is filled: inputs carry data, and an output may be read by the command (in-place forms)
-		RC(widen_matrix(s, sh[j].orig->data.u8, sh[j].kind, (long long)sh[j].n, 1, sh[j].t.data.f32, 1, (int)sh[j].n));
-	}
-	const int rc = F32(cmd, hint, flags, in, input_size, out, output_size, stream_context);
-	if (rc != CCV_NNC_EXEC_SUCCESS)
-		return rc;
-	if (ccv_nnc_stream_context_get_workspace(stream_context, 1, CCV_TENSOR_GPU_MEMORY) != (void*)ws)
-	{
-		set_last_error("functional 16-bit form: the fp32 command moved the workspace under the widened tensors", cudaErrorInvalidValue);
-		return CCV_NNC_EXEC_INVALID;
-	}
-	for (int j = 0; j < n; j++)
-		if (sh[j].is_out)
-			RC(narrow_matrix(s, sh[j].t.data.f32, sh[j].orig->data.u8, sh[j].kind, (long long)sh[j].n, 1, 1, (int)sh[j].n, 0));
-	return CCV_NNC_EXEC_SUCCESS;
-}
-template <ccv_nnc_cmd_exec_f F32>
+template <ccv_nnc_cmd_exec_f F32, staged_inner_f WS = no_workspace>
 int exec_via_f32(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
 {
-	return via_f32(F32, cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
+	return staged(STAGE_F32, 0, F32, WS, cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
 }
 
 // SGD: fp32 parameters / momenta with gradients of any type run natively (the mixed-precision form); 16-bit PARAMETERS
@@ -2272,26 +2334,9 @@ int exec_sgd_any(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int f
 	return exec_sgd_forw(cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
 }
 
-// pooling on NCHW tensors ([N,] C, H, W: pool/gpu/ccv_nnc_max_pool_gpu_cudnn.cu takes both formats; test/int/nnc/cudnn.tests.c:2772-2870):
-// the kernels are NHWC (channel-contiguous 16-byte accesses), NCHW operands are staged like the convolution's
-size_t pool_staged_inner(const ccv_nnc_cmd_t&, const ccv_nnc_hint_t&, ccv_nnc_tensor_t* const*, int, ccv_nnc_tensor_t* const*, int) { return 256; }
-template <ccv_nnc_cmd_exec_f F>
-int exec_pool_any(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
-{
-	if (any_nchw(inputs, input_size, outputs, output_size))
-		return nchw_staged(F, pool_staged_inner, 0, cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
-	return F(cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
-}
-
 // ================================================================================================ palettized (CCV_QX) operands
 // lib/nnc/cmd/blas/gpu/ccv_nnc_gemm_gpu_cublas.cu:291-334, convolution/gpu/ccv_nnc_conv_gpu_cudnn.cu:79,328,
-// convolution/gpu/ccv_nnc_conv_transpose_gpu_cudnn.cu:72,127: a weight operand may be a palettized tensor.  It is decoded into the
-// workspace and the command runs on the decoded tensor, so the result is the dense command's, bit for bit.  The workspace is one
-// request [what the dense command asks for | decoded operands]: the dense command's own requests then never grow (and move) it.
-inline bool is_qx(const ccv_nnc_tensor_t* const t) { return t && CCV_GET_DATA_TYPE(t->info.datatype) == CCV_QX; }
-inline int qx_palette(const ccv_nnc_tensor_t* const t) { return (t->info.datatype & 0xff) << 12; }
-inline int qx_bits(const ccv_nnc_tensor_t* const t) { return (t->info.datatype >> 8) & 0xf; }
-
+// convolution/gpu/ccv_nnc_conv_transpose_gpu_cudnn.cu:72,127: a weight operand may be a palettized tensor (STAGE_QX).
 bool any_qx(ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size)
 {
 	for (int i = 0; i < input_size; i++)
@@ -2301,118 +2346,6 @@ bool any_qx(ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc
 		if (is_qx(outputs[i]))
 			return true;
 	return false;
-}
-
-// what nchw_staged(exec, inner_of, ...) asks the workspace for, or (size_t)-1 when it would refuse the operands
-size_t nchw_staged_request(const staged_inner_f inner_of, const ccv_nnc_cmd_t& cmd, const ccv_nnc_hint_t& hint, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size)
-{
-	if (input_size > 3 || output_size > 3)
-		return (size_t)-1;
-	Staged st[6];
-	ccv_nnc_tensor_t* in[3] = { 0, 0, 0 };
-	ccv_nnc_tensor_t* out[3] = { 0, 0, 0 };
-	int n = 0;
-	size_t staging = 0;
-	for (int i = 0; i < input_size; i++)
-	{
-		in[i] = inputs[i];
-		if (is_nchw(inputs[i]))
-		{
-			if (!stage_plan(inputs[i], st[n]))
-				return (size_t)-1;
-			staging += st[n].bytes, in[i] = &st[n].shadow, n++;
-		}
-	}
-	for (int i = 0; i < output_size; i++)
-	{
-		out[i] = outputs[i];
-		if (is_nchw(outputs[i]))
-		{
-			if (!stage_plan(outputs[i], st[n]))
-				return (size_t)-1;
-			staging += st[n].bytes, out[i] = &st[n].shadow, n++;
-		}
-	}
-	const size_t inner = inner_of(cmd, hint, in, input_size, out, output_size);
-	return inner == (size_t)-1 ? inner : inner + staging;
-}
-
-// `exec` = the dense command, `inner_of` = the most it asks the workspace for (on the decoded operands), `qx_inputs` = bit i set when
-// inputs[i] may be palettized.  Refused (outputs untouched): a palettized output or other operand, qbits outside 4..8, a block size
-// whose index bytes are not whole, a view, a palette that is not fp16 / fp32 or not the type of the command's other tensors.
-typedef size_t (*qx_inner_f)(const ccv_nnc_cmd_t& cmd, const ccv_nnc_hint_t& hint, ccv_nnc_tensor_t* const* in, int input_size, ccv_nnc_tensor_t* const* out, int output_size);
-int exec_depalettized(const ccv_nnc_cmd_exec_f exec, const qx_inner_f inner_of, const unsigned qx_inputs, const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
-{
-	enum { MAXT = 8 };
-	if (input_size > MAXT)
-		return CCV_NNC_EXEC_INVALID;
-	int dense = 0;
-	for (int i = 0; i < output_size && !dense; i++)
-		if (outputs[i])
-		{
-			if (is_qx(outputs[i]))
-				return CCV_NNC_EXEC_INVALID;
-			dense = CCV_GET_DATA_TYPE(outputs[i]->info.datatype);
-		}
-	for (int i = 0; i < input_size && !dense; i++)
-		if (inputs[i] && !is_qx(inputs[i]))
-			dense = CCV_GET_DATA_TYPE(inputs[i]->info.datatype);
-	ccv_nnc_tensor_t shadow[MAXT];
-	ccv_nnc_tensor_t* in[MAXT];
-	size_t off[MAXT], decoded = 0;
-	for (int i = 0; i < input_size; i++)
-	{
-		in[i] = inputs[i];
-		if (!is_qx(inputs[i]))
-			continue;
-		const int pal = qx_palette(inputs[i]);
-		if (!(qx_inputs & (1u << i)) || CCV_IS_TENSOR_VIEW(inputs[i]) || !palettize_params_ok(qx_bits(inputs[i]), inputs[i]->info.reserved) || (pal != CCV_16F && pal != CCV_32F) || pal != dense)
-			return CCV_NNC_EXEC_INVALID;
-		memcpy(&shadow[i], inputs[i], sizeof(ccv_nnc_tensor_t));
-		shadow[i].info.datatype = pal;
-		shadow[i].info.reserved = 0;
-		shadow[i].type = (shadow[i].type & ~0xFF000) | pal;
-		shadow[i].data_size = 0;
-		off[i] = decoded;
-		decoded += (view_of(inputs[i]).count * dtype_size(pal) + 255) & ~(size_t)255;
-		in[i] = &shadow[i];
-	}
-	const size_t inner = inner_of(cmd, hint, in, input_size, outputs, output_size);
-	if (inner == (size_t)-1)
-		return CCV_NNC_EXEC_INVALID;
-	unsigned char* const ws = (unsigned char*)ccv_nnc_stream_context_get_workspace(stream_context, inner + decoded, CCV_TENSOR_GPU_MEMORY);
-	if (!ws)
-		return CCV_NNC_EXEC_OOM;
-	cudaStream_t s = stream_of(stream_context);
-	for (int i = 0; i < input_size; i++)
-		if (is_qx(inputs[i]))
-		{
-			shadow[i].data.u8 = ws + inner + off[i];
-			RC(depalettize(s, inputs[i]->data.u8, qx_palette(inputs[i]), qx_bits(inputs[i]), inputs[i]->info.reserved, shadow[i].data.u8, view_of(inputs[i]).count));
-		}
-	const int rc = exec(cmd, hint, flags, in, input_size, outputs, output_size, stream_context);
-	if (rc != CCV_NNC_EXEC_SUCCESS)
-		return rc;
-	if (ccv_nnc_stream_context_get_workspace(stream_context, 1, CCV_TENSOR_GPU_MEMORY) != (void*)ws)
-	{
-		set_last_error("palettized operands: workspace moved under the decoded tensors", cudaErrorInvalidValue);
-		return CCV_NNC_EXEC_INVALID;
-	}
-	return CCV_NNC_EXEC_SUCCESS;
-}
-
-// GEMM: the contraction scratch, and the column sum of the bias gradient
-size_t gemm_qx_inner(const ccv_nnc_cmd_t&, const ccv_nnc_hint_t&, ccv_nnc_tensor_t* const* const in, const int input_size, ccv_nnc_tensor_t* const*, int)
-{
-	const TV g = view_of(in[0]);
-	return (std::max(CONTRACT_SCRATCH_BYTES, colsum_workspace_bytes(g.nd > 0 ? g.dim[g.nd - 1] : 1)) + 255) & ~(size_t)255;
-}
-template <staged_inner_f INNER>
-size_t conv_qx_inner(const ccv_nnc_cmd_t& cmd, const ccv_nnc_hint_t& hint, ccv_nnc_tensor_t* const* const in, const int input_size, ccv_nnc_tensor_t* const* const out, const int output_size)
-{
-	if (any_nchw(in, input_size, out, output_size))
-		return nchw_staged_request(INNER, cmd, hint, in, input_size, out, output_size);
-	return INNER(cmd, hint, in, input_size, out, output_size);
 }
 
 // The few-row dense layer on a palettized weight, without decoding it: c[M, N] = a[M, K] w[N, K]^T (+ bias), a / c fp16, w with fp16
@@ -2448,8 +2381,6 @@ bool gemm_fused_qx_plan(const ccv_nnc_cmd_t& cmd, ccv_nnc_tensor_t* const* const
 
 int exec_gemm_forw_any(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
 {
-	if (!any_qx(inputs, input_size, outputs, output_size))
-		return exec_gemm_nd4<exec_gemm_forw>(cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
 	int M, N, K;
 	if (gemm_fused_qx_plan(cmd, inputs, input_size, outputs, output_size, M, N, K))
 	{
@@ -2459,26 +2390,23 @@ int exec_gemm_forw_any(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const
 			b32 ? bias_t->data.f32 : 0, bias_t && !b32 ? (const void*)bias_t->data.u8 : 0));
 		return CCV_NNC_EXEC_SUCCESS;
 	}
-	return exec_depalettized(exec_gemm_nd4<exec_gemm_forw>, gemm_qx_inner, 0x3, cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
+	return staged(STAGE_QX, 0x3, exec_gemm_nd4<exec_gemm_forw>, gemm_forw_workspace, cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
 }
 
 int exec_gemm_back_any(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
 {
-	if (!any_qx(inputs, input_size, outputs, output_size))
-		return exec_gemm_nd4<exec_gemm_back>(cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
 	// inputs (g, a, w): a is palettized only for dw, w only for h
 	const unsigned mask = (output_size > 1 && outputs[1] ? 0x2u : 0u) | (output_size > 0 && outputs[0] ? 0x4u : 0u);
-	return exec_depalettized(exec_gemm_nd4<exec_gemm_back>, gemm_qx_inner, mask, cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
+	return staged(STAGE_QX, mask, exec_gemm_nd4<exec_gemm_back>, gemm_back_workspace, cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
 }
 
-// convolutions: the filters, inputs[1] of the forwards and inputs[2] of the backwards when the data gradient (outputs[0]) is asked for
-template <ccv_nnc_cmd_exec_f EXEC, staged_inner_f INNER, int BACKWARD>
+// convolutions (EXEC: the NHWC command, WS: its workspace function): palettized filters, inputs[1] of the forwards and inputs[2] of the
+// backwards when the data gradient (outputs[0]) is asked for, decoded around the NCHW staging
+template <ccv_nnc_cmd_exec_f EXEC, staged_inner_f WS, int BACKWARD>
 int exec_conv_any(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
 {
-	if (!any_qx(inputs, input_size, outputs, output_size))
-		return EXEC(cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
 	const unsigned mask = BACKWARD ? (output_size > 0 && outputs[0] ? 0x4u : 0u) : 0x2u;
-	return exec_depalettized(EXEC, conv_qx_inner<INNER>, mask, cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
+	return staged(STAGE_QX, mask, exec_nchw<EXEC, WS, BACKWARD>, nchw_workspace<WS>, cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
 }
 
 // util/gpu/ccv_nnc_util_gpu_ref.cu:22-24: a palettized tensor moves as its bytes; both sides carry the same datatype word and block size
@@ -2585,6 +2513,14 @@ int backend_gemm_nt_bias(void* stream_context, int kind, int M, int N, int K, co
 		return gemm_dispatch(s, scratch, CCV_NNC_SM100_ALGO_3XTF32, M, N, K, (const float*)a, K, 1, (const float*)w, 1, K, (float*)c, N, 1, (const float*)bias, 0);
 	return gemm_dispatch16(s, scratch, kind, M, N, K, a, K, 1, w, 1, K, c, N, 1, bias && bias_is_f32 ? (const float*)bias : 0, bias && !bias_is_f32 ? bias : 0, 0);
 }
+bool backend_qx_ok(const void* const tensor, const int dense)
+{
+	return qx_ok((const ccv_nnc_tensor_t*)tensor, dense);
+}
+int backend_qx_decode(void* const stream_context, const void* const tensor, void* const out)
+{
+	return qx_decode(stream_of((ccv_nnc_stream_context_t*)stream_context), (const ccv_nnc_tensor_t*)tensor, out);
+}
 } // namespace sm100
 
 // implemented in sm100_backend_ext.cu (attention, layer / rms norm, upsample, allreduce)
@@ -2672,7 +2608,7 @@ extern "C" int ccv_nnc_sm100_fused_conv_stats_forw(const ccv_nnc_cmd_t cmd, cons
 	const int max_rows = stats_t->info.dim[0] / 4;
 	if (outputs[0] && stats_t->info.dim[1] == cmd.info.convolution.count)
 		conv_stats_request(stats_t->data.f32, max_rows, &rows);
-	const int rc = exec_conv_forw(cmd, hint, flags, inputs, input_size, outputs, 1, stream_context);
+	const int rc = exec_nchw<conv_forw_nhwc, conv_forw_workspace, 0>(cmd, hint, flags, inputs, input_size, outputs, 1, stream_context);
 	conv_stats_request(0, 0, 0); // never leave a request pending for an unrelated launch
 	stats_t->sig = rc == CCV_NNC_EXEC_SUCCESS ? (uint64_t)rows : 0;
 	return rc;
@@ -2688,7 +2624,7 @@ extern "C" int ccv_nnc_sm100_fused_sgd_multi(const ccv_nnc_cmd_t cmd, const ccv_
 namespace sm100 {
 int exec_via_f32_rt(ccv_nnc_cmd_exec_f f32, const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
 {
-	return via_f32(f32, cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
+	return staged(STAGE_F32, 0, f32, no_workspace, cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
 }
 }
 
@@ -2696,10 +2632,10 @@ int exec_via_f32_rt(ccv_nnc_cmd_exec_f f32, const ccv_nnc_cmd_t cmd, const ccv_n
 
 REGISTER_SM100(CCV_NNC_GEMM_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_gemm_forw_any); registry->autotune = autotune_contraction<exec_gemm_forw_any>; }
 REGISTER_SM100(CCV_NNC_GEMM_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_gemm_back_any); registry->autotune = autotune_contraction<exec_gemm_back_any>; }
-REGISTER_SM100(CCV_NNC_CONVOLUTION_FORWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_conv_any<exec_conv_forw, conv_staged_inner<0>, 0>); registry->autotune = autotune_contraction<exec_conv_any<exec_conv_forw, conv_staged_inner<0>, 0> >; }
-REGISTER_SM100(CCV_NNC_CONVOLUTION_BACKWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_conv_any<exec_conv_back, conv_staged_inner<1>, 1>); registry->autotune = autotune_contraction<exec_conv_any<exec_conv_back, conv_staged_inner<1>, 1> >; }
-REGISTER_SM100(CCV_NNC_CONVOLUTION_TRANSPOSE_FORWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_conv_any<exec_conv_transpose_forw, conv_transpose_staged_inner<0>, 0>); registry->autotune = autotune_contraction<exec_conv_any<exec_conv_transpose_forw, conv_transpose_staged_inner<0>, 0> >; }
-REGISTER_SM100(CCV_NNC_CONVOLUTION_TRANSPOSE_BACKWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_conv_any<exec_conv_transpose_back, conv_transpose_staged_inner<1>, 1>); registry->autotune = autotune_contraction<exec_conv_any<exec_conv_transpose_back, conv_transpose_staged_inner<1>, 1> >; }
+REGISTER_SM100(CCV_NNC_CONVOLUTION_FORWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_conv_any<conv_forw_nhwc, conv_forw_workspace, 0>); registry->autotune = autotune_contraction<exec_conv_any<conv_forw_nhwc, conv_forw_workspace, 0> >; }
+REGISTER_SM100(CCV_NNC_CONVOLUTION_BACKWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_conv_any<conv_back_nhwc, conv_back_workspace, 1>); registry->autotune = autotune_contraction<exec_conv_any<conv_back_nhwc, conv_back_workspace, 1> >; }
+REGISTER_SM100(CCV_NNC_CONVOLUTION_TRANSPOSE_FORWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_conv_any<conv_transpose_forw_nhwc, conv_transpose_forw_workspace, 0>); registry->autotune = autotune_contraction<exec_conv_any<conv_transpose_forw_nhwc, conv_transpose_forw_workspace, 0> >; }
+REGISTER_SM100(CCV_NNC_CONVOLUTION_TRANSPOSE_BACKWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_conv_any<conv_transpose_back_nhwc, conv_transpose_back_workspace, 1>); registry->autotune = autotune_contraction<exec_conv_any<conv_transpose_back_nhwc, conv_transpose_back_workspace, 1> >; }
 REGISTER_SM100(CCV_NNC_SCALED_DOT_PRODUCT_ATTENTION_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, 1, ccv_nnc_sm100_exec_sdpa_forw); }
 REGISTER_SM100(CCV_NNC_SCALED_DOT_PRODUCT_ATTENTION_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, ccv_nnc_sm100_exec_sdpa_back); }
 REGISTER_SM100(CCV_NNC_SOFTMAX_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_via_f32<exec_softmax_forw>); }
@@ -2717,15 +2653,15 @@ REGISTER_SM100(CCV_NNC_EWSUM_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | C
 REGISTER_SM100(CCV_NNC_ADD_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_via_f32<exec_add_forw>); }
 REGISTER_SM100(CCV_NNC_ADD_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_via_f32<exec_add_back>); }
 REGISTER_SM100(CCV_NNC_MUL_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_via_f32<exec_mul_forw>); }
-REGISTER_SM100(CCV_NNC_MUL_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_via_f32<exec_mul_back>); }
+REGISTER_SM100(CCV_NNC_MUL_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_via_f32<exec_mul_back, mul_back_workspace>); }
 REGISTER_SM100(CCV_NNC_SCALAR_MUL_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_via_f32<exec_scalar_mul_forw>); }
 REGISTER_SM100(CCV_NNC_SCALAR_MUL_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_via_f32<exec_scalar_mul_back>); }
 REGISTER_SM100(CCV_NNC_RELU_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_relu_forw); }
 REGISTER_SM100(CCV_NNC_RELU_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_relu_back); }
-REGISTER_SM100(CCV_NNC_MAX_POOL_FORWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF, 1, exec_pool_any<exec_pool_forw<1> >); }
-REGISTER_SM100(CCV_NNC_MAX_POOL_BACKWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF, 1, exec_pool_any<exec_pool_back<1> >); }
-REGISTER_SM100(CCV_NNC_AVERAGE_POOL_FORWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF, 1, exec_pool_any<exec_pool_forw<0> >); }
-REGISTER_SM100(CCV_NNC_AVERAGE_POOL_BACKWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF, 1, exec_pool_any<exec_pool_back<0> >); }
+REGISTER_SM100(CCV_NNC_MAX_POOL_FORWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF, 1, exec_nchw<exec_pool_forw<1>, no_workspace, 0>); }
+REGISTER_SM100(CCV_NNC_MAX_POOL_BACKWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF, 1, exec_nchw<exec_pool_back<1>, no_workspace, 0>); }
+REGISTER_SM100(CCV_NNC_AVERAGE_POOL_FORWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF, 1, exec_nchw<exec_pool_forw<0>, no_workspace, 0>); }
+REGISTER_SM100(CCV_NNC_AVERAGE_POOL_BACKWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF, 1, exec_nchw<exec_pool_back<0>, no_workspace, 0>); }
 REGISTER_SM100(CCV_NNC_UPSAMPLE_FORWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF, 1, exec_via_f32<ccv_nnc_sm100_exec_upsample_forw>); }
 REGISTER_SM100(CCV_NNC_UPSAMPLE_BACKWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF, 1, exec_via_f32<ccv_nnc_sm100_exec_upsample_back>); }
 REGISTER_SM100(CCV_NNC_SET_FORWARD) { fill(registry, ALL_FORMATS, CCV_64F | CCV_32F | CCV_16F | CCV_16BF | CCV_32S, 1, exec_set_forw); }

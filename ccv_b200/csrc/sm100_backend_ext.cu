@@ -223,9 +223,7 @@ int ccv_nnc_sm100_exec_sdpa_forw(SM100_EXEC_ARGS)
 	// the weights may be palettized (attention/gpu/ccv_nnc_scaled_dot_product_attention_flash_attn.cu registers CCV_QX), with a
 	// palette of the activations' type; no other operand may be
 	const bool w_qx = CCV_GET_DATA_TYPE(w->info.datatype) == CCV_QX;
-	const int w_dt = w_qx ? (w->info.datatype & 0xff) << 12 : CCV_GET_DATA_TYPE(w->info.datatype);
-	const int w_q = (w->info.datatype >> 8) & 0xf;
-	if (w_qx && ((dt != CCV_16F && dt != CCV_32F) || !palettize_params_ok(w_q, w->info.reserved)))
+	if (w_qx ? !backend_qx_ok(w, dt) : CCV_GET_DATA_TYPE(w->info.datatype) != dt)
 		return CCV_NNC_EXEC_INVALID;
 	for (int i = 0; i < input_size; i++)
 		if (i != 4 && inputs[i] && CCV_GET_DATA_TYPE(inputs[i]->info.datatype) == CCV_QX)
@@ -233,7 +231,7 @@ int ccv_nnc_sm100_exec_sdpa_forw(SM100_EXEC_ARGS)
 	for (int i = 0; i < output_size; i++)
 		if (outputs[i] && CCV_GET_DATA_TYPE(outputs[i]->info.datatype) == CCV_QX)
 			return CCV_NNC_EXEC_INVALID;
-	if (CCV_GET_DATA_TYPE(c->info.datatype) != dt || CCV_GET_DATA_TYPE(d->info.datatype) != dt || w_dt != dt)
+	if (CCV_GET_DATA_TYPE(c->info.datatype) != dt || CCV_GET_DATA_TYPE(d->info.datatype) != dt)
 		return CCV_NNC_EXEC_INVALID;
 	const int B = c->info.dim[0], S = c->info.dim[1];
 	const long long hd = c_nd == 4 ? (long long)c->info.dim[2] * c->info.dim[3] : c->info.dim[2];
@@ -261,7 +259,7 @@ int ccv_nnc_sm100_exec_sdpa_forw(SM100_EXEC_ARGS)
 		unsigned char* const ws = (unsigned char*)ccv_nnc_stream_context_get_workspace(stream_context, CONTRACT_SCRATCH_BYTES + (size_t)hd * hd * (dt == CCV_32F ? 4 : 2), CCV_TENSOR_GPU_MEMORY);
 		if (!ws)
 			return CCV_NNC_EXEC_OOM;
-		if (depalettize(stream_of(stream_context), w->data.u8, dt, w_q, w->info.reserved, ws + CONTRACT_SCRATCH_BYTES, (size_t)hd * hd))
+		if (backend_qx_decode(stream_context, w, ws + CONTRACT_SCRATCH_BYTES))
 			return CCV_NNC_EXEC_INVALID;
 		w_data = ws + CONTRACT_SCRATCH_BYTES;
 	}

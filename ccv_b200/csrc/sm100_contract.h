@@ -108,6 +108,11 @@ int sdpa_backward_f16(cudaStream_t s, const SdpaGeom& g, const SdpaGeom& dg, int
 // (the GEMM command's default algorithm, 3xTF32), 1 = bf16, 2 = fp16; bias in the operands' type or fp32 (bias_is_f32).  Used by
 // commands that end in a dense projection (the attention "unify head" output).  Returns 0, or non-zero like the GEMM launchers.
 int backend_gemm_nt_bias(void* stream_context, int kind, int M, int N, int K, const void* a, const void* w, void* c, const void* bias, int bias_is_f32);
+// The palettized-operand checks and decoder of the GEMM / convolution commands, for a weight of another command (the attention's
+// unify-head projection): backend_qx_ok(tensor, dense) = the decoder takes it, with a palette of type `dense`; backend_qx_decode
+// writes its decoded elements to out (device memory) and returns like depalettize.
+bool backend_qx_ok(const void* tensor, int dense);
+int backend_qx_decode(void* stream_context, const void* tensor, void* out);
 
 // palettized (CCV_QX) tensors (sm100_palettize.cu).  qbits 4..8; nib (elements per palette block) must make the block stride
 // nib * qbits / 8 a whole number of bytes.  palette_datatype is CCV_16F, CCV_32F or CCV_64F; out holds `count` decoded elements.

@@ -14,7 +14,7 @@ import numpy as np
 import pytest
 
 from ccv_b200 import abi
-from tests.util import NCHW, NHWC, assert_close, gpu_exec, ref_exec, seeded
+from tests.util import NCHW, NHWC, assert_close, counted, gpu_exec, ref_exec, seeded
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 TOL = {abi.CCV_NNC_SM100_ALGO_TF32: 1e-3, abi.CCV_NNC_SM100_ALGO_3XTF32: 2e-5, abi.CCV_NNC_SM100_ALGO_FFMA: 1e-5}
@@ -261,9 +261,14 @@ def test_convolution_forward_nchw(gpu, ref, N, C, H, K, R, st, groups):
     hint = nnc.hint((st, st), (pad, pad))
     fmts = dict(in_fmts=[NCHW, NCHW, NHWC], out_fmts=[NCHW])
     st_r, (y_r,) = ref_exec(ref, cmd, hint, 0, [x, w, bias], [np.zeros((N, K, P, P), np.float32)], **fmts)
-    st_g, (y_g,) = gpu_exec(nnc, cmd, hint, 0, [x, w, bias], [np.zeros((N, K, P, P), np.float32)], **fmts)
+    st_g, (y_g,), n = counted(nnc, gpu_exec, cmd, hint, 0, [x, w, bias], [np.zeros((N, K, P, P), np.float32)], **fmts)
     assert st_r == 0 and st_g == 0
     assert_close(y_g, y_r, 1e-3, "NCHW convolution")
+    # the same launches as the NHWC command, plus one relayout per NCHW operand in (x, w) and one per NCHW output out (y)
+    t = lambda a: np.ascontiguousarray(a.transpose(0, 2, 3, 1))
+    st_d, (y_d,), n_d = counted(nnc, gpu_exec, cmd, hint, 0, [t(x), t(w), bias], [np.zeros((N, P, P, K), np.float32)])
+    assert st_d == 0 and n == n_d + 3, (n, n_d)
+    assert np.array_equal(y_g, np.ascontiguousarray(y_d.transpose(0, 3, 1, 2)))
 
 
 @pytest.mark.ref
@@ -313,18 +318,26 @@ def test_convolution_backward_nchw_and_mixed(gpu, ref, C, K, st, layout):
     if layout == "filters":
         ins, outs = [g, x, t(w)], [np.zeros_like(x), np.ones_like(t(w)), np.zeros((K,), np.float32)]
         fm = dict(in_fmts=[NHWC, NHWC, NCHW], out_fmts=[NHWC, NCHW, NHWC])
-        st_g, (h_g, dw_g, db_g) = gpu_exec(nnc, cmd, hint, abi.CCV_NNC_ACCUMULATE_OUTPUT, ins, outs, **fm)
+        st_g, (h_g, dw_g, db_g), n = counted(nnc, gpu_exec, cmd, hint, abi.CCV_NNC_ACCUMULATE_OUTPUT, ins, outs, **fm)
         dw_g = dw_g.transpose(0, 2, 3, 1) - 1.0  # accumulated onto ones
+        # relayouts: w in, dw in (it accumulates) and out
+        st_d, _, n_d = counted(nnc, gpu_exec, cmd, hint, abi.CCV_NNC_ACCUMULATE_OUTPUT, [g, x, w], [np.zeros_like(x), np.ones_like(w), np.zeros((K,), np.float32)])
+        staging = 3
     else:
         ins, outs = [t(g), t(x), t(w)], [np.zeros_like(t(x)), np.zeros_like(t(w)), np.zeros((K,), np.float32)]
         fm = dict(in_fmts=[NCHW, NCHW, NCHW], out_fmts=[NCHW, NCHW, NHWC])
+        dense = [g, x, w], [np.zeros_like(x), np.zeros_like(w), np.zeros((K,), np.float32)]
         if half:
             from tests.util import gpu_exec16
-            st_g, (h_g, dw_g, db_g) = gpu_exec16(nnc, cmd, hint, 0, ins, outs, abi.CCV_16F, keep32=(id(outs[2]),), **fm)
+            st_g, (h_g, dw_g, db_g), n = counted(nnc, gpu_exec16, cmd, hint, 0, ins, outs, abi.CCV_16F, keep32=(id(outs[2]),), **fm)
+            st_d, _, n_d = counted(nnc, gpu_exec16, cmd, hint, 0, *dense, abi.CCV_16F, keep32=(id(dense[1][2]),))
         else:
-            st_g, (h_g, dw_g, db_g) = gpu_exec(nnc, cmd, hint, 0, ins, outs, **fm)
+            st_g, (h_g, dw_g, db_g), n = counted(nnc, gpu_exec, cmd, hint, 0, ins, outs, **fm)
+            st_d, _, n_d = counted(nnc, gpu_exec, cmd, hint, 0, *dense)
         h_g, dw_g = h_g.transpose(0, 2, 3, 1), dw_g.transpose(0, 2, 3, 1)
-    assert st_r == 0 and st_g == 0
+        staging = 5  # relayouts: g, x, w in; h, dw out
+    assert st_r == 0 and st_g == 0 and st_d == 0
+    assert n == n_d + staging, (n, n_d)
     tol = 1e-2 if half else 1e-3
     assert_close(h_g, h_r, tol, "dgrad " + layout)
     assert_close(dw_g, dw_r, tol, "wgrad " + layout)

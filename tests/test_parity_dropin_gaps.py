@@ -6,7 +6,7 @@ import numpy as np
 import pytest
 
 from ccv_b200 import abi
-from tests.util import NCHW, NHWC, assert_close, gpu_exec, gpu_exec16, ref_exec, round16, seeded
+from tests.util import NCHW, NHWC, assert_close, counted, gpu_exec, gpu_exec16, ref_exec, round16, seeded
 
 pytestmark = [pytest.mark.gpu, pytest.mark.ref]
 
@@ -28,6 +28,23 @@ def test_mul_backward_broadcast(gpu, ref, with_g):
     st, (da4_g,) = gpu_exec(nnc, cmd, None, 0, [g4, a4, b4], [np.zeros_like(a4)])
     assert st == 0
     assert_close(da4_g, da4_r, 1e-5, "da 4-d")
+
+
+@pytest.mark.parametrize("kind", [abi.CCV_16F, abi.CCV_16BF])
+def test_mul_backward_broadcast_half_without_gradient(gpu, ref, kind):
+    """a [2048, 1] * b [1, 2048] in half precision, no incoming gradient, on the default stream (whose workspace starts empty):
+    each gradient is formed over the 2048 x 2048 broadcast index space, a temporary larger than any operand, next to the widened
+    operands.  Oracle: CPU_REF on the rounded inputs, <= 1e-2.  Launches: the fp32 command's, plus one widen per 16-bit tensor
+    (a, b, da, db) and one narrow per 16-bit output."""
+    nnc = gpu
+    a, b = round16(seeded((2048, 1), 1, -1, 1), kind), round16(seeded((1, 2048), 2, -1, 1), kind)
+    cmd = nnc.CMD_MUL_BACKWARD(0.5)
+    _, (da_r, db_r) = ref_exec(ref, cmd, None, 0, [None, a, b], [np.zeros_like(a), np.zeros_like(b)])
+    st, (da_g, db_g), n = counted(nnc, gpu_exec16, cmd, None, 0, [None, a, b], [np.zeros_like(a), np.zeros_like(b)], kind)
+    assert st == 0, nnc.lib().ccv_nnc_sm100_last_error()
+    assert_close(da_g, da_r, 1e-2, "da"), assert_close(db_g, db_r, 1e-2, "db")
+    st, _, n32 = counted(nnc, gpu_exec, cmd, None, 0, [None, a, b], [np.zeros_like(a), np.zeros_like(b)])
+    assert st == 0 and n == n32 + 4 + 2, (n, n32)
 
 
 @pytest.mark.parametrize("broadcast_w,with_bias", [(False, False), (True, False), (False, True), (True, True)])
@@ -120,16 +137,21 @@ def test_pooling_nchw(gpu, ref, which):
         perm = (2, 0, 1) if len(shape_nhwc) == 3 else (0, 3, 1, 2)
         back = (1, 2, 0) if len(shape_nhwc) == 3 else (0, 2, 3, 1)
         xc = np.ascontiguousarray(x.transpose(perm))
-        st, (y_g,) = gpu_exec(nnc, fwd(k, k), hint, 0, [xc], [np.zeros(tuple(np.array(out_nhwc)[list(perm)]), np.float32)], fmt=NCHW)
+        st, (y_g,), n = counted(nnc, gpu_exec, fwd(k, k), hint, 0, [xc], [np.zeros(tuple(np.array(out_nhwc)[list(perm)]), np.float32)], fmt=NCHW)
         assert st == 0
+        # the NHWC command's launches plus one relayout in (x) and one out (y)
+        st, _, n_d = counted(nnc, gpu_exec, fwd(k, k), hint, 0, [x], [np.zeros(out_nhwc, np.float32)])
+        assert st == 0 and n == n_d + 2, (n, n_d)
         assert np.array_equal(y_g.transpose(back), y_r) if which == "max" else np.abs(y_g.transpose(back) - y_r).max() <= 1e-6
         g = seeded(out_nhwc, 2, -1, 1)
         ins_r = [g, x, y_r] if which == "max" else [g]
         _, (h_r,) = ref_exec(ref, bwd(k, k), hint, 0, ins_r, [np.zeros(shape_nhwc, np.float32)])
         gc, yc = np.ascontiguousarray(g.transpose(perm)), np.ascontiguousarray(y_r.transpose(perm))
         ins_g = [gc, xc, yc] if which == "max" else [gc]
-        st, (h_g,) = gpu_exec(nnc, bwd(k, k), hint, 0, ins_g, [np.zeros(xc.shape, np.float32)], fmt=NCHW)
+        st, (h_g,), n = counted(nnc, gpu_exec, bwd(k, k), hint, 0, ins_g, [np.zeros(xc.shape, np.float32)], fmt=NCHW)
         assert st == 0
+        st, _, n_d = counted(nnc, gpu_exec, bwd(k, k), hint, 0, [g, x, y_r] if which == "max" else [g], [np.zeros(shape_nhwc, np.float32)])
+        assert st == 0 and n == n_d + len(ins_g) + 1, (n, n_d)
         assert_close(h_g.transpose(back), h_r, 1e-6, which + " pool backward NCHW")
 
 

@@ -40,6 +40,13 @@ def gpu_exec(nnc, cmd, hint, flags, in_arrays, out_arrays, fmt=NHWC, in_fmts=Non
     return status, results
 
 
+def counted(nnc, run, *args, **kwargs):
+    """run(nnc, *args, **kwargs) -> (status, outputs, kernels the backend launched meanwhile, ccv_nnc_sm100_launch_count())."""
+    l0 = nnc.launch_count()
+    status, outs = run(nnc, *args, **kwargs)
+    return status, outs, nnc.launch_count() - l0
+
+
 def ref_exec(ref, cmd, hint, flags, in_arrays, out_arrays, fmt=NHWC, in_fmts=None, out_fmts=None):
     """Same command on the reference's CPU_REF. out_arrays are modified in place and returned."""
     cache = {}
