@@ -157,17 +157,21 @@ size_t dtype_size(const int datatype)
 
 // ================================================================================================ GEMM
 struct Mat {
-	float* p;
+	unsigned char* p;
+	size_t esz; // bytes per element
 	int batch, rows, cols;
 	long long batch_inc, rs, cs;
 };
+// the matrix of batch entry i
+inline unsigned char* at(const Mat& m, const int i) { return m.p + i * m.batch_inc * (long long)m.esz; }
 
 // ccv_nnc_tensor_get_matrix_params (lib/nnc/ccv_nnc_easy.h:421-444) for nd <= 3
 bool mat_of(const TV& v, const int transpose[2], Mat& m)
 {
 	if (v.nd < 1 || v.nd > 3)
 		return false;
-	m.p = (float*)v.p;
+	m.p = v.p;
+	m.esz = dtype_size(v.datatype);
 	m.batch = v.nd < 3 ? 1 : v.dim[v.nd - 3];
 	m.batch_inc = v.nd < 3 ? 0 : v.stride[v.nd - 3];
 	m.rows = v.nd == 1 ? 1 : v.dim[v.nd - 2];
@@ -204,8 +208,9 @@ int conv_algorithm(const ccv_nnc_cmd_t& cmd)
 	return CCV_NNC_SM100_ALGO_TF32;
 }
 
-// C[M, N] (+)= A[M, K] * B[K, N] + bias over arbitrary (row, col) element strides
-int gemm_dispatch(cudaStream_t s, const Scratch& scratch, const int algorithm, const int M, const int N, const int K, const float* a, long long a_rs, long long a_cs, const float* b, long long b_rs, long long b_cs, float* c, long long c_rs, long long c_cs, const float* bias, const int accumulate)
+// C[M, N] (+)= A[M, K] * B[K, N] + bias over arbitrary (row, col) element strides, element kind `kind` (0 = fp32, 1 = bf16,
+// 2 = fp16; the algorithm only matters for fp32); bias fp32 (bias32) or of the 16-bit kind (bias16)
+int gemm_dispatch(cudaStream_t s, const Scratch& scratch, const int kind, const int algorithm, const int M, const int N, const int K, const void* a, long long a_rs, long long a_cs, const void* b, long long b_rs, long long b_cs, void* c, long long c_rs, long long c_cs, const float* bias32, const void* bias16, const int accumulate)
 {
 	if (M <= 0 || N <= 0)
 		return 0;
@@ -213,14 +218,11 @@ int gemm_dispatch(cudaStream_t s, const Scratch& scratch, const int algorithm, c
 		return 1;
 	if (c_cs != 1 && N > 1)
 	{
-		if (c_rs != 1 && M > 1)
+		if ((c_rs != 1 && M > 1) || bias32 || bias16)
 			return 1;
-		if (bias)
-			return 1;
-		// C^T = B^T A^T
-		return gemm_dispatch(s, scratch, algorithm, N, M, K, b, b_cs, b_rs, a, a_cs, a_rs, c, c_cs, 1, 0, accumulate);
+		return gemm_dispatch(s, scratch, kind, algorithm, N, M, K, b, b_cs, b_rs, a, a_cs, a_rs, c, c_cs, 1, 0, 0, accumulate); // C^T = B^T A^T
 	}
-	if (algorithm != CCV_NNC_SM100_ALGO_FFMA)
+	if (kind != 0 || algorithm != CCV_NNC_SM100_ALGO_FFMA)
 	{
 		int ta = -1, tb = -1;
 		long long lda = 0, ldb = 0;
@@ -234,44 +236,14 @@ int gemm_dispatch(cudaStream_t s, const Scratch& scratch, const int algorithm, c
 			tb = 1, ldb = b_cs;
 		if (ta >= 0 && tb >= 0)
 		{
-			const int rc = gemm_tf32(s, M, N, K, a, lda, ta, b, ldb, tb, c, c_rs, bias, accumulate, scratch, algorithm == CCV_NNC_SM100_ALGO_3XTF32);
+			const int rc = gemm_any(s, kind, M, N, K, a, lda, ta, b, ldb, tb, c, c_rs, bias32, bias16, accumulate, scratch, algorithm == CCV_NNC_SM100_ALGO_3XTF32);
 			if (rc <= 0)
 				return rc;
 		}
 	}
-	return gemm_ffma(s, M, N, K, a, a_rs, a_cs, b, b_rs, b_cs, c, c_rs, bias, accumulate, scratch);
-}
-
-// the same for 16-bit tensors (kind 1 = bf16, 2 = fp16): tensor-core path only (unit stride along one axis of every operand)
-int gemm_dispatch16(cudaStream_t s, const Scratch& scratch, const int kind, const int M, const int N, const int K, const void* a, long long a_rs, long long a_cs, const void* b, long long b_rs, long long b_cs, void* c, long long c_rs, long long c_cs, const float* bias32, const void* bias16, const int accumulate)
-{
-	if (M <= 0 || N <= 0)
-		return 0;
-	if (K <= 0)
-		return 1;
-	if (c_cs != 1 && N > 1)
-	{
-		if ((c_rs != 1 && M > 1) || bias32 || bias16)
-			return 1;
-		return gemm_dispatch16(s, scratch, kind, N, M, K, b, b_cs, b_rs, a, a_cs, a_rs, c, c_cs, 1, 0, 0, accumulate); // C^T = B^T A^T
-	}
-	int ta = -1, tb = -1;
-	long long lda = 0, ldb = 0;
-	if (a_cs == 1 || K == 1)
-		ta = 0, lda = a_rs;
-	else if (a_rs == 1 || M == 1)
-		ta = 1, lda = a_cs;
-	if (b_cs == 1 || N == 1)
-		tb = 0, ldb = b_rs;
-	else if (b_rs == 1 || K == 1)
-		tb = 1, ldb = b_cs;
-	if (ta >= 0 && tb >= 0)
-	{
-		const int rc = gemm_16(s, kind, M, N, K, a, lda, ta, b, ldb, tb, c, c_rs, bias32, bias16, accumulate, scratch);
-		if (rc <= 0)
-			return rc;
-	}
-	// Shapes the tensor-core path cannot take (a leading dimension that is not a multiple of 16 bytes, e.g. a 10-class head):
+	if (kind == 0)
+		return gemm_ffma(s, M, N, K, (const float*)a, a_rs, a_cs, (const float*)b, b_rs, b_cs, (float*)c, c_rs, bias32, accumulate, scratch);
+	// 16-bit shapes the tensor-core path cannot take (a leading dimension that is not a multiple of 16 bytes, e.g. a 10-class head):
 	// widen the operands into the command's scratch, multiply in fp32 on the CUDA cores, narrow the result (one rounding).  Small
 	// by construction: anything large has TMA-friendly strides.
 	const size_t need = ((size_t)M * K + (size_t)K * N + (size_t)M * N + (size_t)N) * sizeof(float) + 1024;
@@ -354,28 +326,21 @@ int exec_gemm_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 	if (!ws)
 		return CCV_NNC_EXEC_OOM;
 	const Scratch scratch = scratch_at(ws, CONTRACT_SCRATCH_BYTES);
+	const int algorithm = gemm_algorithm(cmd);
 	if (matrix_bias)
 	{
 		for (int i = 0; i < b.batch; i++)
 		{
-			RC(gemm_dispatch(s, scratch, gemm_algorithm(cmd), b.rows, b.cols, a.cols, a.p + i * a.batch_inc, a.rs, a.cs, w.p + i * w.batch_inc, w.rs, w.cs, b.p + i * b.batch_inc, b.rs, b.cs, 0, 0));
+			RC(gemm_dispatch(s, scratch, 0, algorithm, b.rows, b.cols, a.cols, at(a, i), a.rs, a.cs, at(w, i), w.rs, w.cs, at(b, i), b.rs, b.cs, 0, 0, 0));
 			const int d4[4] = { 1, 1, b.rows, b.cols }, cs4[4] = { 0, 0, (int)b.rs, 1 }, ds4[4] = { 0, 0, (int)bias.rs, 1 };
-			RC(ew_axpby_bcast_f32(s, 1.f, b.p + i * b.batch_inc, cs4, 1.f, bias.p + i * bias.batch_inc, ds4, b.p + i * b.batch_inc, cs4, d4));
+			RC(ew_axpby_bcast_f32(s, 1.f, (const float*)at(b, i), cs4, 1.f, (const float*)at(bias, i), ds4, (float*)at(b, i), cs4, d4));
 		}
 		return CCV_NNC_EXEC_SUCCESS;
 	}
-	if (kind != 0)
-	{
-		// 16-bit operands: wgmma (bf16 / fp16), fp32 accumulate; the bias may be fp32 or in the operands' type
-		const char* const bias_p = bias_t ? (const char*)bias.p : 0;
-		const bool bias32 = bias_t && is_f32(bias_t);
-		for (int i = 0; i < b.batch; i++)
-			RC(gemm_dispatch16(s, scratch, kind, b.rows, b.cols, a.cols, (const char*)a.p + (size_t)i * a.batch_inc * 2, a.rs, a.cs, (const char*)w.p + (size_t)i * w.batch_inc * 2, w.rs, w.cs, (char*)b.p + (size_t)i * b.batch_inc * 2, b.rs, b.cs,
-				bias32 ? (const float*)(bias_p + (size_t)i * bias.batch_inc * 4) : 0, bias_t && !bias32 ? bias_p + (size_t)i * bias.batch_inc * 2 : 0, 0));
-		return CCV_NNC_EXEC_SUCCESS;
-	}
+	// the bias is fp32 or in the operands' type
+	const bool bias32 = bias_t && is_f32(bias_t);
 	for (int i = 0; i < b.batch; i++)
-		RC(gemm_dispatch(s, scratch, gemm_algorithm(cmd), b.rows, b.cols, a.cols, a.p + i * a.batch_inc, a.rs, a.cs, w.p + i * w.batch_inc, w.rs, w.cs, b.p + i * b.batch_inc, b.rs, b.cs, bias_t ? bias.p + i * bias.batch_inc : 0, 0));
+		RC(gemm_dispatch(s, scratch, kind, algorithm, b.rows, b.cols, a.cols, at(a, i), a.rs, a.cs, at(w, i), w.rs, w.cs, at(b, i), b.rs, b.cs, bias32 ? (const float*)at(bias, i) : 0, bias_t && !bias32 ? at(bias, i) : 0, 0));
 	return CCV_NNC_EXEC_SUCCESS;
 }
 
@@ -390,7 +355,7 @@ int exec_gemm_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 	const int kind = kind_of(inputs[0]);
 	if (kind < 0 || !mat_of(view_of(inputs[0]), no_transpose, g))
 		return CCV_NNC_EXEC_INVALID;
-	const size_t esz = kind_size(kind);
+	const int algorithm = gemm_algorithm(cmd);
 	cudaStream_t s = stream_of(stream_context);
 	const size_t ws_bytes = gemm_back_workspace(cmd, hint, inputs, input_size, outputs, output_size);
 	void* const ws = ws_bytes ? ccv_nnc_stream_context_get_workspace(stream_context, ws_bytes, CCV_TENSOR_GPU_MEMORY) : 0;
@@ -410,8 +375,10 @@ int exec_gemm_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 		const int db_kind = kind_of(dbias_t);
 		if (db_kind < 0)
 			return CCV_NNC_EXEC_INVALID;
+		if (db.batch == 1)
+			db.batch_inc = 0;
 		for (int i = 0; i < g.batch; i++)
-			RC(colsum_any(s, kind, (const char*)g.p + (size_t)i * g.batch_inc * esz, g.rows, g.cols, g.rs, (char*)db.p + (db.batch == 1 ? 0 : (size_t)i * db.batch_inc * kind_size(db_kind)), db_kind, accumulate || (db.batch == 1 && i > 0), ws));
+			RC(colsum_any(s, kind, at(g, i), g.rows, g.cols, g.rs, at(db, i), db_kind, accumulate || (db.batch == 1 && i > 0), ws));
 	}
 	if (dw_t)
 	{
@@ -424,14 +391,11 @@ int exec_gemm_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 			return CCV_NNC_EXEC_INVALID;
 		if (a.batch == 1)
 			a.batch_inc = 0;
+		if (dw.batch == 1)
+			dw.batch_inc = 0;
 		// dw[K, N] = a^T[K, M] * g[M, N]; a shared dw sums over the batch
-		if (kind != 0)
-		{
-			for (int i = 0; i < g.batch; i++)
-				RC(gemm_dispatch16(s, scratch, kind, dw.rows, dw.cols, g.rows, (const char*)a.p + (size_t)i * a.batch_inc * 2, a.cs, a.rs, (const char*)g.p + (size_t)i * g.batch_inc * 2, g.rs, g.cs, (char*)dw.p + (dw.batch == 1 ? 0 : (size_t)i * dw.batch_inc * 2), dw.rs, dw.cs, 0, 0, accumulate || (dw.batch == 1 && i > 0)));
-		} else
 		for (int i = 0; i < g.batch; i++)
-			RC(gemm_dispatch(s, scratch, gemm_algorithm(cmd), dw.rows, dw.cols, g.rows, a.p + i * a.batch_inc, a.cs, a.rs, g.p + i * g.batch_inc, g.rs, g.cs, dw.p + (dw.batch == 1 ? 0 : i * dw.batch_inc), dw.rs, dw.cs, 0, accumulate || (dw.batch == 1 && i > 0)));
+			RC(gemm_dispatch(s, scratch, kind, algorithm, dw.rows, dw.cols, g.rows, at(a, i), a.cs, a.rs, at(g, i), g.rs, g.cs, at(dw, i), dw.rs, dw.cs, 0, 0, accumulate || (dw.batch == 1 && i > 0)));
 	}
 	if (h_t)
 	{
@@ -444,14 +408,11 @@ int exec_gemm_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 			return CCV_NNC_EXEC_INVALID;
 		if (w.batch == 1)
 			w.batch_inc = 0;
+		if (h.batch == 1)
+			h.batch_inc = 0;
 		// h[M, K] = g[M, N] * w^T[N, K]
-		if (kind != 0)
-		{
-			for (int i = 0; i < g.batch; i++)
-				RC(gemm_dispatch16(s, scratch, kind, h.rows, h.cols, g.cols, (const char*)g.p + (size_t)i * g.batch_inc * 2, g.rs, g.cs, (const char*)w.p + (size_t)i * w.batch_inc * 2, w.cs, w.rs, (char*)h.p + (h.batch == 1 ? 0 : (size_t)i * h.batch_inc * 2), h.rs, h.cs, 0, 0, accumulate || (h.batch == 1 && i > 0)));
-		} else
 		for (int i = 0; i < g.batch; i++)
-			RC(gemm_dispatch(s, scratch, gemm_algorithm(cmd), h.rows, h.cols, g.cols, g.p + i * g.batch_inc, g.rs, g.cs, w.p + i * w.batch_inc, w.cs, w.rs, h.p + (h.batch == 1 ? 0 : i * h.batch_inc), h.rs, h.cs, 0, accumulate || (h.batch == 1 && i > 0)));
+			RC(gemm_dispatch(s, scratch, kind, algorithm, h.rows, h.cols, g.cols, at(g, i), g.rs, g.cs, at(w, i), w.cs, w.rs, at(h, i), h.rs, h.cs, 0, 0, accumulate || (h.batch == 1 && i > 0)));
 	}
 	return CCV_NNC_EXEC_SUCCESS;
 }
@@ -639,7 +600,7 @@ bool group_plan(const ConvGeom& g, const int kind, const int groups, const int p
 	const size_t nx = (size_t)g.N * g.H * g.W * Cg, ny = (size_t)g.N * g.P * g.Q * Kg;
 	p.xb = (nx * es + 255) & ~(size_t)255, p.yb = (ny * es + 255) & ~(size_t)255;
 	// the fp32 data gradient's workspace, else the split-K scratch
-	p.inner = pass == 2 && kind == 0 ? conv_dgrad_workspace_bytes(gg) : CONTRACT_SCRATCH_BYTES;
+	p.inner = pass == 2 ? conv_dgrad_workspace_bytes(gg, kind) : CONTRACT_SCRATCH_BYTES;
 	return true;
 }
 // returns 0 done, 1 not applicable (caller falls back), < 0 error; ws holds the group plan's bytes
@@ -671,10 +632,7 @@ int conv_grouped_tc(cudaStream_t s, unsigned char* const ws, const int kind, con
 			// y_i = conv(x_i, w_i) + bias_i
 			if (copy_strided(s, act_i, xs_t, xg, xs_d, xd, (int)es))
 				return -1;
-			if (kind == 0)
-				rc = conv_fprop_tf32(s, gg, (const float*)xg, (const float*)w_i, bias32 ? bias32 + (size_t)i * Kg : 0, (float*)yg, scratch, x3);
-			else
-				rc = conv_fprop_16(s, kind, gg, xg, w_i, bias32 ? bias32 + (size_t)i * Kg : 0, bias16 ? (const unsigned char*)bias16 + (size_t)i * Kg * 2 : 0, yg, scratch);
+			rc = conv_fprop_any(s, kind, gg, xg, w_i, bias32 ? bias32 + (size_t)i * Kg : 0, bias16 ? (const unsigned char*)bias16 + (size_t)i * Kg * 2 : 0, yg, scratch, x3);
 			if (rc)
 				return i == 0 ? rc : -1;
 			if (copy_strided(s, yg, ys_d, (unsigned char*)out + (size_t)i * Kg * es, ys_t, yd, (int)es))
@@ -683,23 +641,14 @@ int conv_grouped_tc(cudaStream_t s, unsigned char* const ws, const int kind, con
 			// dw_i (+)= wgrad(g_i, x_i): the filter gradient's rows of a group are contiguous
 			if (copy_strided(s, act_i, xs_t, xg, xs_d, xd, (int)es) || copy_strided(s, res_i, ys_t, yg, ys_d, yd, (int)es))
 				return -1;
-			unsigned char* const dw_i = (unsigned char*)out + (size_t)i * wstep;
-			if (kind == 0)
-				rc = conv_wgrad_tf32(s, gg, (const float*)yg, (const float*)xg, (float*)dw_i, accumulate, scratch, x3);
-			else
-				rc = conv_wgrad_16(s, kind, gg, yg, xg, dw_i, accumulate, scratch);
+			rc = conv_wgrad_any(s, kind, gg, yg, xg, (unsigned char*)out + (size_t)i * wstep, accumulate, scratch, x3);
 			if (rc)
 				return i == 0 ? rc : -1;
 		} else {
 			// h_i = dgrad(g_i, w_i) (+ bias_i: the forward of a transposed convolution, whose outputs are the C side)
 			if (copy_strided(s, res_i, ys_t, yg, ys_d, yd, (int)es))
 				return -1;
-			const float* const bias32_i = bias32 ? bias32 + (size_t)i * Cg : 0;
-			const void* const bias16_i = bias16 ? (const unsigned char*)bias16 + (size_t)i * Cg * 2 : 0;
-			if (kind == 0)
-				rc = conv_dgrad_tf32(s, gg, (const float*)yg, (const float*)w_i, bias32_i, (float*)xg, ws, x3);
-			else
-				rc = conv_dgrad_16(s, kind, gg, yg, w_i, bias32_i, bias16_i, xg, scratch);
+			rc = conv_dgrad_any(s, kind, gg, yg, w_i, bias32 ? bias32 + (size_t)i * Cg : 0, bias16 ? (const unsigned char*)bias16 + (size_t)i * Cg * 2 : 0, xg, ws, x3);
 			if (rc)
 				return i == 0 ? rc : -1;
 			if (copy_strided(s, xg, xs_d, (unsigned char*)out + (size_t)i * Cg * es, xs_t, xd, (int)es))
@@ -710,10 +659,10 @@ int conv_grouped_tc(cudaStream_t s, unsigned char* const ws, const int kind, con
 }
 
 // h = dgrad(gb, w) (+ bias[C]) on the geometry gh, returns a CCV_NNC_EXEC_* status: the data gradient of CONVOLUTION_BACKWARD (no
-// bias) and the forward of CONVOLUTION_TRANSPOSE (bias32 fp32, or bias16 of the tensors' 16-bit type).  fp32: tensor cores for one
-// group, per-group dense launches for wide groups, FFMA for narrow groups, unaligned channels and ALGO_FFMA.  16-bit: tensor cores
-// (wide groups only when grouped); shapes they cannot take (3-channel pixels) run in the functional form -- widen g, w and the bias,
-// fp32 FFMA data gradient + bias, one rounding on the way back.
+// bias) and the forward of CONVOLUTION_TRANSPOSE (bias32 fp32, or bias16 of the tensors' 16-bit type).  Tensor cores for one group,
+// per-group dense launches for wide groups (fp32 unless ALGO_FFMA; 16-bit always).  Where they decline, fp32 runs on FFMA (also
+// narrow groups and unaligned channels); 16-bit shapes they cannot take (3-channel pixels, one group) run in the functional form --
+// widen g, w and the bias, fp32 FFMA data gradient + bias, one rounding on the way back.
 // workspace of the 16-bit functional form below: fp32 copies of g, w, h and the bias, 256-byte aligned
 size_t dgrad16_fallback_bytes(const ConvGeom& gh)
 {
@@ -722,42 +671,34 @@ size_t dgrad16_fallback_bytes(const ConvGeom& gh)
 // ws holds conv_workspace(gh, kind, groups, algo, CONV_DGRAD)
 int dgrad_nhwc(cudaStream_t s, unsigned char* const ws, const int kind, const int algo, const int groups, const ConvGeom& gh, const void* const gb, const void* const w, const float* const bias32, const void* const bias16, void* const h)
 {
-	if (kind > 0)
-	{
-		if (groups > 1)
-			return conv_grouped_tc<2>(s, ws, kind, gh, groups, 0, 0, 0, w, bias32, bias16, gb, h) == 0 ? CCV_NNC_EXEC_SUCCESS : CCV_NNC_EXEC_INVALID;
-		const int rc = conv_dgrad_16(s, kind, gh, gb, w, bias32, bias16, h, scratch_at(ws, CONTRACT_SCRATCH_BYTES));
-		if (rc < 0)
-			return CCV_NNC_EXEC_INVALID;
-		if (rc > 0)
-		{
-			// (the image gradient of a stem, test/int/nnc/cudnn.tests.c:499-577; the RGB head of a transposed convolution)  Dense tensors only.
-			const size_t ng = (size_t)gh.N * gh.P * gh.Q * gh.K, nw = (size_t)gh.K * gh.R * gh.S * gh.C, nh = (size_t)gh.N * gh.H * gh.W * gh.C, nb = bias16 ? gh.C : 0;
-			if (gh.bw != gh.K || gh.bh != (long long)gh.Q * gh.K || gh.bn != (long long)gh.P * gh.Q * gh.K || gh.aw != gh.C || gh.ah != (long long)gh.W * gh.C || gh.an != (long long)gh.H * gh.W * gh.C || ng > 0x7fffffffull || nh > 0x7fffffffull)
-				return CCV_NNC_EXEC_INVALID;
-			float* const g32 = (float*)ws;
-			float* const w32 = (float*)(((uintptr_t)(g32 + ng) + 255) & ~(uintptr_t)255);
-			float* const h32 = (float*)(((uintptr_t)(w32 + nw) + 255) & ~(uintptr_t)255);
-			float* const b32 = (float*)(((uintptr_t)(h32 + nh) + 255) & ~(uintptr_t)255);
-			RC(widen_matrix(s, gb, kind, (long long)ng, 1, g32, 1, (int)ng));
-			RC(widen_matrix(s, w, kind, (long long)nw, 1, w32, 1, (int)nw));
-			if (nb)
-				RC(widen_matrix(s, bias16, kind, (long long)nb, 1, b32, 1, (int)nb));
-			RC(conv_dgrad_ffma(s, gh, 1, g32, w32, nb ? b32 : bias32, h32));
-			RC(narrow_matrix(s, h32, h, kind, (long long)nh, 1, 1, (int)nh, 0));
-		}
-		return CCV_NNC_EXEC_SUCCESS;
-	}
 	const int x3 = algo == CCV_NNC_SM100_ALGO_3XTF32;
 	int rc = 1;
-	if (groups == 1 && algo != CCV_NNC_SM100_ALGO_FFMA)
-		rc = conv_dgrad_tf32(s, gh, (const float*)gb, (const float*)w, bias32, (float*)h, ws, x3);
-	if (groups > 1 && algo != CCV_NNC_SM100_ALGO_FFMA)
-		rc = conv_grouped_tc<2>(s, ws, 0, gh, groups, x3, 0, 0, w, bias32, 0, gb, h);
+	if (kind > 0 || algo != CCV_NNC_SM100_ALGO_FFMA)
+		rc = groups > 1 ? conv_grouped_tc<2>(s, ws, kind, gh, groups, x3, 0, 0, w, bias32, bias16, gb, h) : conv_dgrad_any(s, kind, gh, gb, w, bias32, bias16, h, ws, x3);
 	if (rc < 0)
 		return CCV_NNC_EXEC_INVALID;
-	if (rc > 0)
+	if (rc == 0)
+		return CCV_NNC_EXEC_SUCCESS;
+	if (kind == 0)
+	{
 		RC(conv_dgrad_ffma(s, gh, groups, (const float*)gb, (const float*)w, bias32, (float*)h));
+		return CCV_NNC_EXEC_SUCCESS;
+	}
+	// (the image gradient of a stem, test/int/nnc/cudnn.tests.c:499-577; the RGB head of a transposed convolution)  Dense tensors and
+	// one group only.
+	const size_t ng = (size_t)gh.N * gh.P * gh.Q * gh.K, nw = (size_t)gh.K * gh.R * gh.S * gh.C, nh = (size_t)gh.N * gh.H * gh.W * gh.C, nb = bias16 ? gh.C : 0;
+	if (groups > 1 || gh.bw != gh.K || gh.bh != (long long)gh.Q * gh.K || gh.bn != (long long)gh.P * gh.Q * gh.K || gh.aw != gh.C || gh.ah != (long long)gh.W * gh.C || gh.an != (long long)gh.H * gh.W * gh.C || ng > 0x7fffffffull || nh > 0x7fffffffull)
+		return CCV_NNC_EXEC_INVALID;
+	float* const g32 = (float*)ws;
+	float* const w32 = (float*)(((uintptr_t)(g32 + ng) + 255) & ~(uintptr_t)255);
+	float* const h32 = (float*)(((uintptr_t)(w32 + nw) + 255) & ~(uintptr_t)255);
+	float* const b32 = (float*)(((uintptr_t)(h32 + nh) + 255) & ~(uintptr_t)255);
+	RC(widen_matrix(s, gb, kind, (long long)ng, 1, g32, 1, (int)ng));
+	RC(widen_matrix(s, w, kind, (long long)nw, 1, w32, 1, (int)nw));
+	if (nb)
+		RC(widen_matrix(s, bias16, kind, (long long)nb, 1, b32, 1, (int)nb));
+	RC(conv_dgrad_ffma(s, gh, 1, g32, w32, nb ? b32 : bias32, h32));
+	RC(narrow_matrix(s, h32, h, kind, (long long)nh, 1, 1, (int)nh, 0));
 	return CCV_NNC_EXEC_SUCCESS;
 }
 
@@ -779,7 +720,7 @@ size_t conv_workspace(const ConvGeom& g, const int kind, const int groups, const
 		else if (groups > 1)
 			need = std::max(need, group_plan(g, kind, groups, pass, gp) ? gp.inner + gp.xb + gp.yb : kind == 0 && pass == 1 ? CONTRACT_SCRATCH_BYTES : 0);
 		else {
-			need = std::max(need, pass == 2 && kind == 0 ? conv_dgrad_workspace_bytes(g) : CONTRACT_SCRATCH_BYTES);
+			need = std::max(need, pass == 2 ? conv_dgrad_workspace_bytes(g, kind) : CONTRACT_SCRATCH_BYTES);
 			if (pass < 2 && g.C % (kind == 0 ? 4 : 8) != 0)
 				need = std::max(need, conv_im2col_workspace_bytes(g, kind));
 			if (pass == 2 && kind > 0 && conv_dgrad_may_decline(g, kind))
@@ -827,61 +768,40 @@ int conv_forw_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 	unsigned char* const ws = ws_bytes ? (unsigned char*)ccv_nnc_stream_context_get_workspace(stream_context, ws_bytes, CCV_TENSOR_GPU_MEMORY) : 0;
 	if (ws_bytes && !ws)
 		return CCV_NNC_EXEC_OOM;
-	const Scratch scratch = scratch_at(ws, CONTRACT_SCRATCH_BYTES);
+	// every tensor of one kind; the bias fp32 or of that kind
 	const ccv_nnc_tensor_t* const bias_t = input_size > 2 ? inputs[2] : 0;
 	const int kind = kind_of(inputs[0]);
-	if (kind > 0)
-	{
-		// bf16 / fp16 tensors: NHWC, one group, wgmma bf16 / fp16 with fp32 accumulation; the bias is fp32 or of the tensors' type
-		if (kind_of(inputs[1]) != kind || kind_of(outputs[0]) != kind || (bias_t && ((kind_of(bias_t) != kind && !is_f32(bias_t)) || CCV_IS_TENSOR_VIEW(bias_t))))
-			return CCV_NNC_EXEC_INVALID;
-		ConvGeom g16;
-		if (!conv_geom(cmd, hint, view_of(inputs[0]), view_of(inputs[1]), view_of(outputs[0]), g16) || (bias_t && bias_t->info.dim[0] != g16.K))
-			return CCV_NNC_EXEC_INVALID;
-		cudaStream_t s16 = stream_of(stream_context);
-		const float* const bias32 = bias_t && is_f32(bias_t) ? bias_t->data.f32 : 0;
-		const void* const bias16 = bias_t && !is_f32(bias_t) ? (const void*)bias_t->data.u8 : 0;
-		if (cmd.info.convolution.groups > 1) // wide groups only: there is no 16-bit FFMA kernel to fall back to
-			return conv_grouped_tc<0>(s16, ws, kind, g16, cmd.info.convolution.groups, 0, 0, inputs[0]->data.u8, inputs[1]->data.u8, bias32, bias16, 0, outputs[0]->data.u8) == 0 ? CCV_NNC_EXEC_SUCCESS : CCV_NNC_EXEC_INVALID;
-		int rc = conv_fprop_16(s16, kind, g16, inputs[0]->data.u8, inputs[1]->data.u8, bias32, bias16, outputs[0]->data.u8, scratch);
-		if (rc > 0 && g16.C % 8 != 0) // pixels that TMA cannot address (the 3-channel stem): explicit im2col + tensor-core GEMM
-			rc = conv_fprop_im2col_16(s16, kind, g16, inputs[0]->data.u8, inputs[1]->data.u8, bias32, bias16, outputs[0]->data.u8, ws);
-		return rc == 0 ? CCV_NNC_EXEC_SUCCESS : CCV_NNC_EXEC_INVALID;
-	}
-	if (!is_f32(inputs[0]) || !is_f32(inputs[1]) || !is_f32(outputs[0]) || (bias_t && (!is_f32(bias_t) || CCV_IS_TENSOR_VIEW(bias_t))))
+	if (kind_of(inputs[1]) != kind || kind_of(outputs[0]) != kind || (bias_t && ((kind_of(bias_t) != kind && !is_f32(bias_t)) || CCV_IS_TENSOR_VIEW(bias_t))))
 		return CCV_NNC_EXEC_INVALID;
 	ConvGeom g;
-	const int groups = cmd.info.convolution.groups > 0 ? cmd.info.convolution.groups : 1;
-	const int algo = conv_algorithm(cmd), x3 = algo == CCV_NNC_SM100_ALGO_3XTF32;
+	if (!conv_geom(cmd, hint, view_of(inputs[0]), view_of(inputs[1]), view_of(outputs[0]), g) || (bias_t && bias_t->info.dim[0] != g.K))
+		return CCV_NNC_EXEC_INVALID;
+	const int groups = conv_groups(cmd), algo = conv_algorithm(cmd), x3 = algo == CCV_NNC_SM100_ALGO_3XTF32;
 	cudaStream_t s = stream_of(stream_context);
-	const float* a = inputs[0]->data.f32;
-	const float* w = inputs[1]->data.f32;
-	const float* bias = bias_t ? bias_t->data.f32 : 0;
-	float* b = outputs[0]->data.f32;
-	const TV ta = view_of(inputs[0]), tw = view_of(inputs[1]), tb = view_of(outputs[0]);
-	if (!conv_geom(cmd, hint, ta, tw, tb, g))
-		return CCV_NNC_EXEC_INVALID;
-	if (bias_t && bias_t->info.dim[0] != g.K)
-		return CCV_NNC_EXEC_INVALID;
-	if (groups == 1 && algo != CCV_NNC_SM100_ALGO_FFMA)
+	const void* const a = inputs[0]->data.u8;
+	const void* const w = inputs[1]->data.u8;
+	const float* const bias32 = bias_t && is_f32(bias_t) ? bias_t->data.f32 : 0;
+	const void* const bias16 = bias_t && !is_f32(bias_t) ? (const void*)bias_t->data.u8 : 0;
+	void* const b = outputs[0]->data.u8;
+	int rc = 1;
+	if (kind > 0 || algo != CCV_NNC_SM100_ALGO_FFMA)
 	{
-		int rc = conv_fprop_tf32(s, g, a, w, bias, b, scratch, x3);
-		if (rc > 0 && g.C % 4 != 0) // TMA cannot address 12-byte pixels (the 3-channel stem): explicit im2col + tensor-core GEMM
-			rc = conv_fprop_im2col_tf32(s, g, a, w, bias, b, ws, x3);
-		if (rc == 0)
-			return CCV_NNC_EXEC_SUCCESS;
-		if (rc < 0)
-			return CCV_NNC_EXEC_INVALID;
+		if (groups > 1)
+			rc = conv_grouped_tc<0>(s, ws, kind, g, groups, x3, 0, a, w, bias32, bias16, 0, b);
+		else {
+			rc = conv_fprop_any(s, kind, g, a, w, bias32, bias16, b, scratch_at(ws, CONTRACT_SCRATCH_BYTES), x3);
+			if (rc > 0 && g.C % (16 / kind_size(kind)) != 0) // TMA cannot address pixels of other sizes (the 3-channel stem): explicit im2col + tensor-core GEMM
+				rc = conv_fprop_im2col_any(s, kind, g, a, w, bias32, bias16, b, ws, x3);
+		}
 	}
-	if (groups > 1 && algo != CCV_NNC_SM100_ALGO_FFMA)
+	if (rc < 0)
+		return CCV_NNC_EXEC_INVALID;
+	if (rc > 0)
 	{
-		const int rc = conv_grouped_tc<0>(s, ws, 0, g, groups, x3, 0, a, w, bias, 0, 0, b);
-		if (rc == 0)
-			return CCV_NNC_EXEC_SUCCESS;
-		if (rc < 0)
+		if (kind > 0) // there is no 16-bit FFMA kernel to fall back to (narrow groups among others)
 			return CCV_NNC_EXEC_INVALID;
+		RC(conv_fprop_ffma(s, g, groups, (const float*)a, (const float*)w, bias32, (float*)b));
 	}
-	RC(conv_fprop_ffma(s, g, groups, a, w, bias, b));
 	return CCV_NNC_EXEC_SUCCESS;
 }
 
@@ -895,93 +815,52 @@ int conv_back_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 	unsigned char* const ws = ws_bytes ? (unsigned char*)ccv_nnc_stream_context_get_workspace(stream_context, ws_bytes, CCV_TENSOR_GPU_MEMORY) : 0;
 	if (ws_bytes && !ws)
 		return CCV_NNC_EXEC_OOM;
-	const Scratch scratch = scratch_at(ws, CONTRACT_SCRATCH_BYTES);
 	ccv_nnc_tensor_t* const h_t = outputs[0];
 	ccv_nnc_tensor_t* const dw_t = output_size > 1 ? outputs[1] : 0;
 	ccv_nnc_tensor_t* const dbias_t = output_size > 2 ? outputs[2] : 0;
 	const ccv_nnc_tensor_t* const w_t = input_size > 2 ? inputs[2] : 0;
 	const ccv_nnc_tensor_t* const filt = dw_t ? dw_t : w_t;
+	// every operand is checked before the first launch: a refused call leaves the outputs as they were
 	const int kind = kind_of(inputs[0]);
-	if (kind > 0 && filt)
-	{
-		// bf16 / fp16: the same three products on the kind::f16 kernels; dbias in fp32 or the tensors' type
-		if (kind_of(inputs[1]) != kind || kind_of(filt) != kind || (h_t && kind_of(h_t) != kind) || (w_t && kind_of(w_t) != kind))
-			return CCV_NNC_EXEC_INVALID;
-		const int groups16 = cmd.info.convolution.groups > 1 ? cmd.info.convolution.groups : 1;
-		ConvGeom g16;
-		if (!conv_geom(cmd, hint, view_of(inputs[1]), view_of(filt), view_of(inputs[0]), g16))
-			return CCV_NNC_EXEC_INVALID;
-		const int acc16 = (flags & CCV_NNC_ACCUMULATE_OUTPUT) ? 1 : 0;
-		cudaStream_t s16 = stream_of(stream_context);
-		if (dbias_t)
-		{
-			const int db_kind = kind_of(dbias_t);
-			if (db_kind < 0 || dbias_t->info.dim[0] != g16.K || g16.bh != (long long)g16.Q * g16.bw || g16.bn != (long long)g16.P * g16.bh)
-				return CCV_NNC_EXEC_INVALID;
-			RC(colsum_any(s16, kind, inputs[0]->data.u8, (size_t)g16.N * g16.P * g16.Q, g16.K, g16.bw, dbias_t->data.u8, db_kind, acc16, ws));
-		}
-		if (dw_t && groups16 > 1)
-		{
-			if (conv_grouped_tc<1>(s16, ws, kind, g16, groups16, 0, acc16, inputs[1]->data.u8, 0, 0, 0, inputs[0]->data.u8, dw_t->data.u8))
-				return CCV_NNC_EXEC_INVALID;
-		} else if (dw_t) {
-			int rc = conv_wgrad_16(s16, kind, g16, inputs[0]->data.u8, inputs[1]->data.u8, dw_t->data.u8, acc16, scratch);
-			if (rc > 0 && g16.C % 8 != 0)
-				rc = conv_wgrad_im2col_16(s16, kind, g16, inputs[0]->data.u8, inputs[1]->data.u8, dw_t->data.u8, acc16, ws);
-			if (rc)
-				return CCV_NNC_EXEC_INVALID;
-		}
-		if (h_t)
-		{
-			ConvGeom gh16;
-			if (!w_t || !conv_geom(cmd, hint, view_of(h_t), view_of(w_t), view_of(inputs[0]), gh16))
-				return CCV_NNC_EXEC_INVALID;
-			return dgrad_nhwc(s16, ws, kind, CCV_NNC_SM100_ALGO_TF32, groups16, gh16, inputs[0]->data.u8, w_t->data.u8, 0, 0, h_t->data.u8);
-		}
-		return CCV_NNC_EXEC_SUCCESS;
-	}
-	if (!filt || !is_f32(inputs[0]) || !is_f32(inputs[1]))
+	if (!filt || kind_of(inputs[1]) != kind || kind_of(filt) != kind || (h_t && kind_of(h_t) != kind) || (w_t && kind_of(w_t) != kind))
 		return CCV_NNC_EXEC_INVALID;
-	ConvGeom g;
+	ConvGeom g, gh;
 	if (!conv_geom(cmd, hint, view_of(inputs[1]), view_of(filt), view_of(inputs[0]), g))
 		return CCV_NNC_EXEC_INVALID;
-	const int groups = cmd.info.convolution.groups > 0 ? cmd.info.convolution.groups : 1;
+	if (h_t && (!w_t || !conv_geom(cmd, hint, view_of(h_t), view_of(w_t), view_of(inputs[0]), gh)))
+		return CCV_NNC_EXEC_INVALID;
+	// dbias in fp32, or for 16-bit gradients also in their type
+	const int db_kind = dbias_t ? kind_of(dbias_t) : 0;
+	if (dbias_t && (db_kind < 0 || (kind == 0 && db_kind != 0) || dbias_t->info.dim[0] != g.K || g.bh != (long long)g.Q * g.bw || g.bn != (long long)g.P * g.bh))
+		return CCV_NNC_EXEC_INVALID;
+	const int groups = conv_groups(cmd);
 	const int accumulate = (flags & CCV_NNC_ACCUMULATE_OUTPUT) ? 1 : 0;
 	const int algo = conv_algorithm(cmd), x3 = algo == CCV_NNC_SM100_ALGO_3XTF32;
 	cudaStream_t s = stream_of(stream_context);
-	const float* gb = inputs[0]->data.f32;
-	const float* a = inputs[1]->data.f32;
+	const void* const gb = inputs[0]->data.u8;
+	const void* const a = inputs[1]->data.u8;
 	if (dbias_t)
-	{
-		if (dbias_t->info.dim[0] != g.K || g.bh != (long long)g.Q * g.bw || g.bn != (long long)g.P * g.bh)
-			return CCV_NNC_EXEC_INVALID;
-		RC(colsum_f32(s, gb, (size_t)g.N * g.P * g.Q, g.K, g.bw, dbias_t->data.f32, accumulate, ws));
-	}
+		RC(colsum_any(s, kind, gb, (size_t)g.N * g.P * g.Q, g.K, g.bw, dbias_t->data.u8, db_kind, accumulate, ws));
 	if (dw_t)
 	{
 		int rc = 1;
-		if (groups == 1 && algo != CCV_NNC_SM100_ALGO_FFMA)
+		if (kind > 0 || algo != CCV_NNC_SM100_ALGO_FFMA)
 		{
-			rc = conv_wgrad_tf32(s, g, gb, a, dw_t->data.f32, accumulate, scratch, x3);
-			if (rc > 0 && g.C % 4 != 0)
-				rc = conv_wgrad_im2col_tf32(s, g, gb, a, dw_t->data.f32, accumulate, ws, x3);
+			if (groups > 1)
+				rc = conv_grouped_tc<1>(s, ws, kind, g, groups, x3, accumulate, a, 0, 0, 0, gb, dw_t->data.u8);
+			else {
+				rc = conv_wgrad_any(s, kind, g, gb, a, dw_t->data.u8, accumulate, scratch_at(ws, CONTRACT_SCRATCH_BYTES), x3);
+				if (rc > 0 && g.C % (16 / kind_size(kind)) != 0)
+					rc = conv_wgrad_im2col_any(s, kind, g, gb, a, dw_t->data.u8, accumulate, ws, x3);
+			}
 		}
-		if (groups > 1 && algo != CCV_NNC_SM100_ALGO_FFMA)
-			rc = conv_grouped_tc<1>(s, ws, 0, g, groups, x3, accumulate, a, 0, 0, 0, gb, dw_t->data.f32);
-		if (rc < 0)
+		if (rc < 0 || (rc > 0 && kind > 0))
 			return CCV_NNC_EXEC_INVALID;
 		if (rc > 0)
-			RC(conv_wgrad_ffma(s, g, groups, gb, a, dw_t->data.f32, accumulate, scratch));
+			RC(conv_wgrad_ffma(s, g, groups, (const float*)gb, (const float*)a, dw_t->data.f32, accumulate, scratch_at(ws, CONTRACT_SCRATCH_BYTES)));
 	}
 	if (h_t)
-	{
-		if (!w_t || !is_f32(h_t))
-			return CCV_NNC_EXEC_INVALID;
-		ConvGeom gh;
-		if (!conv_geom(cmd, hint, view_of(h_t), view_of(w_t), view_of(inputs[0]), gh))
-			return CCV_NNC_EXEC_INVALID;
-		return dgrad_nhwc(s, ws, 0, algo, groups, gh, gb, w_t->data.f32, 0, 0, h_t->data.f32);
-	}
+		return dgrad_nhwc(s, ws, kind, algo, groups, gh, gb, w_t->data.u8, 0, 0, h_t->data.u8);
 	return CCV_NNC_EXEC_SUCCESS;
 }
 
@@ -1335,10 +1214,7 @@ int conv_transpose_back_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint,
 		// dbias[c] (+)= sum over the pixels of g, which are the mirrored convolution's input pixels
 		const int accumulate = (flags & CCV_NNC_ACCUMULATE_OUTPUT) ? 1 : 0;
 		cudaStream_t s = stream_of(stream_context);
-		if (kind == 0)
-			RC(colsum_f32(s, g_t->data.f32, (size_t)g.N * g.H * g.W, g.C, g.aw, dbias_t->data.f32, accumulate, ws));
-		else
-			RC(colsum_any(s, kind, g_t->data.u8, (size_t)g.N * g.H * g.W, g.C, g.aw, dbias_t->data.u8, db_kind, accumulate, ws));
+		RC(colsum_any(s, kind, g_t->data.u8, (size_t)g.N * g.H * g.W, g.C, g.aw, dbias_t->data.u8, db_kind, accumulate, ws));
 	}
 	return CCV_NNC_EXEC_SUCCESS;
 }
@@ -2509,9 +2385,7 @@ int backend_gemm_nt_bias(void* stream_context, int kind, int M, int N, int K, co
 	ccv_nnc_stream_context_t* const ctx = (ccv_nnc_stream_context_t*)stream_context;
 	const Scratch scratch = scratch_of(ctx);
 	cudaStream_t s = stream_of(ctx);
-	if (kind == 0)
-		return gemm_dispatch(s, scratch, CCV_NNC_SM100_ALGO_3XTF32, M, N, K, (const float*)a, K, 1, (const float*)w, 1, K, (float*)c, N, 1, (const float*)bias, 0);
-	return gemm_dispatch16(s, scratch, kind, M, N, K, a, K, 1, w, 1, K, c, N, 1, bias && bias_is_f32 ? (const float*)bias : 0, bias && !bias_is_f32 ? bias : 0, 0);
+	return gemm_dispatch(s, scratch, kind, CCV_NNC_SM100_ALGO_3XTF32, M, N, K, a, K, 1, w, 1, K, c, N, 1, bias && bias_is_f32 ? (const float*)bias : 0, bias && !bias_is_f32 ? bias : 0, 0);
 }
 bool backend_qx_ok(const void* const tensor, const int dense)
 {

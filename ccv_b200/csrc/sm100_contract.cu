@@ -524,7 +524,7 @@ static inline size_t slice_bytes(long long rows, long long cols)
 }
 
 // C[M, N] (+)= op(A) * op(B) + bias for element kind `kind` (bias: fp32 `bias`, or for 16-bit kinds `bias16` in the element type)
-static int gemm_any(cudaStream_t stream, int kind, int M, int N, int K, const void* a, long long lda, int trans_a, const void* b, long long ldb, int trans_b, void* c, long long ldc, const float* bias, const void* bias16, int accumulate, const Scratch& scratch, int x3)
+int gemm_any(cudaStream_t stream, int kind, int M, int N, int K, const void* a, long long lda, int trans_a, const void* b, long long ldb, int trans_b, void* c, long long ldc, const float* bias, const void* bias16, int accumulate, const Scratch& scratch, int x3)
 {
 	const X3Scope math(kind == 0 ? x3 : 0);
 	if (!tma_api_init() || M <= 0 || N <= 0 || K <= 0)
@@ -561,16 +561,6 @@ static int gemm_any(cudaStream_t stream, int kind, int M, int N, int K, const vo
 		return launch_umma_split<OP_MN2D, OP_K2D>(stream, tmA, tmB, p, bn, kind, scratch, M, N, c, ldc, accumulate);
 	return launch_umma_split<OP_MN2D, OP_MN2D>(stream, tmA, tmB, p, bn, kind, scratch, M, N, c, ldc, accumulate);
 }
-int gemm_tf32(cudaStream_t stream, int M, int N, int K, const float* a, long long lda, int trans_a, const float* b, long long ldb, int trans_b, float* c, long long ldc, const float* bias, int accumulate, const Scratch& scratch, int x3)
-{
-	return gemm_any(stream, 0, M, N, K, a, lda, trans_a, b, ldb, trans_b, c, ldc, bias, 0, accumulate, scratch, x3);
-}
-int gemm_16(cudaStream_t stream, int kind, int M, int N, int K, const void* a, long long lda, int trans_a, const void* b, long long ldb, int trans_b, void* c, long long ldc, const float* bias32, const void* bias16, int accumulate, const Scratch& scratch)
-{
-	if (kind != 1 && kind != 2)
-		return 1;
-	return gemm_any(stream, kind, M, N, K, a, lda, trans_a, b, ldb, trans_b, c, ldc, bias32, bias16, accumulate, scratch, 0);
-}
 
 static bool conv_is_pointwise(const ConvGeom& g)
 {
@@ -595,7 +585,7 @@ static bool conv_shape_consistent(const ConvGeom& g)
 		g.R * g.S <= UMMA_MAX_TAPS && g.C % 4 == 0 && g.K % 4 == 0;
 }
 
-static int conv_fprop_any(cudaStream_t stream, int kind, const ConvGeom& g, const void* a, const void* w, const float* bias, const void* bias16, void* b, const Scratch& scratch, int x3)
+int conv_fprop_any(cudaStream_t stream, int kind, const ConvGeom& g, const void* a, const void* w, const float* bias, const void* bias16, void* b, const Scratch& scratch, int x3)
 {
 	const X3Scope math(kind == 0 ? x3 : 0);
 	if (!tma_api_init() || !conv_shape_consistent(g) || !conv_out_contiguous(g) || g.C % kind_align(kind) || g.K % kind_align(kind))
@@ -634,14 +624,6 @@ static int conv_fprop_any(cudaStream_t stream, int kind, const ConvGeom& g, cons
 	p.rowmap.mode = 0, p.rowmap.ld = g.K;
 	return launch_kind<OP_IM2COL, OP_K2D>(stream, tmA, tmB, p, bn, kind, kind != 0);
 }
-int conv_fprop_tf32(cudaStream_t stream, const ConvGeom& g, const float* a, const float* w, const float* bias, float* b, const Scratch& scratch, int x3)
-{
-	return conv_fprop_any(stream, 0, g, a, w, bias, 0, b, scratch, x3);
-}
-int conv_fprop_16(cudaStream_t stream, int kind, const ConvGeom& g, const void* a, const void* w, const float* bias32, const void* bias16, void* b, const Scratch& scratch)
-{
-	return kind == 1 || kind == 2 ? conv_fprop_any(stream, kind, g, a, w, bias32, bias16, b, scratch, 0) : 1;
-}
 
 // The data gradient reads the filters w[K, R*S*C] as its B operand with k = the output channel.  wgmma reads TF32 operands K-major
 // only, so fp32 filters are first copied to wt[R*S*C, K] ([tap][c][k], the head of the workspace) and taken as a K-major B: the
@@ -651,9 +633,9 @@ static size_t dgrad_filter_copy_bytes(const ConvGeom& g)
 {
 	return ((size_t)g.K * g.R * g.S * g.C * sizeof(float) + 511) & ~(size_t)511;
 }
-size_t conv_dgrad_workspace_bytes(const ConvGeom& g)
+size_t conv_dgrad_workspace_bytes(const ConvGeom& g, int kind)
 {
-	return dgrad_filter_copy_bytes(g) + CONTRACT_SCRATCH_BYTES;
+	return (kind == 0 ? dgrad_filter_copy_bytes(g) : 0) + CONTRACT_SCRATCH_BYTES;
 }
 
 // out[m, c] = bias[c] over a dense [rows, C] tensor of element kind `kind` (fp32 bias32, or bias16 in the output's 16-bit type): the
@@ -681,10 +663,12 @@ bool conv_dgrad_may_decline(const ConvGeom& g, int kind)
 	return span_h > 62 || span_w > 62;
 }
 
-// wt: room for the fp32 filter copy (kind 0; NULL for 16-bit kinds).  bias (fp32) / bias16 (16-bit kinds): added in the epilogue of
+// workspace: [fp32 filter copy (kind 0 only) | split-K scratch].  bias (fp32) / bias16 (16-bit kinds): added in the epilogue of
 // every launch, and broadcast into the pixels of tap-less residue classes
-static int conv_dgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, const void* grad_b, const void* w, const float* bias, const void* bias16, float* wt, void* grad_a, const Scratch& scratch, int x3)
+int conv_dgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, const void* grad_b, const void* w, const float* bias, const void* bias16, void* grad_a, void* workspace, int x3)
 {
+	float* const wt = kind == 0 ? (float*)workspace : 0;
+	const Scratch scratch = { (char*)workspace + (kind == 0 ? dgrad_filter_copy_bytes(g) : 0), CONTRACT_SCRATCH_BYTES };
 	if (bias)
 		bias16 = 0;
 	const X3Scope math(kind == 0 ? x3 : 0);
@@ -826,17 +810,8 @@ static int conv_dgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, cons
 		}
 	return 0;
 }
-int conv_dgrad_tf32(cudaStream_t stream, const ConvGeom& g, const float* grad_b, const float* w, const float* bias, float* grad_a, void* workspace, int x3)
-{
-	const Scratch scratch = { (char*)workspace + dgrad_filter_copy_bytes(g), CONTRACT_SCRATCH_BYTES };
-	return conv_dgrad_any(stream, 0, g, grad_b, w, bias, 0, (float*)workspace, grad_a, scratch, x3);
-}
-int conv_dgrad_16(cudaStream_t stream, int kind, const ConvGeom& g, const void* grad_b, const void* w, const float* bias32, const void* bias16, void* grad_a, const Scratch& scratch)
-{
-	return kind == 1 || kind == 2 ? conv_dgrad_any(stream, kind, g, grad_b, w, bias32, bias16, 0, grad_a, scratch, 0) : 1;
-}
 
-static int conv_wgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, const void* grad_b, const void* a, void* grad_w, int accumulate, const Scratch& scratch, int x3)
+int conv_wgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, const void* grad_b, const void* a, void* grad_w, int accumulate, const Scratch& scratch, int x3)
 {
 	const X3Scope math(kind == 0 ? x3 : 0);
 	if (!tma_api_init() || !conv_shape_consistent(g) || !conv_out_contiguous(g) || g.C % kind_align(kind) || g.K % kind_align(kind))
@@ -883,14 +858,6 @@ static int conv_wgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, cons
 			p.tap_off_w[t] = (unsigned short)(s * g.dil_w);
 		}
 	return launch_umma_split<OP_MN2D, OP_IM2COL>(stream, tmA, tmB, p, bn, kind, scratch, g.K, (int)rsc, grad_w, rsc, accumulate);
-}
-int conv_wgrad_tf32(cudaStream_t stream, const ConvGeom& g, const float* grad_b, const float* a, float* grad_w, int accumulate, const Scratch& scratch, int x3)
-{
-	return conv_wgrad_any(stream, 0, g, grad_b, a, grad_w, accumulate, scratch, x3);
-}
-int conv_wgrad_16(cudaStream_t stream, int kind, const ConvGeom& g, const void* grad_b, const void* a, void* grad_w, int accumulate, const Scratch& scratch)
-{
-	return kind == 1 || kind == 2 ? conv_wgrad_any(stream, kind, g, grad_b, a, grad_w, accumulate, scratch, 0) : 1;
 }
 
 // ------------------------------------------------------------------------------------------------ explicit im2col
@@ -1017,22 +984,18 @@ static int conv_wgrad_im2col_t(cudaStream_t stream, const ConvGeom& g, const T* 
 	count_launch();
 	return 0;
 }
-int conv_fprop_im2col_tf32(cudaStream_t stream, const ConvGeom& g, const float* a, const float* w, const float* bias, float* b, void* workspace, int x3)
+int conv_fprop_im2col_any(cudaStream_t stream, int kind, const ConvGeom& g, const void* a, const void* w, const float* bias32, const void* bias16, void* b, void* workspace, int x3)
 {
-	return conv_fprop_im2col_t<float>(stream, g, a, w, bias, 0, b, workspace, x3);
-}
-int conv_wgrad_im2col_tf32(cudaStream_t stream, const ConvGeom& g, const float* grad_b, const float* a, float* grad_w, int accumulate, void* workspace, int x3)
-{
-	return conv_wgrad_im2col_t<float>(stream, g, grad_b, a, grad_w, accumulate, workspace, x3);
-}
-int conv_fprop_im2col_16(cudaStream_t stream, int kind, const ConvGeom& g, const void* a, const void* w, const float* bias32, const void* bias16, void* b, void* workspace)
-{
+	if (kind == 0)
+		return conv_fprop_im2col_t<float>(stream, g, (const float*)a, (const float*)w, bias32, 0, (float*)b, workspace, x3);
 	if (kind == 1)
 		return conv_fprop_im2col_t<__nv_bfloat16>(stream, g, (const __nv_bfloat16*)a, (const __nv_bfloat16*)w, bias32, bias16, (__nv_bfloat16*)b, workspace, 0);
 	return conv_fprop_im2col_t<__half>(stream, g, (const __half*)a, (const __half*)w, bias32, bias16, (__half*)b, workspace, 0);
 }
-int conv_wgrad_im2col_16(cudaStream_t stream, int kind, const ConvGeom& g, const void* grad_b, const void* a, void* grad_w, int accumulate, void* workspace)
+int conv_wgrad_im2col_any(cudaStream_t stream, int kind, const ConvGeom& g, const void* grad_b, const void* a, void* grad_w, int accumulate, void* workspace, int x3)
 {
+	if (kind == 0)
+		return conv_wgrad_im2col_t<float>(stream, g, (const float*)grad_b, (const float*)a, (float*)grad_w, accumulate, workspace, x3);
 	if (kind == 1)
 		return conv_wgrad_im2col_t<__nv_bfloat16>(stream, g, (const __nv_bfloat16*)grad_b, (const __nv_bfloat16*)a, (__nv_bfloat16*)grad_w, accumulate, workspace, 0);
 	return conv_wgrad_im2col_t<__half>(stream, g, (const __half*)grad_b, (const __half*)a, (__half*)grad_w, accumulate, workspace, 0);

@@ -30,45 +30,41 @@ struct Scratch {
 // ~2 CTAs per SM plus one wave of 128 x 256 fp32 tiles)
 constexpr size_t CONTRACT_SCRATCH_BYTES = (size_t)96 << 20;
 
-// x3 (last argument of every entry point): 0 = one-pass TF32, 1 = error-compensated 3xTF32 (fp32-grade products, a third of
-// the tensor rate; sm100_umma_gemm.cuh).
-// returns 0 on success, 1 if the shape/alignment cannot use the TMA+wgmma path (caller falls back to FFMA), <0 on CUDA error.
+// The tensor-core contractions, one entry per product for every element kind: kind 0 = fp32 (TF32 or 3xTF32 MMAs), 1 = bf16,
+// 2 = fp16 (wgmma bf16 / fp16 with fp32 accumulation in registers, 16-bit result rounded once, to nearest even).  Every leading
+// dimension / channel count must be a multiple of 16 bytes (4 fp32 or 8 16-bit elements).
+// x3 (last argument): 0 = one-pass TF32, 1 = error-compensated 3xTF32 (fp32-grade products, a third of the tensor rate;
+// sm100_umma_gemm.cuh); ignored for 16-bit kinds.
+// bias: fp32 (bias32) or, for 16-bit kinds, in the tensors' 16-bit type (bias16); at most one of them.
+// returns 0 on success, 1 if the shape/alignment cannot use the TMA+wgmma path (the caller falls back), <0 on CUDA error.
 // C[M, N] (+)= op(A) * op(B) + bias; A is [M, K] (lda) or, if trans_a, [K, M]; B is [K, N] (ldb) or, if trans_b, [N, K].
-int gemm_tf32(cudaStream_t stream, int M, int N, int K, const float* a, long long lda, int trans_a, const float* b, long long ldb, int trans_b, float* c, long long ldc, const float* bias, int accumulate, const Scratch& scratch, int x3 = 0);
-int conv_fprop_tf32(cudaStream_t stream, const ConvGeom& g, const float* a, const float* w, const float* bias, float* b, const Scratch& scratch, int x3 = 0);
-// the fp32 data gradient works in a workspace of conv_dgrad_workspace_bytes(g) (which includes CONTRACT_SCRATCH_BYTES for split-K slices).
+int gemm_any(cudaStream_t stream, int kind, int M, int N, int K, const void* a, long long lda, int trans_a, const void* b, long long ldb, int trans_b, void* c, long long ldc, const float* bias32, const void* bias16, int accumulate, const Scratch& scratch, int x3 = 0);
+int conv_fprop_any(cudaStream_t stream, int kind, const ConvGeom& g, const void* a, const void* w, const float* bias32, const void* bias16, void* b, const Scratch& scratch, int x3 = 0);
+// The data gradient works in a workspace of conv_dgrad_workspace_bytes(g, kind): for fp32 a transposed copy of the filters followed
+// by CONTRACT_SCRATCH_BYTES for split-K slices, for 16-bit kinds the split-K scratch alone.
 // bias[C] (NULL: none) is added to every pixel of grad_a, also to those no filter tap reaches: that makes the data gradient the
 // forward of a transposed convolution (CONVOLUTION_TRANSPOSE_FORWARD).
-size_t conv_dgrad_workspace_bytes(const ConvGeom& g);
-int conv_dgrad_tf32(cudaStream_t stream, const ConvGeom& g, const float* grad_b, const float* w, const float* bias, float* grad_a, void* workspace, int x3 = 0);
-int conv_wgrad_tf32(cudaStream_t stream, const ConvGeom& g, const float* grad_b, const float* a, float* grad_w, int accumulate, const Scratch& scratch, int x3 = 0);
-
-// The same contractions on 16-bit tensors (kind 1 = bf16, 2 = fp16): wgmma bf16 / fp16 with fp32 accumulation in registers, 16-bit
-// result (rounded once, to nearest even).  Every leading dimension / channel count must be a multiple of 8 elements (16 bytes).
-// bias: fp32 (bias32) or in the tensors' 16-bit type (bias16); at most one of them.  Returns as above (1 = shape not covered).
-int gemm_16(cudaStream_t stream, int kind, int M, int N, int K, const void* a, long long lda, int trans_a, const void* b, long long ldb, int trans_b, void* c, long long ldc, const float* bias32, const void* bias16, int accumulate, const Scratch& scratch);
-int conv_fprop_16(cudaStream_t stream, int kind, const ConvGeom& g, const void* a, const void* w, const float* bias32, const void* bias16, void* b, const Scratch& scratch);
-int conv_dgrad_16(cudaStream_t stream, int kind, const ConvGeom& g, const void* grad_b, const void* w, const float* bias32, const void* bias16, void* grad_a, const Scratch& scratch);
-// true when conv_dgrad_tf32 / conv_dgrad_16 may return 1 for this geometry and element kind on shape grounds (a superset of the shape
-// tests they make; operand pointers aside): callers that reserve the workspace of their fallback ahead of the call count it in then
+size_t conv_dgrad_workspace_bytes(const ConvGeom& g, int kind);
+int conv_dgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, const void* grad_b, const void* w, const float* bias32, const void* bias16, void* grad_a, void* workspace, int x3 = 0);
+// true when conv_dgrad_any may return 1 for this geometry and element kind on shape grounds (a superset of the shape tests it makes;
+// operand pointers aside): callers that reserve the workspace of their fallback ahead of the call count it in then
 bool conv_dgrad_may_decline(const ConvGeom& g, int kind);
-int conv_wgrad_16(cudaStream_t stream, int kind, const ConvGeom& g, const void* grad_b, const void* a, void* grad_w, int accumulate, const Scratch& scratch);
+int conv_wgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, const void* grad_b, const void* a, void* grad_w, int accumulate, const Scratch& scratch, int x3 = 0);
 
-// Ask the NEXT conv_fprop_tf32 / gemm_tf32 launch of this host thread to also produce per-column statistics of its output
+// Ask the NEXT conv_fprop_any / gemm_any launch of this host thread to also produce per-column statistics of its output
 // (batch-norm forward fused into the producing convolution).  `part` holds four planes of max_rows x N floats -- count,
 // shift k, sum(v - k), sum((v - k)^2) -- one row per (CTA, epilogue warp quarter); *rows_out = rows in use (the plane
 // pitch is *rows_out x N; 0 when the launch took a path without this epilogue; the request is consumed either way).
 // Combined by bn_fwd_train_f32 (ext_part / ext_rows) with a Chan merge in double precision.
 void conv_stats_request(float* part, int max_rows, int* rows_out);
 
-// Small-channel convolutions (C not a multiple of 4, e.g. the 3-channel stem): explicit im2col into `workspace`
-// ([N*P*Q, Kp] with Kp = R*S*C rounded up to 32, zero padded) followed by the tensor-core GEMM.  Returns 1 when not applicable.
+// Small-channel convolutions (C not a multiple of 16 bytes, e.g. the 3-channel stem): explicit im2col into `workspace`
+// ([N*P*Q, Kp] with Kp = R*S*C rounded up to one operand span, zero padded) followed by the tensor-core GEMM.  Returns 1 when not
+// applicable.
 size_t conv_im2col_workspace_bytes(const ConvGeom& g, int kind = 0); // kind: 0 = fp32, 1 = bf16, 2 = fp16
-// (the workspace must hold conv_im2col_workspace_bytes(g), which includes CONTRACT_SCRATCH_BYTES for the GEMM's split-K slices)
-int conv_fprop_im2col_tf32(cudaStream_t stream, const ConvGeom& g, const float* a, const float* w, const float* bias, float* b, void* workspace, int x3 = 0);
-int conv_wgrad_im2col_tf32(cudaStream_t stream, const ConvGeom& g, const float* grad_b, const float* a, float* grad_w, int accumulate, void* workspace, int x3 = 0);
-int conv_fprop_im2col_16(cudaStream_t stream, int kind, const ConvGeom& g, const void* a, const void* w, const float* bias32, const void* bias16, void* b, void* workspace);
-int conv_wgrad_im2col_16(cudaStream_t stream, int kind, const ConvGeom& g, const void* grad_b, const void* a, void* grad_w, int accumulate, void* workspace);
+// (the workspace must hold conv_im2col_workspace_bytes(g, kind), which includes CONTRACT_SCRATCH_BYTES for the GEMM's split-K slices)
+int conv_fprop_im2col_any(cudaStream_t stream, int kind, const ConvGeom& g, const void* a, const void* w, const float* bias32, const void* bias16, void* b, void* workspace, int x3 = 0);
+int conv_wgrad_im2col_any(cudaStream_t stream, int kind, const ConvGeom& g, const void* grad_b, const void* a, void* grad_w, int accumulate, void* workspace, int x3 = 0);
 
 // CUDA-core fp32 versions of the same contractions: any stride/alignment, groups, exact fp32 products.  Long reductions over few
 // output tiles split K into slices of `scratch` (none given: no split), combined in split order like the tensor-core path.

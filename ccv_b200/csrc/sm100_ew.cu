@@ -463,7 +463,7 @@ __global__ void __launch_bounds__(1024) colsum_partials_kernel(const float* __re
 	}
 }
 size_t colsum_workspace_bytes(int cols) { return ((size_t)sms() * 8 + 8) * (size_t)((cols + 3) / 4 * 4) * sizeof(float); }
-int colsum_f32(cudaStream_t s, const float* g, size_t rows, int cols, long long ld, float* out, int accumulate, void* workspace)
+static int colsum_f32(cudaStream_t s, const float* g, size_t rows, int cols, long long ld, float* out, int accumulate, void* workspace)
 {
 	if (cols <= 0)
 		return 0;
@@ -1070,10 +1070,6 @@ int sgd_any(cudaStream_t s, int g_kind, const void* g, const float* a, const flo
 		sgd_kernel<1><<<grid_for(count, 256), 256, 0, s>>>(g, g_kind, a, m, b, n, count, nesterov, rate, scale, decay, momentum, inv_dampening);
 	return check("sgd");
 }
-int sgd_f32(cudaStream_t s, const float* g, const float* a, const float* m, float* b, float* n, size_t count, int nesterov, float rate, float scale, float decay, float momentum, float dampening)
-{
-	return sgd_any(s, 0, g, a, m, b, n, count, nesterov, rate, scale, decay, momentum, dampening);
-}
 
 // Many SGD commands with the same hyper-parameters in one launch (the per-parameter SGD nodes of a model are a run of ~200
 // small tensors): the tensor table travels in the kernel parameters (<= SGD_MULTI_MAX tensors per launch), a block owns
@@ -1130,10 +1126,6 @@ __global__ void __launch_bounds__(256) sgd_multi_kernel(const __grid_constant__ 
 		*reinterpret_cast<float4*>(b + i) = make_float4(bs[0], bs[1], bs[2], bs[3]);
 		*reinterpret_cast<float4*>(n + i) = make_float4(ns[0], ns[1], ns[2], ns[3]);
 	}
-}
-int sgd_multi_f32(cudaStream_t s, int tensors, const float* const* g, const float* const* a, const float* const* m, float* const* b, float* const* n, const size_t* counts, int nesterov, float rate, float scale, float decay, float momentum, float dampening)
-{
-	return sgd_multi_any(s, tensors, 0, reinterpret_cast<const void* const*>(g), a, m, b, n, counts, nesterov, rate, scale, decay, momentum, dampening);
 }
 int sgd_multi_any(cudaStream_t s, int tensors, int g_kind, const void* const* g, const float* const* a, const float* const* m, float* const* b, float* const* n, const size_t* counts, int nesterov, float rate, float scale, float decay, float momentum, float dampening)
 {

@@ -28,7 +28,6 @@ int ew_sum_16(cudaStream_t s, int kind, const void* const* inputs, int k, void* 
 // out[c] (+)= sum over rows of g[row * ld + c]  (bias gradients of GEMM / convolution)
 // workspace (colsum_workspace_bytes(cols), may be NULL): per-block partial rows, combined in a fixed order instead of by atomics
 size_t colsum_workspace_bytes(int cols);
-int colsum_f32(cudaStream_t s, const float* g, size_t rows, int cols, long long ld, float* out, int accumulate, void* workspace);
 // g of element kind g_kind (0 = fp32, 1 = bf16, 2 = fp16), out of kind out_kind; fp32 accumulation
 int colsum_any(cudaStream_t s, int g_kind, const void* g, size_t rows, int cols, long long ld, void* out, int out_kind, int accumulate, void* workspace);
 // reduce a <= 4-d tensor over the axes where rdim == 1 (sum); out has rdim shape, contiguous
@@ -84,14 +83,11 @@ int softmax_cce_fwd_f32(cudaStream_t s, const float* a, const void* label, int l
 int softmax_cce_bwd_f32(cudaStream_t s, const float* g, const void* label, int label_kind, const float* d, float* h, int batch, int count, float trim0, float trim1);
 
 // ---- SGD ------------------------------------------------------------------------------------------------------
-int sgd_f32(cudaStream_t s, const float* g, const float* a, const float* m, float* b, float* n, size_t count, int nesterov, float rate, float scale, float decay, float momentum, float dampening);
-
 // g of element kind g_kind (0 = fp32, 1 = bf16, 2 = fp16) with fp32 parameters / momenta: the reference's mixed-precision form
 // (sgd/gpu/ccv_nnc_sgd_gpu_ref.cu:71-74)
 int sgd_any(cudaStream_t s, int g_kind, const void* g, const float* a, const float* m, float* b, float* n, size_t count, int nesterov, float rate, float scale, float decay, float momentum, float dampening);
-int sgd_multi_any(cudaStream_t s, int tensors, int g_kind, const void* const* g, const float* const* a, const float* const* m, float* const* b, float* const* n, const size_t* counts, int nesterov, float rate, float scale, float decay, float momentum, float dampening);
 // `tensors` independent SGD updates with the same hyper-parameters in ceil(tensors / 32) launches
-int sgd_multi_f32(cudaStream_t s, int tensors, const float* const* g, const float* const* a, const float* const* m, float* const* b, float* const* n, const size_t* counts, int nesterov, float rate, float scale, float decay, float momentum, float dampening);
+int sgd_multi_any(cudaStream_t s, int tensors, int g_kind, const void* const* g, const float* const* a, const float* const* m, float* const* b, float* const* n, const size_t* counts, int nesterov, float rate, float scale, float decay, float momentum, float dampening);
 
 // strided matrix of element kind `kind` (0 fp32, 1 bf16, 2 fp16) <-> dense fp32 (16-bit GEMM operands with strides TMA cannot take)
 int widen_matrix(cudaStream_t s, const void* src, int kind, long long rs, long long cs, float* dst, int rows, int cols);

@@ -119,7 +119,7 @@ int sdpa_forward_f32(cudaStream_t s, const SdpaGeom& g, const float* q, const fl
 			const float* vp = v + b * g.v_b + (h / ratio) * g.v_h;
 			float* op = o + b * g.o_b + h * g.o_h;
 			// S = Q K^T
-			int rc = gemm_tf32(s, g.Sq, g.Sk, g.D, qp, g.q_s, 0, kp, g.k_s, 1, S, g.Sk, 0, 0, no_scratch);
+			int rc = gemm_any(s, 0, g.Sq, g.Sk, g.D, qp, g.q_s, 0, kp, g.k_s, 1, S, g.Sk, 0, 0, 0, no_scratch);
 			if (rc > 0)
 				rc = gemm_ffma(s, g.Sq, g.Sk, g.D, qp, g.q_s, 1, kp, 1, g.k_s, S, g.Sk, 0, 0);
 			if (rc)
@@ -129,7 +129,7 @@ int sdpa_forward_f32(cudaStream_t s, const SdpaGeom& g, const float* q, const fl
 			if (check("sdpa_softmax"))
 				return -1;
 			// O = P V
-			rc = gemm_tf32(s, g.Sq, g.Dv, g.Sk, S, g.Sk, 0, vp, g.v_s, 0, op, g.o_s, 0, 0, no_scratch);
+			rc = gemm_any(s, 0, g.Sq, g.Dv, g.Sk, S, g.Sk, 0, vp, g.v_s, 0, op, g.o_s, 0, 0, 0, no_scratch);
 			if (rc > 0)
 				rc = gemm_ffma(s, g.Sq, g.Dv, g.Sk, S, g.Sk, 1, vp, g.v_s, 1, op, g.o_s, 0, 0);
 			if (rc)
@@ -140,7 +140,7 @@ int sdpa_forward_f32(cudaStream_t s, const SdpaGeom& g, const float* q, const fl
 
 static int mm(cudaStream_t s, int M, int N, int K, const float* a, long long lda, int ta, const float* b, long long ldb, int tb, float* c, long long ldc, int accumulate)
 {
-	int rc = gemm_tf32(s, M, N, K, a, lda, ta, b, ldb, tb, c, ldc, 0, accumulate, no_scratch);
+	int rc = gemm_any(s, 0, M, N, K, a, lda, ta, b, ldb, tb, c, ldc, 0, 0, accumulate, no_scratch);
 	if (rc > 0)
 		rc = gemm_ffma(s, M, N, K, a, ta ? 1 : lda, ta ? lda : 1, b, tb ? 1 : ldb, tb ? ldb : 1, c, ldc, 0, accumulate);
 	return rc;

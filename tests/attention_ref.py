@@ -88,7 +88,7 @@ def _flash_ok(D, Dv, H, Hk, aligned):
 
 
 def _fp32_gemms(D, Dv, Sk, aligned4=True):
-    """gemm_tf32 declines (and gemm_ffma runs) when an operand's tensor map cannot be encoded: fp32 rows must start on 16 bytes.
+    """The fp32 gemm_any declines (and gemm_ffma runs) when an operand's tensor map cannot be encoded: fp32 rows must start on 16 bytes.
     S = Q K^T reads q / k rows of D floats; P V, P^T dO, dS K and dS^T Q read the [Sq, Sk] score matrix with pitch Sk."""
     return dict(gemm_s="tf32" if D % 4 == 0 and Dv % 4 == 0 and aligned4 else "ffma", gemm_p="tf32" if Sk % 4 == 0 and D % 4 == 0 and Dv % 4 == 0 and aligned4 else "ffma")
 

@@ -14,7 +14,7 @@ import numpy as np
 import pytest
 
 from ccv_b200 import abi
-from tests.util import NCHW, NHWC, assert_close, counted, gpu_exec, ref_exec, seeded
+from tests.util import NCHW, NHWC, assert_close, counted, gpu_exec, ref_exec, seeded, to_bf16
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 TOL = {abi.CCV_NNC_SM100_ALGO_TF32: 1e-3, abi.CCV_NNC_SM100_ALGO_3XTF32: 2e-5, abi.CCV_NNC_SM100_ALGO_FFMA: 1e-5}
@@ -342,6 +342,42 @@ def test_convolution_backward_nchw_and_mixed(gpu, ref, C, K, st, layout):
     assert_close(h_g, h_r, tol, "dgrad " + layout)
     assert_close(dw_g, dw_r, tol, "wgrad " + layout)
     assert_close(db_g, db_r, tol, "dbias " + layout)
+
+
+@pytest.mark.parametrize("case", ["fp16 dw", "fp16 w", "fp16 dbias", "fp16 h", "h channels", "bf16 g, fp16 dw"])
+def test_convolution_backward_refuses_mixed_operands_before_any_launch(gpu, case):
+    """The backend is chosen on the union of the operands' types, so CONVOLUTION_BACKWARD receives calls whose operands differ in type.
+    It checks every operand (types, the dbias type, h's geometry) before its first launch: such a call returns INVALID, launches
+    nothing and leaves h, dw and dbias as they were, also when dw and dbias would have been computable."""
+    nnc = gpu
+    N, H, C, K, R = 2, 8, 16, 32, 3
+    F32, F16, BF16 = abi.CCV_32F, abi.CCV_16F, abi.CCV_16BF
+    types = dict(g=F32, a=F32, w=F32, h=F32, dw=F32, dbias=F32)
+    h_c = C
+    if case == "h channels":
+        h_c = C + 8
+    elif case == "bf16 g, fp16 dw":
+        types.update(g=BF16, a=BF16, w=BF16, h=BF16, dw=F16)
+    else:
+        types[case.split()[1]] = F16
+    shapes = dict(g=(N, H, H, K), a=(N, H, H, C), w=(K, R, R, C), h=(N, H, H, h_c), dw=(K, R, R, C), dbias=(K,))
+    tensors, before = {}, {}
+    for i, name in enumerate(("g", "a", "w", "h", "dw", "dbias")):
+        v = seeded(shapes[name], 10 + i, -1, 1)
+        v = to_bf16(v) if types[name] == BF16 else v.astype(np.float16) if types[name] == F16 else v
+        tensors[name] = nnc.gpu_tensor(list(shapes[name]), NHWC, types[name])
+        tensors[name].upload(v)
+        before[name] = tensors[name].download().tobytes()
+    l0 = nnc.launch_count()
+    status = nnc.cmd_exec(nnc.CMD_CONVOLUTION_BACKWARD(1, K, R, R, C), nnc.hint((1, 1), (1, 1)), 0, [tensors[n] for n in ("g", "a", "w")], [tensors[n] for n in ("h", "dw", "dbias")])
+    launches = nnc.launch_count() - l0
+    after = {name: t.download().tobytes() for name, t in tensors.items()}
+    for t in tensors.values():
+        t.free()
+    assert status == abi.CCV_NNC_EXEC_INVALID, (case, status)
+    assert launches == 0, (case, launches)
+    for name in ("h", "dw", "dbias"):
+        assert after[name] == before[name], (case, name + " changed")
 
 
 # ------------------------------------------------------------------------------------------------ BASELINE configs at full size
