@@ -661,8 +661,9 @@ int conv_grouped_tc(cudaStream_t s, unsigned char* const ws, const int kind, con
 // h = dgrad(gb, w) (+ bias[C]) on the geometry gh, returns a CCV_NNC_EXEC_* status: the data gradient of CONVOLUTION_BACKWARD (no
 // bias) and the forward of CONVOLUTION_TRANSPOSE (bias32 fp32, or bias16 of the tensors' 16-bit type).  Tensor cores for one group,
 // per-group dense launches for wide groups (fp32 unless ALGO_FFMA; 16-bit always).  Where they decline, fp32 runs on FFMA (also
-// narrow groups and unaligned channels); 16-bit shapes they cannot take (3-channel pixels, one group) run in the functional form --
-// widen g, w and the bias, fp32 FFMA data gradient + bias, one rounding on the way back.
+// narrow groups and unaligned channels); 16-bit groups they cannot take run on the direct grouped kernels (sm100_conv_grouped.cu),
+// 16-bit single-group shapes they cannot take (3-channel pixels) in the functional form -- widen g, w and the bias, fp32 FFMA data
+// gradient + bias, one rounding on the way back.
 // workspace of the 16-bit functional form below: fp32 copies of g, w, h and the bias, 256-byte aligned
 size_t dgrad16_fallback_bytes(const ConvGeom& gh)
 {
@@ -684,10 +685,14 @@ int dgrad_nhwc(cudaStream_t s, unsigned char* const ws, const int kind, const in
 		RC(conv_dgrad_ffma(s, gh, groups, (const float*)gb, (const float*)w, bias32, (float*)h));
 		return CCV_NNC_EXEC_SUCCESS;
 	}
-	// (the image gradient of a stem, test/int/nnc/cudnn.tests.c:499-577; the RGB head of a transposed convolution)  Dense tensors and
-	// one group only.
+	if (groups > 1) // groups the tensor cores do not take: the direct CUDA-core kernels
+	{
+		RC(conv_dgrad_grouped16(s, kind, gh, groups, gb, w, bias32, bias16, h));
+		return CCV_NNC_EXEC_SUCCESS;
+	}
+	// (the image gradient of a stem, test/int/nnc/cudnn.tests.c:499-577; the RGB head of a transposed convolution)  Dense tensors.
 	const size_t ng = (size_t)gh.N * gh.P * gh.Q * gh.K, nw = (size_t)gh.K * gh.R * gh.S * gh.C, nh = (size_t)gh.N * gh.H * gh.W * gh.C, nb = bias16 ? gh.C : 0;
-	if (groups > 1 || gh.bw != gh.K || gh.bh != (long long)gh.Q * gh.K || gh.bn != (long long)gh.P * gh.Q * gh.K || gh.aw != gh.C || gh.ah != (long long)gh.W * gh.C || gh.an != (long long)gh.H * gh.W * gh.C || ng > 0x7fffffffull || nh > 0x7fffffffull)
+	if (gh.bw != gh.K || gh.bh != (long long)gh.Q * gh.K || gh.bn != (long long)gh.P * gh.Q * gh.K || gh.aw != gh.C || gh.ah != (long long)gh.W * gh.C || gh.an != (long long)gh.H * gh.W * gh.C || ng > 0x7fffffffull || nh > 0x7fffffffull)
 		return CCV_NNC_EXEC_INVALID;
 	float* const g32 = (float*)ws;
 	float* const w32 = (float*)(((uintptr_t)(g32 + ng) + 255) & ~(uintptr_t)255);
@@ -705,7 +710,7 @@ int dgrad_nhwc(cudaStream_t s, unsigned char* const ws, const int kind, const in
 // The workspace of the products `which` of a convolution on g: the most any path the shapes permit uses -- the split-K scratch or
 // the fp32 data gradient's workspace, the grouped [contraction | group activations | group results], im2col for unaligned channels,
 // the 16-bit functional data gradient where the tensor cores may decline.  The FFMA kernels use none, except the weight gradient's
-// split-K scratch.
+// split-K scratch; the direct 16-bit grouped kernels likewise (their weight gradient's pixel-chunk slices).
 enum { CONV_FPROP = 1, CONV_WGRAD = 2, CONV_DGRAD = 4 };
 size_t conv_workspace(const ConvGeom& g, const int kind, const int groups, const int algo, const unsigned which)
 {
@@ -718,7 +723,11 @@ size_t conv_workspace(const ConvGeom& g, const int kind, const int groups, const
 		if (kind == 0 && algo == CCV_NNC_SM100_ALGO_FFMA)
 			need = std::max(need, pass == 1 ? CONTRACT_SCRATCH_BYTES : 0);
 		else if (groups > 1)
+		{
 			need = std::max(need, group_plan(g, kind, groups, pass, gp) ? gp.inner + gp.xb + gp.yb : kind == 0 && pass == 1 ? CONTRACT_SCRATCH_BYTES : 0);
+			if (kind > 0 && pass == 1) // where the tensor cores decline, the direct kernels' weight gradient
+				need = std::max(need, conv_grouped16_wgrad_bytes(g, groups));
+		}
 		else {
 			need = std::max(need, pass == 2 ? conv_dgrad_workspace_bytes(g, kind) : CONTRACT_SCRATCH_BYTES);
 			if (pass < 2 && g.C % (kind == 0 ? 4 : 8) != 0)
@@ -798,9 +807,12 @@ int conv_forw_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 		return CCV_NNC_EXEC_INVALID;
 	if (rc > 0)
 	{
-		if (kind > 0) // there is no 16-bit FFMA kernel to fall back to (narrow groups among others)
+		if (kind > 0 && groups > 1) // groups the tensor cores do not take: the direct CUDA-core kernels
+			RC(conv_fprop_grouped16(s, kind, g, groups, a, w, bias32, bias16, b));
+		else if (kind > 0) // there is no 16-bit FFMA kernel to fall back to
 			return CCV_NNC_EXEC_INVALID;
-		RC(conv_fprop_ffma(s, g, groups, (const float*)a, (const float*)w, bias32, (float*)b));
+		else
+			RC(conv_fprop_ffma(s, g, groups, (const float*)a, (const float*)w, bias32, (float*)b));
 	}
 	return CCV_NNC_EXEC_SUCCESS;
 }
@@ -854,6 +866,8 @@ int conv_back_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 					rc = conv_wgrad_im2col_any(s, kind, g, gb, a, dw_t->data.u8, accumulate, ws, x3);
 			}
 		}
+		if (rc > 0 && kind > 0 && groups > 1) // groups the tensor cores do not take: the direct CUDA-core kernels
+			rc = conv_wgrad_grouped16(s, kind, g, groups, gb, a, dw_t->data.u8, accumulate, scratch_at(ws, ws_bytes));
 		if (rc < 0 || (rc > 0 && kind > 0))
 			return CCV_NNC_EXEC_INVALID;
 		if (rc > 0)
@@ -1176,8 +1190,9 @@ int conv_transpose_back_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint,
 		return CCV_NNC_EXEC_INVALID;
 	if ((dw_t && !conv_transpose_geom(cmd, hint, view_of(g_t), view_of(dw_t), view_of(a_t), gchk)) || (da_t && !conv_transpose_geom(cmd, hint, view_of(g_t), view_of(w_t), view_of(da_t), gchk)))
 		return CCV_NNC_EXEC_INVALID;
-	// 16-bit forwards and weight gradients run on the tensor cores only: Cin a multiple of 8, grouped ones with wide groups
-	if (kind > 0 && (da_t || dw_t) && (g.K % 8 || (groups > 1 && (g.C / groups % 8 || g.K / groups % 8 || g.C / groups < 16 || g.K / groups < 16))))
+	// 16-bit forwards and weight gradients of one group run on the tensor cores only: Cin a multiple of 8 (grouped ones also on the
+	// direct kernels)
+	if (kind > 0 && (da_t || dw_t) && groups == 1 && g.K % 8)
 		return CCV_NNC_EXEC_INVALID;
 	const int db_kind = dbias_t ? kind_of(dbias_t) : 0;
 	if (dbias_t && (db_kind < 0 || (kind == 0 && db_kind != 0) || dbias_t->info.dim[0] != g.C || g.ah != (long long)g.W * g.aw || g.an != (long long)g.H * g.ah))

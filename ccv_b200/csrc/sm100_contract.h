@@ -72,6 +72,15 @@ int gemm_ffma(cudaStream_t stream, int M, int N, int K, const float* a, long lon
 int conv_fprop_ffma(cudaStream_t stream, const ConvGeom& g, int groups, const float* a, const float* w, const float* bias, float* b);
 int conv_dgrad_ffma(cudaStream_t stream, const ConvGeom& g, int groups, const float* grad_b, const float* w, const float* bias, float* grad_a);
 int conv_wgrad_ffma(cudaStream_t stream, const ConvGeom& g, int groups, const float* grad_b, const float* a, float* grad_w, int accumulate, const Scratch& scratch = Scratch());
+// Direct CUDA-core grouped convolutions for 16-bit tensors (sm100_conv_grouped.cu), kind 1 = bf16, 2 = fp16: any C / groups and
+// K / groups (depthwise, channel multipliers, groups too narrow or unaligned for the tensor cores), pitched activations, 64-bit
+// offsets; fp32 accumulation in a fixed order, one rounding to nearest even.  Bias fp32 (bias32) or of the tensors' type (bias16).
+// The weight gradient sums fixed pixel chunks into fp32 slices of `scratch` (conv_grouped16_wgrad_bytes(g, groups) of them) and
+// combines them in order with splitk_reduce.  Return 0, 1 when the kind or the group count does not fit, < 0 on errors.
+size_t conv_grouped16_wgrad_bytes(const ConvGeom& g, int groups);
+int conv_fprop_grouped16(cudaStream_t stream, int kind, const ConvGeom& g, int groups, const void* a, const void* w, const float* bias32, const void* bias16, void* b);
+int conv_dgrad_grouped16(cudaStream_t stream, int kind, const ConvGeom& g, int groups, const void* grad_b, const void* w, const float* bias32, const void* bias16, void* grad_a);
+int conv_wgrad_grouped16(cudaStream_t stream, int kind, const ConvGeom& g, int groups, const void* grad_b, const void* a, void* grad_w, int accumulate, const Scratch& scratch);
 // out[r, c] = (accumulate ? out[r, c] : 0) + part[0][r, c] + part[1][r, c] + ... (fp32 slices [rows, cols] of pitch ldp, split_stride apart)
 int splitk_reduce(cudaStream_t stream, const float* part, int splits, long long split_stride, int rows, int cols, long long ldp, float* out, long long ldo, int accumulate, int out_kind = 0);
 
