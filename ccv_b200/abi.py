@@ -35,6 +35,7 @@ CMD_IDS = dict(
     SIGMOID=0xf2f69650, TANH=0x6a62be30, LEAKY_RELU=0x507144e0, EWEXP=0xd784b170, EWLOG=0xf4191bf2, EWSQRT=0x8870a61e, CLAMP=0x2640d854,
     EWDIV=0x1cd2fa18, REDUCE_SUM=0x52970f06, REDUCE_MEAN=0xf23556c6, REDUCE_MAX=0x80f1a506, REDUCE_MIN=0x6785ef96, REDUCE_NORM2=0xb3034e16,
     MASKED_FILL=0x7f992d84, DROPOUT=0x7f2dc3e4, ADAM=0xe30099dc, RANDOM_UNIFORM=0xa0cd1d5e, RANDOM_NORMAL=0x7062c8b4,
+    CMUL=0xead486e6,
 )
 for _k, _v in CMD_IDS.items():
     globals()["CCV_NNC_%s_FORWARD" % _k] = _v

@@ -685,6 +685,7 @@ CMD_EWEXP_FORWARD, CMD_EWEXP_BACKWARD = _make_simple("EWEXP")
 CMD_EWLOG_FORWARD, CMD_EWLOG_BACKWARD = _make_simple("EWLOG")
 CMD_EWSQRT_FORWARD, CMD_EWSQRT_BACKWARD = _make_simple("EWSQRT")
 CMD_EWDIV_FORWARD, CMD_EWDIV_BACKWARD = _make_simple("EWDIV")
+CMD_CMUL_FORWARD, CMD_CMUL_BACKWARD = _make_simple("CMUL")  # complex multiplication (cmd/blas/ccv_nnc_cmul_cpu_ref.c)
 
 
 def CMD_LEAKY_RELU_FORWARD(negative_slope, **kw):

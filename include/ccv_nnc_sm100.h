@@ -439,6 +439,9 @@ enum {
 	CCV_NNC_RANDOM_UNIFORM_BACKWARD = 0xa0cd1d5f,
 	CCV_NNC_RANDOM_NORMAL_FORWARD = 0x7062c8b4,
 	CCV_NNC_RANDOM_NORMAL_BACKWARD = 0x7062c8b5,
+	/* cmd/blas (CMUL: the complex multiplication of rotary position embeddings) */
+	CCV_NNC_CMUL_FORWARD = 0xead486e6,
+	CCV_NNC_CMUL_BACKWARD = 0xead486e7,
 };
 
 enum {
@@ -499,7 +502,8 @@ enum {
 	X(CCV_NNC_COMM_ALLREDUCE_FORWARD) X(CCV_NNC_COMM_ALLREDUCE_BACKWARD) \
 	X(CCV_NNC_SIGMOID_FORWARD) X(CCV_NNC_SIGMOID_BACKWARD) X(CCV_NNC_TANH_FORWARD) X(CCV_NNC_TANH_BACKWARD) X(CCV_NNC_LEAKY_RELU_FORWARD) X(CCV_NNC_LEAKY_RELU_BACKWARD) X(CCV_NNC_EWEXP_FORWARD) X(CCV_NNC_EWEXP_BACKWARD) X(CCV_NNC_EWLOG_FORWARD) X(CCV_NNC_EWLOG_BACKWARD) X(CCV_NNC_EWSQRT_FORWARD) X(CCV_NNC_EWSQRT_BACKWARD) X(CCV_NNC_CLAMP_FORWARD) X(CCV_NNC_CLAMP_BACKWARD) \
 	X(CCV_NNC_EWDIV_FORWARD) X(CCV_NNC_EWDIV_BACKWARD) X(CCV_NNC_REDUCE_SUM_FORWARD) X(CCV_NNC_REDUCE_SUM_BACKWARD) X(CCV_NNC_REDUCE_MEAN_FORWARD) X(CCV_NNC_REDUCE_MEAN_BACKWARD) X(CCV_NNC_REDUCE_MAX_FORWARD) X(CCV_NNC_REDUCE_MAX_BACKWARD) X(CCV_NNC_REDUCE_MIN_FORWARD) X(CCV_NNC_REDUCE_MIN_BACKWARD) X(CCV_NNC_REDUCE_NORM2_FORWARD) X(CCV_NNC_REDUCE_NORM2_BACKWARD) X(CCV_NNC_MASKED_FILL_FORWARD) X(CCV_NNC_MASKED_FILL_BACKWARD) \
-	X(CCV_NNC_RANDOM_UNIFORM_FORWARD) X(CCV_NNC_RANDOM_UNIFORM_BACKWARD) X(CCV_NNC_RANDOM_NORMAL_FORWARD) X(CCV_NNC_RANDOM_NORMAL_BACKWARD) X(CCV_NNC_ADAM_FORWARD) X(CCV_NNC_ADAM_BACKWARD) X(CCV_NNC_DROPOUT_FORWARD) X(CCV_NNC_DROPOUT_BACKWARD)
+	X(CCV_NNC_RANDOM_UNIFORM_FORWARD) X(CCV_NNC_RANDOM_UNIFORM_BACKWARD) X(CCV_NNC_RANDOM_NORMAL_FORWARD) X(CCV_NNC_RANDOM_NORMAL_BACKWARD) X(CCV_NNC_ADAM_FORWARD) X(CCV_NNC_ADAM_BACKWARD) X(CCV_NNC_DROPOUT_FORWARD) X(CCV_NNC_DROPOUT_BACKWARD) \
+	X(CCV_NNC_CMUL_FORWARD) X(CCV_NNC_CMUL_BACKWARD)
 
 #define CCV_SM100_DECLARE_REGISTER(cmd) void _register_command_ ## cmd ## _backend_CCV_NNC_BACKEND_GPU_SM100(ccv_nnc_cmd_backend_registry_t* const registry);
 CCV_NNC_SM100_COMMANDS(CCV_SM100_DECLARE_REGISTER)
