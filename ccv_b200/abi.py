@@ -15,6 +15,7 @@ CCV_STREAM_CONTEXT_CPU, CCV_STREAM_CONTEXT_GPU = 0x1, 0x2
 CCV_NNC_ACCUMULATE_OUTPUT, CCV_NNC_ZERO_MEMORY_ALLOC = 0x01, 0x02
 CCV_NNC_EXEC_SUCCESS, CCV_NNC_EXEC_INVALID, CCV_NNC_EXEC_NO_KERNEL, CCV_NNC_EXEC_OOM = 0, -1, -2, -3
 CCV_NNC_UPSAMPLE_NEAREST, CCV_NNC_UPSAMPLE_BILINEAR = 0, 1
+CCV_NNC_MSE_REDUCE_MEAN, CCV_NNC_MSE_REDUCE_SUM = 0, 1  # lib/nnc/ccv_nnc.h:81-84 (cmd.info.mse.reduce_op)
 
 # backends (lib/nnc/cmd/ccv_nnc_backend.h + the new one)
 CCV_NNC_BACKEND_CPU_OPT = 0x46deb194
@@ -35,7 +36,7 @@ CMD_IDS = dict(
     SIGMOID=0xf2f69650, TANH=0x6a62be30, LEAKY_RELU=0x507144e0, EWEXP=0xd784b170, EWLOG=0xf4191bf2, EWSQRT=0x8870a61e, CLAMP=0x2640d854,
     EWDIV=0x1cd2fa18, REDUCE_SUM=0x52970f06, REDUCE_MEAN=0xf23556c6, REDUCE_MAX=0x80f1a506, REDUCE_MIN=0x6785ef96, REDUCE_NORM2=0xb3034e16,
     MASKED_FILL=0x7f992d84, DROPOUT=0x7f2dc3e4, ADAM=0xe30099dc, RANDOM_UNIFORM=0xa0cd1d5e, RANDOM_NORMAL=0x7062c8b4,
-    CMUL=0xead486e6,
+    CMUL=0xead486e6, BINARY_CROSSENTROPY=0xcd2107ec, SIGMOID_BINARY_CROSSENTROPY=0xd9e0e4a, MSE=0x6904a9a2, SMOOTH_L1=0x4e428e,
 )
 for _k, _v in CMD_IDS.items():
     globals()["CCV_NNC_%s_FORWARD" % _k] = _v
@@ -132,6 +133,18 @@ class _LeakyRelu(C.Structure):
     _fields_ = [("negative_slope", C.c_float)]
 
 
+class _BinaryCrossentropy(C.Structure):
+    _fields_ = [("pos_weight", C.c_float)]
+
+
+class _SmoothL1(C.Structure):
+    _fields_ = [("beta", C.c_float)]
+
+
+class _Mse(C.Structure):
+    _fields_ = [("reduce_op", C.c_int)]
+
+
 class _Dropout(C.Structure):
     _fields_ = [("p", C.c_float), ("entirety", C.c_int)]
 
@@ -139,7 +152,8 @@ class _Dropout(C.Structure):
 class _CmdUnion(C.Union):
     _fields_ = [("convolution", _Convolution), ("convolution_transpose", _ConvolutionTranspose), ("pool", _Pool), ("bnorm", _Bnorm), ("lnorm", _Lnorm), ("gnorm", _Gnorm), ("rmsnorm", _Rmsnorm),
                 ("sgd", _Sgd), ("adam", _Adam), ("gelu", _Gelu), ("blas", _Blas), ("label_smoothing", _LabelSmoothing), ("reduce", _Reduce), ("transpose", _Transpose),
-                ("upsample", _Upsample), ("clamp", _Clamp), ("leaky_relu", _LeakyRelu), ("dropout", _Dropout), ("scaled_dot_product_attention", _Sdpa), ("userdata", C.c_void_p)]
+                ("upsample", _Upsample), ("clamp", _Clamp), ("leaky_relu", _LeakyRelu), ("dropout", _Dropout), ("scaled_dot_product_attention", _Sdpa),
+                ("binary_crossentropy", _BinaryCrossentropy), ("smooth_l1", _SmoothL1), ("mse", _Mse), ("userdata", C.c_void_p)]
 
 
 class CmdParam(C.Structure):

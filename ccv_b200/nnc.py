@@ -688,6 +688,48 @@ CMD_EWDIV_FORWARD, CMD_EWDIV_BACKWARD = _make_simple("EWDIV")
 CMD_CMUL_FORWARD, CMD_CMUL_BACKWARD = _make_simple("CMUL")  # complex multiplication (cmd/blas/ccv_nnc_cmul_cpu_ref.c)
 
 
+# ---- losses over [batch, count] rows (cmd/loss, cmd/sigmoid_loss; cmd/ccv_nnc_cmd_easy.h) ----
+def _loss(name, arm, field, value, **kw):
+    def make(cmd_id):
+        c = _simple(cmd_id, **kw)
+        setattr(getattr(c.info, arm), field, value)
+        return c
+    return make(getattr(abi, "CCV_NNC_%s_FORWARD" % name)), make(getattr(abi, "CCV_NNC_%s_BACKWARD" % name))
+
+
+def CMD_BINARY_CROSSENTROPY_FORWARD(pos_weight=1.0, **kw):
+    return _loss("BINARY_CROSSENTROPY", "binary_crossentropy", "pos_weight", pos_weight, **kw)[0]
+
+
+def CMD_BINARY_CROSSENTROPY_BACKWARD(pos_weight=1.0, **kw):
+    return _loss("BINARY_CROSSENTROPY", "binary_crossentropy", "pos_weight", pos_weight, **kw)[1]
+
+
+def CMD_SIGMOID_BINARY_CROSSENTROPY_FORWARD(pos_weight=1.0, **kw):
+    return _loss("SIGMOID_BINARY_CROSSENTROPY", "binary_crossentropy", "pos_weight", pos_weight, **kw)[0]
+
+
+def CMD_SIGMOID_BINARY_CROSSENTROPY_BACKWARD(pos_weight=1.0, **kw):
+    return _loss("SIGMOID_BINARY_CROSSENTROPY", "binary_crossentropy", "pos_weight", pos_weight, **kw)[1]
+
+
+def CMD_MSE_FORWARD(reduce_op, **kw):
+    """reduce_op: abi.CCV_NNC_MSE_REDUCE_MEAN or abi.CCV_NNC_MSE_REDUCE_SUM"""
+    return _loss("MSE", "mse", "reduce_op", reduce_op, **kw)[0]
+
+
+def CMD_MSE_BACKWARD(reduce_op, **kw):
+    return _loss("MSE", "mse", "reduce_op", reduce_op, **kw)[1]
+
+
+def CMD_SMOOTH_L1_FORWARD(beta, **kw):
+    return _loss("SMOOTH_L1", "smooth_l1", "beta", beta, **kw)[0]
+
+
+def CMD_SMOOTH_L1_BACKWARD(beta, **kw):
+    return _loss("SMOOTH_L1", "smooth_l1", "beta", beta, **kw)[1]
+
+
 def CMD_LEAKY_RELU_FORWARD(negative_slope, **kw):
     c = _simple(abi.CCV_NNC_LEAKY_RELU_FORWARD, **kw)
     c.info.leaky_relu.negative_slope = negative_slope

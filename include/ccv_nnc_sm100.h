@@ -266,6 +266,15 @@ typedef struct {
 			float negative_slope;
 		} leaky_relu;
 		struct {
+			float pos_weight; /* BINARY_CROSSENTROPY / SIGMOID_BINARY_CROSSENTROPY: -(pos_weight y log(x) + (1 - y) log(1 - x)) */
+		} binary_crossentropy;
+		struct {
+			float beta;
+		} smooth_l1;
+		struct {
+			int reduce_op; /* CCV_NNC_MSE_REDUCE_MEAN / _SUM */
+		} mse;
+		struct {
 			float p;
 			int entirety;
 		} dropout;
@@ -442,6 +451,21 @@ enum {
 	/* cmd/blas (CMUL: the complex multiplication of rotary position embeddings) */
 	CCV_NNC_CMUL_FORWARD = 0xead486e6,
 	CCV_NNC_CMUL_BACKWARD = 0xead486e7,
+	/* cmd/loss, cmd/sigmoid_loss (BINARY_CROSSENTROPY, MSE, SMOOTH_L1; SIGMOID_BINARY_CROSSENTROPY) */
+	CCV_NNC_BINARY_CROSSENTROPY_FORWARD = 0xcd2107ec,
+	CCV_NNC_BINARY_CROSSENTROPY_BACKWARD = 0xcd2107ed,
+	CCV_NNC_SIGMOID_BINARY_CROSSENTROPY_FORWARD = 0xd9e0e4a,
+	CCV_NNC_SIGMOID_BINARY_CROSSENTROPY_BACKWARD = 0xd9e0e4b,
+	CCV_NNC_MSE_FORWARD = 0x6904a9a2,
+	CCV_NNC_MSE_BACKWARD = 0x6904a9a3,
+	CCV_NNC_SMOOTH_L1_FORWARD = 0x4e428e,
+	CCV_NNC_SMOOTH_L1_BACKWARD = 0x4e428f,
+};
+
+/* lib/nnc/ccv_nnc.h:81-84 (cmd.info.mse.reduce_op) */
+enum {
+	CCV_NNC_MSE_REDUCE_MEAN = 0,
+	CCV_NNC_MSE_REDUCE_SUM = 1,
 };
 
 enum {
@@ -503,7 +527,9 @@ enum {
 	X(CCV_NNC_SIGMOID_FORWARD) X(CCV_NNC_SIGMOID_BACKWARD) X(CCV_NNC_TANH_FORWARD) X(CCV_NNC_TANH_BACKWARD) X(CCV_NNC_LEAKY_RELU_FORWARD) X(CCV_NNC_LEAKY_RELU_BACKWARD) X(CCV_NNC_EWEXP_FORWARD) X(CCV_NNC_EWEXP_BACKWARD) X(CCV_NNC_EWLOG_FORWARD) X(CCV_NNC_EWLOG_BACKWARD) X(CCV_NNC_EWSQRT_FORWARD) X(CCV_NNC_EWSQRT_BACKWARD) X(CCV_NNC_CLAMP_FORWARD) X(CCV_NNC_CLAMP_BACKWARD) \
 	X(CCV_NNC_EWDIV_FORWARD) X(CCV_NNC_EWDIV_BACKWARD) X(CCV_NNC_REDUCE_SUM_FORWARD) X(CCV_NNC_REDUCE_SUM_BACKWARD) X(CCV_NNC_REDUCE_MEAN_FORWARD) X(CCV_NNC_REDUCE_MEAN_BACKWARD) X(CCV_NNC_REDUCE_MAX_FORWARD) X(CCV_NNC_REDUCE_MAX_BACKWARD) X(CCV_NNC_REDUCE_MIN_FORWARD) X(CCV_NNC_REDUCE_MIN_BACKWARD) X(CCV_NNC_REDUCE_NORM2_FORWARD) X(CCV_NNC_REDUCE_NORM2_BACKWARD) X(CCV_NNC_MASKED_FILL_FORWARD) X(CCV_NNC_MASKED_FILL_BACKWARD) \
 	X(CCV_NNC_RANDOM_UNIFORM_FORWARD) X(CCV_NNC_RANDOM_UNIFORM_BACKWARD) X(CCV_NNC_RANDOM_NORMAL_FORWARD) X(CCV_NNC_RANDOM_NORMAL_BACKWARD) X(CCV_NNC_ADAM_FORWARD) X(CCV_NNC_ADAM_BACKWARD) X(CCV_NNC_DROPOUT_FORWARD) X(CCV_NNC_DROPOUT_BACKWARD) \
-	X(CCV_NNC_CMUL_FORWARD) X(CCV_NNC_CMUL_BACKWARD)
+	X(CCV_NNC_CMUL_FORWARD) X(CCV_NNC_CMUL_BACKWARD) \
+	X(CCV_NNC_BINARY_CROSSENTROPY_FORWARD) X(CCV_NNC_BINARY_CROSSENTROPY_BACKWARD) X(CCV_NNC_SIGMOID_BINARY_CROSSENTROPY_FORWARD) X(CCV_NNC_SIGMOID_BINARY_CROSSENTROPY_BACKWARD) \
+	X(CCV_NNC_MSE_FORWARD) X(CCV_NNC_MSE_BACKWARD) X(CCV_NNC_SMOOTH_L1_FORWARD) X(CCV_NNC_SMOOTH_L1_BACKWARD)
 
 #define CCV_SM100_DECLARE_REGISTER(cmd) void _register_command_ ## cmd ## _backend_CCV_NNC_BACKEND_GPU_SM100(ccv_nnc_cmd_backend_registry_t* const registry);
 CCV_NNC_SM100_COMMANDS(CCV_SM100_DECLARE_REGISTER)
