@@ -1369,6 +1369,10 @@ int bnorm_back(const int fused_relu, const ccv_nnc_cmd_t cmd, const ccv_nnc_hint
 		return CCV_NNC_EXEC_INVALID;
 	if (h_t && (!same_shape(view_of(h_t), a) || !view_of(h_t).contiguous))
 		return CCV_NNC_EXEC_INVALID;
+	// every per-channel tensor is read or written as C packed floats
+	for (const ccv_nnc_tensor_t* const t : { (const ccv_nnc_tensor_t*)mean_t, (const ccv_nnc_tensor_t*)istd_t, bias_t, (const ccv_nnc_tensor_t*)dscale_t, (const ccv_nnc_tensor_t*)dbias_t })
+		if (t && (view_of(t).count != (size_t)C || !view_of(t).contiguous))
+			return CCV_NNC_EXEC_INVALID;
 	cudaStream_t s = stream_of(stream_context);
 	void* const ws = ccv_nnc_stream_context_get_workspace(stream_context, bn_workspace_bytes(C), CCV_TENSOR_GPU_MEMORY);
 	if (!ws)

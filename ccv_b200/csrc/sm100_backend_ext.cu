@@ -33,6 +33,12 @@ bool packed_f32(const ccv_nnc_tensor_t* const t)
 	return CCV_GET_DATA_TYPE(t->info.datatype) == CCV_32F && CCV_IS_TENSOR_CONTIGUOUS(t);
 }
 
+// a packed fp32 tensor of exactly `count` elements: what the row-norm kernels assume of every operand they index as [rows, inner]
+bool packed_f32_of(const ccv_nnc_tensor_t* const t, const size_t count)
+{
+	return packed_f32(t) && count_of(t) == count;
+}
+
 // the normalised axes must be the trailing ones: x is then [rows, inner]
 bool rows_inner(const ccv_nnc_tensor_t* const x, const int* const axis, const int axis_count, int& rows, int& inner)
 {
@@ -372,7 +378,7 @@ int ccv_nnc_sm100_exec_lnorm_forw(SM100_EXEC_ARGS)
 		return CCV_NNC_EXEC_INVALID;
 	float* sm = output_size > 1 && outputs[1] ? outputs[1]->data.f32 : 0;
 	float* sis = output_size > 2 && outputs[2] ? outputs[2]->data.f32 : 0;
-	if ((sm && count_of(outputs[1]) != (size_t)rows) || (sis && count_of(outputs[2]) != (size_t)rows))
+	if ((sm && !packed_f32_of(outputs[1], rows)) || (sis && !packed_f32_of(outputs[2], rows)))
 		return CCV_NNC_EXEC_INVALID;
 	if (layer_norm_fwd_f32(stream_of(stream_context), inputs[0]->data.f32, affine ? inputs[1]->data.f32 : 0, affine ? inputs[2]->data.f32 : 0, outputs[0]->data.f32, sm, sis, rows, inner, cmd.info.lnorm.epsilon))
 		return CCV_NNC_EXEC_INVALID;
@@ -389,12 +395,17 @@ int ccv_nnc_sm100_exec_lnorm_back(SM100_EXEC_ARGS)
 	int rows, inner;
 	if (!rows_inner(inputs[3], cmd.info.lnorm.axis, cmd.info.lnorm.count, rows, inner) || !packed_f32(inputs[0]) || count_of(inputs[0]) != (size_t)rows * inner)
 		return CCV_NNC_EXEC_INVALID;
-	if (count_of(inputs[mi]) != (size_t)rows || count_of(inputs[si]) != (size_t)rows)
+	if (!packed_f32_of(inputs[mi], rows) || !packed_f32_of(inputs[si], rows) || (affine && !packed_f32_of(inputs[4], inner)))
 		return CCV_NNC_EXEC_INVALID;
 	float* h = outputs[0] ? outputs[0]->data.f32 : 0;
 	float* ds = output_size > 1 && outputs[1] ? outputs[1]->data.f32 : 0;
 	float* db = output_size > 2 && outputs[2] ? outputs[2]->data.f32 : 0;
-	if (layer_norm_bwd_f32(stream_of(stream_context), inputs[0]->data.f32, inputs[3]->data.f32, affine ? inputs[4]->data.f32 : 0, inputs[mi]->data.f32, inputs[si]->data.f32, h, ds, db, rows, inner, 0))
+	if ((h && !packed_f32_of(outputs[0], (size_t)rows * inner)) || (ds && !packed_f32_of(outputs[1], inner)) || (db && !packed_f32_of(outputs[2], inner)))
+		return CCV_NNC_EXEC_INVALID;
+	void* const ws = ds || db ? ccv_nnc_stream_context_get_workspace(stream_context, norm_bwd_workspace_bytes(rows, inner), CCV_TENSOR_GPU_MEMORY) : 0;
+	if ((ds || db) && !ws)
+		return CCV_NNC_EXEC_OOM;
+	if (layer_norm_bwd_f32(stream_of(stream_context), inputs[0]->data.f32, inputs[3]->data.f32, affine ? inputs[4]->data.f32 : 0, inputs[mi]->data.f32, inputs[si]->data.f32, h, ds, db, rows, inner, ws))
 		return CCV_NNC_EXEC_INVALID;
 	return CCV_NNC_EXEC_SUCCESS;
 }
@@ -434,8 +445,11 @@ static bool gn_geom(const ccv_nnc_tensor_t* const x, const ccv_nnc_tensor_t* con
 		g.sdim[i] = 1;
 	if (scale && (!packed_f32(scale) || nd_of(scale) != nd_of(x) || !gn_dims(scale, g.sdim, 0)))
 		return false;
+	// Slots must divide the axis.  Where they do not, the reference divides every slot's sums by the one integer
+	// n = count(x) / count(statistics) (norm/ccv_nnc_group_norm_cpu_ref.c:52-57, :464) although the slots hold different numbers of
+	// elements, so its "mean" is not a mean; there is nothing meaningful to agree with, and the command is refused.
 	for (int i = 0; i < 4; i++)
-		if (g.rdim[i] < 1 || g.rdim[i] > g.dim[i] || g.sdim[i] < 1 || g.sdim[i] > g.dim[i])
+		if (g.rdim[i] < 1 || g.dim[i] % g.rdim[i] != 0 || g.sdim[i] < 1 || g.dim[i] % g.sdim[i] != 0)
 			return false;
 	return true;
 }
@@ -489,10 +503,10 @@ int ccv_nnc_sm100_exec_rmsnorm_forw(SM100_EXEC_ARGS)
 	if (input_size < 2 || output_size < 1 || !inputs[0] || !inputs[1] || !outputs[0])
 		return CCV_NNC_EXEC_INVALID;
 	int rows, inner;
-	if (!rows_inner(inputs[0], cmd.info.rmsnorm.axis, cmd.info.rmsnorm.count, rows, inner) || !packed_f32(outputs[0]) || !packed_f32(inputs[1]) || count_of(inputs[1]) != (size_t)inner)
+	if (!rows_inner(inputs[0], cmd.info.rmsnorm.axis, cmd.info.rmsnorm.count, rows, inner) || !packed_f32_of(outputs[0], (size_t)rows * inner) || !packed_f32_of(inputs[1], inner))
 		return CCV_NNC_EXEC_INVALID;
 	float* sis = output_size > 1 && outputs[1] ? outputs[1]->data.f32 : 0;
-	if (sis && count_of(outputs[1]) != (size_t)rows)
+	if (sis && !packed_f32_of(outputs[1], rows))
 		return CCV_NNC_EXEC_INVALID;
 	if (rmsnorm_fwd_f32(stream_of(stream_context), inputs[0]->data.f32, inputs[1]->data.f32, outputs[0]->data.f32, sis, rows, inner, cmd.info.rmsnorm.epsilon))
 		return CCV_NNC_EXEC_INVALID;
@@ -505,11 +519,16 @@ int ccv_nnc_sm100_exec_rmsnorm_back(SM100_EXEC_ARGS)
 	if (input_size < 6 || output_size < 1 || !inputs[0] || !inputs[2] || !inputs[3] || !inputs[5])
 		return CCV_NNC_EXEC_INVALID;
 	int rows, inner;
-	if (!rows_inner(inputs[2], cmd.info.rmsnorm.axis, cmd.info.rmsnorm.count, rows, inner) || !packed_f32(inputs[0]) || count_of(inputs[5]) != (size_t)rows || count_of(inputs[3]) != (size_t)inner)
+	if (!rows_inner(inputs[2], cmd.info.rmsnorm.axis, cmd.info.rmsnorm.count, rows, inner) || !packed_f32_of(inputs[0], (size_t)rows * inner) || !packed_f32_of(inputs[5], rows) || !packed_f32_of(inputs[3], inner))
 		return CCV_NNC_EXEC_INVALID;
 	float* h = outputs[0] ? outputs[0]->data.f32 : 0;
 	float* ds = output_size > 1 && outputs[1] ? outputs[1]->data.f32 : 0;
-	if (rmsnorm_bwd_f32(stream_of(stream_context), inputs[0]->data.f32, inputs[2]->data.f32, inputs[3]->data.f32, inputs[5]->data.f32, h, ds, rows, inner, 0))
+	if ((h && !packed_f32_of(outputs[0], (size_t)rows * inner)) || (ds && !packed_f32_of(outputs[1], inner)))
+		return CCV_NNC_EXEC_INVALID;
+	void* const ws = ds ? ccv_nnc_stream_context_get_workspace(stream_context, norm_bwd_workspace_bytes(rows, inner), CCV_TENSOR_GPU_MEMORY) : 0;
+	if (ds && !ws)
+		return CCV_NNC_EXEC_OOM;
+	if (rmsnorm_bwd_f32(stream_of(stream_context), inputs[0]->data.f32, inputs[2]->data.f32, inputs[3]->data.f32, inputs[5]->data.f32, h, ds, rows, inner, ws))
 		return CCV_NNC_EXEC_INVALID;
 	return CCV_NNC_EXEC_SUCCESS;
 }

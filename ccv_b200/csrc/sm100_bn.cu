@@ -779,8 +779,10 @@ static int bn_bwd_t(cudaStream_t s, const T* g, const T* x, const float* scale, 
 	float* const part = dx_colsum ? ws_part(workspace, C) : 0;
 	if (mask ? run_apply<T, 1, 1>(s, x, g, dx, coef, outer, C, inner, part, dx_colsum, colsum_kind, &done) : run_apply<T, 1, 0>(s, x, g, dx, coef, outer, C, inner, part, dx_colsum, colsum_kind, &done))
 		return -1;
-	if (dx_colsum && !done) // layouts the vector path does not take: a separate column sum over dx
-		return colsum_any(s, ElemKind<T>::value, dx, outer * inner, C, C, dx_colsum, colsum_kind, 0, 0);
+	if (dx_colsum && !done) // layouts the vector path does not take: a separate column sum over dx, with the partial area (sms * 4 + 8
+		// rows of 2C floats, at least the sms * 8 rows of C it needs) as its workspace so that its row blocks are combined in a fixed
+		// order and not with atomics
+		return colsum_any(s, ElemKind<T>::value, dx, outer * inner, C, C, dx_colsum, colsum_kind, 0, part);
 	return 0;
 }
 

@@ -101,6 +101,8 @@ int copy_strided(cudaStream_t s, const void* a, const int* astride, void* b, con
 
 // ---- layer norm / rms norm over the last `inner` elements of each of `rows` rows -----------------------------
 int layer_norm_fwd_f32(cudaStream_t s, const float* x, const float* scale, const float* bias, float* y, float* saved_mean, float* saved_inv_std, int rows, int inner, float epsilon);
+// the backward's workspace when dscale / dbias are requested: one row of partial column sums per row block
+size_t norm_bwd_workspace_bytes(int rows, int inner);
 int layer_norm_bwd_f32(cudaStream_t s, const float* g, const float* x, const float* scale, const float* saved_mean, const float* saved_inv_std, float* dx, float* dscale, float* dbias, int rows, int inner, void* workspace);
 int rmsnorm_fwd_f32(cudaStream_t s, const float* x, const float* scale, float* y, float* saved_inv_std, int rows, int inner, float epsilon);
 int rmsnorm_bwd_f32(cudaStream_t s, const float* g, const float* x, const float* scale, const float* saved_inv_std, float* dx, float* dscale, int rows, int inner, void* workspace);

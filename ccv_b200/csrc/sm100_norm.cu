@@ -115,9 +115,13 @@ __global__ void norm_bwd_dx_kernel(const float* __restrict__ g, const float* __r
 		dx[o + j] = r * (gs - s1 - (x[o + j] - mean) * r * s2);
 	}
 }
-// dscale[j] = sum_rows g * xhat, dbias[j] = sum_rows g: column reductions with one atomic per (block, column)
+// dscale[j] = sum_rows g * xhat, dbias[j] = sum_rows g.  Row block y (rows y, y + gridDim.y, ..) leaves its two partial sums of column j
+// in part[y][j] and part[y][inner + j]; norm_bwd_dparam_rows_kernel then adds the gridDim.y rows in a fixed order, so the result does
+// not depend on the order in which blocks finish (one atomicAdd per (block, column) did).
+static int dparam_row_blocks(int rows) { return rows < 296 ? rows : 296; }
+size_t norm_bwd_workspace_bytes(int rows, int inner) { return rows <= 0 || inner <= 0 ? 0 : (size_t)dparam_row_blocks(rows) * 2 * (size_t)inner * sizeof(float); }
 template <int RMS>
-__global__ void norm_bwd_dparam_kernel(const float* __restrict__ g, const float* __restrict__ x, const float* __restrict__ saved_mean, const float* __restrict__ saved_inv_std, float* __restrict__ dscale, float* __restrict__ dbias, const int rows, const int inner)
+__global__ void norm_bwd_dparam_kernel(const float* __restrict__ g, const float* __restrict__ x, const float* __restrict__ saved_mean, const float* __restrict__ saved_inv_std, float* __restrict__ part, const int rows, const int inner)
 {
 	const int j = blockIdx.x * blockDim.x + threadIdx.x;
 	if (j >= inner)
@@ -129,16 +133,47 @@ __global__ void norm_bwd_dparam_kernel(const float* __restrict__ g, const float*
 		a += gv * (x[(size_t)r * inner + j] - (RMS ? 0.f : saved_mean[r])) * saved_inv_std[r];
 		b += gv;
 	}
+	float* const row = part + (size_t)blockIdx.y * 2 * inner;
+	row[j] = a;
+	if (!RMS)
+		row[inner + j] = b;
+}
+// 32 columns x 32 row-lanes per block: lane l adds rows l, l + 32, .. in order, then the 32 lane sums are added in order
+__global__ void __launch_bounds__(1024) norm_bwd_dparam_rows_kernel(const float* __restrict__ part, const int gy, const int inner, float* __restrict__ dscale, float* __restrict__ dbias)
+{
+	__shared__ float sh[2][32][33];
+	const int cx = threadIdx.x & 31, yl = threadIdx.x >> 5;
+	const int j = blockIdx.x * 32 + cx;
+	float a = 0.f, b = 0.f;
+	if (j < inner)
+		for (int y = yl; y < gy; y += 32)
+		{
+			const float* const row = part + (size_t)y * 2 * inner;
+			if (dscale)
+				a += row[j];
+			if (dbias)
+				b += row[inner + j];
+		}
+	sh[0][yl][cx] = a, sh[1][yl][cx] = b;
+	__syncthreads();
+	if (yl != 0 || j >= inner)
+		return;
+	a = b = 0.f;
+#pragma unroll
+	for (int l = 0; l < 32; l++)
+		a += sh[0][l][cx], b += sh[1][l][cx];
 	if (dscale)
-		atomicAdd(dscale + j, a);
+		dscale[j] = a;
 	if (dbias)
-		atomicAdd(dbias + j, b);
+		dbias[j] = b;
 }
 template <int RMS>
-static int norm_bwd(cudaStream_t s, const float* g, const float* x, const float* scale, const float* saved_mean, const float* saved_inv_std, float* dx, float* dscale, float* dbias, int rows, int inner)
+static int norm_bwd(cudaStream_t s, const float* g, const float* x, const float* scale, const float* saved_mean, const float* saved_inv_std, float* dx, float* dscale, float* dbias, int rows, int inner, void* workspace)
 {
 	if (rows <= 0 || inner <= 0)
 		return 0;
+	if ((dscale || dbias) && !workspace)
+		return -1;
 	if (dx)
 	{
 		norm_bwd_dx_kernel<RMS><<<rows, row_threads(inner), 0, s>>>(g, x, scale, saved_mean, saved_inv_std, dx, inner);
@@ -147,24 +182,23 @@ static int norm_bwd(cudaStream_t s, const float* g, const float* x, const float*
 	}
 	if (dscale || dbias)
 	{
-		if (dscale && cudaMemsetAsync(dscale, 0, (size_t)inner * 4, s) != cudaSuccess)
-			return -1;
-		if (dbias && cudaMemsetAsync(dbias, 0, (size_t)inner * 4, s) != cudaSuccess)
-			return -1;
-		int gy = rows < 296 ? rows : 296;
-		norm_bwd_dparam_kernel<RMS><<<dim3((inner + 127) / 128, gy), 128, 0, s>>>(g, x, saved_mean, saved_inv_std, dscale, dbias, rows, inner);
+		const int gy = dparam_row_blocks(rows);
+		norm_bwd_dparam_kernel<RMS><<<dim3((inner + 127) / 128, gy), 128, 0, s>>>(g, x, saved_mean, saved_inv_std, (float*)workspace, rows, inner);
 		if (check("norm_bwd_dparam"))
+			return -1;
+		norm_bwd_dparam_rows_kernel<<<(inner + 31) / 32, 1024, 0, s>>>((const float*)workspace, gy, inner, dscale, dbias);
+		if (check("norm_bwd_dparam_rows"))
 			return -1;
 	}
 	return 0;
 }
 int layer_norm_bwd_f32(cudaStream_t s, const float* g, const float* x, const float* scale, const float* saved_mean, const float* saved_inv_std, float* dx, float* dscale, float* dbias, int rows, int inner, void* workspace)
 {
-	return norm_bwd<0>(s, g, x, scale, saved_mean, saved_inv_std, dx, dscale, dbias, rows, inner);
+	return norm_bwd<0>(s, g, x, scale, saved_mean, saved_inv_std, dx, dscale, dbias, rows, inner, workspace);
 }
 int rmsnorm_bwd_f32(cudaStream_t s, const float* g, const float* x, const float* scale, const float* saved_inv_std, float* dx, float* dscale, int rows, int inner, void* workspace)
 {
-	return norm_bwd<1>(s, g, x, scale, 0, saved_inv_std, dx, dscale, 0, rows, inner);
+	return norm_bwd<1>(s, g, x, scale, 0, saved_inv_std, dx, dscale, 0, rows, inner, workspace);
 }
 
 // ------------------------------------------------------------------------------------------------ upsample
@@ -450,19 +484,22 @@ int group_norm_bwd_f32(cudaStream_t s, const GroupNormGeom& g, const float* grad
 	{
 		float* const sums = (float*)workspace;
 		gn_bwd_stats_kernel<<<(unsigned)slots, 512, 0, s>>>(g, grad, x, scale, saved_mean, saved_inv_std, sums);
-		count_launch();
+		if (check("group_norm_bwd_stats"))
+			return -1;
 		long long blocks = (total + 255) / 256;
 		if (blocks > 132 * 16)
 			blocks = 132 * 16;
 		gn_bwd_apply_kernel<<<(unsigned)blocks, 256, 0, s>>>(g, grad, x, scale, saved_mean, saved_inv_std, sums, h, total, (float)slots / (float)total);
-		count_launch();
+		if (check("group_norm_bwd_apply"))
+			return -1;
 	}
 	if (dscale || dbias)
 	{
 		gn_bwd_dparam_kernel<<<(unsigned)gn_count(g.sdim), 256, 0, s>>>(g, grad, x, saved_mean, saved_inv_std, dscale, dbias);
-		count_launch();
+		if (check("group_norm_bwd_dparam"))
+			return -1;
 	}
-	return check("group_norm_bwd") ;
+	return 0;
 }
 
 } // namespace sm100
