@@ -342,12 +342,13 @@ static int launch_umma(cudaStream_t stream, const CUtensorMap& tmA, const CUtens
 		}
 	}
 	const long long sms = num_sms(), columns = (long long)grid.y * grid.z, ctas = tiles_m * columns;
-	if (!q.stats && p.splits == 1 && p.grid_taps == 1 && ctas > sms)
+	if (!q.stats && p.splits == 1 && p.grid_taps == 1 && BMODE != OP_IM2COL && ctas > sms)
 	{
 		// more tiles than one wave of one CTA per SM: gx CTAs per column walk the M tiles, so the producer loads the next tile while the
 		// consumers store this one.  Taken only when it costs no more rounds of tiles than one tile per CTA does.  Not for split-K or
-		// per-tap launches (the weight gradients): their few M tiles share one large B slice per column, which side-by-side CTAs read
-		// from L2 once and walking CTAs read again from HBM (walked, ResNet-50's 1x1 weight gradients ran 12-19 % slower on an H100)
+		// im2col-B launches (the weight gradients with filter taps): their few M tiles share one large B slice per column, which
+		// side-by-side CTAs read from L2 once and walking CTAs read again from HBM (walked, ResNet-50's 1x1 weight gradients ran 12-19 %
+		// slower on an H100)
 		long long gx = sms / columns;
 		gx = gx < 1 ? 1 : (gx > tiles_m ? tiles_m : gx);
 		if ((gx * columns + sms - 1) / sms * ((tiles_m + gx - 1) / gx) <= (ctas + sms - 1) / sms)
@@ -820,22 +821,36 @@ int conv_wgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, const void*
 	const long long npq = (long long)g.N * g.P * g.Q;
 	if (npq > 0x7fffffffll)
 		return 1;
-	const int bn = pick_bn(g.C);
 	const long long rsc = (long long)g.R * g.S * g.C;
+	// Split-K: the factor the per-tap grid below is planned with (tiles of pick_bn(C) columns, one per tap), for every layout, so that
+	// each dW element is the same sum over the same pixel ranges, combined in the same order, whichever layout computes it
+	const int grid_bn = pick_bn(g.C);
+	const int k_iters = (int)((npq + bk - 1) / bk);
+	const long long tiles_m = (g.K + 127) / 128, grid_tiles = tiles_m * ((g.C + grid_bn - 1) / grid_bn) * g.R * g.S;
+	// split-K slices have the layout of dW itself ([K, RSC]); splitk_reduce adds them (and the old dW when accumulating)
+	const size_t dw_bytes = (size_t)g.K * rsc * sizeof(float);
+	const int splits = fit_splits(pick_splits(grid_tiles, k_iters, 16), k_iters, dw_bytes, scratch);
+	// Taps along the columns: dW[K, R*S*C] = grad_b^T [K, NPQ] x im2col(a) [NPQ, R*S*C], column n = tap * C + c, each bk-channel B box
+	// of a tile loading the tap its columns belong to, so one read of a pixel block serves every tap of the tile.  A tile then carries
+	// several taps' work, so this layout is taken when it needs fewer rounds of CTAs over the SMs than the per-tap grid does (the
+	// 32-channel layers, whose per-tap tiles are a 64-column eighth of the work of a 128-column one), and needs C to be a multiple of
+	// bk (else two taps would share a box).  Otherwise one launch with the filter tap on gridDim.z writes the columns [tap * C, +C).
+	const int col_bn = pick_bn((int)rsc);
+	const long long sms = num_sms(), col_ctas = tiles_m * ((rsc + col_bn - 1) / col_bn) * splits;
+	const bool tap_cols = !conv_is_pointwise(g) && g.C % bk == 0 && (col_ctas + sms - 1) / sms < (grid_tiles * splits + sms - 1) / sms;
+	const int cols = tap_cols || conv_is_pointwise(g) ? (int)rsc : g.C;
+	const int bn = tap_cols ? col_bn : grid_bn;
 	CUtensorMap tmA, tmB;
 	// A = grad_b^T: [K, NPQ] read from the [NPQ, K] tensor as an MN-major operand
 	if (!map_2d(&tmA, kind, grad_b, npq, g.K, g.K, bk, true))
 		return 1;
 	UmmaGemmParams p;
 	init_params_kind(p, kind);
-	p.M = g.K, p.N = g.C;
-	p.k_iters = (int)((npq + bk - 1) / bk);
+	p.M = g.K, p.N = cols;
+	p.k_iters = k_iters;
 	p.chunks_per_tap = p.k_iters;
 	p.rowmap.mode = 0, p.rowmap.ld = rsc;
-	const long long tiles = (long long)((g.K + 127) / 128) * ((g.C + bn - 1) / bn) * g.R * g.S;
-	// split-K slices have the layout of dW itself ([K, RSC]); splitk_reduce adds them (and the old dW when accumulating)
-	const size_t dw_bytes = (size_t)g.K * rsc * sizeof(float);
-	p.splits = fit_splits(pick_splits(tiles, p.k_iters, 16), p.k_iters, dw_bytes, scratch);
+	p.splits = splits;
 	if (conv_is_pointwise(g))
 	{
 		// B = a: [NHW, C], also MN-major
@@ -845,8 +860,9 @@ int conv_wgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, const void*
 	}
 	if (!map_im2col(&tmB, kind, a, g.N, g.H, g.W, g.C, g.an, g.ah, g.aw, -g.pad_h0, -g.pad_w0, g.pad_h1 - (g.R - 1) * g.dil_h, g.pad_w1 - (g.S - 1) * g.dil_w, g.stride_h, g.stride_w, bk, true))
 		return 1;
-	p.grid_taps = g.R * g.S;
-	p.grid_tap_out_stride = g.C;
+	p.C_tap = g.C;
+	if (!tap_cols)
+		p.grid_taps = g.R * g.S, p.grid_tap_out_stride = g.C;
 	p.P = g.P, p.Q = g.Q;
 	p.stride_h = g.stride_h, p.stride_w = g.stride_w;
 	p.base_h = -g.pad_h0, p.base_w = -g.pad_w0;

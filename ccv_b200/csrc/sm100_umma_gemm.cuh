@@ -52,6 +52,7 @@ struct UmmaGemmParams {
 	long long split_out_stride;
 	int grid_taps;      // > 1 only for wgrad: the filter tap is a grid dimension
 	long long grid_tap_out_stride; // output column offset per grid tap
+	int C_tap;          // B = OP_IM2COL (wgrad): channels per filter tap.  B column n < N reads the grid tap + n / C_tap, channel n % C_tap
 	// im2col geometry of the operand that uses OP_IM2COL: base pixel p -> (w, h, n) TMA coordinates
 	int P, Q;
 	int stride_h, stride_w;
@@ -201,6 +202,19 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) umma_gemm_kernel(const __grid
 		{
 			tma_prefetch_desc(&tmA);
 			tma_prefetch_desc(&tmB);
+			// B = OP_IM2COL: each BK-column box of the tile loads one filter tap's channel span (C_tap is a multiple of BK when a
+			// tile holds several taps; with the tap on the grid, N = C_tap and every box is at the grid tap); a box past the last
+			// column asks for channels beyond C, which the TMA unit fills with zeros
+			int b_ch[BN / BK], b_off_w[BN / BK], b_off_h[BN / BK];
+#pragma unroll
+			for (int j = 0; j < BN / BK; j++)
+			{
+				const int col = n0 + BK * j;
+				const int t = BMODE == OP_IM2COL && col < p.N ? col / p.C_tap : 0;
+				b_ch[j] = col - t * p.C_tap;
+				if (BMODE == OP_IM2COL)
+					b_off_w[j] = p.tap_off_w[gtap + t], b_off_h[j] = p.tap_off_h[gtap + t];
+			}
 			int stage = 0;
 			uint32_t phase = 0;
 			for (int mt = blockIdx.x; mt < tiles_m; mt += gridDim.x)
@@ -247,7 +261,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) umma_gemm_kernel(const __grid
 					const int b_n = t / p.P;
 #pragma unroll
 					for (int j = 0; j < BN / BK; j++)
-						tma_load_im2col_4d(sB + j * MN_BOX_BYTES, &tmB, &full_bar[stage], n0 + BK * j, b_w, b_h, b_n, p.tap_off_w[gtap], p.tap_off_h[gtap]);
+						tma_load_im2col_4d(sB + j * MN_BOX_BYTES, &tmB, &full_bar[stage], b_ch[j], b_w, b_h, b_n, (uint16_t)b_off_w[j], (uint16_t)b_off_h[j]);
 				}
 				if (++stage == STAGES) { stage = 0; phase ^= 1; }
 			}
