@@ -995,6 +995,14 @@ int ccv_nnc_sm100_graph_fuse(ccv_nnc_sm100_graph_t* const graph)
 			// hyper-parameters (weights with decay, biases / norm parameters without) even when the groups interleave
 			while (j < n && is_gpu_sm100(nodes[j]) && nodes[j].cmd.cmd == CCV_NNC_SGD_FORWARD && nodes[j].inputs.size() == 3 && nodes[j].outputs.size() == 2 && independent(nodes[j], i, j))
 				j++;
+			// the multi-tensor kernel takes fp32 parameters and momenta only; a node with 16-bit ones runs on its own (through the
+			// functional form of exec_sgd_any)
+			auto fp32_state = [](const ccv_nnc_sm100_graph_node_t& x) {
+				for (ccv_nnc_tensor_t* t : { x.inputs[1], x.inputs[2], x.outputs[0], x.outputs[1] })
+					if (!t || CCV_GET_DATA_TYPE(t->info.datatype) != CCV_32F)
+						return false;
+				return true;
+			};
 			std::vector<char> done(j - i, 0);
 			for (size_t k = i; k < j; k++)
 			{
@@ -1002,8 +1010,8 @@ int ccv_nnc_sm100_graph_fuse(ccv_nnc_sm100_graph_t* const graph)
 					continue;
 				ccv_nnc_sm100_graph_node_t f = nodes[k];
 				int members = 1;
-				for (size_t q = k + 1; q < j; q++)
-					if (!done[q - i] && memcmp(&nodes[q].cmd.info.sgd, &f.cmd.info.sgd, sizeof(f.cmd.info.sgd)) == 0 && nodes[q].flags == f.flags && nodes[q].cmd.algorithm == f.cmd.algorithm &&
+				for (size_t q = k + 1; q < j && fp32_state(f); q++)
+					if (!done[q - i] && fp32_state(nodes[q]) && memcmp(&nodes[q].cmd.info.sgd, &f.cmd.info.sgd, sizeof(f.cmd.info.sgd)) == 0 && nodes[q].flags == f.flags && nodes[q].cmd.algorithm == f.cmd.algorithm &&
 					nodes[q].inputs[0] && f.inputs[0] && nodes[q].inputs[0]->info.datatype == f.inputs[0]->info.datatype) // one gradient type per launch (16-bit and fp32 gradients of a mixed-precision model go separately)
 					{
 						f.inputs.insert(f.inputs.end(), nodes[q].inputs.begin(), nodes[q].inputs.end());

@@ -1885,12 +1885,24 @@ bool label_kind_of(const ccv_nnc_tensor_t* const b_t, const int batch, int& kind
 	return true;
 }
 
+// the label holds one class index per row (kind 0 / 1) or one row of `count` probabilities per row (kind 2)
+bool label_fits(const ccv_nnc_tensor_t* const b_t, const int kind, const int batch, const int count)
+{
+	return view_of(b_t).count == (size_t)batch * (kind == 2 ? (size_t)count : 1);
+}
+
+// a loss c or a gradient g of the loss: one fp32 value per row (absent: g reads as ones)
+bool per_row_ok(const ccv_nnc_tensor_t* const t, const int batch)
+{
+	return !t || (is_f32(t) && view_of(t).contiguous && view_of(t).count == (size_t)batch);
+}
+
 int exec_cce_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
 {
 	if (input_size != 2 || output_size < 1 || !inputs[0] || !inputs[1] || !outputs[0])
 		return CCV_NNC_EXEC_INVALID;
 	int batch, count, kind;
-	if (!is_f32(inputs[0]) || !rows_of(view_of(inputs[0]), batch, count) || !label_kind_of(inputs[1], batch, kind) || !view_of(outputs[0]).contiguous)
+	if (!is_f32(inputs[0]) || !rows_of(view_of(inputs[0]), batch, count) || !label_kind_of(inputs[1], batch, kind) || !label_fits(inputs[1], kind, batch, count) || !per_row_ok(outputs[0], batch))
 		return CCV_NNC_EXEC_INVALID;
 	RC(cce_fwd_f32(stream_of(stream_context), inputs[0]->data.f32, inputs[1]->data.ptr, kind, outputs[0]->data.f32, batch, count, cmd.info.label_smoothing.trim0, cmd.info.label_smoothing.trim1));
 	return CCV_NNC_EXEC_SUCCESS;
@@ -1902,7 +1914,7 @@ int exec_cce_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int 
 	if (input_size < 3 || output_size < 1 || !inputs[1] || !inputs[2] || !outputs[0])
 		return CCV_NNC_EXEC_INVALID;
 	int batch, count, kind;
-	if (!is_f32(inputs[1]) || !rows_of(view_of(inputs[1]), batch, count) || !label_kind_of(inputs[2], batch, kind) || !view_of(outputs[0]).contiguous || !same_shape(view_of(inputs[1]), view_of(outputs[0])))
+	if (!is_f32(inputs[1]) || !rows_of(view_of(inputs[1]), batch, count) || !label_kind_of(inputs[2], batch, kind) || !label_fits(inputs[2], kind, batch, count) || !per_row_ok(inputs[0], batch) || !view_of(outputs[0]).contiguous || !same_shape(view_of(inputs[1]), view_of(outputs[0])))
 		return CCV_NNC_EXEC_INVALID;
 	RC(cce_bwd_f32(stream_of(stream_context), inputs[0] ? inputs[0]->data.f32 : 0, inputs[1]->data.f32, inputs[2]->data.ptr, kind, outputs[0]->data.f32, batch, count, cmd.info.label_smoothing.trim0, cmd.info.label_smoothing.trim1));
 	return CCV_NNC_EXEC_SUCCESS;
@@ -1914,7 +1926,7 @@ int exec_softmax_cce_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, co
 	if (input_size != 2 || output_size != 2 || !inputs[0] || !inputs[1] || !outputs[1])
 		return CCV_NNC_EXEC_INVALID;
 	int batch, count, kind;
-	if (!is_f32(inputs[0]) || !rows_of(view_of(inputs[0]), batch, count) || !label_kind_of(inputs[1], batch, kind) || !view_of(outputs[1]).contiguous || !same_shape(view_of(inputs[0]), view_of(outputs[1])))
+	if (!is_f32(inputs[0]) || !rows_of(view_of(inputs[0]), batch, count) || !label_kind_of(inputs[1], batch, kind) || !label_fits(inputs[1], kind, batch, count) || !per_row_ok(outputs[0], batch) || !view_of(outputs[1]).contiguous || !same_shape(view_of(inputs[0]), view_of(outputs[1])))
 		return CCV_NNC_EXEC_INVALID;
 	RC(softmax_cce_fwd_f32(stream_of(stream_context), inputs[0]->data.f32, inputs[1]->data.ptr, kind, outputs[0] ? outputs[0]->data.f32 : 0, outputs[1]->data.f32, batch, count, cmd.info.label_smoothing.trim0, cmd.info.label_smoothing.trim1));
 	return CCV_NNC_EXEC_SUCCESS;
@@ -1926,7 +1938,7 @@ int exec_softmax_cce_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, co
 	if (input_size < 6 || output_size < 1 || !inputs[3] || !inputs[5] || !outputs[0])
 		return CCV_NNC_EXEC_INVALID;
 	int batch, count, kind;
-	if (!is_f32(inputs[5]) || !rows_of(view_of(inputs[5]), batch, count) || !label_kind_of(inputs[3], batch, kind) || !view_of(outputs[0]).contiguous || !same_shape(view_of(inputs[5]), view_of(outputs[0])))
+	if (!is_f32(inputs[5]) || !rows_of(view_of(inputs[5]), batch, count) || !label_kind_of(inputs[3], batch, kind) || !label_fits(inputs[3], kind, batch, count) || !per_row_ok(inputs[0], batch) || !view_of(outputs[0]).contiguous || !same_shape(view_of(inputs[5]), view_of(outputs[0])))
 		return CCV_NNC_EXEC_INVALID;
 	RC(softmax_cce_bwd_f32(stream_of(stream_context), inputs[0] ? inputs[0]->data.f32 : 0, inputs[3]->data.ptr, kind, inputs[5]->data.f32, outputs[0]->data.f32, batch, count, cmd.info.label_smoothing.trim0, cmd.info.label_smoothing.trim1));
 	return CCV_NNC_EXEC_SUCCESS;

@@ -690,10 +690,10 @@ __global__ void pool_bwd_kernel(const PoolGeom g, const T* __restrict__ gb, cons
 			h = (int)(r % g.H);
 			n = (int)(r / g.H);
 		}
-		if (!IS_MAX && VEC > 1 && g.R == g.stride_h && g.S == g.stride_w && g.pad_h == 0 && g.pad_w == 0)
+		if (!IS_MAX && VEC > 1 && g.R == g.stride_h && g.S == g.stride_w && g.pad_h == 0 && g.pad_w == 0 && g.P * g.stride_h <= g.H && g.Q * g.stride_w <= g.W)
 		{
 			// non-overlapping windows (the 2 x 2 / 2 shortcut pools, the global pool): every input position belongs to at most one
-			// window, whose size is never clipped -> one load, one divide per lane, one store
+			// window, and with P * R <= H, Q * S <= W (no end border) none is clipped -> one load, one divide per lane, one store
 			const int p = h / g.stride_h, q = w / g.stride_w;
 			float o[VEC];
 #pragma unroll
@@ -825,8 +825,9 @@ int pool_avg_bwd_16(cudaStream_t s, int kind, const PoolGeom& g, const void* gra
 }
 
 // =============================================================================================== softmax / losses
-// softmax/ccv_nnc_softmax_cpu_ref.c:13-40: per row, b = exp(a - max) / sum; one block per row
-__global__ void softmax_fwd_kernel(const float* __restrict__ a, float* __restrict__ b, const int count)
+// softmax/ccv_nnc_softmax_cpu_ref.c:13-40: per row, b = exp(a - max) / sum; one block per row.  b may be a (in place), so neither
+// pointer is __restrict__: each element is read before the same thread writes it
+__global__ void softmax_fwd_kernel(const float* a, float* b, const int count)
 {
 	__shared__ float sh[32];
 	const float* ap = a + (size_t)blockIdx.x * count;
@@ -855,8 +856,8 @@ int softmax_fwd_f32(cudaStream_t s, const float* a, float* b, int batch, int cou
 	softmax_fwd_kernel<<<batch, softmax_threads(count), 0, s>>>(a, b, count);
 	return check("softmax_fwd");
 }
-// softmax/ccv_nnc_softmax_cpu_ref.c:42-75: h = (g - sum(g * b)) * b
-__global__ void softmax_bwd_kernel(const float* __restrict__ g, const float* __restrict__ b, float* __restrict__ h, const int count)
+// softmax/ccv_nnc_softmax_cpu_ref.c:42-75: h = (g - sum(g * b)) * b; h may be g (in place)
+__global__ void softmax_bwd_kernel(const float* g, const float* __restrict__ b, float* h, const int count)
 {
 	__shared__ float sh[32];
 	const size_t o = (size_t)blockIdx.x * count;
@@ -945,7 +946,9 @@ int cce_bwd_f32(cudaStream_t s, const float* g, const float* a, const void* labe
 }
 // softmax_loss/ccv_nnc_softmax_crossentropy_cpu_ref.c:13-170: d = softmax(a); c = sum_j t_j * (max - a_j).
 // (The reference's "loss" deliberately leaves out log(sum exp): it is assigned before the exponentials, :46,:71,:98.)
-__global__ void softmax_cce_fwd_kernel(const float* __restrict__ a, const void* __restrict__ label, const int kind, float* __restrict__ c, float* __restrict__ d, const int count, const float trim0, const float trim1)
+// d may be a (softmax_loss/ccv_nnc_softmax_crossentropy.c:17-20 lets the graph allocator alias them), so neither is __restrict__ and
+// the loss term of a_j is taken in the exponential pass, from the value in a register, before d_j overwrites it
+__global__ void softmax_cce_fwd_kernel(const float* a, const void* __restrict__ label, const int kind, float* __restrict__ c, float* d, const int count, const float trim0, const float trim1)
 {
 	__shared__ float sh[32];
 	const int i = blockIdx.x;
@@ -955,28 +958,26 @@ __global__ void softmax_cce_fwd_kernel(const float* __restrict__ a, const void* 
 	for (int j = threadIdx.x; j < count; j += blockDim.x)
 		m = fmaxf(m, ap[j]);
 	m = block_max(m, sh);
-	float sum = 0.f;
+	const int l = kind == 2 ? -1 : label_of(label, kind, i);
+	const float* bp = kind == 2 ? reinterpret_cast<const float*>(label) + (size_t)i * count : 0;
+	float sum = 0.f, p = 0.f;
 	for (int j = threadIdx.x; j < count; j += blockDim.x)
 	{
-		const float e = expf(ap[j] - m);
+		const float x = ap[j];
+		if (c)
+		{
+			const float t = kind == 2 ? bp[j] : (j == l ? trim1 : trim0);
+			if (t != 0.f)
+				p += t * (m - x);
+		}
+		const float e = expf(x - m);
 		dp[j] = e;
 		sum += e;
 	}
 	sum = block_sum(sum, sh);
 	const float inv = 1.f / sum;
-	const int l = kind == 2 ? -1 : label_of(label, kind, i);
-	const float* bp = kind == 2 ? reinterpret_cast<const float*>(label) + (size_t)i * count : 0;
-	float p = 0.f;
 	for (int j = threadIdx.x; j < count; j += blockDim.x)
-	{
 		dp[j] *= inv;
-		if (c)
-		{
-			const float t = kind == 2 ? bp[j] : (j == l ? trim1 : trim0);
-			if (t != 0.f)
-				p += t * (m - ap[j]);
-		}
-	}
 	if (c)
 	{
 		p = block_sum(p, sh);
@@ -991,8 +992,9 @@ int softmax_cce_fwd_f32(cudaStream_t s, const float* a, const void* label, int l
 	softmax_cce_fwd_kernel<<<batch, softmax_threads(count), 0, s>>>(a, label, label_kind, c, d, count, trim0, trim1);
 	return check("softmax_cce_fwd");
 }
-// softmax_loss/ccv_nnc_softmax_crossentropy_cpu_ref.c:172-340: h = g * (d - t); g == NULL means 1
-__global__ void softmax_cce_bwd_kernel(const float* __restrict__ g, const void* __restrict__ label, const int kind, const float* __restrict__ d, float* __restrict__ h, const int count, const float trim0, const float trim1)
+// softmax_loss/ccv_nnc_softmax_crossentropy_cpu_ref.c:172-340: h = g * (d - t); g == NULL means 1.  h may be d
+// (softmax_loss/ccv_nnc_softmax_crossentropy.c:31-40)
+__global__ void softmax_cce_bwd_kernel(const float* __restrict__ g, const void* __restrict__ label, const int kind, const float* d, float* h, const int count, const float trim0, const float trim1)
 {
 	const int i = blockIdx.x;
 	const float gp = g ? g[i] : 1.f;
@@ -1018,9 +1020,10 @@ int softmax_cce_bwd_f32(cudaStream_t s, const float* g, const void* label, int l
 }
 
 // =============================================================================================== SGD
-// sgd/ccv_nnc_sgd_cpu_ref.c:16-126
+// sgd/ccv_nnc_sgd_cpu_ref.c:16-126.  b may be a and n may be m (sgd/ccv_nnc_sgd.c:14-19: how models call it), so those are not
+// __restrict__
 template <int VEC>
-__global__ void sgd_kernel(const void* __restrict__ g, const int g_kind, const float* __restrict__ a, const float* __restrict__ m, float* __restrict__ b, float* __restrict__ n, const size_t count, const int nesterov, const float rate, const float scale, const float decay, const float momentum, const float inv_dampening)
+__global__ void sgd_kernel(const void* __restrict__ g, const int g_kind, const float* a, const float* m, float* b, float* n, const size_t count, const int nesterov, const float rate, const float scale, const float decay, const float momentum, const float inv_dampening)
 {
 	const size_t cv = VEC == 4 ? count >> 2 : count;
 	for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < cv; i += (size_t)gridDim.x * blockDim.x)
