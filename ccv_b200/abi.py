@@ -16,6 +16,7 @@ CCV_NNC_ACCUMULATE_OUTPUT, CCV_NNC_ZERO_MEMORY_ALLOC = 0x01, 0x02
 CCV_NNC_EXEC_SUCCESS, CCV_NNC_EXEC_INVALID, CCV_NNC_EXEC_NO_KERNEL, CCV_NNC_EXEC_OOM = 0, -1, -2, -3
 CCV_NNC_UPSAMPLE_NEAREST, CCV_NNC_UPSAMPLE_BILINEAR = 0, 1
 CCV_NNC_MSE_REDUCE_MEAN, CCV_NNC_MSE_REDUCE_SUM = 0, 1  # lib/nnc/ccv_nnc.h:81-84 (cmd.info.mse.reduce_op)
+CCV_NNC_PAD_ZERO, CCV_NNC_PAD_REPLICATE = 0, 1  # lib/nnc/ccv_nnc.h:97-100 (cmd.info.pad.type)
 
 # backends (lib/nnc/cmd/ccv_nnc_backend.h + the new one)
 CCV_NNC_BACKEND_CPU_OPT = 0x46deb194
@@ -37,6 +38,7 @@ CMD_IDS = dict(
     EWDIV=0x1cd2fa18, REDUCE_SUM=0x52970f06, REDUCE_MEAN=0xf23556c6, REDUCE_MAX=0x80f1a506, REDUCE_MIN=0x6785ef96, REDUCE_NORM2=0xb3034e16,
     MASKED_FILL=0x7f992d84, DROPOUT=0x7f2dc3e4, ADAM=0xe30099dc, RANDOM_UNIFORM=0xa0cd1d5e, RANDOM_NORMAL=0x7062c8b4,
     CMUL=0xead486e6, BINARY_CROSSENTROPY=0xcd2107ec, SIGMOID_BINARY_CROSSENTROPY=0xd9e0e4a, MSE=0x6904a9a2, SMOOTH_L1=0x4e428e,
+    PAD=0xd8aaca60, MIN=0x972fbd26, MAX=0xdf6f014c, ARGMAX=0x68af2804, ARGMIN=0xeb8747f2, REDUCE_ISNAN=0xee0a4ade,
 )
 for _k, _v in CMD_IDS.items():
     globals()["CCV_NNC_%s_FORWARD" % _k] = _v
@@ -149,11 +151,15 @@ class _Dropout(C.Structure):
     _fields_ = [("p", C.c_float), ("entirety", C.c_int)]
 
 
+class _Pad(C.Structure):
+    _fields_ = [("type", C.c_int), ("end", C.c_int * MAX_DIM_ALLOC)]
+
+
 class _CmdUnion(C.Union):
     _fields_ = [("convolution", _Convolution), ("convolution_transpose", _ConvolutionTranspose), ("pool", _Pool), ("bnorm", _Bnorm), ("lnorm", _Lnorm), ("gnorm", _Gnorm), ("rmsnorm", _Rmsnorm),
                 ("sgd", _Sgd), ("adam", _Adam), ("gelu", _Gelu), ("blas", _Blas), ("label_smoothing", _LabelSmoothing), ("reduce", _Reduce), ("transpose", _Transpose),
                 ("upsample", _Upsample), ("clamp", _Clamp), ("leaky_relu", _LeakyRelu), ("dropout", _Dropout), ("scaled_dot_product_attention", _Sdpa),
-                ("binary_crossentropy", _BinaryCrossentropy), ("smooth_l1", _SmoothL1), ("mse", _Mse), ("userdata", C.c_void_p)]
+                ("binary_crossentropy", _BinaryCrossentropy), ("smooth_l1", _SmoothL1), ("mse", _Mse), ("pad", _Pad), ("userdata", C.c_void_p)]
 
 
 class CmdParam(C.Structure):

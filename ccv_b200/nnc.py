@@ -779,6 +779,46 @@ CMD_REDUCE_MIN_FORWARD, CMD_REDUCE_MIN_BACKWARD = _make_reduce("MIN")
 CMD_REDUCE_NORM2_FORWARD, CMD_REDUCE_NORM2_BACKWARD = _make_reduce("NORM2")
 
 
+def CMD_REDUCE_ISNAN_FORWARD(*axes, **kw):
+    """b (int32) = 1 where an element of a mapping to it is NaN; b's unit axes are the reduced ones (cmd/isnan)"""
+    return _reduce(abi.CCV_NNC_REDUCE_ISNAN_FORWARD, axes, **kw)
+
+
+def CMD_REDUCE_ISNAN_BACKWARD(*axes, **kw):
+    return _reduce(abi.CCV_NNC_REDUCE_ISNAN_BACKWARD, axes, **kw)
+
+
+def CMD_ARGMAX_FORWARD(axis, **kw):
+    """index (int32, or fp32 holding it) of the first maximum along `axis` (cmd/reduce/ccv_nnc_argmax_cpu_ref.c)"""
+    return _reduce(abi.CCV_NNC_ARGMAX_FORWARD, (axis,), **kw)
+
+
+def CMD_ARGMIN_FORWARD(axis, **kw):
+    return _reduce(abi.CCV_NNC_ARGMIN_FORWARD, (axis,), **kw)
+
+
+CMD_MIN_FORWARD, CMD_MIN_BACKWARD = _make_simple("MIN")  # element-wise a < b ? a : b (cmd/compare)
+CMD_MAX_FORWARD, CMD_MAX_BACKWARD = _make_simple("MAX")
+
+
+def _pad(cmd_id, pad_type, begin, end, **kw):
+    c = _simple(cmd_id, size=(), **kw)
+    _size(c.info, tuple(begin) + (0,) * (abi.MAX_DIM_ALLOC - len(begin)))
+    c.info.pad.type = pad_type
+    for i, e in enumerate(end):
+        c.info.pad.end[i] = int(e)
+    return c
+
+
+def CMD_PAD_FORWARD(pad_type, begin, end, **kw):
+    """pad_type: abi.CCV_NNC_PAD_ZERO or abi.CCV_NNC_PAD_REPLICATE; begin / end: per-axis widths (cmd/pad)"""
+    return _pad(abi.CCV_NNC_PAD_FORWARD, pad_type, begin, end, **kw)
+
+
+def CMD_PAD_BACKWARD(pad_type, begin, end, **kw):
+    return _pad(abi.CCV_NNC_PAD_BACKWARD, pad_type, begin, end, **kw)
+
+
 def CMD_MASKED_FILL_FORWARD(eq, fill, **kw):
     c = _simple(abi.CCV_NNC_MASKED_FILL_FORWARD, **kw)
     c.info.blas.a[0], c.info.blas.a[1] = eq, fill

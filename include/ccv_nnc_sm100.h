@@ -279,6 +279,10 @@ typedef struct {
 			int entirety;
 		} dropout;
 		struct {
+			int type; /* CCV_NNC_PAD_ZERO / _REPLICATE; size.dim holds the leading pad of each axis */
+			int end[CCV_NNC_MAX_DIM_ALLOC];
+		} pad;
+		struct {
 			float scale;
 			int is_causal;
 			int flags;
@@ -460,6 +464,25 @@ enum {
 	CCV_NNC_MSE_BACKWARD = 0x6904a9a3,
 	CCV_NNC_SMOOTH_L1_FORWARD = 0x4e428e,
 	CCV_NNC_SMOOTH_L1_BACKWARD = 0x4e428f,
+	/* cmd/pad, cmd/compare, cmd/reduce (ARGMAX / ARGMIN), cmd/isnan */
+	CCV_NNC_PAD_FORWARD = 0xd8aaca60,
+	CCV_NNC_PAD_BACKWARD = 0xd8aaca61,
+	CCV_NNC_MIN_FORWARD = 0x972fbd26,
+	CCV_NNC_MIN_BACKWARD = 0x972fbd27,
+	CCV_NNC_MAX_FORWARD = 0xdf6f014c,
+	CCV_NNC_MAX_BACKWARD = 0xdf6f014d,
+	CCV_NNC_ARGMAX_FORWARD = 0x68af2804,
+	CCV_NNC_ARGMAX_BACKWARD = 0x68af2805,
+	CCV_NNC_ARGMIN_FORWARD = 0xeb8747f2,
+	CCV_NNC_ARGMIN_BACKWARD = 0xeb8747f3,
+	CCV_NNC_REDUCE_ISNAN_FORWARD = 0xee0a4ade,
+	CCV_NNC_REDUCE_ISNAN_BACKWARD = 0xee0a4adf,
+};
+
+/* lib/nnc/ccv_nnc.h:97-100 (cmd.info.pad.type) */
+enum {
+	CCV_NNC_PAD_ZERO = 0,
+	CCV_NNC_PAD_REPLICATE = 1,
 };
 
 /* lib/nnc/ccv_nnc.h:81-84 (cmd.info.mse.reduce_op) */
@@ -529,7 +552,9 @@ enum {
 	X(CCV_NNC_RANDOM_UNIFORM_FORWARD) X(CCV_NNC_RANDOM_UNIFORM_BACKWARD) X(CCV_NNC_RANDOM_NORMAL_FORWARD) X(CCV_NNC_RANDOM_NORMAL_BACKWARD) X(CCV_NNC_ADAM_FORWARD) X(CCV_NNC_ADAM_BACKWARD) X(CCV_NNC_DROPOUT_FORWARD) X(CCV_NNC_DROPOUT_BACKWARD) \
 	X(CCV_NNC_CMUL_FORWARD) X(CCV_NNC_CMUL_BACKWARD) \
 	X(CCV_NNC_BINARY_CROSSENTROPY_FORWARD) X(CCV_NNC_BINARY_CROSSENTROPY_BACKWARD) X(CCV_NNC_SIGMOID_BINARY_CROSSENTROPY_FORWARD) X(CCV_NNC_SIGMOID_BINARY_CROSSENTROPY_BACKWARD) \
-	X(CCV_NNC_MSE_FORWARD) X(CCV_NNC_MSE_BACKWARD) X(CCV_NNC_SMOOTH_L1_FORWARD) X(CCV_NNC_SMOOTH_L1_BACKWARD)
+	X(CCV_NNC_MSE_FORWARD) X(CCV_NNC_MSE_BACKWARD) X(CCV_NNC_SMOOTH_L1_FORWARD) X(CCV_NNC_SMOOTH_L1_BACKWARD) \
+	X(CCV_NNC_PAD_FORWARD) X(CCV_NNC_PAD_BACKWARD) X(CCV_NNC_MIN_FORWARD) X(CCV_NNC_MIN_BACKWARD) X(CCV_NNC_MAX_FORWARD) X(CCV_NNC_MAX_BACKWARD) \
+	X(CCV_NNC_ARGMAX_FORWARD) X(CCV_NNC_ARGMAX_BACKWARD) X(CCV_NNC_ARGMIN_FORWARD) X(CCV_NNC_ARGMIN_BACKWARD) X(CCV_NNC_REDUCE_ISNAN_FORWARD) X(CCV_NNC_REDUCE_ISNAN_BACKWARD)
 
 #define CCV_SM100_DECLARE_REGISTER(cmd) void _register_command_ ## cmd ## _backend_CCV_NNC_BACKEND_GPU_SM100(ccv_nnc_cmd_backend_registry_t* const registry);
 CCV_NNC_SM100_COMMANDS(CCV_SM100_DECLARE_REGISTER)
