@@ -39,6 +39,7 @@ CMD_IDS = dict(
     MASKED_FILL=0x7f992d84, DROPOUT=0x7f2dc3e4, ADAM=0xe30099dc, RANDOM_UNIFORM=0xa0cd1d5e, RANDOM_NORMAL=0x7062c8b4,
     CMUL=0xead486e6, BINARY_CROSSENTROPY=0xcd2107ec, SIGMOID_BINARY_CROSSENTROPY=0xd9e0e4a, MSE=0x6904a9a2, SMOOTH_L1=0x4e428e,
     PAD=0xd8aaca60, MIN=0x972fbd26, MAX=0xdf6f014c, ARGMAX=0x68af2804, ARGMIN=0xeb8747f2, REDUCE_ISNAN=0xee0a4ade,
+    ROI_ALIGN=0xfef55168, NMS=0xdba26106,
 )
 for _k, _v in CMD_IDS.items():
     globals()["CCV_NNC_%s_FORWARD" % _k] = _v
@@ -151,6 +152,10 @@ class _Dropout(C.Structure):
     _fields_ = [("p", C.c_float), ("entirety", C.c_int)]
 
 
+class _Nms(C.Structure):
+    _fields_ = [("iou_threshold", C.c_float)]
+
+
 class _Pad(C.Structure):
     _fields_ = [("type", C.c_int), ("end", C.c_int * MAX_DIM_ALLOC)]
 
@@ -159,7 +164,7 @@ class _CmdUnion(C.Union):
     _fields_ = [("convolution", _Convolution), ("convolution_transpose", _ConvolutionTranspose), ("pool", _Pool), ("bnorm", _Bnorm), ("lnorm", _Lnorm), ("gnorm", _Gnorm), ("rmsnorm", _Rmsnorm),
                 ("sgd", _Sgd), ("adam", _Adam), ("gelu", _Gelu), ("blas", _Blas), ("label_smoothing", _LabelSmoothing), ("reduce", _Reduce), ("transpose", _Transpose),
                 ("upsample", _Upsample), ("clamp", _Clamp), ("leaky_relu", _LeakyRelu), ("dropout", _Dropout), ("scaled_dot_product_attention", _Sdpa),
-                ("binary_crossentropy", _BinaryCrossentropy), ("smooth_l1", _SmoothL1), ("mse", _Mse), ("pad", _Pad), ("userdata", C.c_void_p)]
+                ("binary_crossentropy", _BinaryCrossentropy), ("smooth_l1", _SmoothL1), ("mse", _Mse), ("nms", _Nms), ("pad", _Pad), ("userdata", C.c_void_p)]
 
 
 class CmdParam(C.Structure):

@@ -127,6 +127,7 @@ void ccv_nnc_init(void)
 		// what the generated _ccv_nnc_cmd_init() does for every (command, backend) pair (integration/ccv_nnc_cmd_sm100_init.inc)
 #define CCV_SM100_CALL_REGISTER(cmd) _register_command_ ## cmd ## _backend_CCV_NNC_BACKEND_GPU_SM100(&init_map[_ccv_nnc_cmd_ph((uint32_t)cmd)].backends[_ccv_nnc_cmd_backend_ph(CCV_NNC_BACKEND_GPU_SM100)]);
 		CCV_NNC_SM100_COMMANDS(CCV_SM100_CALL_REGISTER)
+		CCV_NNC_SM100_DETECTION_COMMANDS(CCV_SM100_CALL_REGISTER)
 #undef CCV_SM100_CALL_REGISTER
 	});
 }

@@ -819,6 +819,28 @@ def CMD_PAD_BACKWARD(pad_type, begin, end, **kw):
     return _pad(abi.CCV_NNC_PAD_BACKWARD, pad_type, begin, end, **kw)
 
 
+def CMD_ROI_ALIGN_FORWARD(rows, cols, **kw):
+    """c[n, rows, cols, C] = bilinear ROI align of a[n % a_n] over ROI b[n % b_n] = (x, y, w, h), normalised (cmd/roi)"""
+    return _simple(abi.CCV_NNC_ROI_ALIGN_FORWARD, size=(rows, cols, 1), **kw)
+
+
+def CMD_ROI_ALIGN_BACKWARD(rows, cols, **kw):
+    return _simple(abi.CCV_NNC_ROI_ALIGN_BACKWARD, size=(rows, cols, 1), **kw)
+
+
+def CMD_NMS_FORWARD(iou, **kw):
+    """rows (score, x, y, w, h) -> kept rows first in score order (b) and their input indices, -1 after the last (c) (cmd/nms)"""
+    c = _simple(abi.CCV_NNC_NMS_FORWARD, size=(), **kw)
+    c.info.nms.iou_threshold = iou
+    return c
+
+
+def CMD_NMS_BACKWARD(iou, **kw):
+    c = _simple(abi.CCV_NNC_NMS_BACKWARD, size=(), **kw)
+    c.info.nms.iou_threshold = iou
+    return c
+
+
 def CMD_MASKED_FILL_FORWARD(eq, fill, **kw):
     c = _simple(abi.CCV_NNC_MASKED_FILL_FORWARD, **kw)
     c.info.blas.a[0], c.info.blas.a[1] = eq, fill

@@ -279,6 +279,9 @@ typedef struct {
 			int entirety;
 		} dropout;
 		struct {
+			float iou_threshold; /* NMS: a lower-scored box is suppressed when its IoU with a kept one is >= this */
+		} nms;
+		struct {
 			int type; /* CCV_NNC_PAD_ZERO / _REPLICATE; size.dim holds the leading pad of each axis */
 			int end[CCV_NNC_MAX_DIM_ALLOC];
 		} pad;
@@ -477,6 +480,11 @@ enum {
 	CCV_NNC_ARGMIN_BACKWARD = 0xeb8747f3,
 	CCV_NNC_REDUCE_ISNAN_FORWARD = 0xee0a4ade,
 	CCV_NNC_REDUCE_ISNAN_BACKWARD = 0xee0a4adf,
+	/* cmd/roi, cmd/nms */
+	CCV_NNC_ROI_ALIGN_FORWARD = 0xfef55168,
+	CCV_NNC_ROI_ALIGN_BACKWARD = 0xfef55169,
+	CCV_NNC_NMS_FORWARD = 0xdba26106,
+	CCV_NNC_NMS_BACKWARD = 0xdba26107,
 };
 
 /* lib/nnc/ccv_nnc.h:97-100 (cmd.info.pad.type) */
@@ -558,6 +566,12 @@ enum {
 
 #define CCV_SM100_DECLARE_REGISTER(cmd) void _register_command_ ## cmd ## _backend_CCV_NNC_BACKEND_GPU_SM100(ccv_nnc_cmd_backend_registry_t* const registry);
 CCV_NNC_SM100_COMMANDS(CCV_SM100_DECLARE_REGISTER)
+
+/* Families registered after the first 118 commands are listed by family, one list each; every list is expanded wherever
+ * CCV_NNC_SM100_COMMANDS is (the declarations here, ccv_nnc_init, tools/gen_backend_ph.py). */
+#define CCV_NNC_SM100_DETECTION_COMMANDS(X) \
+	X(CCV_NNC_ROI_ALIGN_FORWARD) X(CCV_NNC_ROI_ALIGN_BACKWARD) X(CCV_NNC_NMS_FORWARD) X(CCV_NNC_NMS_BACKWARD)
+CCV_NNC_SM100_DETECTION_COMMANDS(CCV_SM100_DECLARE_REGISTER)
 #undef CCV_SM100_DECLARE_REGISTER
 
 /* What the backend needs back from its host (ccv's own when linked into libccv: lib/nnc/gpu/ccv_nnc_compat.h:95-97,

@@ -186,7 +186,9 @@ def main():
     open(os.path.join(out, "ccv_nnc_cmd_backend.inc"), "w").write(
         "/* regenerated by tools/gen_backend_ph.py: the two backend-side pieces of lib/nnc/cmd/ccv_nnc_cmd.inc (lines 142-190) for 8 backends */\n" + init_map + "\n" + backend_ph)
     header = open(os.path.join(ROOT, "include", "ccv_nnc_sm100.h")).read()
+    # the first list, then the per-family lists that follow the declaration macro
     sm100_cmds = re.findall(r"X\((CCV_NNC_[A-Z0-9_]+)\)", header[header.index("#define CCV_NNC_SM100_COMMANDS(X)"):header.index("#define CCV_SM100_DECLARE_REGISTER")])
+    sm100_cmds += re.findall(r"X\((CCV_NNC_[A-Z0-9_]+)\)", header[header.index("#define CCV_NNC_SM100_DETECTION_COMMANDS(X)"):header.index("CCV_NNC_SM100_DETECTION_COMMANDS(CCV_SM100_DECLARE_REGISTER)")])
     ids = dict(cmds)
     lines = ["/* regenerated by tools/gen_backend_ph.py: what build-cmd.rb adds to ccv_nnc_cmd.inc for every (command, GPU_SM100) pair */"]
     for c in sm100_cmds:
