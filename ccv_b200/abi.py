@@ -39,7 +39,7 @@ CMD_IDS = dict(
     MASKED_FILL=0x7f992d84, DROPOUT=0x7f2dc3e4, ADAM=0xe30099dc, RANDOM_UNIFORM=0xa0cd1d5e, RANDOM_NORMAL=0x7062c8b4,
     CMUL=0xead486e6, BINARY_CROSSENTROPY=0xcd2107ec, SIGMOID_BINARY_CROSSENTROPY=0xd9e0e4a, MSE=0x6904a9a2, SMOOTH_L1=0x4e428e,
     PAD=0xd8aaca60, MIN=0x972fbd26, MAX=0xdf6f014c, ARGMAX=0x68af2804, ARGMIN=0xeb8747f2, REDUCE_ISNAN=0xee0a4ade,
-    ROI_ALIGN=0xfef55168, NMS=0xdba26106,
+    ROI_ALIGN=0xfef55168, NMS=0xdba26106, LAMB=0x450edb1a, RMSPROP=0x9c886b1c,
 )
 for _k, _v in CMD_IDS.items():
     globals()["CCV_NNC_%s_FORWARD" % _k] = _v
@@ -98,6 +98,14 @@ class _Sgd(C.Structure):
 
 class _Adam(C.Structure):
     _fields_ = [("step", C.c_int), ("rate", C.c_float), ("scale", C.c_float), ("beta1", C.c_float), ("beta2", C.c_float), ("decay", C.c_float), ("epsilon", C.c_float), ("amsgrad", C.c_int)]
+
+
+class _Lamb(C.Structure):
+    _fields_ = [("step", C.c_int), ("rate", C.c_float), ("scale", C.c_float), ("beta1", C.c_float), ("beta2", C.c_float), ("decay", C.c_float), ("epsilon", C.c_float)]
+
+
+class _Rmsprop(C.Structure):
+    _fields_ = [("rate", C.c_float), ("scale", C.c_float), ("decay", C.c_float), ("alpha", C.c_float), ("momentum", C.c_float), ("epsilon", C.c_float)]
 
 
 class _Gelu(C.Structure):
@@ -162,7 +170,7 @@ class _Pad(C.Structure):
 
 class _CmdUnion(C.Union):
     _fields_ = [("convolution", _Convolution), ("convolution_transpose", _ConvolutionTranspose), ("pool", _Pool), ("bnorm", _Bnorm), ("lnorm", _Lnorm), ("gnorm", _Gnorm), ("rmsnorm", _Rmsnorm),
-                ("sgd", _Sgd), ("adam", _Adam), ("gelu", _Gelu), ("blas", _Blas), ("label_smoothing", _LabelSmoothing), ("reduce", _Reduce), ("transpose", _Transpose),
+                ("sgd", _Sgd), ("adam", _Adam), ("lamb", _Lamb), ("rmsprop", _Rmsprop), ("gelu", _Gelu), ("blas", _Blas), ("label_smoothing", _LabelSmoothing), ("reduce", _Reduce), ("transpose", _Transpose),
                 ("upsample", _Upsample), ("clamp", _Clamp), ("leaky_relu", _LeakyRelu), ("dropout", _Dropout), ("scaled_dot_product_attention", _Sdpa),
                 ("binary_crossentropy", _BinaryCrossentropy), ("smooth_l1", _SmoothL1), ("mse", _Mse), ("nms", _Nms), ("pad", _Pad), ("userdata", C.c_void_p)]
 

@@ -128,6 +128,7 @@ void ccv_nnc_init(void)
 #define CCV_SM100_CALL_REGISTER(cmd) _register_command_ ## cmd ## _backend_CCV_NNC_BACKEND_GPU_SM100(&init_map[_ccv_nnc_cmd_ph((uint32_t)cmd)].backends[_ccv_nnc_cmd_backend_ph(CCV_NNC_BACKEND_GPU_SM100)]);
 		CCV_NNC_SM100_COMMANDS(CCV_SM100_CALL_REGISTER)
 		CCV_NNC_SM100_DETECTION_COMMANDS(CCV_SM100_CALL_REGISTER)
+		CCV_NNC_SM100_OPTIMIZER_COMMANDS(CCV_SM100_CALL_REGISTER)
 #undef CCV_SM100_CALL_REGISTER
 	});
 }
@@ -815,6 +816,8 @@ int ccv_nnc_sm100_fused_relu_bn_back(const ccv_nnc_cmd_t, const ccv_nnc_hint_t, 
 int ccv_nnc_sm100_fused_add_relu_forw(const ccv_nnc_cmd_t, const ccv_nnc_hint_t, const int, ccv_nnc_tensor_t* const*, const int, ccv_nnc_tensor_t* const*, const int, ccv_nnc_stream_context_t*);
 int ccv_nnc_sm100_fused_add_relu_back(const ccv_nnc_cmd_t, const ccv_nnc_hint_t, const int, ccv_nnc_tensor_t* const*, const int, ccv_nnc_tensor_t* const*, const int, ccv_nnc_stream_context_t*);
 int ccv_nnc_sm100_fused_sgd_multi(const ccv_nnc_cmd_t, const ccv_nnc_hint_t, const int, ccv_nnc_tensor_t* const*, const int, ccv_nnc_tensor_t* const*, const int, ccv_nnc_stream_context_t*);
+int ccv_nnc_sm100_fused_lamb_multi(const ccv_nnc_cmd_t, const ccv_nnc_hint_t, const int, ccv_nnc_tensor_t* const*, const int, ccv_nnc_tensor_t* const*, const int, ccv_nnc_stream_context_t*);
+int ccv_nnc_sm100_fused_rmsprop_multi(const ccv_nnc_cmd_t, const ccv_nnc_hint_t, const int, ccv_nnc_tensor_t* const*, const int, ccv_nnc_tensor_t* const*, const int, ccv_nnc_stream_context_t*);
 int ccv_nnc_sm100_fused_conv_stats_forw(const ccv_nnc_cmd_t, const ccv_nnc_hint_t, const int, ccv_nnc_tensor_t* const*, const int, ccv_nnc_tensor_t* const*, const int, ccv_nnc_stream_context_t*);
 int ccv_nnc_sm100_fused_bn_forw(const ccv_nnc_cmd_t, const ccv_nnc_hint_t, const int, ccv_nnc_tensor_t* const*, const int, ccv_nnc_tensor_t* const*, const int, ccv_nnc_stream_context_t*);
 int ccv_nnc_sm100_fused_bn_back(const ccv_nnc_cmd_t, const ccv_nnc_hint_t, const int, ccv_nnc_tensor_t* const*, const int, ccv_nnc_tensor_t* const*, const int, ccv_nnc_stream_context_t*);
@@ -966,7 +969,8 @@ int ccv_nnc_sm100_graph_run(ccv_nnc_sm100_graph_t* const graph, const int begin,
 //  (c) EWSUM(a, b -> y) ; RELU_FORWARD in place on y                          -> y = relu(a + b)
 //  (d) EWSUM(a, b -> a) ; RELU_BACKWARD in place on a (mask y)                -> a = y > 0 ? a + b : 0
 //  (e) a run of SGD_FORWARD nodes with identical parameters (the per-parameter updates of a model; none of them reads
-//      what another one writes) -> one multi-tensor command; counts as (run length - 1) fused nodes
+//      what another one writes) -> one multi-tensor command; counts as (run length - 1) fused nodes.  Runs of LAMB_FORWARD and
+//      of RMSPROP_FORWARD nodes are rewritten the same way (each LAMB tensor keeps its own trust ratio).
 int ccv_nnc_sm100_graph_fuse(ccv_nnc_sm100_graph_t* const graph)
 {
 	std::vector<ccv_nnc_sm100_graph_node_t>& nodes = graph->nodes;
@@ -979,8 +983,22 @@ int ccv_nnc_sm100_graph_fuse(ccv_nnc_sm100_graph_t* const graph)
 	for (size_t i = 0; i < n; i++)
 	{
 		ccv_nnc_sm100_graph_node_t& a = nodes[i];
-		// (e)
-		if (is_gpu_sm100(a) && a.cmd.cmd == CCV_NNC_SGD_FORWARD && a.inputs.size() == 3 && a.outputs.size() == 2)
+		// (e): the optimizer of the run, its operand counts, the size of its cmd.info arm and the multi-tensor exec
+		struct optimizer_run_t {
+			uint32_t cmd;
+			size_t inputs, outputs, arm;
+			ccv_nnc_cmd_exec_f exec;
+		};
+		static const optimizer_run_t optimizer_runs[] = {
+			{ CCV_NNC_SGD_FORWARD, 3, 2, sizeof(a.cmd.info.sgd), ccv_nnc_sm100_fused_sgd_multi },
+			{ CCV_NNC_LAMB_FORWARD, 4, 3, sizeof(a.cmd.info.lamb), ccv_nnc_sm100_fused_lamb_multi },
+			{ CCV_NNC_RMSPROP_FORWARD, 4, 3, sizeof(a.cmd.info.rmsprop), ccv_nnc_sm100_fused_rmsprop_multi },
+		};
+		const optimizer_run_t* run = 0;
+		for (const optimizer_run_t& r : optimizer_runs)
+			if (is_gpu_sm100(a) && a.cmd.cmd == r.cmd && a.inputs.size() == r.inputs && a.outputs.size() == r.outputs)
+				run = &r;
+		if (run)
 		{
 			size_t j = i + 1;
 			auto independent = [&](const ccv_nnc_sm100_graph_node_t& x, size_t from, size_t to) {
@@ -994,15 +1012,21 @@ int ccv_nnc_sm100_graph_fuse(ccv_nnc_sm100_graph_t* const graph)
 			};
 			// the maximal run of mutually independent SGD nodes: inside it the order is free, so nodes are grouped by their
 			// hyper-parameters (weights with decay, biases / norm parameters without) even when the groups interleave
-			while (j < n && is_gpu_sm100(nodes[j]) && nodes[j].cmd.cmd == CCV_NNC_SGD_FORWARD && nodes[j].inputs.size() == 3 && nodes[j].outputs.size() == 2 && independent(nodes[j], i, j))
+			while (j < n && is_gpu_sm100(nodes[j]) && nodes[j].cmd.cmd == run->cmd && nodes[j].inputs.size() == run->inputs && nodes[j].outputs.size() == run->outputs && independent(nodes[j], i, j))
 				j++;
-			// the multi-tensor kernel takes fp32 parameters and momenta only; a node with 16-bit ones runs on its own (through the
+			// the SGD multi-tensor kernel takes fp32 parameters and momenta only; a node with 16-bit ones runs on its own (through the
 			// functional form of exec_sgd_any)
 			auto fp32_state = [](const ccv_nnc_sm100_graph_node_t& x) {
 				for (ccv_nnc_tensor_t* t : { x.inputs[1], x.inputs[2], x.outputs[0], x.outputs[1] })
 					if (!t || CCV_GET_DATA_TYPE(t->info.datatype) != CCV_32F)
 						return false;
 				return true;
+			};
+			// LAMB / RMSPROP take fp32, bf16 or fp16 state, one type per launch
+			auto same_state = [&](const ccv_nnc_sm100_graph_node_t& f, const ccv_nnc_sm100_graph_node_t& x) {
+				if (run->cmd == CCV_NNC_SGD_FORWARD)
+					return fp32_state(f) && fp32_state(x);
+				return f.inputs[1] && x.inputs[1] && f.inputs[1]->info.datatype == x.inputs[1]->info.datatype;
 			};
 			std::vector<char> done(j - i, 0);
 			for (size_t k = i; k < j; k++)
@@ -1011,8 +1035,10 @@ int ccv_nnc_sm100_graph_fuse(ccv_nnc_sm100_graph_t* const graph)
 					continue;
 				ccv_nnc_sm100_graph_node_t f = nodes[k];
 				int members = 1;
-				for (size_t q = k + 1; q < j && fp32_state(f); q++)
-					if (!done[q - i] && fp32_state(nodes[q]) && memcmp(&nodes[q].cmd.info.sgd, &f.cmd.info.sgd, sizeof(f.cmd.info.sgd)) == 0 && nodes[q].flags == f.flags && nodes[q].cmd.algorithm == f.cmd.algorithm &&
+				// every arm of the cmd.info union starts at the same address, so the sgd arm's address with the run's arm size compares
+				// that arm
+				for (size_t q = k + 1; q < j; q++)
+					if (!done[q - i] && same_state(f, nodes[q]) && memcmp(&nodes[q].cmd.info.sgd, &f.cmd.info.sgd, run->arm) == 0 && nodes[q].flags == f.flags && nodes[q].cmd.algorithm == f.cmd.algorithm &&
 					nodes[q].inputs[0] && f.inputs[0] && nodes[q].inputs[0]->info.datatype == f.inputs[0]->info.datatype) // one gradient type per launch (16-bit and fp32 gradients of a mixed-precision model go separately)
 					{
 						f.inputs.insert(f.inputs.end(), nodes[q].inputs.begin(), nodes[q].inputs.end());
@@ -1022,7 +1048,7 @@ int ccv_nnc_sm100_graph_fuse(ccv_nnc_sm100_graph_t* const graph)
 					}
 				if (members > 1)
 				{
-					f.fused = ccv_nnc_sm100_fused_sgd_multi;
+					f.fused = run->exec;
 					fused += members - 1;
 				}
 				out.push_back(f);
@@ -1156,7 +1182,8 @@ int ccv_nnc_sm100_graph_node(const ccv_nnc_sm100_graph_t* const graph, const int
 		return -1;
 	const ccv_nnc_sm100_graph_node_t& n = graph->nodes[i];
 	*cmd = n.cmd.cmd;
-	*fused_kind = n.fused == ccv_nnc_sm100_fused_bn_relu_forw ? 1 : n.fused == ccv_nnc_sm100_fused_relu_bn_back ? 2 : n.fused == ccv_nnc_sm100_fused_add_relu_forw ? 3 : n.fused == ccv_nnc_sm100_fused_add_relu_back ? 4 : n.fused == ccv_nnc_sm100_fused_sgd_multi ? 5 : n.fused == ccv_nnc_sm100_fused_conv_stats_forw ? 6 : n.fused == ccv_nnc_sm100_fused_bn_forw ? 7 : n.fused == ccv_nnc_sm100_fused_bn_back ? 8 : 0;
+	*fused_kind = n.fused == ccv_nnc_sm100_fused_bn_relu_forw ? 1 : n.fused == ccv_nnc_sm100_fused_relu_bn_back ? 2 : n.fused == ccv_nnc_sm100_fused_add_relu_forw ? 3 : n.fused == ccv_nnc_sm100_fused_add_relu_back ? 4 : n.fused == ccv_nnc_sm100_fused_sgd_multi ? 5 : n.fused == ccv_nnc_sm100_fused_conv_stats_forw ? 6 : n.fused == ccv_nnc_sm100_fused_bn_forw ? 7 : n.fused == ccv_nnc_sm100_fused_bn_back ? 8 :
+		n.fused == ccv_nnc_sm100_fused_lamb_multi ? 9 : n.fused == ccv_nnc_sm100_fused_rmsprop_multi ? 10 : 0;
 	*input_size = (int)n.inputs.size();
 	*output_size = (int)n.outputs.size();
 	return 0;

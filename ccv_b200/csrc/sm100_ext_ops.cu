@@ -367,11 +367,6 @@ int exec_adam_any(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int 
 		return exec_via_f32_rt(exec_adam_f32<L2>, cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
 	return exec_adam_f32<L2>(cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
 }
-int exec_no_backward(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
-{
-	return CCV_NNC_EXEC_INVALID; // an optimizer has no backward (adam/ccv_nnc_adamw_cpu_ref.c: _ccv_nnc_adamw_back)
-}
-
 void fill(ccv_nnc_cmd_backend_registry_t* const registry, const int datatypes, const ccv_nnc_cmd_exec_f exec)
 {
 	registry->tensor_formats = CCV_TENSOR_FORMAT_NCHW | CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_CHWN;
@@ -384,6 +379,14 @@ void fill(ccv_nnc_cmd_backend_registry_t* const registry, const int datatypes, c
 }
 
 } // namespace
+
+namespace sm100 {
+// an optimizer has no backward (adam/ccv_nnc_adamw_cpu_ref.c: _ccv_nnc_adamw_back); also LAMB's and RMSPROP's (sm100_optim.cu)
+int exec_no_backward(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
+{
+	return CCV_NNC_EXEC_INVALID;
+}
+}
 
 #define REGISTER_SM100(cmd) extern "C" void _register_command_ ## cmd ## _backend_CCV_NNC_BACKEND_GPU_SM100(ccv_nnc_cmd_backend_registry_t* const registry)
 REGISTER_SM100(CCV_NNC_GELU_FORWARD) { fill(registry, CCV_32F | CCV_16F | CCV_16BF, exec_act<0, 0>); }

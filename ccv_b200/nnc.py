@@ -871,6 +871,34 @@ def CMD_ADAM_FORWARD(step, rate, beta1, beta2, decay, epsilon, amsgrad=0, scale=
     return c
 
 
+def CMD_LAMB_FORWARD(step, rate, beta1, beta2, decay, epsilon, scale=1.0, **kw):
+    """LAMB (cmd/lamb): inputs (g, a, m, v) -> outputs (b, n, u); b = a - rate * trust * update, trust = |a| / |update| per tensor"""
+    c = _simple(abi.CCV_NNC_LAMB_FORWARD, **kw)
+    l = c.info.lamb
+    l.step, l.rate, l.scale, l.beta1, l.beta2, l.decay, l.epsilon = step, rate, scale, beta1, beta2, decay, epsilon
+    return c
+
+
+def CMD_LAMB_BACKWARD(step, rate, beta1, beta2, decay, epsilon, scale=1.0, **kw):
+    c = CMD_LAMB_FORWARD(step, rate, beta1, beta2, decay, epsilon, scale, **kw)
+    c.cmd = abi.CCV_NNC_LAMB_BACKWARD
+    return c
+
+
+def CMD_RMSPROP_FORWARD(rate, decay, alpha, momentum, epsilon, scale=1.0, **kw):
+    """RMSPROP (cmd/rmsprop): inputs (g, a, m, v) -> outputs (b, n, u)"""
+    c = _simple(abi.CCV_NNC_RMSPROP_FORWARD, **kw)
+    r = c.info.rmsprop
+    r.rate, r.scale, r.decay, r.alpha, r.momentum, r.epsilon = rate, scale, decay, alpha, momentum, epsilon
+    return c
+
+
+def CMD_RMSPROP_BACKWARD(rate, decay, alpha, momentum, epsilon, scale=1.0, **kw):
+    c = CMD_RMSPROP_FORWARD(rate, decay, alpha, momentum, epsilon, scale, **kw)
+    c.cmd = abi.CCV_NNC_RMSPROP_BACKWARD
+    return c
+
+
 def CMD_DROPOUT_FORWARD(p, entirety=0, **kw):
     c = _simple(abi.CCV_NNC_DROPOUT_FORWARD, **kw)
     c.info.dropout.p, c.info.dropout.entirety = p, entirety

@@ -233,6 +233,23 @@ typedef struct {
 			int amsgrad;
 		} adam;
 		struct {
+			int step;
+			float rate;
+			float scale;
+			float beta1;
+			float beta2;
+			float decay; /* added to the update (not an L2 term of the gradient) */
+			float epsilon;
+		} lamb;
+		struct {
+			float rate;
+			float scale;
+			float decay; /* L2 term of the gradient */
+			float alpha;
+			float momentum;
+			float epsilon;
+		} rmsprop;
+		struct {
 			int tanh;
 		} gelu;
 		struct {
@@ -485,6 +502,11 @@ enum {
 	CCV_NNC_ROI_ALIGN_BACKWARD = 0xfef55169,
 	CCV_NNC_NMS_FORWARD = 0xdba26106,
 	CCV_NNC_NMS_BACKWARD = 0xdba26107,
+	/* cmd/lamb, cmd/rmsprop */
+	CCV_NNC_LAMB_FORWARD = 0x450edb1a,
+	CCV_NNC_LAMB_BACKWARD = 0x450edb1b,
+	CCV_NNC_RMSPROP_FORWARD = 0x9c886b1c,
+	CCV_NNC_RMSPROP_BACKWARD = 0x9c886b1d,
 };
 
 /* lib/nnc/ccv_nnc.h:97-100 (cmd.info.pad.type) */
@@ -572,6 +594,9 @@ CCV_NNC_SM100_COMMANDS(CCV_SM100_DECLARE_REGISTER)
 #define CCV_NNC_SM100_DETECTION_COMMANDS(X) \
 	X(CCV_NNC_ROI_ALIGN_FORWARD) X(CCV_NNC_ROI_ALIGN_BACKWARD) X(CCV_NNC_NMS_FORWARD) X(CCV_NNC_NMS_BACKWARD)
 CCV_NNC_SM100_DETECTION_COMMANDS(CCV_SM100_DECLARE_REGISTER)
+#define CCV_NNC_SM100_OPTIMIZER_COMMANDS(X) \
+	X(CCV_NNC_LAMB_FORWARD) X(CCV_NNC_LAMB_BACKWARD) X(CCV_NNC_RMSPROP_FORWARD) X(CCV_NNC_RMSPROP_BACKWARD)
+CCV_NNC_SM100_OPTIMIZER_COMMANDS(CCV_SM100_DECLARE_REGISTER)
 #undef CCV_SM100_DECLARE_REGISTER
 
 /* What the backend needs back from its host (ccv's own when linked into libccv: lib/nnc/gpu/ccv_nnc_compat.h:95-97,
@@ -687,14 +712,16 @@ int ccv_nnc_sm100_graph_size(const ccv_nnc_sm100_graph_t* const graph);
 int ccv_nnc_sm100_graph_exec_set_side_stream(ccv_nnc_sm100_graph_t* const graph, const int i, const int side);
 /* runs nodes [begin, end) in order on the stream; returns the first non-zero exec status */
 int ccv_nnc_sm100_graph_run(ccv_nnc_sm100_graph_t* const graph, const int begin, const int end, ccv_nnc_stream_context_t* const stream_context);
-/* peephole fusion of adjacent nodes (BN+ReLU forward, ReLU+BN backward, residual add + ReLU forward / backward); node
+/* peephole fusion of adjacent nodes (BN+ReLU forward, ReLU+BN backward, residual add + ReLU forward / backward, runs of SGD / LAMB /
+ * RMSPROP updates); node
  * indices change, so call it before choosing capture ranges. Returns the number of pairs fused. */
 int ccv_nnc_sm100_graph_fuse(ccv_nnc_sm100_graph_t* const graph);
 /* introspection and per-node device timing (CUDA events, best of reps) of the (possibly fused) node list;
  * fused_kind: 0 plain command, 1 bn+relu forward, 2 relu+bn backward, 3 add+relu forward, 4 add+relu backward,
  * 5 a run of SGD commands as one multi-tensor launch, 6 convolution forward that also produces the batch-norm statistics of
  * its output (extra output: the statistics tensor), 7 batch-norm forward consuming them (extra input), 8 batch-norm backward
- * that also writes the bias gradient of the convolution in front of it (extra output; kind 2 may carry it too) */
+ * that also writes the bias gradient of the convolution in front of it (extra output; kind 2 may carry it too), 9 a run of LAMB
+ * commands as one multi-tensor command (each tensor keeps its own trust ratio), 10 a run of RMSPROP commands as one multi-tensor command */
 int ccv_nnc_sm100_graph_node(const ccv_nnc_sm100_graph_t* const graph, const int i, uint32_t* const cmd, int* const fused_kind, int* const input_size, int* const output_size);
 void* ccv_nnc_sm100_graph_node_tensor(const ccv_nnc_sm100_graph_t* const graph, const int i, const int is_output, const int k);
 int ccv_nnc_sm100_graph_profile(ccv_nnc_sm100_graph_t* const graph, ccv_nnc_stream_context_t* const stream_context, const int reps, float* const ms);
