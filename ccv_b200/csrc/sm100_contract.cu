@@ -307,9 +307,9 @@ void conv_stats_request(float* part, int max_rows, int* rows_out)
 template <int AMODE, int BMODE, int BN, int X3 = 0, int K16 = 0, int OUT16 = 0>
 static int launch_umma(cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB, const UmmaGemmParams& p)
 {
-	constexpr bool XF = GemmXform<AMODE, BMODE, K16, X3>::ANY;
-	constexpr int STAGES = GemmStages<BN, XF, X3>::value;
-	using S = UmmaSmem<BN, STAGES, XF, X3>;
+	constexpr bool XF = GemmXform<AMODE, BMODE, K16, X3>::ANY, ARS = GemmXform<AMODE, BMODE, K16, X3>::A_RS;
+	constexpr int STAGES = GemmStages<BN, XF, X3, ARS>::value;
+	using S = UmmaSmem<BN, STAGES, XF, X3, ARS>;
 	auto kern = umma_gemm_kernel<AMODE, BMODE, BN, STAGES, X3, K16, OUT16>;
 	static bool configured[MAX_DEVICES];
 	if (ensure_dynamic_smem(kern, S::TOTAL, configured, "cudaFuncSetAttribute(umma_gemm_kernel)"))
@@ -354,7 +354,7 @@ static int launch_umma(cudaStream_t stream, const CUtensorMap& tmA, const CUtens
 		if ((gx * columns + sms - 1) / sms * ((tiles_m + gx - 1) / gx) <= (ctas + sms - 1) / sms)
 			grid.x = (unsigned)gx;
 	}
-	kern<<<grid, GEMM_THREADS, S::TOTAL, stream>>>(tmA, tmB, q);
+	kern<<<grid, ARS ? GEMM_THREADS_RS : GEMM_THREADS, S::TOTAL, stream>>>(tmA, tmB, q);
 	count_launch();
 	cudaError_t e = cudaGetLastError();
 	if (e != cudaSuccess)
@@ -482,16 +482,21 @@ static int launch_kind16(cudaStream_t stream, const CUtensorMap& tmA, const CUte
 		return bn == 64 ? launch_umma<AMODE, BMODE, 64, 0, 2, 1>(stream, tmA, tmB, p) : launch_umma<AMODE, BMODE, 128, 0, 2, 1>(stream, tmA, tmB, p);
 	return bn == 64 ? launch_umma<AMODE, BMODE, 64, 0, 2, 0>(stream, tmA, tmB, p) : launch_umma<AMODE, BMODE, 128, 0, 2, 0>(stream, tmA, tmB, p);
 }
+// AMODE = OP_MN2D_RS: TF32 reads A into registers (bn 64, 128 or 256); 3xTF32 and the 16-bit kinds read the same operand as OP_MN2D.
 template <int AMODE, int BMODE>
 static int launch_kind(cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB, const UmmaGemmParams& p, int bn, int kind, bool out16)
 {
+	constexpr int A_SS = AMODE == OP_MN2D_RS ? OP_MN2D : AMODE;
 	if (kind == 0)
 	{
 		if (t_x3)
-			return bn == 64 ? launch_umma<AMODE, BMODE, 64, 1>(stream, tmA, tmB, p) : launch_umma<AMODE, BMODE, 128, 1>(stream, tmA, tmB, p);
-		return bn == 64 ? launch_umma<AMODE, BMODE, 64>(stream, tmA, tmB, p) : launch_umma<AMODE, BMODE, 128>(stream, tmA, tmB, p);
+			return bn == 64 ? launch_umma<A_SS, BMODE, 64, 1>(stream, tmA, tmB, p) : launch_umma<A_SS, BMODE, 128, 1>(stream, tmA, tmB, p);
+		if constexpr (AMODE == OP_MN2D_RS)
+			return bn == 64 ? launch_umma<AMODE, BMODE, 64>(stream, tmA, tmB, p) : bn == 128 ? launch_umma<AMODE, BMODE, 128>(stream, tmA, tmB, p) : launch_umma<AMODE, BMODE, 256>(stream, tmA, tmB, p);
+		else
+			return bn == 64 ? launch_umma<AMODE, BMODE, 64>(stream, tmA, tmB, p) : launch_umma<AMODE, BMODE, 128>(stream, tmA, tmB, p);
 	}
-	return launch_kind16<AMODE, BMODE>(stream, tmA, tmB, p, bn, kind, out16);
+	return launch_kind16<A_SS, BMODE>(stream, tmA, tmB, p, bn, kind, out16);
 }
 
 // Launch with the split factor already chosen in p.splits.  One split: straight into `out` (pitch ldo, element kind `kind`).
@@ -831,18 +836,41 @@ int conv_wgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, const void*
 	const size_t dw_bytes = (size_t)g.K * rsc * sizeof(float);
 	const int splits = fit_splits(pick_splits(grid_tiles, k_iters, 16), k_iters, dw_bytes, scratch);
 	// Taps along the columns: dW[K, R*S*C] = grad_b^T [K, NPQ] x im2col(a) [NPQ, R*S*C], column n = tap * C + c, each bk-channel B box
-	// of a tile loading the tap its columns belong to, so one read of a pixel block serves every tap of the tile.  A tile then carries
-	// several taps' work, so this layout is taken when it needs fewer rounds of CTAs over the SMs than the per-tap grid does (the
-	// 32-channel layers, whose per-tap tiles are a 64-column eighth of the work of a 128-column one), and needs C to be a multiple of
-	// bk (else two taps would share a box).  Otherwise one launch with the filter tap on gridDim.z writes the columns [tap * C, +C).
-	const int col_bn = pick_bn((int)rsc);
-	const long long sms = num_sms(), col_ctas = tiles_m * ((rsc + col_bn - 1) / col_bn) * splits;
-	const bool tap_cols = !conv_is_pointwise(g) && g.C % bk == 0 && (col_ctas + sms - 1) / sms < (grid_tiles * splits + sms - 1) / sms;
-	const int cols = tap_cols || conv_is_pointwise(g) ? (int)rsc : g.C;
-	const int bn = tap_cols ? col_bn : grid_bn;
+	// of a tile loading the tap its columns belong to, so one read of a pixel block serves every tap of the tile; needs C to be a
+	// multiple of bk (else two taps would share a box).  Otherwise one launch with the filter tap on gridDim.z writes the columns
+	// [tap * C, +C).  A tile of the column layout carries several taps' work, and the per-tap grid reads grad_b and a once per tap.
+	const bool pointwise = conv_is_pointwise(g), rs = kind == 0 && !x3;
+	const long long sms = num_sms();
+	const auto rounds = [sms](long long ctas) { return (ctas + sms - 1) / sms; };
+	int bn = 0;
+	bool tap_cols = false;
+	if (rs)
+	{
+		// TF32 (A from registers, tiles 64, 128 or 256 wide): the fewest rounds of CTAs over the SMs, then the narrower tile, then the
+		// fewer CTAs, the per-tap grid on a tie.  A wider tile runs nearer the tensor rate (its B transform and B reads serve more
+		// columns per A fragment), so it pays when it saves a round: ResNet-50's layer1 3 x 3 64 -> 64 goes from a per-tap grid of 261 CTAs
+		// (two rounds on 132 SMs) to 3 column tiles of 256 x 29 splits, most later layers from two rounds at 128 to one at 256.
+		long long best = 0, best_ctas = 0;
+		for (int w = 64; w <= 256; w *= 2)
+			for (int c = 0; c < 2; c++)
+			{
+				if (c && (pointwise || g.C % bk))
+					continue;
+				const long long ctas = tiles_m * (c || pointwise ? (rsc + w - 1) / w : (g.C + w - 1) / w * g.R * g.S) * splits;
+				if (!bn || rounds(ctas) < best || (rounds(ctas) == best && w == bn && ctas < best_ctas))
+					bn = w, tap_cols = c, best = rounds(ctas), best_ctas = ctas;
+			}
+	} else {
+		// 3xTF32 and 16-bit: the column layout when it needs fewer rounds than the per-tap grid (the 32-channel layers, whose per-tap
+		// tiles are a 64-column eighth of the work of a 128-column one)
+		const int col_bn = pick_bn((int)rsc);
+		tap_cols = !pointwise && g.C % bk == 0 && rounds(tiles_m * ((rsc + col_bn - 1) / col_bn) * splits) < rounds(grid_tiles * splits);
+		bn = tap_cols ? col_bn : grid_bn;
+	}
+	const int cols = tap_cols || pointwise ? (int)rsc : g.C;
 	CUtensorMap tmA, tmB;
-	// A = grad_b^T: [K, NPQ] read from the [NPQ, K] tensor as an MN-major operand
-	if (!map_2d(&tmA, kind, grad_b, npq, g.K, g.K, bk, true))
+	// A = grad_b^T: [K, NPQ] read from the [NPQ, K] tensor as an MN-major operand (TF32: 128-byte swizzled, see load_a_frags)
+	if (!map_2d(&tmA, kind, grad_b, npq, g.K, g.K, bk, !rs))
 		return 1;
 	UmmaGemmParams p;
 	init_params_kind(p, kind);
@@ -851,12 +879,12 @@ int conv_wgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, const void*
 	p.chunks_per_tap = p.k_iters;
 	p.rowmap.mode = 0, p.rowmap.ld = rsc;
 	p.splits = splits;
-	if (conv_is_pointwise(g))
+	if (pointwise)
 	{
 		// B = a: [NHW, C], also MN-major
 		if (!map_2d(&tmB, kind, a, npq, g.C, g.C, bk, true))
 			return 1;
-		return launch_umma_split<OP_MN2D, OP_MN2D>(stream, tmA, tmB, p, bn, kind, scratch, g.K, (int)rsc, grad_w, rsc, accumulate);
+		return launch_umma_split<OP_MN2D_RS, OP_MN2D>(stream, tmA, tmB, p, bn, kind, scratch, g.K, (int)rsc, grad_w, rsc, accumulate);
 	}
 	if (!map_im2col(&tmB, kind, a, g.N, g.H, g.W, g.C, g.an, g.ah, g.aw, -g.pad_h0, -g.pad_w0, g.pad_h1 - (g.R - 1) * g.dil_h, g.pad_w1 - (g.S - 1) * g.dil_w, g.stride_h, g.stride_w, bk, true))
 		return 1;
@@ -873,7 +901,7 @@ int conv_wgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, const void*
 			p.tap_off_h[t] = (unsigned short)(r * g.dil_h);
 			p.tap_off_w[t] = (unsigned short)(s * g.dil_w);
 		}
-	return launch_umma_split<OP_MN2D, OP_IM2COL>(stream, tmA, tmB, p, bn, kind, scratch, g.K, (int)rsc, grad_w, rsc, accumulate);
+	return launch_umma_split<OP_MN2D_RS, OP_IM2COL>(stream, tmA, tmB, p, bn, kind, scratch, g.K, (int)rsc, grad_w, rsc, accumulate);
 }
 
 // ------------------------------------------------------------------------------------------------ explicit im2col

@@ -14,7 +14,8 @@
 // fp32 operands run as TF32 (kind 0; the TMA unit rounds them to TF32 on the way in) or as 3xTF32 (X3).  wgmma reads TF32 operands
 // K-major only, so the fp32 kernels whose operands arrive MN-major, and the 3xTF32 kernels, pass every stage through a transform
 // step first: the consumers copy the staged tiles into one of two K-major operand slots (transposing MN-major tiles, splitting
-// 3xTF32 operands into hi / lo) and release the stage to the producer before the MMAs run.
+// 3xTF32 operands into hi / lo) and release the stage to the producer before the MMAs run.  The TF32 weight gradient (A =
+// OP_MN2D_RS) transposes only B: its A = grad^T goes from the stage into registers, and its tiles are up to 256 columns wide.
 #pragma once
 #include "sm100_ptx.cuh"
 #include <cuda_bf16.h>
@@ -27,12 +28,17 @@ enum OperandMode {
 	OP_MN2D = 1,   // MN-major 2-D tensor [K, rows]: boxes {BK mn, BK k} per stage
 	OP_IM2COL = 2, // NHWC tensor through im2col-mode TMA.  As A: pixels are rows (K-major, channels = K).
 	               //                                       As B: pixels are K   (MN-major, channels = N).
+	OP_MN2D_RS = 3, // A only, TF32 only: an OP_MN2D tile staged 128-byte swizzled, which the consumers read straight into wgmma A
+	                // fragments (see load_a_frags): it never goes through the transform step
 };
 
 constexpr int UMMA_BLOCK_M = 128;
 constexpr int UMMA_BLOCK_K = 32; // fp32 elements per stage along K = one 128-byte span
 constexpr int UMMA_MAX_TAPS = 64;
 constexpr int GEMM_THREADS = 288;
+// A from registers: a producer warpgroup, so that setmaxnreg can hand the consumers 224 registers (128 accumulators at BN = 256);
+// without it the register file's split over the four schedulers caps 9 warps at 168
+constexpr int GEMM_THREADS_RS = 384;
 
 struct UmmaRowMap {
 	// output row m -> element offset.  mode 0: m * ld.  mode 1: m = (n, i, j) over a (Pc x Qc) grid per image:
@@ -100,17 +106,19 @@ __device__ __forceinline__ float cvt16(const uint16_t x, const int kind)
 // (the reference's fp32 GEMM is CUBLAS_COMPUTE_32F, lib/nnc/gpu/ccv_nnc_compat.cu:786-803) at a third of the tensor rate.
 template <int AMODE, int BMODE, int K16, int X3>
 struct GemmXform {
+	static constexpr bool A_RS = AMODE == OP_MN2D_RS;     // A from registers (TF32 only)
 	static constexpr bool A_T = !K16 && AMODE == OP_MN2D; // fp32 MN-major A: transposed into the K-major slot
 	static constexpr bool B_T = !K16 && BMODE != OP_K2D;  // fp32 MN-major B (2-D or im2col)
 	static constexpr bool ANY = A_T || B_T || X3;
 };
 
-template <int BN, int STAGES, bool XF, int X3>
+template <int BN, int STAGES, bool XF, int X3, bool ARS = false>
 struct UmmaSmem {
 	static constexpr int A_BYTES = UMMA_BLOCK_M * 128;
 	static constexpr int B_BYTES = BN * 128;
 	static constexpr int RAW_BYTES = A_BYTES + B_BYTES;            // one TMA stage
-	static constexpr int SLOT_BYTES = RAW_BYTES * (X3 ? 2 : 1);     // one K-major operand slot: [A hi][B hi] ([A lo][B lo])
+	static constexpr int SLOT_A_BYTES = ARS ? 0 : A_BYTES;          // where B starts in the operand the MMAs read (A from registers: B alone)
+	static constexpr int SLOT_BYTES = (SLOT_A_BYTES + B_BYTES) * (X3 ? 2 : 1); // one K-major operand slot: [A hi][B hi] ([A lo][B lo])
 	static constexpr int SLOT_OFFSET = STAGES * RAW_BYTES;
 	static constexpr int STATS_OFFSET = SLOT_OFFSET + (XF ? 2 * SLOT_BYTES : 0);
 	static constexpr int STATS_BYTES = XF ? 0 : 4 * BN * 4 * 4 + 2 * 4 * BN * 3 * 4; // running (n, k, s1, s2) per slot + per-warp partials
@@ -118,10 +126,11 @@ struct UmmaSmem {
 	static constexpr int TOTAL = BAR_OFFSET + 256 + 1024;           // barriers + slack for the 1024-byte alignment
 };
 
-// stages per kernel: as deep as 227 KB of shared memory allows with the transform slots
-template <int BN, bool XF, int X3>
+// stages per kernel: as deep as 227 KB of shared memory allows with the transform slots (A from registers: 3 stages of 48 KB and
+// two 32 KB B slots at BN = 256; 4 at BN = 64 / 128, which ran ResNet-50's weight gradients no slower than 6)
+template <int BN, bool XF, int X3, bool ARS = false>
 struct GemmStages {
-	static constexpr int value = X3 ? (BN == 128 ? 3 : 4) : (XF ? 4 : (BN == 128 ? 5 : 6));
+	static constexpr int value = ARS ? (BN == 256 ? 3 : 4) : X3 ? (BN == 128 ? 3 : 4) : (XF ? 4 : (BN == 128 ? 5 : 6));
 };
 
 // one staged fp32 operand tile (rows x 32 k) -> K-major 128-byte-swizzled slot (16-byte chunk c of row r at chunk c ^ (r & 7)).
@@ -158,14 +167,40 @@ __device__ __forceinline__ void xform_tile(const float* __restrict__ raw, float*
 	}
 }
 
+// A = OP_MN2D_RS: one consumer warp's wgmma A fragments of a stage (4 MMA steps of k = 8) from the staged MN-major tile, four
+// 32-row boxes of 32 k-rows of 128 B.  The stage is 128-byte swizzled: 16-byte chunk c of k-row k sits at c ^ (k & 7).  A fragment
+// load takes 8 rows (lane / 4) x 4 k (lane % 4); rows are contiguous, so unswizzled those 32 words fall in 8 banks (4-way conflict)
+// and swizzled with the natural rows in 16 (2-way).  So fragment row lane / 4 = i (a0 / a2; a1 / a3: h = 1) of warp w holds row
+// a_row(w, lane, h) = 32 (w >> 1) + 16 (i >> 2) + 8 (w & 1) + 4 h + (i & 3) of the warpgroup's 64: chunk (4 (i >> 2) + 2 (w & 1) + h)
+// ^ (k & 7), word i & 3, 32 distinct banks.  The accumulator rows follow the A rows, so the epilogue stores them by the same map.
+__device__ __forceinline__ int a_row(const int warp, const int lane, const int h)
+{
+	const int i = lane >> 2;
+	return 32 * ((warp >> 1) & 1) + 16 * (i >> 2) + 8 * (warp & 1) + 4 * h + (i & 3);
+}
+__device__ __forceinline__ void load_a_frags(uint32_t (&af)[4][4], const float* __restrict__ raw_wg, const int warp, const int lane)
+{
+	const int i = lane >> 2, j = lane & 3;
+	// k = 8 step + j + 4 e: k-row offset 32 k; chunk ((4 (i >> 2) + 2 (w & 1)) ^ j) ^ h ^ 4 e
+	const float* const src = raw_wg + ((warp >> 1) & 1) * 1024 + j * 32 + (i & 3);
+	const int c = ((4 * (i >> 2) + 2 * (warp & 1)) ^ j) << 2;
+#pragma unroll
+	for (int step = 0; step < 4; step++)
+#pragma unroll
+		for (int e = 0; e < 2; e++)
+#pragma unroll
+			for (int h = 0; h < 2; h++)
+				af[step][2 * e + h] = __float_as_uint(src[step * 256 + e * 128 + (c ^ (h << 2) ^ (e << 4))]);
+}
+
 // K16 = 1 / 2: bf16 / fp16 operands (p.out_kind holds the same kind), 64 elements per 128-byte row, K = 16 per MMA; K16 = 0: fp32
 // operands (32 per row, K = 8 per MMA).  The element type is a template parameter so that every wgmma of a k-step sits in one basic
 // block (a runtime type branch makes ptxas fence each MMA on its own).  OUT16 = 1: the output tensor (and an optional 16-bit bias) is bf16 / fp16 (p.out_kind).
 template <int AMODE, int BMODE, int BN, int STAGES, int X3 = 0, int K16 = 0, int OUT16 = 0>
-__global__ void __launch_bounds__(GEMM_THREADS, 1) umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const UmmaGemmParams p)
+__global__ void __launch_bounds__(AMODE == OP_MN2D_RS ? GEMM_THREADS_RS : GEMM_THREADS, 1) umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const UmmaGemmParams p)
 {
 	using XF = GemmXform<AMODE, BMODE, K16, X3>;
-	using S = UmmaSmem<BN, STAGES, XF::ANY, X3>;
+	using S = UmmaSmem<BN, STAGES, XF::ANY, X3, XF::A_RS>;
 	extern __shared__ uint8_t smem_raw[];
 	uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
 	uint64_t* full_bar = (uint64_t*)(smem + S::BAR_OFFSET);
@@ -195,9 +230,15 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) umma_gemm_kernel(const __grid
 	}
 	__syncthreads();
 
-	if (warp == 8)
+	if (XF::A_RS ? warp >= 8 : warp == 8)
 	{
 		// ------------------------------------------------------------------ TMA producer
+		if constexpr (XF::A_RS)
+		{
+			setmaxnreg_dec<56>(); // 2 x 224 + 56 registers per scheduler: the whole file
+			if (warp != 8)
+				return;
+		}
 		if (elect_one())
 		{
 			tma_prefetch_desc(&tmA);
@@ -239,7 +280,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) umma_gemm_kernel(const __grid
 				mbar_expect_tx(&full_bar[stage], S::RAW_BYTES);
 				if (AMODE == OP_K2D)
 					tma_load_2d(sA, &tmA, &full_bar[stage], chunk * BK, m0);
-				else if (AMODE == OP_MN2D) {
+				else if (AMODE == OP_MN2D || AMODE == OP_MN2D_RS) {
 #pragma unroll
 					for (int j = 0; j < UMMA_BLOCK_M / BK; j++)
 						tma_load_2d(sA + j * MN_BOX_BYTES, &tmA, &full_bar[stage], m0 + BK * j, it * BK);
@@ -271,6 +312,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) umma_gemm_kernel(const __grid
 	}
 
 	// ------------------------------------------------------------------ consumers (warps 0..7)
+	if constexpr (XF::A_RS)
+		setmaxnreg_inc<224>();
 	const int wg = warp >> 2; // output rows [64 * wg, +64) of the tile
 	float acc[BN / 2];
 	constexpr bool A_MN16 = K16 && AMODE == OP_MN2D, B_MN16 = K16 && BMODE != OP_K2D;
@@ -291,6 +334,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) umma_gemm_kernel(const __grid
 #pragma unroll
 	for (int i = 0; i < BN / 2; i++)
 		acc[i] = 0.f;
+	uint32_t af[4][4]; // A from registers: this k-iteration's A fragments
 	for (int it = 0; it < n_it; it++, gi++)
 	{
 		mbar_wait(&full_bar[stage], phase);
@@ -303,8 +347,17 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) umma_gemm_kernel(const __grid
 			const float* const raw = reinterpret_cast<const float*>(smem + stage * S::RAW_BYTES);
 			float* const hi = reinterpret_cast<float*>(op);
 			float* const lo = reinterpret_cast<float*>(op + S::RAW_BYTES);
-			xform_tile<XF::A_T, X3>(raw, hi, lo, UMMA_BLOCK_M, threadIdx.x);
-			xform_tile<XF::B_T, X3>(raw + S::A_BYTES / 4, hi + S::A_BYTES / 4, lo + S::A_BYTES / 4, BN, threadIdx.x);
+			if constexpr (!XF::A_RS)
+				xform_tile<XF::A_T, X3>(raw, hi, lo, UMMA_BLOCK_M, threadIdx.x);
+			xform_tile<XF::B_T, X3>(raw + S::A_BYTES / 4, hi + S::SLOT_A_BYTES / 4, lo + S::SLOT_A_BYTES / 4, BN, threadIdx.x);
+			if constexpr (XF::A_RS)
+			{
+				// B went into slot gi & 1 while the MMAs of iteration it - 1 still ran.  Those read the fragment registers until they
+				// complete (overwritten in flight, ptxas would serialise every wgmma), so only now load this stage's; the stage is
+				// released below
+				wgmma_wait<0>();
+				load_a_frags(af, raw + wg * 2048, warp, lane);
+			}
 			fence_proxy_async(); // the tensor core reads shared memory through the async proxy
 			named_bar_sync(1, 256);
 			if (threadIdx.x == 0)
@@ -312,7 +365,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) umma_gemm_kernel(const __grid
 		}
 		const uint32_t base = smem_u32(op);
 		const uint64_t da0 = wgmma_desc(base + wg * 8192, 16, 1024);
-		const uint64_t db0 = wgmma_desc(base + S::A_BYTES, 8192, 1024);
+		const uint64_t db0 = wgmma_desc(base + S::SLOT_A_BYTES, 8192, 1024);
 		fence_regs(acc);
 		wgmma_fence();
 #pragma unroll
@@ -333,6 +386,13 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) umma_gemm_kernel(const __grid
 					else
 						wgmma_f16_ss_n64<A_MN16, B_MN16>(*reinterpret_cast<float(*)[32]>(acc), da, db);
 				}
+			} else if constexpr (XF::A_RS) {
+				if constexpr (BN == 256)
+					wgmma_tf32_rs_n256(*reinterpret_cast<float(*)[128]>(acc), af[k], db);
+				else if constexpr (BN == 128)
+					wgmma_tf32_rs_n128(*reinterpret_cast<float(*)[64]>(acc), af[k], db);
+				else
+					wgmma_tf32_rs_n64(*reinterpret_cast<float(*)[32]>(acc), af[k], db);
 			} else {
 				constexpr uint32_t LO = (uint32_t)(S::RAW_BYTES >> 4);
 				if constexpr (BN == 128)
@@ -378,7 +438,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) umma_gemm_kernel(const __grid
 #pragma unroll
 	for (int h = 0; h < 2; h++)
 	{
-		const int row = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+		const int row = m0 + wg * 64 + (XF::A_RS ? a_row(warp, lane, h) : (warp & 3) * 16 + (lane >> 2) + 8 * h);
 		long long off;
 		if (p.rowmap.mode == 0)
 			off = (long long)row * p.rowmap.ld;
