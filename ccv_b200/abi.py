@@ -40,6 +40,7 @@ CMD_IDS = dict(
     CMUL=0xead486e6, BINARY_CROSSENTROPY=0xcd2107ec, SIGMOID_BINARY_CROSSENTROPY=0xd9e0e4a, MSE=0x6904a9a2, SMOOTH_L1=0x4e428e,
     PAD=0xd8aaca60, MIN=0x972fbd26, MAX=0xdf6f014c, ARGMAX=0x68af2804, ARGMIN=0xeb8747f2, REDUCE_ISNAN=0xee0a4ade,
     ROI_ALIGN=0xfef55168, NMS=0xdba26106, LAMB=0x450edb1a, RMSPROP=0x9c886b1c,
+    COMPRESSION_LSSC=0x17ea8f72,
 )
 for _k, _v in CMD_IDS.items():
     globals()["CCV_NNC_%s_FORWARD" % _k] = _v

@@ -1402,25 +1402,7 @@ int narrow_matrix(cudaStream_t s, const float* src, void* dst, int kind, long lo
 }
 
 // =============================================================================================== dtype conversion
-// f32 -> f16 follows the reference's CPU table method bit for bit (lib/ccv_util.c:1434-1440; van der Zijp's
-// base/shift tables): the mantissa is TRUNCATED, values below 2^-24 flush to signed zero, values >= 2^16 become inf,
-// NaN keeps its top mantissa bits.  This is not __float2half_rn.
-__device__ __forceinline__ uint16_t f32_to_f16_trunc(const float f)
-{
-	const uint32_t u = __float_as_uint(f);
-	const uint32_t sign = (u >> 16) & 0x8000u;
-	const int e = (int)((u >> 23) & 0xff) - 127;
-	const uint32_t m = u & 0x007fffffu;
-	if (e < -24)
-		return (uint16_t)sign;
-	if (e < -14)
-		return (uint16_t)(sign | ((0x0400u >> (-e - 14)) + (m >> (-e - 1))));
-	if (e <= 15)
-		return (uint16_t)(sign | (((uint32_t)(e + 15) << 10) + (m >> 13)));
-	if (e < 128)
-		return (uint16_t)(sign | 0x7c00u);
-	return (uint16_t)(sign | (0x7c00u + (m >> 13)));
-}
+// f32 -> f16 is f32_to_f16_trunc (sm100_elem.cuh): the reference's truncating table method, not __float2half_rn.
 template <int AD, int BD>
 __global__ void convert_kernel(const void* __restrict__ a, void* __restrict__ b, const size_t n)
 {

@@ -899,6 +899,27 @@ def CMD_RMSPROP_BACKWARD(rate, decay, alpha, momentum, epsilon, scale=1.0, **kw)
     return c
 
 
+def CMD_COMPRESSION_LSSC_FORWARD(**kw):
+    """LSSC (cmd/compression): inputs (x_1 .. x_n) fp16 -> outputs (y_1 .. y_n), y_i of lssc_compressed_dims(x_i); 4 bits per element"""
+    return _simple(abi.CCV_NNC_COMPRESSION_LSSC_FORWARD, **kw)
+
+
+def CMD_COMPRESSION_LSSC_BACKWARD(**kw):
+    """inputs (y_1 .. y_m) -> outputs (x_1 .. x_n), n <= m: each block's cells set to one of four levels between its min and max"""
+    return _simple(abi.CCV_NNC_COMPRESSION_LSSC_BACKWARD, **kw)
+
+
+def lssc_compressed_dims(dims, fmt):
+    """The compressed shape of an fp16 tensor of dims in fmt (the reference's _ccv_nnc_lssc_tensor_auto_forw): NCHW [N, C, H, W] or
+    [C, H, W] -> [N, C, ceil(H/4), 4 ceil(W/4)]; NHWC [N, H, W, C] or [H, W, C] -> [N, ceil(H/4), 4 ceil(W/4), C]"""
+    dims = list(dims)
+    if len(dims) not in (3, 4) or fmt not in (abi.CCV_TENSOR_FORMAT_NCHW, abi.CCV_TENSOR_FORMAT_NHWC):
+        raise ValueError("LSSC takes 3-d or 4-d NCHW / NHWC tensors, not %s in format %d" % (dims, fmt))
+    hw = len(dims) - 2 if fmt == abi.CCV_TENSOR_FORMAT_NCHW else len(dims) - 3
+    dims[hw], dims[hw + 1] = (dims[hw] + 3) // 4, (dims[hw + 1] + 3) // 4 * 4
+    return dims
+
+
 def CMD_DROPOUT_FORWARD(p, entirety=0, **kw):
     c = _simple(abi.CCV_NNC_DROPOUT_FORWARD, **kw)
     c.info.dropout.p, c.info.dropout.entirety = p, entirety

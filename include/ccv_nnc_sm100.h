@@ -507,6 +507,9 @@ enum {
 	CCV_NNC_LAMB_BACKWARD = 0x450edb1b,
 	CCV_NNC_RMSPROP_FORWARD = 0x9c886b1c,
 	CCV_NNC_RMSPROP_BACKWARD = 0x9c886b1d,
+	/* cmd/compression */
+	CCV_NNC_COMPRESSION_LSSC_FORWARD = 0x17ea8f72,
+	CCV_NNC_COMPRESSION_LSSC_BACKWARD = 0x17ea8f73,
 };
 
 /* lib/nnc/ccv_nnc.h:97-100 (cmd.info.pad.type) */
@@ -597,6 +600,9 @@ CCV_NNC_SM100_DETECTION_COMMANDS(CCV_SM100_DECLARE_REGISTER)
 #define CCV_NNC_SM100_OPTIMIZER_COMMANDS(X) \
 	X(CCV_NNC_LAMB_FORWARD) X(CCV_NNC_LAMB_BACKWARD) X(CCV_NNC_RMSPROP_FORWARD) X(CCV_NNC_RMSPROP_BACKWARD)
 CCV_NNC_SM100_OPTIMIZER_COMMANDS(CCV_SM100_DECLARE_REGISTER)
+#define CCV_NNC_SM100_COMPRESSION_COMMANDS(X) \
+	X(CCV_NNC_COMPRESSION_LSSC_FORWARD) X(CCV_NNC_COMPRESSION_LSSC_BACKWARD)
+CCV_NNC_SM100_COMPRESSION_COMMANDS(CCV_SM100_DECLARE_REGISTER)
 #undef CCV_SM100_DECLARE_REGISTER
 
 /* What the backend needs back from its host (ccv's own when linked into libccv: lib/nnc/gpu/ccv_nnc_compat.h:95-97,
