@@ -2547,12 +2547,12 @@ REGISTER_SM100(CCV_NNC_SOFTMAX_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | 
 REGISTER_SM100(CCV_NNC_SOFTMAX_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_via_f32<exec_softmax_back>); }
 REGISTER_SM100(CCV_NNC_BATCH_NORM_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_bnorm_forw); }
 REGISTER_SM100(CCV_NNC_BATCH_NORM_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_bnorm_back); }
-REGISTER_SM100(CCV_NNC_LAYER_NORM_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F, 1, ccv_nnc_sm100_exec_lnorm_forw); }
-REGISTER_SM100(CCV_NNC_LAYER_NORM_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F, 1, ccv_nnc_sm100_exec_lnorm_back); }
-REGISTER_SM100(CCV_NNC_GROUP_NORM_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F, 1, ccv_nnc_sm100_exec_gnorm_forw); }
-REGISTER_SM100(CCV_NNC_GROUP_NORM_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F, 1, ccv_nnc_sm100_exec_gnorm_back); }
-REGISTER_SM100(CCV_NNC_RMSNORM_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F, 1, ccv_nnc_sm100_exec_rmsnorm_forw); }
-REGISTER_SM100(CCV_NNC_RMSNORM_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F, 1, ccv_nnc_sm100_exec_rmsnorm_back); }
+REGISTER_SM100(CCV_NNC_LAYER_NORM_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, ccv_nnc_sm100_exec_lnorm_forw); }
+REGISTER_SM100(CCV_NNC_LAYER_NORM_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, ccv_nnc_sm100_exec_lnorm_back); }
+REGISTER_SM100(CCV_NNC_GROUP_NORM_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, ccv_nnc_sm100_exec_gnorm_forw); }
+REGISTER_SM100(CCV_NNC_GROUP_NORM_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, ccv_nnc_sm100_exec_gnorm_back); }
+REGISTER_SM100(CCV_NNC_RMSNORM_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, ccv_nnc_sm100_exec_rmsnorm_forw); }
+REGISTER_SM100(CCV_NNC_RMSNORM_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, ccv_nnc_sm100_exec_rmsnorm_back); }
 REGISTER_SM100(CCV_NNC_EWSUM_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF | CCV_32S, 1, exec_ewsum_forw); }
 REGISTER_SM100(CCV_NNC_EWSUM_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_ewsum_back); }
 REGISTER_SM100(CCV_NNC_ADD_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_via_f32<exec_add_forw>); }

@@ -33,16 +33,55 @@ bool packed_f32(const ccv_nnc_tensor_t* const t)
 	return CCV_GET_DATA_TYPE(t->info.datatype) == CCV_32F && CCV_IS_TENSOR_CONTIGUOUS(t);
 }
 
-// a packed fp32 tensor of exactly `count` elements: what the row-norm kernels assume of every operand they index as [rows, inner]
-bool packed_f32_of(const ccv_nnc_tensor_t* const t, const size_t count)
+// element kind of an fp32 / bf16 / fp16 tensor (ElemKind: 0, 1, 2); -1 for every other type, palettized ones included
+int kind_of(const ccv_nnc_tensor_t* const t)
 {
-	return packed_f32(t) && count_of(t) == count;
+	switch (CCV_GET_DATA_TYPE(t->info.datatype))
+	{
+		case CCV_32F:
+			return 0;
+		case CCV_16BF:
+			return 1;
+		case CCV_16F:
+			return 2;
+	}
+	return -1;
+}
+
+// The normalisations' datatype rule.  The activations (x and y; g, x and h) share one kind kx: fp32, bf16 or fp16.  Each parameter
+// tensor (scale, bias, dscale, dbias) is fp32 or kx, and so are the statistics (saved_mean, saved_inv_std), which share one kind.
+// With fp32 activations everything is fp32.
+//
+// an activation: packed, of kind kx, exactly `count` elements (what the row-norm kernels assume of every operand they index as
+// [rows, inner])
+bool packed_act(const ccv_nnc_tensor_t* const t, const int kx, const size_t count)
+{
+	return kind_of(t) == kx && CCV_IS_TENSOR_CONTIGUOUS(t) && count_of(t) == count;
+}
+// a parameter or statistics tensor: packed, fp32 or kx; its kind in k
+bool packed_param(const ccv_nnc_tensor_t* const t, const int kx, int& k)
+{
+	k = kind_of(t);
+	return kx >= 0 && (k == 0 || k == kx) && CCV_IS_TENSOR_CONTIGUOUS(t);
+}
+bool packed_param_of(const ccv_nnc_tensor_t* const t, const int kx, const size_t count, int& k)
+{
+	return packed_param(t, kx, k) && count_of(t) == count;
+}
+// the two statistics (either may be absent): each a packed `count` elements, the pair of one kind, k = that kind
+bool packed_stats_of(const ccv_nnc_tensor_t* const mean, const ccv_nnc_tensor_t* const inv_std, const int kx, const size_t count, int& k)
+{
+	int km = 0, ki = 0;
+	if ((mean && !packed_param_of(mean, kx, count, km)) || (inv_std && !packed_param_of(inv_std, kx, count, ki)))
+		return false;
+	k = mean ? km : ki;
+	return !mean || !inv_std || km == ki;
 }
 
 // the normalised axes must be the trailing ones: x is then [rows, inner]
 bool rows_inner(const ccv_nnc_tensor_t* const x, const int* const axis, const int axis_count, int& rows, int& inner)
 {
-	if (!packed_f32(x))
+	if (kind_of(x) < 0 || !CCV_IS_TENSOR_CONTIGUOUS(x))
 		return false;
 	const int nd = nd_of(x);
 	if (axis_count < 1 || axis_count > nd)
@@ -372,15 +411,18 @@ int ccv_nnc_sm100_exec_lnorm_forw(SM100_EXEC_ARGS)
 	if (affine && (input_size < 3 || !inputs[1] || !inputs[2]))
 		return CCV_NNC_EXEC_INVALID;
 	int rows, inner;
-	if (!rows_inner(inputs[0], cmd.info.lnorm.axis, cmd.info.lnorm.count, rows, inner) || !packed_f32(outputs[0]) || count_of(outputs[0]) != (size_t)rows * inner)
+	if (!rows_inner(inputs[0], cmd.info.lnorm.axis, cmd.info.lnorm.count, rows, inner))
 		return CCV_NNC_EXEC_INVALID;
-	if (affine && (!packed_f32(inputs[1]) || !packed_f32(inputs[2]) || count_of(inputs[1]) != (size_t)inner || count_of(inputs[2]) != (size_t)inner))
+	NormKinds k = { kind_of(inputs[0]), 0, 0, 0, 0, 0 };
+	if (!packed_act(outputs[0], k.x, (size_t)rows * inner))
 		return CCV_NNC_EXEC_INVALID;
-	float* sm = output_size > 1 && outputs[1] ? outputs[1]->data.f32 : 0;
-	float* sis = output_size > 2 && outputs[2] ? outputs[2]->data.f32 : 0;
-	if ((sm && !packed_f32_of(outputs[1], rows)) || (sis && !packed_f32_of(outputs[2], rows)))
+	if (affine && (!packed_param_of(inputs[1], k.x, inner, k.scale) || !packed_param_of(inputs[2], k.x, inner, k.bias)))
 		return CCV_NNC_EXEC_INVALID;
-	if (layer_norm_fwd_f32(stream_of(stream_context), inputs[0]->data.f32, affine ? inputs[1]->data.f32 : 0, affine ? inputs[2]->data.f32 : 0, outputs[0]->data.f32, sm, sis, rows, inner, cmd.info.lnorm.epsilon))
+	ccv_nnc_tensor_t* const sm = output_size > 1 ? outputs[1] : 0;
+	ccv_nnc_tensor_t* const sis = output_size > 2 ? outputs[2] : 0;
+	if (!packed_stats_of(sm, sis, k.x, rows, k.stat))
+		return CCV_NNC_EXEC_INVALID;
+	if (layer_norm_fwd(stream_of(stream_context), k, inputs[0]->data.u8, affine ? inputs[1]->data.u8 : 0, affine ? inputs[2]->data.u8 : 0, outputs[0]->data.u8, sm ? sm->data.u8 : 0, sis ? sis->data.u8 : 0, rows, inner, cmd.info.lnorm.epsilon))
 		return CCV_NNC_EXEC_INVALID;
 	return CCV_NNC_EXEC_SUCCESS;
 }
@@ -393,19 +435,20 @@ int ccv_nnc_sm100_exec_lnorm_back(SM100_EXEC_ARGS)
 	if (input_size <= si || output_size < 1 || !inputs[0] || !inputs[3] || !inputs[mi] || !inputs[si] || (affine && !inputs[4]))
 		return CCV_NNC_EXEC_INVALID;
 	int rows, inner;
-	if (!rows_inner(inputs[3], cmd.info.lnorm.axis, cmd.info.lnorm.count, rows, inner) || !packed_f32(inputs[0]) || count_of(inputs[0]) != (size_t)rows * inner)
+	if (!rows_inner(inputs[3], cmd.info.lnorm.axis, cmd.info.lnorm.count, rows, inner))
 		return CCV_NNC_EXEC_INVALID;
-	if (!packed_f32_of(inputs[mi], rows) || !packed_f32_of(inputs[si], rows) || (affine && !packed_f32_of(inputs[4], inner)))
+	NormKinds k = { kind_of(inputs[3]), 0, 0, 0, 0, 0 };
+	if (!packed_act(inputs[0], k.x, (size_t)rows * inner) || !packed_stats_of(inputs[mi], inputs[si], k.x, rows, k.stat) || (affine && !packed_param_of(inputs[4], k.x, inner, k.scale)))
 		return CCV_NNC_EXEC_INVALID;
-	float* h = outputs[0] ? outputs[0]->data.f32 : 0;
-	float* ds = output_size > 1 && outputs[1] ? outputs[1]->data.f32 : 0;
-	float* db = output_size > 2 && outputs[2] ? outputs[2]->data.f32 : 0;
-	if ((h && !packed_f32_of(outputs[0], (size_t)rows * inner)) || (ds && !packed_f32_of(outputs[1], inner)) || (db && !packed_f32_of(outputs[2], inner)))
+	ccv_nnc_tensor_t* const h = outputs[0];
+	ccv_nnc_tensor_t* const ds = output_size > 1 ? outputs[1] : 0;
+	ccv_nnc_tensor_t* const db = output_size > 2 ? outputs[2] : 0;
+	if ((h && !packed_act(h, k.x, (size_t)rows * inner)) || (ds && !packed_param_of(ds, k.x, inner, k.dscale)) || (db && !packed_param_of(db, k.x, inner, k.dbias)))
 		return CCV_NNC_EXEC_INVALID;
 	void* const ws = ds || db ? ccv_nnc_stream_context_get_workspace(stream_context, norm_bwd_workspace_bytes(rows, inner), CCV_TENSOR_GPU_MEMORY) : 0;
 	if ((ds || db) && !ws)
 		return CCV_NNC_EXEC_OOM;
-	if (layer_norm_bwd_f32(stream_of(stream_context), inputs[0]->data.f32, inputs[3]->data.f32, affine ? inputs[4]->data.f32 : 0, inputs[mi]->data.f32, inputs[si]->data.f32, h, ds, db, rows, inner, ws))
+	if (layer_norm_bwd(stream_of(stream_context), k, inputs[0]->data.u8, inputs[3]->data.u8, affine ? inputs[4]->data.u8 : 0, inputs[mi]->data.u8, inputs[si]->data.u8, h ? h->data.u8 : 0, ds ? ds->data.u8 : 0, db ? db->data.u8 : 0, rows, inner, ws))
 		return CCV_NNC_EXEC_INVALID;
 	return CCV_NNC_EXEC_SUCCESS;
 }
@@ -415,8 +458,6 @@ int ccv_nnc_sm100_exec_lnorm_back(SM100_EXEC_ARGS)
 // statistics tensor's own dims say which elements share a slot (group axis -> groups, reduced axes -> 1).
 static bool gn_dims(const ccv_nnc_tensor_t* const t, int dim[4], long long stride[4])
 {
-	if (CCV_GET_DATA_TYPE(t->info.datatype) != CCV_32F)
-		return false;
 	const int nd = nd_of(t);
 	if (nd < 1 || nd > 4)
 		return false;
@@ -432,18 +473,23 @@ static bool gn_dims(const ccv_nnc_tensor_t* const t, int dim[4], long long strid
 	return true;
 }
 
-static bool gn_geom(const ccv_nnc_tensor_t* const x, const ccv_nnc_tensor_t* const y, const ccv_nnc_tensor_t* const h, const ccv_nnc_tensor_t* const stat, const ccv_nnc_tensor_t* const scale, GroupNormGeom& g)
+// x, y (forward) or g (backward) and h are activations and may be strided views; the statistics and the tensor that gives the
+// parameters' dims are packed.  Sets k.x, k.stat (from `stat`) and k.scale (from `scale`).
+static bool gn_geom(const ccv_nnc_tensor_t* const x, const ccv_nnc_tensor_t* const y, const ccv_nnc_tensor_t* const h, const ccv_nnc_tensor_t* const stat, const ccv_nnc_tensor_t* const scale, GroupNormGeom& g, NormKinds& k)
 {
+	k.x = kind_of(x);
+	if (k.x < 0 || kind_of(y) != k.x || (h && kind_of(h) != k.x))
+		return false;
 	int d2[4];
 	if (!gn_dims(x, g.dim, g.xstride) || !gn_dims(y, d2, g.ystride) || memcmp(d2, g.dim, sizeof(d2)) != 0)
 		return false;
 	if (h && (!gn_dims(h, d2, g.hstride) || memcmp(d2, g.dim, sizeof(d2)) != 0))
 		return false;
-	if (!packed_f32(stat) || nd_of(stat) != nd_of(x) || !gn_dims(stat, g.rdim, 0))
+	if (!packed_param(stat, k.x, k.stat) || nd_of(stat) != nd_of(x) || !gn_dims(stat, g.rdim, 0))
 		return false;
 	for (int i = 0; i < 4; i++)
 		g.sdim[i] = 1;
-	if (scale && (!packed_f32(scale) || nd_of(scale) != nd_of(x) || !gn_dims(scale, g.sdim, 0)))
+	if (scale && (!packed_param(scale, k.x, k.scale) || nd_of(scale) != nd_of(x) || !gn_dims(scale, g.sdim, 0)))
 		return false;
 	// Slots must divide the axis.  Where they do not, the reference divides every slot's sums by the one integer
 	// n = count(x) / count(statistics) (norm/ccv_nnc_group_norm_cpu_ref.c:52-57, :464) although the slots hold different numbers of
@@ -462,14 +508,16 @@ int ccv_nnc_sm100_exec_gnorm_forw(SM100_EXEC_ARGS)
 	if (affine && (input_size < 3 || !inputs[1] || !inputs[2] || count_of(inputs[1]) != count_of(inputs[2])))
 		return CCV_NNC_EXEC_INVALID;
 	GroupNormGeom g;
-	if (!gn_geom(inputs[0], outputs[0], 0, outputs[1], affine ? inputs[1] : 0, g) || !packed_f32(outputs[2]) || count_of(outputs[2]) != count_of(outputs[1]) || (affine && !packed_f32(inputs[2])))
+	NormKinds k = { 0, 0, 0, 0, 0, 0 };
+	int kis;
+	if (!gn_geom(inputs[0], outputs[0], 0, outputs[1], affine ? inputs[1] : 0, g, k) || !packed_param(outputs[2], k.x, kis) || kis != k.stat || count_of(outputs[2]) != count_of(outputs[1]) || (affine && !packed_param(inputs[2], k.x, k.bias)))
 		return CCV_NNC_EXEC_INVALID;
 	// Both reference implementations read the epsilon through the LAYER-norm arm of the parameter union
 	// (norm/ccv_nnc_group_norm_cpu_ref.c:46, norm/gpu/ccv_nnc_group_norm_gpu_cudnn.cu:117: `cmd.info.lnorm.epsilon`), which aliases
 	// gnorm.reduce_count -- a small integer whose bits read as a denormal float (~0), NOT gnorm.epsilon.  Parity is with what the
 	// reference computes, so the same word is read here (its own tests hold the two backends to 1e-5 on statistics over 4 values,
 	// test/int/nnc/cudnn.tests.c:1491-1560, where a 1e-5 epsilon would show).
-	if (group_norm_fwd_f32(stream_of(stream_context), g, inputs[0]->data.f32, affine ? inputs[1]->data.f32 : 0, affine ? inputs[2]->data.f32 : 0, outputs[0]->data.f32, outputs[1]->data.f32, outputs[2]->data.f32, cmd.info.lnorm.epsilon))
+	if (group_norm_fwd(stream_of(stream_context), k, g, inputs[0]->data.u8, affine ? inputs[1]->data.u8 : 0, affine ? inputs[2]->data.u8 : 0, outputs[0]->data.u8, outputs[1]->data.u8, outputs[2]->data.u8, cmd.info.lnorm.epsilon))
 		return CCV_NNC_EXEC_INVALID;
 	return CCV_NNC_EXEC_SUCCESS;
 }
@@ -485,14 +533,18 @@ int ccv_nnc_sm100_exec_gnorm_back(SM100_EXEC_ARGS)
 	ccv_nnc_tensor_t* const ds = output_size > 1 ? outputs[1] : 0;
 	ccv_nnc_tensor_t* const db = output_size > 2 ? outputs[2] : 0;
 	GroupNormGeom g;
-	if (!gn_geom(inputs[3], inputs[0], h, inputs[mi], affine ? inputs[4] : (ds ? ds : db), g) || !packed_f32(inputs[si]) || count_of(inputs[si]) != count_of(inputs[mi]))
+	NormKinds k = { 0, 0, 0, 0, 0, 0 };
+	int kis;
+	if (!gn_geom(inputs[3], inputs[0], h, inputs[mi], affine ? inputs[4] : (ds ? ds : db), g, k) || !packed_param(inputs[si], k.x, kis) || kis != k.stat || count_of(inputs[si]) != count_of(inputs[mi]))
 		return CCV_NNC_EXEC_INVALID;
-	if ((ds && (!packed_f32(ds) || (long long)count_of(ds) != (long long)g.sdim[0] * g.sdim[1] * g.sdim[2] * g.sdim[3])) || (db && (!packed_f32(db) || (long long)count_of(db) != (long long)g.sdim[0] * g.sdim[1] * g.sdim[2] * g.sdim[3])))
+	if (!affine)
+		k.scale = 0;
+	if ((ds && (!packed_param(ds, k.x, k.dscale) || (long long)count_of(ds) != (long long)g.sdim[0] * g.sdim[1] * g.sdim[2] * g.sdim[3])) || (db && (!packed_param(db, k.x, k.dbias) || (long long)count_of(db) != (long long)g.sdim[0] * g.sdim[1] * g.sdim[2] * g.sdim[3])))
 		return CCV_NNC_EXEC_INVALID;
 	void* const ws = h ? ccv_nnc_stream_context_get_workspace(stream_context, group_norm_bwd_workspace_bytes(g), CCV_TENSOR_GPU_MEMORY) : 0;
 	if (h && !ws)
 		return CCV_NNC_EXEC_OOM;
-	if (group_norm_bwd_f32(stream_of(stream_context), g, inputs[0]->data.f32, inputs[3]->data.f32, affine ? inputs[4]->data.f32 : 0, inputs[mi]->data.f32, inputs[si]->data.f32, h ? h->data.f32 : 0, ds ? ds->data.f32 : 0, db ? db->data.f32 : 0, ws))
+	if (group_norm_bwd(stream_of(stream_context), k, g, inputs[0]->data.u8, inputs[3]->data.u8, affine ? inputs[4]->data.u8 : 0, inputs[mi]->data.u8, inputs[si]->data.u8, h ? h->data.u8 : 0, ds ? ds->data.u8 : 0, db ? db->data.u8 : 0, ws))
 		return CCV_NNC_EXEC_INVALID;
 	return CCV_NNC_EXEC_SUCCESS;
 }
@@ -503,12 +555,15 @@ int ccv_nnc_sm100_exec_rmsnorm_forw(SM100_EXEC_ARGS)
 	if (input_size < 2 || output_size < 1 || !inputs[0] || !inputs[1] || !outputs[0])
 		return CCV_NNC_EXEC_INVALID;
 	int rows, inner;
-	if (!rows_inner(inputs[0], cmd.info.rmsnorm.axis, cmd.info.rmsnorm.count, rows, inner) || !packed_f32_of(outputs[0], (size_t)rows * inner) || !packed_f32_of(inputs[1], inner))
+	if (!rows_inner(inputs[0], cmd.info.rmsnorm.axis, cmd.info.rmsnorm.count, rows, inner))
 		return CCV_NNC_EXEC_INVALID;
-	float* sis = output_size > 1 && outputs[1] ? outputs[1]->data.f32 : 0;
-	if (sis && !packed_f32_of(outputs[1], rows))
+	NormKinds k = { kind_of(inputs[0]), 0, 0, 0, 0, 0 };
+	if (!packed_act(outputs[0], k.x, (size_t)rows * inner) || !packed_param_of(inputs[1], k.x, inner, k.scale))
 		return CCV_NNC_EXEC_INVALID;
-	if (rmsnorm_fwd_f32(stream_of(stream_context), inputs[0]->data.f32, inputs[1]->data.f32, outputs[0]->data.f32, sis, rows, inner, cmd.info.rmsnorm.epsilon))
+	ccv_nnc_tensor_t* const sis = output_size > 1 ? outputs[1] : 0;
+	if (!packed_stats_of(0, sis, k.x, rows, k.stat))
+		return CCV_NNC_EXEC_INVALID;
+	if (rmsnorm_fwd(stream_of(stream_context), k, inputs[0]->data.u8, inputs[1]->data.u8, outputs[0]->data.u8, sis ? sis->data.u8 : 0, rows, inner, cmd.info.rmsnorm.epsilon))
 		return CCV_NNC_EXEC_INVALID;
 	return CCV_NNC_EXEC_SUCCESS;
 }
@@ -519,16 +574,19 @@ int ccv_nnc_sm100_exec_rmsnorm_back(SM100_EXEC_ARGS)
 	if (input_size < 6 || output_size < 1 || !inputs[0] || !inputs[2] || !inputs[3] || !inputs[5])
 		return CCV_NNC_EXEC_INVALID;
 	int rows, inner;
-	if (!rows_inner(inputs[2], cmd.info.rmsnorm.axis, cmd.info.rmsnorm.count, rows, inner) || !packed_f32_of(inputs[0], (size_t)rows * inner) || !packed_f32_of(inputs[5], rows) || !packed_f32_of(inputs[3], inner))
+	if (!rows_inner(inputs[2], cmd.info.rmsnorm.axis, cmd.info.rmsnorm.count, rows, inner))
 		return CCV_NNC_EXEC_INVALID;
-	float* h = outputs[0] ? outputs[0]->data.f32 : 0;
-	float* ds = output_size > 1 && outputs[1] ? outputs[1]->data.f32 : 0;
-	if ((h && !packed_f32_of(outputs[0], (size_t)rows * inner)) || (ds && !packed_f32_of(outputs[1], inner)))
+	NormKinds k = { kind_of(inputs[2]), 0, 0, 0, 0, 0 };
+	if (!packed_act(inputs[0], k.x, (size_t)rows * inner) || !packed_stats_of(0, inputs[5], k.x, rows, k.stat) || !packed_param_of(inputs[3], k.x, inner, k.scale))
+		return CCV_NNC_EXEC_INVALID;
+	ccv_nnc_tensor_t* const h = outputs[0];
+	ccv_nnc_tensor_t* const ds = output_size > 1 ? outputs[1] : 0;
+	if ((h && !packed_act(h, k.x, (size_t)rows * inner)) || (ds && !packed_param_of(ds, k.x, inner, k.dscale)))
 		return CCV_NNC_EXEC_INVALID;
 	void* const ws = ds ? ccv_nnc_stream_context_get_workspace(stream_context, norm_bwd_workspace_bytes(rows, inner), CCV_TENSOR_GPU_MEMORY) : 0;
 	if (ds && !ws)
 		return CCV_NNC_EXEC_OOM;
-	if (rmsnorm_bwd_f32(stream_of(stream_context), inputs[0]->data.f32, inputs[2]->data.f32, inputs[3]->data.f32, inputs[5]->data.f32, h, ds, rows, inner, ws))
+	if (rmsnorm_bwd(stream_of(stream_context), k, inputs[0]->data.u8, inputs[2]->data.u8, inputs[3]->data.u8, inputs[5]->data.u8, h ? h->data.u8 : 0, ds ? ds->data.u8 : 0, rows, inner, ws))
 		return CCV_NNC_EXEC_INVALID;
 	return CCV_NNC_EXEC_SUCCESS;
 }

@@ -100,12 +100,17 @@ int convert_dtype(cudaStream_t s, const void* a, int a_dtype, void* b, int b_dty
 int copy_strided(cudaStream_t s, const void* a, const int* astride, void* b, const int* bstride, const int* dim, int elem_size);
 
 // ---- layer norm / rms norm over the last `inner` elements of each of `rows` rows -----------------------------
-int layer_norm_fwd_f32(cudaStream_t s, const float* x, const float* scale, const float* bias, float* y, float* saved_mean, float* saved_inv_std, int rows, int inner, float epsilon);
+// Element kinds of one normalisation call (0 fp32, 1 bf16, 2 fp16): x is the activations' kind (x and y; g, x and h), every other
+// operand is fp32 or that kind; the statistics share one kind.  Absent operands may carry any of the two.
+struct NormKinds {
+	int x, scale, bias, stat, dscale, dbias;
+};
+int layer_norm_fwd(cudaStream_t s, const NormKinds& k, const void* x, const void* scale, const void* bias, void* y, void* saved_mean, void* saved_inv_std, int rows, int inner, float epsilon);
 // the backward's workspace when dscale / dbias are requested: one row of partial column sums per row block
 size_t norm_bwd_workspace_bytes(int rows, int inner);
-int layer_norm_bwd_f32(cudaStream_t s, const float* g, const float* x, const float* scale, const float* saved_mean, const float* saved_inv_std, float* dx, float* dscale, float* dbias, int rows, int inner, void* workspace);
-int rmsnorm_fwd_f32(cudaStream_t s, const float* x, const float* scale, float* y, float* saved_inv_std, int rows, int inner, float epsilon);
-int rmsnorm_bwd_f32(cudaStream_t s, const float* g, const float* x, const float* scale, const float* saved_inv_std, float* dx, float* dscale, int rows, int inner, void* workspace);
+int layer_norm_bwd(cudaStream_t s, const NormKinds& k, const void* g, const void* x, const void* scale, const void* saved_mean, const void* saved_inv_std, void* dx, void* dscale, void* dbias, int rows, int inner, void* workspace);
+int rmsnorm_fwd(cudaStream_t s, const NormKinds& k, const void* x, const void* scale, void* y, void* saved_inv_std, int rows, int inner, float epsilon);
+int rmsnorm_bwd(cudaStream_t s, const NormKinds& k, const void* g, const void* x, const void* scale, const void* saved_inv_std, void* dx, void* dscale, int rows, int inner, void* workspace);
 
 // ---- group norm: <= 4-d index space, statistics / scale / bias tensors with dims dividing it (slot = i * rdim / dim) ----
 struct GroupNormGeom {
@@ -114,9 +119,9 @@ struct GroupNormGeom {
 	int sdim[4];           // scale / bias / dscale / dbias dims (packed)
 	long long xstride[4], ystride[4], hstride[4]; // element strides of x, of y (forward) or g (backward), of h
 };
-int group_norm_fwd_f32(cudaStream_t s, const GroupNormGeom& g, const float* x, const float* scale, const float* bias, float* y, float* saved_mean, float* saved_inv_std, float epsilon);
+int group_norm_fwd(cudaStream_t s, const NormKinds& k, const GroupNormGeom& g, const void* x, const void* scale, const void* bias, void* y, void* saved_mean, void* saved_inv_std, float epsilon);
 size_t group_norm_bwd_workspace_bytes(const GroupNormGeom& g);
-int group_norm_bwd_f32(cudaStream_t s, const GroupNormGeom& g, const float* grad, const float* x, const float* scale, const float* saved_mean, const float* saved_inv_std, float* h, float* dscale, float* dbias, void* workspace);
+int group_norm_bwd(cudaStream_t s, const NormKinds& k, const GroupNormGeom& g, const void* grad, const void* x, const void* scale, const void* saved_mean, const void* saved_inv_std, void* h, void* dscale, void* dbias, void* workspace);
 
 // ---- upsample (NHWC) ------------------------------------------------------------------------------------------
 int upsample_fwd_f32(cudaStream_t s, const float* a, float* b, int N, int H, int W, int C, int OH, int OW, int type, int align_corners, int nchw);

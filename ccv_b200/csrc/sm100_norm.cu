@@ -3,7 +3,9 @@
 // upsample/ccv_nnc_upsample_cpu_ref.c:16-509 (paths relative to /root/reference/lib/nnc/cmd).
 #include "sm100_ew.h"
 #include "sm100_contract.h"
+#include "sm100_elem.cuh"
 #include <float.h>
+#include <type_traits>
 
 namespace sm100 {
 
@@ -39,89 +41,243 @@ __device__ __forceinline__ float bsum(float v, float* sh)
 }
 static int row_threads(int inner) { return inner >= 2048 ? 512 : (inner >= 512 ? 256 : (inner >= 128 ? 128 : (inner >= 64 ? 64 : 32))); }
 
-// one block per row: mean, biased variance of (x - mean) (two passes over a row that sits in L1/L2), y = xhat * scale + bias
-template <int RMS>
-__global__ void norm_fwd_kernel(const float* __restrict__ x, const float* __restrict__ scale, const float* __restrict__ bias, float* __restrict__ y, float* __restrict__ saved_mean, float* __restrict__ saved_inv_std, const int inner, const float epsilon)
+// Element types.  The activations (x, y / g, x, dx) are TX: float, __nv_bfloat16 or __half.  Every other operand has its own type,
+// float or TX: TP scale, TB bias, TS both statistics, TDS dscale, TDB dbias.  16-bit values are widened exactly, all arithmetic is
+// fp32 in the order of the fp32 kernels, and every output is rounded to its type once (round to nearest even, stf / stv).
+//
+// Rows of a 16-bit TX take 16-byte accesses (8 elements) when inner % 8 == 0 and every row operand is 16-byte aligned; every other
+// row, and every fp32 row, takes single-element accesses.  The choice is the same for every row of a call and for a single row.
+template <typename TX>
+__device__ __forceinline__ bool row_vec(const int inner, const void* a, const void* b, const void* c, const void* d)
+{
+	return sizeof(TX) == 2 && inner % 8 == 0 && ((((uintptr_t)a) | ((uintptr_t)b) | ((uintptr_t)c) | ((uintptr_t)d)) & 15) == 0;
+}
+// 8 consecutive elements: one 16-byte access of a 16-bit type, two of fp32
+__device__ __forceinline__ void ld8(const float* p, float (&v)[8])
+{
+	float a[4], b[4];
+	ldv(p, a), ldv(p + 4, b);
+#pragma unroll
+	for (int k = 0; k < 4; k++)
+		v[k] = a[k], v[4 + k] = b[k];
+}
+__device__ __forceinline__ void ld8(const __nv_bfloat16* p, float (&v)[8]) { ldv(p, v); }
+__device__ __forceinline__ void ld8(const __half* p, float (&v)[8]) { ldv(p, v); }
+__device__ __forceinline__ void st8(float* p, const float (&v)[8])
+{
+	const float a[4] = { v[0], v[1], v[2], v[3] }, b[4] = { v[4], v[5], v[6], v[7] };
+	stv(p, a), stv(p + 4, b);
+}
+__device__ __forceinline__ void st8(__nv_bfloat16* p, const float (&v)[8]) { stv(p, v); }
+__device__ __forceinline__ void st8(__half* p, const float (&v)[8]) { stv(p, v); }
+// the value v has once stored as T and read back (v itself for fp32)
+template <typename T>
+__device__ __forceinline__ float stored(const float v)
+{
+	T t;
+	stf(&t, v);
+	return ldf(&t);
+}
+
+// one block per row: mean, biased variance of (x - mean) (two passes over a row that sits in L1/L2), y = xhat * scale + bias.
+// y is computed from the statistics as stored (rounded to TS when they are 16-bit), which is what the backward reads.
+template <int RMS, typename TX, typename TP, typename TB, typename TS>
+__global__ void norm_fwd_kernel(const TX* __restrict__ x, const TP* __restrict__ scale, const TB* __restrict__ bias, TX* __restrict__ y, TS* __restrict__ saved_mean, TS* __restrict__ saved_inv_std, const int inner, const float epsilon)
 {
 	__shared__ float sh[32];
-	const float* xp = x + (size_t)blockIdx.x * inner;
-	float* yp = y + (size_t)blockIdx.x * inner;
+	const TX* xp = x + (size_t)blockIdx.x * inner;
+	TX* yp = y + (size_t)blockIdx.x * inner;
+	const bool vec = row_vec<TX>(inner, x, y, scale, bias);
 	float mean = 0.f;
 	if (!RMS)
 	{
 		float s = 0.f;
-		for (int j = threadIdx.x; j < inner; j += blockDim.x)
-			s += xp[j];
+		if (vec)
+			for (int j = 8 * threadIdx.x; j < inner; j += 8 * blockDim.x)
+			{
+				float xv[8];
+				ld8(xp + j, xv);
+#pragma unroll
+				for (int k = 0; k < 8; k++)
+					s += xv[k];
+			}
+		else
+			for (int j = threadIdx.x; j < inner; j += blockDim.x)
+				s += ldf(xp + j);
 		mean = bsum(s, sh) * (1.f / inner);
 	}
 	float v = 0.f;
-	for (int j = threadIdx.x; j < inner; j += blockDim.x)
-	{
-		const float d = xp[j] - mean;
-		v += d * d;
-	}
+	if (vec)
+		for (int j = 8 * threadIdx.x; j < inner; j += 8 * blockDim.x)
+		{
+			float xv[8];
+			ld8(xp + j, xv);
+#pragma unroll
+			for (int k = 0; k < 8; k++)
+			{
+				const float d = xv[k] - mean;
+				v += d * d;
+			}
+		}
+	else
+		for (int j = threadIdx.x; j < inner; j += blockDim.x)
+		{
+			const float d = ldf(xp + j) - mean;
+			v += d * d;
+		}
 	v = bsum(v, sh);
 	const float inv_std = 1.f / sqrtf(v * (1.f / inner) + epsilon);
 	if (threadIdx.x == 0)
 	{
 		if (!RMS && saved_mean)
-			saved_mean[blockIdx.x] = mean;
+			stf(saved_mean + blockIdx.x, mean);
 		if (saved_inv_std)
-			saved_inv_std[blockIdx.x] = inv_std;
+			stf(saved_inv_std + blockIdx.x, inv_std);
 	}
-	for (int j = threadIdx.x; j < inner; j += blockDim.x)
-	{
-		float o = (xp[j] - mean) * inv_std;
-		if (scale)
-			o *= scale[j];
-		if (bias)
-			o += bias[j];
-		yp[j] = o;
-	}
+	const float ym = saved_mean ? stored<TS>(mean) : mean, yr = saved_inv_std ? stored<TS>(inv_std) : inv_std;
+	if (vec)
+		for (int j = 8 * threadIdx.x; j < inner; j += 8 * blockDim.x)
+		{
+			float o[8], sc[8], b[8];
+			ld8(xp + j, o);
+			if (scale)
+				ld8(scale + j, sc);
+			if (bias)
+				ld8(bias + j, b);
+#pragma unroll
+			for (int k = 0; k < 8; k++)
+			{
+				o[k] = (o[k] - ym) * yr;
+				if (scale)
+					o[k] *= sc[k];
+				if (bias)
+					o[k] += b[k];
+			}
+			st8(yp + j, o);
+		}
+	else
+		for (int j = threadIdx.x; j < inner; j += blockDim.x)
+		{
+			float o = (ldf(xp + j) - ym) * yr;
+			if (scale)
+				o *= ldf(scale + j);
+			if (bias)
+				o += ldf(bias + j);
+			stf(yp + j, o);
+		}
 }
-int layer_norm_fwd_f32(cudaStream_t s, const float* x, const float* scale, const float* bias, float* y, float* saved_mean, float* saved_inv_std, int rows, int inner, float epsilon)
+
+// calls f with a null pointer whose element type is that of `kind` (0 fp32, 1 bf16, 2 fp16: ElemKind)
+template <typename F>
+static int with_kind(const int kind, F&& f)
+{
+	return kind == 1 ? f((__nv_bfloat16*)0) : kind == 2 ? f((__half*)0) : f((float*)0);
+}
+// the same for an operand that is either fp32 (kind 0) or of the activations' type TX
+template <typename TX, typename F>
+static int with_kind_of(const int kind, F&& f)
+{
+	return kind ? f((TX*)0) : f((float*)0);
+}
+template <typename P> using elem_t = typename std::remove_pointer<P>::type;
+
+template <int RMS, typename TX, typename TP, typename TB, typename TS>
+static int norm_fwd(cudaStream_t s, const void* x, const void* scale, const void* bias, void* y, void* saved_mean, void* saved_inv_std, int rows, int inner, float epsilon)
+{
+	norm_fwd_kernel<RMS, TX, TP, TB, TS><<<rows, row_threads(inner), 0, s>>>((const TX*)x, (const TP*)scale, (const TB*)bias, (TX*)y, (TS*)saved_mean, (TS*)saved_inv_std, inner, epsilon);
+	return check(RMS ? "rmsnorm_fwd" : "layer_norm_fwd");
+}
+int layer_norm_fwd(cudaStream_t s, const NormKinds& k, const void* x, const void* scale, const void* bias, void* y, void* saved_mean, void* saved_inv_std, int rows, int inner, float epsilon)
 {
 	if (rows <= 0 || inner <= 0)
 		return 0;
-	norm_fwd_kernel<0><<<rows, row_threads(inner), 0, s>>>(x, scale, bias, y, saved_mean, saved_inv_std, inner, epsilon);
-	return check("layer_norm_fwd");
+	return with_kind(k.x, [&](auto tx) {
+		using TX = elem_t<decltype(tx)>;
+		return with_kind_of<TX>(k.scale, [&](auto tp) {
+			return with_kind_of<TX>(k.bias, [&](auto tb) {
+				return with_kind_of<TX>(k.stat, [&](auto ts) {
+					return norm_fwd<0, TX, elem_t<decltype(tp)>, elem_t<decltype(tb)>, elem_t<decltype(ts)> >(s, x, scale, bias, y, saved_mean, saved_inv_std, rows, inner, epsilon);
+				});
+			});
+		});
+	});
 }
-int rmsnorm_fwd_f32(cudaStream_t s, const float* x, const float* scale, float* y, float* saved_inv_std, int rows, int inner, float epsilon)
+int rmsnorm_fwd(cudaStream_t s, const NormKinds& k, const void* x, const void* scale, void* y, void* saved_inv_std, int rows, int inner, float epsilon)
 {
 	if (rows <= 0 || inner <= 0)
 		return 0;
-	norm_fwd_kernel<1><<<rows, row_threads(inner), 0, s>>>(x, scale, 0, y, 0, saved_inv_std, inner, epsilon);
-	return check("rmsnorm_fwd");
+	return with_kind(k.x, [&](auto tx) {
+		using TX = elem_t<decltype(tx)>;
+		return with_kind_of<TX>(k.scale, [&](auto tp) {
+			return with_kind_of<TX>(k.stat, [&](auto ts) {
+				return norm_fwd<1, TX, elem_t<decltype(tp)>, float, elem_t<decltype(ts)> >(s, x, scale, 0, y, 0, saved_inv_std, rows, inner, epsilon);
+			});
+		});
+	});
 }
 // dx per row.  layer norm: r * (gs - mean(gs) - xhat * mean(gs * xhat)); rms norm: r * (gs - xhat * mean(gs * xhat)), gs = g * scale
-template <int RMS>
-__global__ void norm_bwd_dx_kernel(const float* __restrict__ g, const float* __restrict__ x, const float* __restrict__ scale, const float* __restrict__ saved_mean, const float* __restrict__ saved_inv_std, float* __restrict__ dx, const int inner)
+template <int RMS, typename TX, typename TP, typename TS>
+__global__ void norm_bwd_dx_kernel(const TX* __restrict__ g, const TX* __restrict__ x, const TP* __restrict__ scale, const TS* __restrict__ saved_mean, const TS* __restrict__ saved_inv_std, TX* __restrict__ dx, const int inner)
 {
 	__shared__ float sh[32];
 	const size_t o = (size_t)blockIdx.x * inner;
-	const float mean = RMS ? 0.f : saved_mean[blockIdx.x], r = saved_inv_std[blockIdx.x];
+	const float mean = RMS ? 0.f : ldf(saved_mean + blockIdx.x), r = ldf(saved_inv_std + blockIdx.x);
+	const bool vec = row_vec<TX>(inner, g, x, scale, dx);
 	float s1 = 0.f, s2 = 0.f;
-	for (int j = threadIdx.x; j < inner; j += blockDim.x)
-	{
-		const float gs = g[o + j] * (scale ? scale[j] : 1.f);
-		s1 += gs;
-		s2 += gs * (x[o + j] - mean) * r;
-	}
+	if (vec)
+		for (int j = 8 * threadIdx.x; j < inner; j += 8 * blockDim.x)
+		{
+			float gv[8], xv[8], sc[8];
+			ld8(g + o + j, gv), ld8(x + o + j, xv);
+			if (scale)
+				ld8(scale + j, sc);
+#pragma unroll
+			for (int k = 0; k < 8; k++)
+			{
+				const float gs = gv[k] * (scale ? sc[k] : 1.f);
+				s1 += gs;
+				s2 += gs * (xv[k] - mean) * r;
+			}
+		}
+	else
+		for (int j = threadIdx.x; j < inner; j += blockDim.x)
+		{
+			const float gs = ldf(g + o + j) * (scale ? ldf(scale + j) : 1.f);
+			s1 += gs;
+			s2 += gs * (ldf(x + o + j) - mean) * r;
+		}
 	s1 = RMS ? 0.f : bsum(s1, sh) * (1.f / inner);
 	s2 = bsum(s2, sh) * (1.f / inner);
-	for (int j = threadIdx.x; j < inner; j += blockDim.x)
-	{
-		const float gs = g[o + j] * (scale ? scale[j] : 1.f);
-		dx[o + j] = r * (gs - s1 - (x[o + j] - mean) * r * s2);
-	}
+	if (vec)
+		for (int j = 8 * threadIdx.x; j < inner; j += 8 * blockDim.x)
+		{
+			float gv[8], xv[8], sc[8];
+			ld8(g + o + j, gv), ld8(x + o + j, xv);
+			if (scale)
+				ld8(scale + j, sc);
+#pragma unroll
+			for (int k = 0; k < 8; k++)
+			{
+				const float gs = gv[k] * (scale ? sc[k] : 1.f);
+				gv[k] = r * (gs - s1 - (xv[k] - mean) * r * s2);
+			}
+			st8(dx + o + j, gv);
+		}
+	else
+		for (int j = threadIdx.x; j < inner; j += blockDim.x)
+		{
+			const float gs = ldf(g + o + j) * (scale ? ldf(scale + j) : 1.f);
+			const float d = r * (gs - s1 - (ldf(x + o + j) - mean) * r * s2);
+			stf(dx + o + j, d);
+		}
 }
 // dscale[j] = sum_rows g * xhat, dbias[j] = sum_rows g.  Row block y (rows y, y + gridDim.y, ..) leaves its two partial sums of column j
-// in part[y][j] and part[y][inner + j]; norm_bwd_dparam_rows_kernel then adds the gridDim.y rows in a fixed order, so the result does
-// not depend on the order in which blocks finish (one atomicAdd per (block, column) did).
+// in part[y][j] and part[y][inner + j] (fp32 whatever the operands' types); norm_bwd_dparam_rows_kernel then adds the gridDim.y rows in a
+// fixed order and rounds once, so the result does not depend on the order in which blocks finish (one atomicAdd per (block, column) did).
 static int dparam_row_blocks(int rows) { return rows < 296 ? rows : 296; }
 size_t norm_bwd_workspace_bytes(int rows, int inner) { return rows <= 0 || inner <= 0 ? 0 : (size_t)dparam_row_blocks(rows) * 2 * (size_t)inner * sizeof(float); }
-template <int RMS>
-__global__ void norm_bwd_dparam_kernel(const float* __restrict__ g, const float* __restrict__ x, const float* __restrict__ saved_mean, const float* __restrict__ saved_inv_std, float* __restrict__ part, const int rows, const int inner)
+template <int RMS, typename TX, typename TS>
+__global__ void norm_bwd_dparam_kernel(const TX* __restrict__ g, const TX* __restrict__ x, const TS* __restrict__ saved_mean, const TS* __restrict__ saved_inv_std, float* __restrict__ part, const int rows, const int inner)
 {
 	const int j = blockIdx.x * blockDim.x + threadIdx.x;
 	if (j >= inner)
@@ -129,8 +285,8 @@ __global__ void norm_bwd_dparam_kernel(const float* __restrict__ g, const float*
 	float a = 0.f, b = 0.f;
 	for (int r = blockIdx.y; r < rows; r += gridDim.y)
 	{
-		const float gv = g[(size_t)r * inner + j];
-		a += gv * (x[(size_t)r * inner + j] - (RMS ? 0.f : saved_mean[r])) * saved_inv_std[r];
+		const float gv = ldf(g + (size_t)r * inner + j);
+		a += gv * (ldf(x + (size_t)r * inner + j) - (RMS ? 0.f : ldf(saved_mean + r))) * ldf(saved_inv_std + r);
 		b += gv;
 	}
 	float* const row = part + (size_t)blockIdx.y * 2 * inner;
@@ -139,7 +295,8 @@ __global__ void norm_bwd_dparam_kernel(const float* __restrict__ g, const float*
 		row[inner + j] = b;
 }
 // 32 columns x 32 row-lanes per block: lane l adds rows l, l + 32, .. in order, then the 32 lane sums are added in order
-__global__ void __launch_bounds__(1024) norm_bwd_dparam_rows_kernel(const float* __restrict__ part, const int gy, const int inner, float* __restrict__ dscale, float* __restrict__ dbias)
+template <typename TDS, typename TDB>
+__global__ void __launch_bounds__(1024) norm_bwd_dparam_rows_kernel(const float* __restrict__ part, const int gy, const int inner, TDS* __restrict__ dscale, TDB* __restrict__ dbias)
 {
 	__shared__ float sh[2][32][33];
 	const int cx = threadIdx.x & 31, yl = threadIdx.x >> 5;
@@ -163,42 +320,58 @@ __global__ void __launch_bounds__(1024) norm_bwd_dparam_rows_kernel(const float*
 	for (int l = 0; l < 32; l++)
 		a += sh[0][l][cx], b += sh[1][l][cx];
 	if (dscale)
-		dscale[j] = a;
+		stf(dscale + j, a);
 	if (dbias)
-		dbias[j] = b;
+		stf(dbias + j, b);
 }
-template <int RMS>
-static int norm_bwd(cudaStream_t s, const float* g, const float* x, const float* scale, const float* saved_mean, const float* saved_inv_std, float* dx, float* dscale, float* dbias, int rows, int inner, void* workspace)
+template <int RMS, typename TX, typename TP, typename TS, typename TDS, typename TDB>
+static int norm_bwd(cudaStream_t s, const void* g, const void* x, const void* scale, const void* saved_mean, const void* saved_inv_std, void* dx, void* dscale, void* dbias, int rows, int inner, void* workspace)
 {
-	if (rows <= 0 || inner <= 0)
-		return 0;
-	if ((dscale || dbias) && !workspace)
-		return -1;
 	if (dx)
 	{
-		norm_bwd_dx_kernel<RMS><<<rows, row_threads(inner), 0, s>>>(g, x, scale, saved_mean, saved_inv_std, dx, inner);
+		norm_bwd_dx_kernel<RMS, TX, TP, TS><<<rows, row_threads(inner), 0, s>>>((const TX*)g, (const TX*)x, (const TP*)scale, (const TS*)saved_mean, (const TS*)saved_inv_std, (TX*)dx, inner);
 		if (check("norm_bwd_dx"))
 			return -1;
 	}
 	if (dscale || dbias)
 	{
 		const int gy = dparam_row_blocks(rows);
-		norm_bwd_dparam_kernel<RMS><<<dim3((inner + 127) / 128, gy), 128, 0, s>>>(g, x, saved_mean, saved_inv_std, (float*)workspace, rows, inner);
+		norm_bwd_dparam_kernel<RMS, TX, TS><<<dim3((inner + 127) / 128, gy), 128, 0, s>>>((const TX*)g, (const TX*)x, (const TS*)saved_mean, (const TS*)saved_inv_std, (float*)workspace, rows, inner);
 		if (check("norm_bwd_dparam"))
 			return -1;
-		norm_bwd_dparam_rows_kernel<<<(inner + 31) / 32, 1024, 0, s>>>((const float*)workspace, gy, inner, dscale, dbias);
+		norm_bwd_dparam_rows_kernel<TDS, TDB><<<(inner + 31) / 32, 1024, 0, s>>>((const float*)workspace, gy, inner, (TDS*)dscale, (TDB*)dbias);
 		if (check("norm_bwd_dparam_rows"))
 			return -1;
 	}
 	return 0;
 }
-int layer_norm_bwd_f32(cudaStream_t s, const float* g, const float* x, const float* scale, const float* saved_mean, const float* saved_inv_std, float* dx, float* dscale, float* dbias, int rows, int inner, void* workspace)
+template <int RMS>
+static int norm_bwd_any(cudaStream_t s, const NormKinds& k, const void* g, const void* x, const void* scale, const void* saved_mean, const void* saved_inv_std, void* dx, void* dscale, void* dbias, int rows, int inner, void* workspace)
 {
-	return norm_bwd<0>(s, g, x, scale, saved_mean, saved_inv_std, dx, dscale, dbias, rows, inner, workspace);
+	if (rows <= 0 || inner <= 0)
+		return 0;
+	if ((dscale || dbias) && !workspace)
+		return -1;
+	return with_kind(k.x, [&](auto tx) {
+		using TX = elem_t<decltype(tx)>;
+		return with_kind_of<TX>(k.scale, [&](auto tp) {
+			return with_kind_of<TX>(k.stat, [&](auto ts) {
+				return with_kind_of<TX>(k.dscale, [&](auto tds) {
+					return with_kind_of<TX>(RMS ? 0 : k.dbias, [&](auto tdb) {
+						return norm_bwd<RMS, TX, elem_t<decltype(tp)>, elem_t<decltype(ts)>, elem_t<decltype(tds)>, elem_t<decltype(tdb)> >(s, g, x, scale, saved_mean, saved_inv_std, dx, dscale, dbias, rows, inner, workspace);
+					});
+				});
+			});
+		});
+	});
 }
-int rmsnorm_bwd_f32(cudaStream_t s, const float* g, const float* x, const float* scale, const float* saved_inv_std, float* dx, float* dscale, int rows, int inner, void* workspace)
+int layer_norm_bwd(cudaStream_t s, const NormKinds& k, const void* g, const void* x, const void* scale, const void* saved_mean, const void* saved_inv_std, void* dx, void* dscale, void* dbias, int rows, int inner, void* workspace)
 {
-	return norm_bwd<1>(s, g, x, scale, 0, saved_inv_std, dx, dscale, 0, rows, inner, workspace);
+	return norm_bwd_any<0>(s, k, g, x, scale, saved_mean, saved_inv_std, dx, dscale, dbias, rows, inner, workspace);
+}
+int rmsnorm_bwd(cudaStream_t s, const NormKinds& k, const void* g, const void* x, const void* scale, const void* saved_inv_std, void* dx, void* dscale, int rows, int inner, void* workspace)
+{
+	return norm_bwd_any<1>(s, k, g, x, scale, 0, saved_inv_std, dx, dscale, 0, rows, inner, workspace);
 }
 
 // ------------------------------------------------------------------------------------------------ upsample
@@ -345,7 +518,9 @@ __device__ __forceinline__ long long gn_slot(const GroupNormGeom& g, const int c
 
 __device__ __forceinline__ float gn_block_sum(float v, float* const red) { return bsum(v, red); }
 
-__global__ void gn_stats_kernel(const GroupNormGeom g, const float* __restrict__ x, float* __restrict__ saved_mean, float* __restrict__ saved_inv_std, const float epsilon)
+// element types as for the row norms: TX x / y / grad / h, TP scale, TB bias, TS statistics, TDS dscale, TDB dbias
+template <typename TX, typename TS>
+__global__ void gn_stats_kernel(const GroupNormGeom g, const TX* __restrict__ x, TS* __restrict__ saved_mean, TS* __restrict__ saved_inv_std, const float epsilon)
 {
 	__shared__ float red[32];
 	const GnBox b = gn_box(g, g.rdim, blockIdx.x);
@@ -354,7 +529,7 @@ __global__ void gn_stats_kernel(const GroupNormGeom g, const float* __restrict__
 	for (long long i = threadIdx.x; i < b.count; i += blockDim.x)
 	{
 		gn_coord(b, i, c);
-		sum += x[gn_offset(c, g.xstride)];
+		sum += ldf(x + gn_offset(c, g.xstride));
 	}
 	const float inv_n = 1.f / (float)b.count;
 	const float mean = gn_block_sum(sum, red) * inv_n;
@@ -362,18 +537,20 @@ __global__ void gn_stats_kernel(const GroupNormGeom g, const float* __restrict__
 	for (long long i = threadIdx.x; i < b.count; i += blockDim.x)
 	{
 		gn_coord(b, i, c);
-		const float w = x[gn_offset(c, g.xstride)] - mean;
+		const float w = ldf(x + gn_offset(c, g.xstride)) - mean;
 		sq += w * w;
 	}
 	const float var = gn_block_sum(sq, red) * inv_n;
 	if (threadIdx.x == 0)
 	{
-		saved_mean[blockIdx.x] = mean;
-		saved_inv_std[blockIdx.x] = 1.f / sqrtf(var + epsilon);
+		stf(saved_mean + blockIdx.x, mean);
+		stf(saved_inv_std + blockIdx.x, 1.f / sqrtf(var + epsilon));
 	}
 }
 
-__global__ void gn_apply_kernel(const GroupNormGeom g, const float* __restrict__ x, const float* __restrict__ scale, const float* __restrict__ bias, const float* __restrict__ saved_mean, const float* __restrict__ saved_inv_std, float* __restrict__ y, const long long total)
+// y from the statistics as stored (what the backward reads)
+template <typename TX, typename TP, typename TB, typename TS>
+__global__ void gn_apply_kernel(const GroupNormGeom g, const TX* __restrict__ x, const TP* __restrict__ scale, const TB* __restrict__ bias, const TS* __restrict__ saved_mean, const TS* __restrict__ saved_inv_std, TX* __restrict__ y, const long long total)
 {
 	GnBox all;
 	for (int d = 0; d < 4; d++)
@@ -383,28 +560,29 @@ __global__ void gn_apply_kernel(const GroupNormGeom g, const float* __restrict__
 	{
 		gn_coord(all, i, c);
 		const long long r = gn_slot(g, c, g.rdim);
-		float v = (x[gn_offset(c, g.xstride)] - saved_mean[r]) * saved_inv_std[r];
+		float v = (ldf(x + gn_offset(c, g.xstride)) - ldf(saved_mean + r)) * ldf(saved_inv_std + r);
 		if (scale)
-			v = v * scale[gn_slot(g, c, g.sdim)] + bias[gn_slot(g, c, g.sdim)];
-		y[gn_offset(c, g.ystride)] = v;
+			v = v * ldf(scale + gn_slot(g, c, g.sdim)) + ldf(bias + gn_slot(g, c, g.sdim));
+		stf(y + gn_offset(c, g.ystride), v);
 	}
 }
 
 // per statistic slot: gssr = sum g * scale * inv_std, ahgssr = sum xhat * g * scale * inv_std (:412-470)
-__global__ void gn_bwd_stats_kernel(const GroupNormGeom g, const float* __restrict__ grad, const float* __restrict__ x, const float* __restrict__ scale, const float* __restrict__ saved_mean, const float* __restrict__ saved_inv_std, float* __restrict__ sums)
+template <typename TX, typename TP, typename TS>
+__global__ void gn_bwd_stats_kernel(const GroupNormGeom g, const TX* __restrict__ grad, const TX* __restrict__ x, const TP* __restrict__ scale, const TS* __restrict__ saved_mean, const TS* __restrict__ saved_inv_std, float* __restrict__ sums)
 {
 	__shared__ float red[32];
 	const GnBox b = gn_box(g, g.rdim, blockIdx.x);
-	const float mean = saved_mean[blockIdx.x], inv_std = saved_inv_std[blockIdx.x];
+	const float mean = ldf(saved_mean + blockIdx.x), inv_std = ldf(saved_inv_std + blockIdx.x);
 	int c[4];
 	float s0 = 0, s1 = 0;
 	for (long long i = threadIdx.x; i < b.count; i += blockDim.x)
 	{
 		gn_coord(b, i, c);
-		const float ah = (x[gn_offset(c, g.xstride)] - mean) * inv_std;
-		float gss = grad[gn_offset(c, g.ystride)] * inv_std;
+		const float ah = (ldf(x + gn_offset(c, g.xstride)) - mean) * inv_std;
+		float gss = ldf(grad + gn_offset(c, g.ystride)) * inv_std;
 		if (scale)
-			gss *= scale[gn_slot(g, c, g.sdim)];
+			gss *= ldf(scale + gn_slot(g, c, g.sdim));
 		s0 += gss, s1 += ah * gss;
 	}
 	s0 = gn_block_sum(s0, red), s1 = gn_block_sum(s1, red);
@@ -413,7 +591,8 @@ __global__ void gn_bwd_stats_kernel(const GroupNormGeom g, const float* __restri
 }
 
 // h = gss - (gssr + xhat * ahgssr) / n (:472-500)
-__global__ void gn_bwd_apply_kernel(const GroupNormGeom g, const float* __restrict__ grad, const float* __restrict__ x, const float* __restrict__ scale, const float* __restrict__ saved_mean, const float* __restrict__ saved_inv_std, const float* __restrict__ sums, float* __restrict__ h, const long long total, const float inv_n)
+template <typename TX, typename TP, typename TS>
+__global__ void gn_bwd_apply_kernel(const GroupNormGeom g, const TX* __restrict__ grad, const TX* __restrict__ x, const TP* __restrict__ scale, const TS* __restrict__ saved_mean, const TS* __restrict__ saved_inv_std, const float* __restrict__ sums, TX* __restrict__ h, const long long total, const float inv_n)
 {
 	GnBox all;
 	for (int d = 0; d < 4; d++)
@@ -423,17 +602,18 @@ __global__ void gn_bwd_apply_kernel(const GroupNormGeom g, const float* __restri
 	{
 		gn_coord(all, i, c);
 		const long long r = gn_slot(g, c, g.rdim);
-		const float inv_std = saved_inv_std[r];
-		const float ah = (x[gn_offset(c, g.xstride)] - saved_mean[r]) * inv_std;
-		float gss = grad[gn_offset(c, g.ystride)] * inv_std;
+		const float inv_std = ldf(saved_inv_std + r);
+		const float ah = (ldf(x + gn_offset(c, g.xstride)) - ldf(saved_mean + r)) * inv_std;
+		float gss = ldf(grad + gn_offset(c, g.ystride)) * inv_std;
 		if (scale)
-			gss *= scale[gn_slot(g, c, g.sdim)];
-		h[gn_offset(c, g.hstride)] = gss - (sums[2 * r] + ah * sums[2 * r + 1]) * inv_n;
+			gss *= ldf(scale + gn_slot(g, c, g.sdim));
+		stf(h + gn_offset(c, g.hstride), gss - (sums[2 * r] + ah * sums[2 * r + 1]) * inv_n);
 	}
 }
 
-// per scale / bias slot: dscale = sum xhat * g, dbias = sum g (:322-345, :254)
-__global__ void gn_bwd_dparam_kernel(const GroupNormGeom g, const float* __restrict__ grad, const float* __restrict__ x, const float* __restrict__ saved_mean, const float* __restrict__ saved_inv_std, float* __restrict__ dscale, float* __restrict__ dbias)
+// per scale / bias slot: dscale = sum xhat * g, dbias = sum g (:322-345, :254); fp32 sums in a fixed order, rounded once
+template <typename TX, typename TS, typename TDS, typename TDB>
+__global__ void gn_bwd_dparam_kernel(const GroupNormGeom g, const TX* __restrict__ grad, const TX* __restrict__ x, const TS* __restrict__ saved_mean, const TS* __restrict__ saved_inv_std, TDS* __restrict__ dscale, TDB* __restrict__ dbias)
 {
 	__shared__ float red[32];
 	const GnBox b = gn_box(g, g.sdim, blockIdx.x);
@@ -443,63 +623,95 @@ __global__ void gn_bwd_dparam_kernel(const GroupNormGeom g, const float* __restr
 	{
 		gn_coord(b, i, c);
 		const long long r = gn_slot(g, c, g.rdim);
-		const float gv = grad[gn_offset(c, g.ystride)];
-		s0 += (x[gn_offset(c, g.xstride)] - saved_mean[r]) * saved_inv_std[r] * gv;
+		const float gv = ldf(grad + gn_offset(c, g.ystride));
+		s0 += (ldf(x + gn_offset(c, g.xstride)) - ldf(saved_mean + r)) * ldf(saved_inv_std + r) * gv;
 		s1 += gv;
 	}
 	s0 = gn_block_sum(s0, red), s1 = gn_block_sum(s1, red);
 	if (threadIdx.x == 0)
 	{
 		if (dscale)
-			dscale[blockIdx.x] = s0;
+			stf(dscale + blockIdx.x, s0);
 		if (dbias)
-			dbias[blockIdx.x] = s1;
+			stf(dbias + blockIdx.x, s1);
 	}
 }
 
 static long long gn_count(const int* d) { return (long long)d[0] * d[1] * d[2] * d[3]; }
 
-int group_norm_fwd_f32(cudaStream_t s, const GroupNormGeom& g, const float* x, const float* scale, const float* bias, float* y, float* saved_mean, float* saved_inv_std, float epsilon)
+template <typename TX, typename TP, typename TB, typename TS>
+static int gn_fwd(cudaStream_t s, const GroupNormGeom& g, const void* x, const void* scale, const void* bias, void* y, void* saved_mean, void* saved_inv_std, float epsilon, long long total, long long slots)
 {
-	const long long total = gn_count(g.dim), slots = gn_count(g.rdim);
-	if (total == 0)
-		return 0;
-	gn_stats_kernel<<<(unsigned)slots, 512, 0, s>>>(g, x, saved_mean, saved_inv_std, epsilon);
+	gn_stats_kernel<TX, TS><<<(unsigned)slots, 512, 0, s>>>(g, (const TX*)x, (TS*)saved_mean, (TS*)saved_inv_std, epsilon);
 	count_launch();
 	long long blocks = (total + 255) / 256;
 	if (blocks > 132 * 16)
 		blocks = 132 * 16;
-	gn_apply_kernel<<<(unsigned)blocks, 256, 0, s>>>(g, x, scale, bias, saved_mean, saved_inv_std, y, total);
+	gn_apply_kernel<TX, TP, TB, TS><<<(unsigned)blocks, 256, 0, s>>>(g, (const TX*)x, (const TP*)scale, (const TB*)bias, (const TS*)saved_mean, (const TS*)saved_inv_std, (TX*)y, total);
 	return check("group_norm_fwd");
 }
 
-size_t group_norm_bwd_workspace_bytes(const GroupNormGeom& g) { return (size_t)gn_count(g.rdim) * 2 * sizeof(float); }
-
-int group_norm_bwd_f32(cudaStream_t s, const GroupNormGeom& g, const float* grad, const float* x, const float* scale, const float* saved_mean, const float* saved_inv_std, float* h, float* dscale, float* dbias, void* workspace)
+int group_norm_fwd(cudaStream_t s, const NormKinds& k, const GroupNormGeom& g, const void* x, const void* scale, const void* bias, void* y, void* saved_mean, void* saved_inv_std, float epsilon)
 {
 	const long long total = gn_count(g.dim), slots = gn_count(g.rdim);
 	if (total == 0)
 		return 0;
+	return with_kind(k.x, [&](auto tx) {
+		using TX = elem_t<decltype(tx)>;
+		return with_kind_of<TX>(k.scale, [&](auto tp) {
+			return with_kind_of<TX>(k.bias, [&](auto tb) {
+				return with_kind_of<TX>(k.stat, [&](auto ts) {
+					return gn_fwd<TX, elem_t<decltype(tp)>, elem_t<decltype(tb)>, elem_t<decltype(ts)> >(s, g, x, scale, bias, y, saved_mean, saved_inv_std, epsilon, total, slots);
+				});
+			});
+		});
+	});
+}
+
+size_t group_norm_bwd_workspace_bytes(const GroupNormGeom& g) { return (size_t)gn_count(g.rdim) * 2 * sizeof(float); }
+
+template <typename TX, typename TP, typename TS, typename TDS, typename TDB>
+static int gn_bwd(cudaStream_t s, const GroupNormGeom& g, const void* grad, const void* x, const void* scale, const void* saved_mean, const void* saved_inv_std, void* h, void* dscale, void* dbias, void* workspace, long long total, long long slots)
+{
 	if (h)
 	{
 		float* const sums = (float*)workspace;
-		gn_bwd_stats_kernel<<<(unsigned)slots, 512, 0, s>>>(g, grad, x, scale, saved_mean, saved_inv_std, sums);
+		gn_bwd_stats_kernel<TX, TP, TS><<<(unsigned)slots, 512, 0, s>>>(g, (const TX*)grad, (const TX*)x, (const TP*)scale, (const TS*)saved_mean, (const TS*)saved_inv_std, sums);
 		if (check("group_norm_bwd_stats"))
 			return -1;
 		long long blocks = (total + 255) / 256;
 		if (blocks > 132 * 16)
 			blocks = 132 * 16;
-		gn_bwd_apply_kernel<<<(unsigned)blocks, 256, 0, s>>>(g, grad, x, scale, saved_mean, saved_inv_std, sums, h, total, (float)slots / (float)total);
+		gn_bwd_apply_kernel<TX, TP, TS><<<(unsigned)blocks, 256, 0, s>>>(g, (const TX*)grad, (const TX*)x, (const TP*)scale, (const TS*)saved_mean, (const TS*)saved_inv_std, sums, (TX*)h, total, (float)slots / (float)total);
 		if (check("group_norm_bwd_apply"))
 			return -1;
 	}
 	if (dscale || dbias)
 	{
-		gn_bwd_dparam_kernel<<<(unsigned)gn_count(g.sdim), 256, 0, s>>>(g, grad, x, saved_mean, saved_inv_std, dscale, dbias);
+		gn_bwd_dparam_kernel<TX, TS, TDS, TDB><<<(unsigned)gn_count(g.sdim), 256, 0, s>>>(g, (const TX*)grad, (const TX*)x, (const TS*)saved_mean, (const TS*)saved_inv_std, (TDS*)dscale, (TDB*)dbias);
 		if (check("group_norm_bwd_dparam"))
 			return -1;
 	}
 	return 0;
+}
+
+int group_norm_bwd(cudaStream_t s, const NormKinds& k, const GroupNormGeom& g, const void* grad, const void* x, const void* scale, const void* saved_mean, const void* saved_inv_std, void* h, void* dscale, void* dbias, void* workspace)
+{
+	const long long total = gn_count(g.dim), slots = gn_count(g.rdim);
+	if (total == 0)
+		return 0;
+	return with_kind(k.x, [&](auto tx) {
+		using TX = elem_t<decltype(tx)>;
+		return with_kind_of<TX>(k.scale, [&](auto tp) {
+			return with_kind_of<TX>(k.stat, [&](auto ts) {
+				return with_kind_of<TX>(k.dscale, [&](auto tds) {
+					return with_kind_of<TX>(k.dbias, [&](auto tdb) {
+						return gn_bwd<TX, elem_t<decltype(tp)>, elem_t<decltype(ts)>, elem_t<decltype(tds)>, elem_t<decltype(tdb)> >(s, g, grad, x, scale, saved_mean, saved_inv_std, h, dscale, dbias, workspace, total, slots);
+					});
+				});
+			});
+		});
+	});
 }
 
 } // namespace sm100
