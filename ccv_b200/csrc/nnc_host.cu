@@ -822,6 +822,23 @@ int ccv_nnc_sm100_fused_rmsprop_multi(const ccv_nnc_cmd_t, const ccv_nnc_hint_t,
 int ccv_nnc_sm100_fused_conv_stats_forw(const ccv_nnc_cmd_t, const ccv_nnc_hint_t, const int, ccv_nnc_tensor_t* const*, const int, ccv_nnc_tensor_t* const*, const int, ccv_nnc_stream_context_t*);
 int ccv_nnc_sm100_fused_bn_forw(const ccv_nnc_cmd_t, const ccv_nnc_hint_t, const int, ccv_nnc_tensor_t* const*, const int, ccv_nnc_tensor_t* const*, const int, ccv_nnc_stream_context_t*);
 int ccv_nnc_sm100_fused_bn_back(const ccv_nnc_cmd_t, const ccv_nnc_hint_t, const int, ccv_nnc_tensor_t* const*, const int, ccv_nnc_tensor_t* const*, const int, ccv_nnc_stream_context_t*);
+int ccv_nnc_sm100_fused_bn_add_relu_forw(const ccv_nnc_cmd_t, const ccv_nnc_hint_t, const int, ccv_nnc_tensor_t* const*, const int, ccv_nnc_tensor_t* const*, const int, ccv_nnc_stream_context_t*);
+int ccv_nnc_sm100_fused_avgpool_add_relu_back(const ccv_nnc_cmd_t, const ccv_nnc_hint_t, const int, ccv_nnc_tensor_t* const*, const int, ccv_nnc_tensor_t* const*, const int, ccv_nnc_stream_context_t*);
+}
+
+// the byte range [first, second) a tensor or tensor view spans
+static std::pair<const unsigned char*, const unsigned char*> tensor_range(const ccv_nnc_tensor_t* const t)
+{
+	size_t elems = 1;
+	if (CCV_IS_TENSOR_VIEW(t))
+	{
+		const ccv_nnc_tensor_view_t* const tv = (const ccv_nnc_tensor_view_t*)t;
+		for (int d = 0; d < CCV_NNC_MAX_DIM_ALLOC && t->info.dim[d] > 0; d++)
+			elems += (size_t)(t->info.dim[d] - 1) * (size_t)tv->stride[d];
+	} else
+		for (int d = 0; d < CCV_NNC_MAX_DIM_ALLOC && t->info.dim[d] > 0; d++)
+			elems *= (size_t)t->info.dim[d];
+	return std::make_pair((const unsigned char*)t->data.u8, (const unsigned char*)t->data.u8 + elems * datatype_size(t->info.datatype));
 }
 
 struct ccv_nnc_sm100_graph_s {
@@ -888,18 +905,6 @@ int ccv_nnc_sm100_graph_run(ccv_nnc_sm100_graph_t* const graph, const int begin,
 	// byte ranges written by side-stream nodes that have not been joined yet: a main-stream node that touches one of them is a
 	// consumer (or an overwriter) of that result, so the join is issued in front of it instead of at the end of the run
 	std::vector<std::pair<const unsigned char*, const unsigned char*> > side_writes;
-	auto range_of = [](const ccv_nnc_tensor_t* const t) {
-		size_t elems = 1;
-		if (CCV_IS_TENSOR_VIEW(t))
-		{
-			const ccv_nnc_tensor_view_t* const tv = (const ccv_nnc_tensor_view_t*)t;
-			for (int d = 0; d < CCV_NNC_MAX_DIM_ALLOC && t->info.dim[d] > 0; d++)
-				elems += (size_t)(t->info.dim[d] - 1) * (size_t)tv->stride[d];
-		} else
-			for (int d = 0; d < CCV_NNC_MAX_DIM_ALLOC && t->info.dim[d] > 0; d++)
-				elems *= (size_t)t->info.dim[d];
-		return std::make_pair((const unsigned char*)t->data.u8, (const unsigned char*)t->data.u8 + elems * datatype_size(t->info.datatype));
-	};
 	auto join = [&]() {
 		ccv_nnc_stream_context_emit_signal(graph->side_stream, graph->join_signal);
 		ccv_nnc_stream_context_wait_signal(stream_context, graph->join_signal);
@@ -917,7 +922,7 @@ int ccv_nnc_sm100_graph_run(ccv_nnc_sm100_graph_t* const graph, const int begin,
 				for (ccv_nnc_tensor_t* t : (pass ? n.outputs : n.inputs))
 					if (t && t->data.u8)
 					{
-						const auto r = range_of(t);
+						const auto r = tensor_range(t);
 						for (const auto& w : side_writes)
 							if (r.first < w.second && w.first < r.second)
 								touches = true;
@@ -946,7 +951,7 @@ int ccv_nnc_sm100_graph_run(ccv_nnc_sm100_graph_t* const graph, const int begin,
 				side_pending = true;
 				for (ccv_nnc_tensor_t* t : n.outputs)
 					if (t && t->data.u8)
-						side_writes.push_back(range_of(t));
+						side_writes.push_back(tensor_range(t));
 			}
 		}
 		const int ret = n.fused ? n.fused(n.cmd, n.hint, n.flags, n.inputs.data(), (int)n.inputs.size(), n.outputs.data(), (int)n.outputs.size(), sc) :
@@ -969,6 +974,11 @@ int ccv_nnc_sm100_graph_run(ccv_nnc_sm100_graph_t* const graph, const int begin,
 //      unmasked, so the rewrite is only applied when no later node reads g
 //  (c) EWSUM(a, b -> y) ; RELU_FORWARD in place on y                          -> y = relu(a + b)
 //  (d) EWSUM(a, b -> a) ; RELU_BACKWARD in place on a (mask y)                -> a = y > 0 ? a + b : 0
+//  (h) BATCH_NORM_FORWARD(train) -> m ; EWSUM(m, s -> y) ; RELU_FORWARD in place on y -> y = relu(bn(x) + s), m is not written, so
+//      the rewrite is only applied when no later node reads m's memory (the end of a residual block: the batch-norm backward
+//      reads x and the saved statistics, not m)
+//  (i) AVERAGE_POOL_BACKWARD(g -> s) ; EWSUM(r, s -> out) ; RELU_BACKWARD in place on out (mask y) -> out = y > 0 ? r + s : 0, s is
+//      not written, so the rewrite is only applied when no later node reads s's memory (the shortcut of a strided residual block)
 //  (e) a run of SGD_FORWARD nodes with identical parameters (the per-parameter updates of a model; none of them reads
 //      what another one writes) -> one multi-tensor command; counts as (run length - 1) fused nodes.  Runs of LAMB_FORWARD and
 //      of RMSPROP_FORWARD nodes are rewritten the same way (each LAMB tensor keeps its own trust ratio).
@@ -981,6 +991,19 @@ int ccv_nnc_sm100_graph_fuse(ccv_nnc_sm100_graph_t* const graph)
 	int fused = 0;
 	const size_t n = nodes.size();
 	auto is_gpu_sm100 = [](const ccv_nnc_sm100_graph_node_t& x) { return x.fused == 0 && !x.side && (x.cmd.backend == CCV_NNC_BACKEND_GPU_SM100 || x.cmd.backend == CCV_NNC_NO_BACKEND); };
+	// whether a node from `from` on reads any byte of t (through t itself or through another tensor or view of its memory)
+	auto read_later = [&](const ccv_nnc_tensor_t* const t, const size_t from) {
+		const auto m = tensor_range(t);
+		for (size_t j = from; j < n; j++)
+			for (ccv_nnc_tensor_t* x : nodes[j].inputs)
+				if (x && x->data.u8)
+				{
+					const auto r = tensor_range(x);
+					if (r.first < m.second && m.first < r.second)
+						return true;
+				}
+		return false;
+	};
 	for (size_t i = 0; i < n; i++)
 	{
 		ccv_nnc_sm100_graph_node_t& a = nodes[i];
@@ -1070,6 +1093,37 @@ int ccv_nnc_sm100_graph_fuse(ccv_nnc_sm100_graph_t* const graph)
 				fused++, i++;
 				continue;
 			}
+			// (h)
+			if (i + 2 < n && a.cmd.cmd == CCV_NNC_BATCH_NORM_FORWARD && !a.cmd.info.bnorm.is_test && a.inputs.size() == 5 && a.outputs.size() == 5 && a.outputs[0] && a.outputs[0]->data.u8 &&
+				!CCV_IS_TENSOR_VIEW(a.outputs[0]) && b.cmd.cmd == CCV_NNC_EWSUM_FORWARD && b.inputs.size() == 2 && b.outputs.size() == 1 && b.outputs[0] && b.inputs[0] && b.inputs[1] &&
+				(b.inputs[0] == a.outputs[0]) != (b.inputs[1] == a.outputs[0]) && is_gpu_sm100(nodes[i + 2]) && nodes[i + 2].cmd.cmd == CCV_NNC_RELU_FORWARD &&
+				nodes[i + 2].inputs.size() == 1 && nodes[i + 2].outputs.size() == 1 && nodes[i + 2].inputs[0] == b.outputs[0] && nodes[i + 2].outputs[0] == b.outputs[0] &&
+				!read_later(a.outputs[0], i + 3))
+			{
+				// s rides as a 6th output (read, never written): the inputs stay the batch norm's, where rule (f) appends the statistics
+				ccv_nnc_sm100_graph_node_t f = a;
+				f.outputs[0] = b.outputs[0];
+				f.outputs.push_back(b.inputs[b.inputs[0] == a.outputs[0] ? 1 : 0]);
+				f.fused = ccv_nnc_sm100_fused_bn_add_relu_forw;
+				out.push_back(f);
+				fused += 2, i += 2;
+				continue;
+			}
+			// (i)
+			if (i + 2 < n && a.cmd.cmd == CCV_NNC_AVERAGE_POOL_BACKWARD && a.inputs.size() >= 1 && a.inputs[0] && a.outputs.size() == 1 && a.outputs[0] && a.outputs[0]->data.u8 &&
+				!CCV_IS_TENSOR_VIEW(a.outputs[0]) && b.cmd.cmd == CCV_NNC_EWSUM_FORWARD && b.inputs.size() == 2 && b.outputs.size() == 1 && b.outputs[0] && b.inputs[0] && b.inputs[1] &&
+				(b.inputs[0] == a.outputs[0]) != (b.inputs[1] == a.outputs[0]) && is_gpu_sm100(nodes[i + 2]) && nodes[i + 2].cmd.cmd == CCV_NNC_RELU_BACKWARD &&
+				nodes[i + 2].inputs.size() == 3 && nodes[i + 2].inputs[0] == b.outputs[0] && nodes[i + 2].inputs[2] && nodes[i + 2].outputs.size() == 1 && nodes[i + 2].outputs[0] == b.outputs[0] &&
+				!read_later(a.outputs[0], i + 3))
+			{
+				ccv_nnc_sm100_graph_node_t f = a;
+				f.inputs.assign({ a.inputs[0], b.inputs[b.inputs[0] == a.outputs[0] ? 1 : 0], nodes[i + 2].inputs[2] });
+				f.outputs[0] = b.outputs[0];
+				f.fused = ccv_nnc_sm100_fused_avgpool_add_relu_back;
+				out.push_back(f);
+				fused += 2, i += 2;
+				continue;
+			}
 			// (c)
 			if (a.cmd.cmd == CCV_NNC_EWSUM_FORWARD && a.inputs.size() == 2 && a.outputs.size() == 1 && b.cmd.cmd == CCV_NNC_RELU_FORWARD && b.inputs.size() == 1 && b.inputs[0] == a.outputs[0] && b.outputs[0] == a.outputs[0])
 			{
@@ -1121,7 +1175,7 @@ int ccv_nnc_sm100_graph_fuse(ccv_nnc_sm100_graph_t* const graph)
 		}
 		out.push_back(a);
 	}
-	// (f) CONVOLUTION_FORWARD ; BATCH_NORM_FORWARD(train) (plain or already fused with its ReLU) reading the convolution's output:
+	// (f) CONVOLUTION_FORWARD ; BATCH_NORM_FORWARD(train) (plain or already fused with its ReLU, or by (h)) reading the convolution's output:
 	//     the convolution's tensor-core epilogue also produces the per-channel sums the batch norm needs, through a small
 	//     statistics tensor owned by the graph (one fewer pass over the activation).  CCV_NNC_SM100_FUSE_CONV_BN=0 turns it off.
 	const char* const env = getenv("CCV_NNC_SM100_FUSE_CONV_BN");
@@ -1132,7 +1186,7 @@ int ccv_nnc_sm100_graph_fuse(ccv_nnc_sm100_graph_t* const graph)
 			ccv_nnc_sm100_graph_node_t& b = out[i + 1];
 			if (c.fused || c.cmd.cmd != CCV_NNC_CONVOLUTION_FORWARD || c.outputs.size() != 1 || !c.outputs[0] || c.cmd.algorithm == CCV_NNC_SM100_ALGO_FFMA || c.cmd.info.convolution.groups != 1)
 				continue;
-			if (b.cmd.cmd != CCV_NNC_BATCH_NORM_FORWARD || b.cmd.info.bnorm.is_test || b.inputs.size() != 5 || b.inputs[0] != c.outputs[0] || (b.fused && b.fused != ccv_nnc_sm100_fused_bn_relu_forw))
+			if (b.cmd.cmd != CCV_NNC_BATCH_NORM_FORWARD || b.cmd.info.bnorm.is_test || b.inputs.size() != 5 || b.inputs[0] != c.outputs[0] || (b.fused && b.fused != ccv_nnc_sm100_fused_bn_relu_forw && b.fused != ccv_nnc_sm100_fused_bn_add_relu_forw))
 				continue;
 			if (CCV_IS_TENSOR_VIEW(c.outputs[0]) || CCV_TENSOR_GET_MEMORY(c.outputs[0]->info.type) != CCV_TENSOR_GPU_MEMORY)
 				continue;
@@ -1183,7 +1237,7 @@ int ccv_nnc_sm100_graph_node(const ccv_nnc_sm100_graph_t* const graph, const int
 		return -1;
 	const ccv_nnc_sm100_graph_node_t& n = graph->nodes[i];
 	*cmd = n.cmd.cmd;
-	*fused_kind = n.fused == ccv_nnc_sm100_fused_bn_relu_forw ? 1 : n.fused == ccv_nnc_sm100_fused_relu_bn_back ? 2 : n.fused == ccv_nnc_sm100_fused_add_relu_forw ? 3 : n.fused == ccv_nnc_sm100_fused_add_relu_back ? 4 : n.fused == ccv_nnc_sm100_fused_sgd_multi ? 5 : n.fused == ccv_nnc_sm100_fused_conv_stats_forw ? 6 : n.fused == ccv_nnc_sm100_fused_bn_forw ? 7 : n.fused == ccv_nnc_sm100_fused_bn_back ? 8 :
+	*fused_kind = n.fused == ccv_nnc_sm100_fused_bn_relu_forw ? 1 : n.fused == ccv_nnc_sm100_fused_relu_bn_back ? 2 : n.fused == ccv_nnc_sm100_fused_add_relu_forw ? 3 : n.fused == ccv_nnc_sm100_fused_add_relu_back ? 4 : n.fused == ccv_nnc_sm100_fused_sgd_multi ? 5 : n.fused == ccv_nnc_sm100_fused_conv_stats_forw ? 6 : n.fused == ccv_nnc_sm100_fused_bn_forw || n.fused == ccv_nnc_sm100_fused_bn_add_relu_forw ? 7 : n.fused == ccv_nnc_sm100_fused_bn_back ? 8 :
 		n.fused == ccv_nnc_sm100_fused_lamb_multi ? 9 : n.fused == ccv_nnc_sm100_fused_rmsprop_multi ? 10 : 0;
 	*input_size = (int)n.inputs.size();
 	*output_size = (int)n.outputs.size();

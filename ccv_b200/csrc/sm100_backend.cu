@@ -1269,7 +1269,8 @@ bool bn_layout(const TV& a, const TV& scale, size_t& outer, int& C, size_t& inne
 	return true;
 }
 
-int bnorm_forw(const int fuse_relu, const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
+// resid (training only): y = relu(bn(x) + resid), the batch norm at the end of a residual block fused with the block's sum and ReLU
+int bnorm_forw(const int fuse_relu, const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context, const ccv_nnc_tensor_t* const resid = 0)
 {
 	// a 6th input is the statistics tensor of a fused convolution -> batch norm pair (ccv_nnc_sm100_graph_fuse): its `sig`
 	// field carries the number of valid partial rows the convolution produced for this issue (0 = none: reduce here)
@@ -1287,6 +1288,8 @@ int bnorm_forw(const int fuse_relu, const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_
 	size_t outer, inner;
 	int C;
 	if (!same_shape(a, b) || !b.contiguous || !bn_layout(a, scale, outer, C, inner))
+		return CCV_NNC_EXEC_INVALID;
+	if (resid && (fuse_relu || cmd.info.bnorm.is_test || kind_of(resid) != kind || !view_of(resid).contiguous || view_of(resid).count != b.count))
 		return CCV_NNC_EXEC_INVALID;
 	for (int i = 2; i < 5; i++)
 		if (view_of(inputs[i]).count != (size_t)C)
@@ -1320,10 +1323,10 @@ int bnorm_forw(const int fuse_relu, const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_
 			return CCV_NNC_EXEC_INVALID;
 	if (kind == 0)
 		RC(bn_fwd_train_f32(s, inputs[0]->data.f32, outputs[0]->data.f32, inputs[1]->data.f32, inputs[2]->data.f32, outputs[1]->data.f32, outputs[2]->data.f32, outputs[3]->data.f32, outputs[4]->data.f32, outer, C, inner, cmd.info.bnorm.epsilon, cmd.info.bnorm.momentum, ws, fuse_relu,
-			stats_t && inner == 1 ? stats_t->data.f32 : 0, stats_t ? (int)stats_t->sig : 0));
+			stats_t && inner == 1 ? stats_t->data.f32 : 0, stats_t ? (int)stats_t->sig : 0, resid ? resid->data.f32 : 0));
 	else
 		RC(bn_fwd_train_16(s, kind, inputs[0]->data.u8, outputs[0]->data.u8, inputs[1]->data.f32, inputs[2]->data.f32, outputs[1]->data.f32, outputs[2]->data.f32, outputs[3]->data.f32, outputs[4]->data.f32, outer, C, inner, cmd.info.bnorm.epsilon, cmd.info.bnorm.momentum, ws, fuse_relu,
-			stats_t && inner == 1 ? stats_t->data.f32 : 0, stats_t ? (int)stats_t->sig : 0));
+			stats_t && inner == 1 ? stats_t->data.f32 : 0, stats_t ? (int)stats_t->sig : 0, resid ? resid->data.u8 : 0));
 	return CCV_NNC_EXEC_SUCCESS;
 }
 
@@ -1825,6 +1828,38 @@ int exec_pool_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 		RC(pool_avg_bwd_16(stream_of(stream_context), kind, g, inputs[0]->data.u8, outputs[0]->data.u8));
 	else
 		RC(pool_avg_bwd_f32(stream_of(stream_context), g, inputs[0]->data.f32, outputs[0]->data.f32));
+	return CCV_NNC_EXEC_SUCCESS;
+}
+
+// AVERAGE_POOL_BACKWARD(g -> s) ; EWSUM(r, s -> out) ; RELU_BACKWARD in place on out (mask y), as one pass out = y > 0 ? r + s : 0 that
+// never writes s: inputs (g, r, y), outputs (out).  Geometries the one-pass kernel does not take run the three steps with s in the
+// workspace.
+int exec_avgpool_add_relu_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
+{
+	if (input_size != 3 || output_size != 1 || !inputs[0] || !inputs[1] || !inputs[2] || !outputs[0])
+		return CCV_NNC_EXEC_INVALID;
+	const int kind = kind_of(outputs[0]);
+	const TV r = view_of(inputs[1]), y = view_of(inputs[2]), o = view_of(outputs[0]);
+	if (kind < 0 || kind_of(inputs[0]) != kind || kind_of(inputs[1]) != kind || kind_of(inputs[2]) != kind || !r.contiguous || !y.contiguous || !o.contiguous || !same_shape(r, o) || !same_shape(y, o))
+		return CCV_NNC_EXEC_INVALID;
+	PoolGeom g;
+	if (!pool_geom(cmd, hint, o, view_of(inputs[0]), g))
+		return CCV_NNC_EXEC_INVALID;
+	cudaStream_t s = stream_of(stream_context);
+	const int rc = pool_avg_bwd_add_relu(s, kind, g, inputs[0]->data.u8, inputs[1]->data.u8, inputs[2]->data.u8, outputs[0]->data.u8);
+	if (rc <= 0)
+		return rc ? CCV_NNC_EXEC_INVALID : CCV_NNC_EXEC_SUCCESS;
+	void* const ws = ccv_nnc_stream_context_get_workspace(stream_context, o.count * (kind == 0 ? 4 : 2), CCV_TENSOR_GPU_MEMORY);
+	if (!ws)
+		return CCV_NNC_EXEC_OOM;
+	if (kind != 0)
+	{
+		RC(pool_avg_bwd_16(s, kind, g, inputs[0]->data.u8, ws));
+		RC(ew_add_relu_bwd_16(s, kind, inputs[1]->data.u8, ws, inputs[2]->data.u8, outputs[0]->data.u8, o.count));
+	} else {
+		RC(pool_avg_bwd_f32(s, g, inputs[0]->data.f32, (float*)ws));
+		RC(ew_add_relu_bwd_f32(s, inputs[1]->data.f32, (const float*)ws, inputs[2]->data.f32, outputs[0]->data.f32, o.count));
+	}
 	return CCV_NNC_EXEC_SUCCESS;
 }
 
@@ -2455,6 +2490,22 @@ extern "C" int ccv_nnc_sm100_fused_bn_relu_forw(const ccv_nnc_cmd_t cmd, const c
 extern "C" int ccv_nnc_sm100_fused_bn_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
 {
 	return bnorm_forw(0, cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
+}
+
+// BATCH_NORM_FORWARD(train) ; EWSUM(bn output, s -> y) ; RELU_FORWARD in place on y, as one pass y = relu(bn(x) + s) that never
+// writes the batch norm's own output.  inputs: the batch norm's five (and the statistics tensor of a linked convolution); outputs: y,
+// the batch norm's four statistics outputs, then s (read only).
+extern "C" int ccv_nnc_sm100_fused_bn_add_relu_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
+{
+	if (output_size != 6 || !outputs[5])
+		return CCV_NNC_EXEC_INVALID;
+	return bnorm_forw(0, cmd, hint, flags, inputs, input_size, outputs, 5, stream_context, outputs[5]);
+}
+
+// AVERAGE_POOL_BACKWARD ; EWSUM ; RELU_BACKWARD at the shortcut of a strided residual block (exec_avgpool_add_relu_back)
+extern "C" int ccv_nnc_sm100_fused_avgpool_add_relu_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
+{
+	return exec_avgpool_add_relu_back(cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
 }
 
 // BATCH_NORM_BACKWARD with the bias gradient of the producing convolution as a 4th output (no ReLU in front)

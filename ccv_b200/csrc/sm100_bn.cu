@@ -417,7 +417,9 @@ __global__ void __launch_bounds__(1024) bn_finalize_ext_kernel(const float* __re
 }
 
 // ------------------------------------------------------------------------------------------------ elementwise passes
-// forward: y = x * a + b (optionally relu'd).  backward: dx = a * g' + p * x + q with the optional relu mask on g.
+// forward: y = x * a + b (RELU 1: relu'd; RELU 2: y = relu(x * a + b + r) with the residual r read through `g`, the end of a
+// residual block, where x * a + b is first rounded to T as a stored batch-norm output would be).  backward: dx = a * g' + p * x + q
+// with the optional relu mask on g.
 // COLSUM (backward only): also leaves per-channel sums of the values written in `part` (rows of C floats; the caller guarantees
 // stride % CV == 0, so a thread stays on one channel group, and 256 % CV == 0 or CV % 256 == 0) -- the bias gradient of the
 // convolution that consumes dx, without another pass over dx.
@@ -433,7 +435,7 @@ __global__ void __launch_bounds__(256) bn_apply_vec_kernel(const T* __restrict__
 		const bool two = j < total4;
 		const float4 x0 = ld4(x + i * 4), x1 = two ? ld4(x + j * 4) : x0;
 		float4 g0 = x0, g1 = x0;
-		if (BWD)
+		if (BWD || RELU == 2)
 			g0 = ld4(g + i * 4), g1 = two ? ld4(g + j * 4) : g0;
 #pragma unroll
 		for (int u = 0; u < 2; u++)
@@ -448,6 +450,8 @@ __global__ void __launch_bounds__(256) bn_apply_vec_kernel(const T* __restrict__
 			if (!BWD)
 			{
 				o.x = fmaf(xv.x, a.x, b.x), o.y = fmaf(xv.y, a.y, b.y), o.z = fmaf(xv.z, a.z, b.z), o.w = fmaf(xv.w, a.w, b.w);
+				if (RELU == 2)
+					o.x = rnd(x, o.x) + gv.x, o.y = rnd(x, o.y) + gv.y, o.z = rnd(x, o.z) + gv.z, o.w = rnd(x, o.w) + gv.w;
 				if (RELU)
 					o.x = fmaxf(o.x, 0.f), o.y = fmaxf(o.y, 0.f), o.z = fmaxf(o.z, 0.f), o.w = fmaxf(o.w, 0.f);
 			} else {
@@ -516,7 +520,7 @@ __global__ void __launch_bounds__(256) bn_apply_fixed_kernel(const T* __restrict
 			if (i + u * stride < totalw)
 			{
 				ldv(x + (i + u * stride) * W, xv[u]);
-				if (BWD)
+				if (BWD || RELU == 2)
 					ldv(g + (i + u * stride) * W, gv[u]);
 			}
 #pragma unroll
@@ -530,6 +534,8 @@ __global__ void __launch_bounds__(256) bn_apply_fixed_kernel(const T* __restrict
 					if (!BWD)
 					{
 						o[k] = fmaf(xv[u][k], a[k], b[k]);
+						if (RELU == 2)
+							o[k] = rnd(x, o[k]) + gv[u][k];
 						if (RELU)
 							o[k] = fmaxf(o[k], 0.f);
 					} else {
@@ -606,7 +612,9 @@ __global__ void bn_apply_generic_kernel(const T* __restrict__ x, const T* __rest
 		const float a = coef[c], b = coef[C + c], xv = ldf(x + i);
 		if (!BWD)
 		{
-			const float o = fmaf(xv, a, b);
+			float o = fmaf(xv, a, b);
+			if (RELU == 2)
+				o = rnd(x, o) + ldf(g + i);
 			stf(out + i, RELU ? fmaxf(o, 0.f) : o);
 		} else {
 			float h = ldf(g + i);
@@ -658,7 +666,7 @@ static int run_apply(cudaStream_t s, const T* x, const T* g, T* out, const float
 	const size_t total = outer * C * inner;
 	constexpr int W = Vec16<T>::W;
 	const int CW = C / W;
-	if (inner == 1 && C % W == 0 && (256 % CW == 0 || CW % 256 == 0) && aligned_v16(x) && aligned_v16(out) && (!BWD || aligned_v16(g)))
+	if (inner == 1 && C % W == 0 && (256 % CW == 0 || CW % 256 == 0) && aligned_v16(x) && aligned_v16(out) && ((!BWD && RELU != 2) || aligned_v16(g)))
 	{
 		// channel-stationary threads: the grid stride is a multiple of the channel groups per pixel
 		int grid = grid_for(total / W / 4, 256);
@@ -677,7 +685,7 @@ static int run_apply(cudaStream_t s, const T* x, const T* g, T* out, const float
 		bn_apply_fixed_kernel<T, BWD, RELU, 0><<<grid, 256, 0, s>>>(x, g, out, coef, total / W, C, 0);
 		return check("bn_apply");
 	}
-	if (inner == 1 && C % 4 == 0 && aligned_v4(x) && aligned_v4(out) && (!BWD || aligned_v4(g)))
+	if (inner == 1 && C % 4 == 0 && aligned_v4(x) && aligned_v4(out) && ((!BWD && RELU != 2) || aligned_v4(g)))
 	{
 		int grid = grid_for(total / 8, 256);
 		const int CV = C / 4;
@@ -700,10 +708,14 @@ static int run_apply(cudaStream_t s, const T* x, const T* g, T* out, const float
 }
 
 template <typename T>
-static int bn_fwd_train_t(cudaStream_t s, const T* x, T* y, const float* scale, const float* bias, float* running_mean, float* running_var, float* saved_mean, float* saved_inv_std, size_t outer, int C, size_t inner, float epsilon, float momentum, void* workspace, int fuse_relu, const float* ext_part, int ext_rows)
+static int bn_fwd_train_t(cudaStream_t s, const T* x, T* y, const float* scale, const float* bias, float* running_mean, float* running_var, float* saved_mean, float* saved_inv_std, size_t outer, int C, size_t inner, float epsilon, float momentum, void* workspace, int fuse_relu, const float* ext_part, int ext_rows, const T* resid)
 {
 	if (outer * C * inner == 0)
 		return 0;
+	// y = fuse_relu ? relu(bn(x)) : bn(x), or with a residual: y = relu(bn(x) + resid)
+	auto apply = [&](const float* coef) {
+		return resid ? run_apply<T, 0, 2>(s, x, resid, y, coef, outer, C, inner) : fuse_relu ? run_apply<T, 0, 1>(s, x, (const T*)0, y, coef, outer, C, inner) : run_apply<T, 0, 0>(s, x, (const T*)0, y, coef, outer, C, inner);
+	};
 	double* ws = ws_sums(workspace);
 	float* coef = ws_coef(workspace, C);
 	int part_rows = 0;
@@ -713,7 +725,7 @@ static int bn_fwd_train_t(cudaStream_t s, const T* x, T* y, const float* scale, 
 		bn_finalize_ext_kernel<<<(C + 31) / 32, 1024, 0, s>>>(ext_part, ext_rows, C, epsilon, momentum, scale, bias, running_mean, running_var, saved_mean, saved_inv_std, coef);
 		if (check("bn_fwd_finalize(ext)"))
 			return -1;
-		return fuse_relu ? run_apply<T, 0, 1>(s, x, (const T*)0, y, coef, outer, C, inner) : run_apply<T, 0, 0>(s, x, (const T*)0, y, coef, outer, C, inner);
+		return apply(coef);
 	}
 	if (run_reduce<T, 0, 0>(s, x, (const T*)0, 0, 0, outer, C, inner, ws, ws_part(workspace, C), &part_rows))
 		return -1;
@@ -723,7 +735,7 @@ static int bn_fwd_train_t(cudaStream_t s, const T* x, T* y, const float* scale, 
 		bn_fwd_finalize_kernel<T><<<(C + 127) / 128, 128, 0, s>>>(x, inner, ws, C, (double)outer * (double)inner, epsilon, momentum, scale, bias, running_mean, running_var, saved_mean, saved_inv_std, coef);
 	if (check("bn_fwd_finalize"))
 		return -1;
-	return fuse_relu ? run_apply<T, 0, 1>(s, x, (const T*)0, y, coef, outer, C, inner) : run_apply<T, 0, 0>(s, x, (const T*)0, y, coef, outer, C, inner);
+	return apply(coef);
 }
 
 template <typename T>
@@ -786,9 +798,9 @@ static int bn_bwd_t(cudaStream_t s, const T* g, const T* x, const float* scale, 
 	return 0;
 }
 
-int bn_fwd_train_f32(cudaStream_t s, const float* x, float* y, const float* scale, const float* bias, float* running_mean, float* running_var, float* saved_mean, float* saved_inv_std, size_t outer, int C, size_t inner, float epsilon, float momentum, void* workspace, int fuse_relu, const float* ext_part, int ext_rows)
+int bn_fwd_train_f32(cudaStream_t s, const float* x, float* y, const float* scale, const float* bias, float* running_mean, float* running_var, float* saved_mean, float* saved_inv_std, size_t outer, int C, size_t inner, float epsilon, float momentum, void* workspace, int fuse_relu, const float* ext_part, int ext_rows, const float* resid)
 {
-	return bn_fwd_train_t<float>(s, x, y, scale, bias, running_mean, running_var, saved_mean, saved_inv_std, outer, C, inner, epsilon, momentum, workspace, fuse_relu, ext_part, ext_rows);
+	return bn_fwd_train_t<float>(s, x, y, scale, bias, running_mean, running_var, saved_mean, saved_inv_std, outer, C, inner, epsilon, momentum, workspace, fuse_relu, ext_part, ext_rows, resid);
 }
 int bn_fwd_test_f32(cudaStream_t s, const float* x, float* y, const float* scale, const float* bias, const float* mean, const float* var, size_t outer, int C, size_t inner, float epsilon, void* workspace)
 {
@@ -800,11 +812,11 @@ int bn_bwd_f32(cudaStream_t s, const float* g, const float* x, const float* scal
 }
 // 16-bit activations (kind 1 = bf16, 2 = fp16); scale / bias / statistics / parameter gradients stay fp32
 // (lib/nnc/ccv_cnnp_model_addons.c:954-956)
-int bn_fwd_train_16(cudaStream_t s, int kind, const void* x, void* y, const float* scale, const float* bias, float* running_mean, float* running_var, float* saved_mean, float* saved_inv_std, size_t outer, int C, size_t inner, float epsilon, float momentum, void* workspace, int fuse_relu, const float* ext_part, int ext_rows)
+int bn_fwd_train_16(cudaStream_t s, int kind, const void* x, void* y, const float* scale, const float* bias, float* running_mean, float* running_var, float* saved_mean, float* saved_inv_std, size_t outer, int C, size_t inner, float epsilon, float momentum, void* workspace, int fuse_relu, const float* ext_part, int ext_rows, const void* resid)
 {
 	if (kind == 1)
-		return bn_fwd_train_t<__nv_bfloat16>(s, (const __nv_bfloat16*)x, (__nv_bfloat16*)y, scale, bias, running_mean, running_var, saved_mean, saved_inv_std, outer, C, inner, epsilon, momentum, workspace, fuse_relu, ext_part, ext_rows);
-	return bn_fwd_train_t<__half>(s, (const __half*)x, (__half*)y, scale, bias, running_mean, running_var, saved_mean, saved_inv_std, outer, C, inner, epsilon, momentum, workspace, fuse_relu, ext_part, ext_rows);
+		return bn_fwd_train_t<__nv_bfloat16>(s, (const __nv_bfloat16*)x, (__nv_bfloat16*)y, scale, bias, running_mean, running_var, saved_mean, saved_inv_std, outer, C, inner, epsilon, momentum, workspace, fuse_relu, ext_part, ext_rows, (const __nv_bfloat16*)resid);
+	return bn_fwd_train_t<__half>(s, (const __half*)x, (__half*)y, scale, bias, running_mean, running_var, saved_mean, saved_inv_std, outer, C, inner, epsilon, momentum, workspace, fuse_relu, ext_part, ext_rows, (const __half*)resid);
 }
 int bn_fwd_test_16(cudaStream_t s, int kind, const void* x, void* y, const float* scale, const float* bias, const float* mean, const float* var, size_t outer, int C, size_t inner, float epsilon, void* workspace)
 {

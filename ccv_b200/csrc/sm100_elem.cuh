@@ -45,6 +45,10 @@ __device__ __forceinline__ float ldf(const __half* p) { return __half2float(*p);
 __device__ __forceinline__ void stf(float* p, const float v) { *p = v; }
 __device__ __forceinline__ void stf(__nv_bfloat16* p, const float v) { *p = __float2bfloat16_rn(v); }
 __device__ __forceinline__ void stf(__half* p, const float v) { *p = __float2half_rn(v); }
+// v as a store to a T tensor and a load back would give it: rounded to nearest even for the 16-bit types, unchanged for fp32
+__device__ __forceinline__ float rnd(const float*, const float v) { return v; }
+__device__ __forceinline__ float rnd(const __nv_bfloat16*, const float v) { return __bfloat162float(__float2bfloat16_rn(v)); }
+__device__ __forceinline__ float rnd(const __half*, const float v) { return __half2float(__float2half_rn(v)); }
 
 // element i of a buffer whose kind is only known at run time
 __device__ __forceinline__ float ld_kind(const void* p, const size_t i, const int kind)

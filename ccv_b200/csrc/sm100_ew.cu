@@ -769,8 +769,12 @@ static int pool_max_bwd_t(cudaStream_t s, const PoolGeom& g, const T* grad_b, co
 // Average-pool backward when the windows tile the input exactly (window = stride, no padding, H = P * R, W = Q * S: the 2 x 2 / 2
 // shortcut pools and the global pool of a ResNet): one thread per OUTPUT gradient group -- one 16-byte load, one multiply per
 // element, R * S 16-byte stores -- instead of one thread (and three integer divisions) per input group.
-template <typename T>
-__global__ void __launch_bounds__(256) avgpool_bwd_tiles_kernel(const PoolGeom g, const T* __restrict__ gb, T* __restrict__ ga)
+// MASK = 1: the pool is the shortcut of a residual block whose input gradient is the sum of both branches behind a ReLU: the store is
+// ga = y > 0 ? add + v : 0 with add (the other branch's gradient) and y (the block input) laid out as ga, v rounded to T first as a
+// stored pool gradient would be.  add may be ga itself: every element is read before the same thread writes it, so ga is not
+// __restrict__.
+template <typename T, int MASK>
+__global__ void __launch_bounds__(256) avgpool_bwd_tiles_kernel(const PoolGeom g, const T* __restrict__ gb, T* ga, const T* add, const T* y)
 {
 	constexpr int W = Vec16<T>::W;
 	const unsigned CW = (unsigned)g.C / W;
@@ -787,11 +791,35 @@ __global__ void __launch_bounds__(256) avgpool_bwd_tiles_kernel(const PoolGeom g
 #pragma unroll
 		for (int k = 0; k < W; k++)
 			v[k] = v[k] / (float)(g.R * g.S); // the reference divides (pool/ccv_nnc_avg_pool_cpu_ref.c:60-110); keep its rounding
-		T* const base = ga + n * g.an + (long long)p * g.R * g.ah + (long long)q * g.S * g.aw + c;
+		const long long base = n * g.an + (long long)p * g.R * g.ah + (long long)q * g.S * g.aw + c;
+		if (MASK)
+#pragma unroll
+			for (int k = 0; k < W; k++)
+				v[k] = rnd(gb, v[k]);
 		for (int dh = 0; dh < g.R; dh++)
 			for (int dw = 0; dw < g.S; dw++)
-				stv(base + dh * g.ah + dw * g.aw, v);
+			{
+				const long long o = base + dh * g.ah + dw * g.aw;
+				if (MASK)
+				{
+					float rv[W], yv[W], ov[W];
+					ldv(add + o, rv), ldv(y + o, yv);
+#pragma unroll
+					for (int k = 0; k < W; k++)
+						ov[k] = yv[k] > 0.f ? rv[k] + v[k] : 0.f;
+					stv(ga + o, ov);
+				} else
+					stv(ga + o, v);
+			}
 	}
+}
+// the tiles kernel's geometry: every window lies inside the input and no two overlap
+template <typename T>
+static bool avgpool_tiles_ok(const PoolGeom& g, const T* grad_b, const T* grad_a)
+{
+	constexpr int W = Vec16<T>::W;
+	return g.R == g.stride_h && g.S == g.stride_w && g.pad_h == 0 && g.pad_w == 0 && g.H == g.P * g.R && g.W == g.Q * g.S && g.C % W == 0 && aligned_v16(grad_b) && aligned_v16(grad_a) &&
+		g.aw % W == 0 && g.ah % W == 0 && g.an % W == 0 && g.bw % W == 0 && g.bh % W == 0 && g.bn % W == 0;
 }
 template <typename T>
 static int pool_avg_bwd_t(cudaStream_t s, const PoolGeom& g, const T* grad_b, T* grad_a)
@@ -800,10 +828,9 @@ static int pool_avg_bwd_t(cudaStream_t s, const PoolGeom& g, const T* grad_b, T*
 	if (total == 0)
 		return 0;
 	constexpr int W = Vec16<T>::W;
-	if (g.R == g.stride_h && g.S == g.stride_w && g.pad_h == 0 && g.pad_w == 0 && g.H == g.P * g.R && g.W == g.Q * g.S && g.C % W == 0 && aligned_v16(grad_b) && aligned_v16(grad_a) &&
-		g.aw % W == 0 && g.ah % W == 0 && g.an % W == 0 && g.bw % W == 0 && g.bh % W == 0 && g.bn % W == 0)
+	if (avgpool_tiles_ok(g, grad_b, grad_a))
 	{
-		avgpool_bwd_tiles_kernel<T><<<grid_for((size_t)g.N * g.P * g.Q * (g.C / W), 256), 256, 0, s>>>(g, grad_b, grad_a);
+		avgpool_bwd_tiles_kernel<T, 0><<<grid_for((size_t)g.N * g.P * g.Q * (g.C / W), 256), 256, 0, s>>>(g, grad_b, grad_a, (const T*)0, (const T*)0);
 		return check("pool_avg_bwd");
 	}
 	if (pool_vec_ok(g, (const T*)grad_a, grad_b))
@@ -811,6 +838,26 @@ static int pool_avg_bwd_t(cudaStream_t s, const PoolGeom& g, const T* grad_b, T*
 	else
 		pool_bwd_kernel<T, 1, 0><<<grid_for(total, 256), 256, 0, s>>>(g, grad_b, (const T*)0, (const T*)0, grad_a);
 	return check("pool_avg_bwd");
+}
+// grad_a = y > 0 ? r + avgpool_backward(grad_b) : 0 in one pass; r and y are addressed with grad_a's strides.  1 (nothing launched)
+// when the geometry is not the tiles kernel's
+template <typename T>
+static int pool_avg_bwd_add_relu_t(cudaStream_t s, const PoolGeom& g, const T* grad_b, const T* r, const T* y, T* grad_a)
+{
+	if (!avgpool_tiles_ok(g, grad_b, grad_a) || !aligned_v16(r) || !aligned_v16(y))
+		return 1;
+	if ((size_t)g.N * g.H * g.W * g.C == 0)
+		return 0;
+	avgpool_bwd_tiles_kernel<T, 1><<<grid_for((size_t)g.N * g.P * g.Q * (g.C / Vec16<T>::W), 256), 256, 0, s>>>(g, grad_b, grad_a, r, y);
+	return check("pool_avg_bwd_add_relu") ? -1 : 0;
+}
+int pool_avg_bwd_add_relu(cudaStream_t s, int kind, const PoolGeom& g, const void* grad_b, const void* r, const void* y, void* grad_a)
+{
+	if (kind == 0)
+		return pool_avg_bwd_add_relu_t<float>(s, g, (const float*)grad_b, (const float*)r, (const float*)y, (float*)grad_a);
+	if (kind == 1)
+		return pool_avg_bwd_add_relu_t<__nv_bfloat16>(s, g, (const __nv_bfloat16*)grad_b, (const __nv_bfloat16*)r, (const __nv_bfloat16*)y, (__nv_bfloat16*)grad_a);
+	return pool_avg_bwd_add_relu_t<__half>(s, g, (const __half*)grad_b, (const __half*)r, (const __half*)y, (__half*)grad_a);
 }
 int pool_max_bwd_f32(cudaStream_t s, const PoolGeom& g, const float* grad_b, const float* a, const float* b, float* grad_a) { return pool_max_bwd_t<float>(s, g, grad_b, a, b, grad_a); }
 int pool_avg_bwd_f32(cudaStream_t s, const PoolGeom& g, const float* grad_b, float* grad_a) { return pool_avg_bwd_t<float>(s, g, grad_b, grad_a); }

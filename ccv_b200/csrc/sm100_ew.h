@@ -48,13 +48,16 @@ int pool_max_fwd_16(cudaStream_t s, int kind, const PoolGeom& g, const void* a, 
 int pool_max_bwd_16(cudaStream_t s, int kind, const PoolGeom& g, const void* grad_b, const void* a, const void* b, void* grad_a);
 int pool_avg_fwd_16(cudaStream_t s, int kind, const PoolGeom& g, const void* a, void* b);
 int pool_avg_bwd_16(cudaStream_t s, int kind, const PoolGeom& g, const void* grad_b, void* grad_a);
+// kind 0 fp32, 1 bf16, 2 fp16: grad_a = y > 0 ? r + avgpool_backward(grad_b) : 0 (r and y laid out as grad_a; r may be grad_a);
+// 0 done, 1 the geometry is not one this pass takes (nothing launched), -1 launch error
+int pool_avg_bwd_add_relu(cudaStream_t s, int kind, const PoolGeom& g, const void* grad_b, const void* r, const void* y, void* grad_a);
 
 // ---- batch norm over [outer, C, inner] (NHWC: inner = 1; NCHW: outer = N, inner = H * W) ----------------------
 // training forward: writes y, saved_mean, saved_inv_std and updates the running mean / var in place
 // fuse_relu: y = relu(bn(x)) in the same pass (BATCH_NORM_FORWARD followed by an in-place RELU_FORWARD)
 // ext_part / ext_rows: per-channel statistics slots (four planes [ext_rows][C]: count, shift, shifted sum, shifted sum of squares) produced by the convolution that wrote x
 // (conv_stats_request); the statistics pass over x is then skipped
-int bn_fwd_train_f32(cudaStream_t s, const float* x, float* y, const float* scale, const float* bias, float* running_mean, float* running_var, float* saved_mean, float* saved_inv_std, size_t outer, int C, size_t inner, float epsilon, float momentum, void* workspace, int fuse_relu, const float* ext_part = 0, int ext_rows = 0);
+int bn_fwd_train_f32(cudaStream_t s, const float* x, float* y, const float* scale, const float* bias, float* running_mean, float* running_var, float* saved_mean, float* saved_inv_std, size_t outer, int C, size_t inner, float epsilon, float momentum, void* workspace, int fuse_relu, const float* ext_part = 0, int ext_rows = 0, const float* resid = 0);
 size_t bn_workspace_bytes(int C);
 int bn_fwd_test_f32(cudaStream_t s, const float* x, float* y, const float* scale, const float* bias, const float* mean, const float* var, size_t outer, int C, size_t inner, float epsilon, void* workspace);
 // backward: dx, dscale, dbias from g, x, scale, saved_mean, saved_inv_std.  bias != NULL = fused with the RELU_BACKWARD
@@ -63,7 +66,7 @@ int bn_fwd_test_f32(cudaStream_t s, const float* x, float* y, const float* scale
 int bn_bwd_f32(cudaStream_t s, const float* g, const float* x, const float* scale, const float* bias, const float* saved_mean, const float* saved_inv_std, float* dx, float* dscale, float* dbias, size_t outer, int C, size_t inner, void* workspace, float* dx_colsum = 0);
 // the same on 16-bit activations (kind 1 = bf16, 2 = fp16): scale / bias / running and saved statistics / dscale / dbias stay fp32
 // (lib/nnc/ccv_cnnp_model_addons.c:954-956); dx_colsum is written in element kind colsum_kind (0 = fp32)
-int bn_fwd_train_16(cudaStream_t s, int kind, const void* x, void* y, const float* scale, const float* bias, float* running_mean, float* running_var, float* saved_mean, float* saved_inv_std, size_t outer, int C, size_t inner, float epsilon, float momentum, void* workspace, int fuse_relu, const float* ext_part = 0, int ext_rows = 0);
+int bn_fwd_train_16(cudaStream_t s, int kind, const void* x, void* y, const float* scale, const float* bias, float* running_mean, float* running_var, float* saved_mean, float* saved_inv_std, size_t outer, int C, size_t inner, float epsilon, float momentum, void* workspace, int fuse_relu, const float* ext_part = 0, int ext_rows = 0, const void* resid = 0);
 int bn_fwd_test_16(cudaStream_t s, int kind, const void* x, void* y, const float* scale, const float* bias, const float* mean, const float* var, size_t outer, int C, size_t inner, float epsilon, void* workspace);
 int bn_bwd_16(cudaStream_t s, int kind, const void* g, const void* x, const float* scale, const float* bias, const float* saved_mean, const float* saved_inv_std, void* dx, float* dscale, float* dbias, size_t outer, int C, size_t inner, void* workspace, void* dx_colsum = 0, int colsum_kind = 0);
 int ew_add_relu_fwd_16(cudaStream_t s, int kind, const void* a, const void* b, void* out, size_t n);
