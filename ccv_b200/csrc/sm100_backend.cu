@@ -1427,6 +1427,22 @@ int exec_relu_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 	return CCV_NNC_EXEC_SUCCESS;
 }
 
+// the order EWSUM adds its operands in (ew/ccv_nnc_ew_cpu_ref.c:29-45): when the output is the storage of an operand z >= 1, that
+// operand comes first and the rest follow left to right; otherwise plain left to right.  Starting from the aliased operand also keeps
+// it from being overwritten before it is read: the fp32 sum runs in chunks of 8 operands, and every chunk after the first adds onto
+// the output.
+void ewsum_order(ccv_nnc_tensor_t* const* const inputs, const int input_size, const void* const out, int* const order)
+{
+	int k = 0;
+	for (int z = 1; z < input_size && !k; z++)
+		if (inputs[z]->data.u8 == out)
+			k = z;
+	order[0] = k;
+	for (int z = 0, j = 1; z < input_size; z++)
+		if (z != k)
+			order[j++] = z;
+}
+
 // ew/ccv_nnc_ew_cpu_ref.c:15-110,207-214
 int exec_ewsum_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
 {
@@ -1462,8 +1478,11 @@ int exec_ewsum_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const in
 		{
 			if (!inputs[i] || kind_of(inputs[i]) != kind || !view_of(inputs[i]).contiguous || view_of(inputs[i]).count != c.count)
 				return CCV_NNC_EXEC_INVALID;
-			p16[i] = inputs[i]->data.u8;
 		}
+		int order[8];
+		ewsum_order(inputs, input_size, outputs[0]->data.u8, order);
+		for (int i = 0; i < input_size; i++)
+			p16[i] = inputs[order[i]]->data.u8;
 		if (input_size == 1)
 		{
 			if (p16[0] != outputs[0]->data.u8 && cudaMemcpyAsync(outputs[0]->data.u8, p16[0], c.count * 2, cudaMemcpyDeviceToDevice, stream_of(stream_context)) != cudaSuccess)
@@ -1481,8 +1500,11 @@ int exec_ewsum_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const in
 		const TV a = view_of(inputs[i]);
 		if (!a.contiguous || a.count != c.count)
 			return CCV_NNC_EXEC_INVALID;
-		ptrs[i] = inputs[i]->data.f32;
 	}
+	int order[64];
+	ewsum_order(inputs, input_size, outputs[0]->data.u8, order);
+	for (int i = 0; i < input_size; i++)
+		ptrs[i] = inputs[order[i]]->data.f32;
 	cudaStream_t s = stream_of(stream_context);
 	if (input_size == 1)
 	{

@@ -1386,7 +1386,8 @@ int colsum_any(cudaStream_t s, int g_kind, const void* g, size_t rows, int cols,
 		return colsum_f32(s, (const float*)g, rows, cols, ld, (float*)out, accumulate, workspace);
 	if (cols <= 0)
 		return 0;
-	if (cols % 4 || ld % 4 || !workspace || (((uintptr_t)g) & 7))
+	// the vector kernel loads 4 elements of g at once: 16 bytes of fp32, 8 of bf16 / fp16
+	if (cols % 4 || ld % 4 || !workspace || (((uintptr_t)g) & (g_kind == 0 ? 15 : 7)))
 	{
 		colsum_scalar_kernel<<<cols, 256, 0, s>>>(g, g_kind, rows, ld, out, out_kind, accumulate);
 		return check("colsum_scalar");

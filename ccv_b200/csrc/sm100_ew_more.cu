@@ -18,6 +18,7 @@
 #include "sm100_elem.cuh"
 #include "sm100_ew.h"
 #include <cuda_runtime.h>
+#include <float.h>
 #include <math.h>
 #include <string.h>
 
@@ -280,7 +281,10 @@ struct Red4 {
 	long long as[4], bs[4]; // element strides of a and b
 	long long rcount;
 };
-template <int MODE> __device__ __forceinline__ float red_identity() { return MODE == RED_MAX ? -INFINITY : MODE == RED_MIN ? INFINITY : 0.f; }
+// MAX / MIN start from -FLT_MAX / FLT_MAX as the reference does (reduce_max_cpu_ref.c:36, reduce_min_cpu_ref.c:36), not from -inf /
+// inf: a slice of only -inf (a masked row) or only NaN gives -FLT_MAX, so that the backward (a == b) sends none of its gradient there.
+// In bf16 / fp16, -FLT_MAX rounds to -inf on the way out.
+template <int MODE> __device__ __forceinline__ float red_identity() { return MODE == RED_MAX ? -FLT_MAX : MODE == RED_MIN ? FLT_MAX : 0.f; }
 template <int MODE> __device__ __forceinline__ float red_combine(const float x, const float y) { return MODE == RED_MAX ? fmaxf(x, y) : MODE == RED_MIN ? fminf(x, y) : x + y; }
 template <int MODE> __device__ __forceinline__ float red_map(const float v) { return MODE == RED_NORM2 ? v * v : v; }
 template <typename T, int MODE, int THREADS>
