@@ -17,6 +17,7 @@ CCV_NNC_EXEC_SUCCESS, CCV_NNC_EXEC_INVALID, CCV_NNC_EXEC_NO_KERNEL, CCV_NNC_EXEC
 CCV_NNC_UPSAMPLE_NEAREST, CCV_NNC_UPSAMPLE_BILINEAR = 0, 1
 CCV_NNC_MSE_REDUCE_MEAN, CCV_NNC_MSE_REDUCE_SUM = 0, 1  # lib/nnc/ccv_nnc.h:81-84 (cmd.info.mse.reduce_op)
 CCV_NNC_PAD_ZERO, CCV_NNC_PAD_REPLICATE = 0, 1  # lib/nnc/ccv_nnc.h:97-100 (cmd.info.pad.type)
+CCV_NNC_HISTOGRAM_EVEN, CCV_NNC_HISTOGRAM_LOGARITHMIC, CCV_NNC_HISTOGRAM_BINS = 0, 1, 2  # lib/nnc/ccv_nnc.h:86-90 (cmd.info.histogram.type)
 
 # backends (lib/nnc/cmd/ccv_nnc_backend.h + the new one)
 CCV_NNC_BACKEND_CPU_OPT = 0x46deb194
@@ -40,7 +41,7 @@ CMD_IDS = dict(
     CMUL=0xead486e6, BINARY_CROSSENTROPY=0xcd2107ec, SIGMOID_BINARY_CROSSENTROPY=0xd9e0e4a, MSE=0x6904a9a2, SMOOTH_L1=0x4e428e,
     PAD=0xd8aaca60, MIN=0x972fbd26, MAX=0xdf6f014c, ARGMAX=0x68af2804, ARGMIN=0xeb8747f2, REDUCE_ISNAN=0xee0a4ade,
     ROI_ALIGN=0xfef55168, NMS=0xdba26106, LAMB=0x450edb1a, RMSPROP=0x9c886b1c,
-    COMPRESSION_LSSC=0x17ea8f72,
+    COMPRESSION_LSSC=0x17ea8f72, HISTOGRAM=0xc5473e44, EWPROD=0xee07e8fe,
 )
 for _k, _v in CMD_IDS.items():
     globals()["CCV_NNC_%s_FORWARD" % _k] = _v
@@ -141,6 +142,10 @@ class _Clamp(C.Structure):
     _fields_ = [("min", C.c_float), ("max", C.c_float)]
 
 
+class _Histogram(C.Structure):
+    _fields_ = [("type", C.c_int), ("bins", C.c_int), ("min", C.c_float), ("max", C.c_float), ("rate", C.c_float)]
+
+
 class _LeakyRelu(C.Structure):
     _fields_ = [("negative_slope", C.c_float)]
 
@@ -172,7 +177,7 @@ class _Pad(C.Structure):
 class _CmdUnion(C.Union):
     _fields_ = [("convolution", _Convolution), ("convolution_transpose", _ConvolutionTranspose), ("pool", _Pool), ("bnorm", _Bnorm), ("lnorm", _Lnorm), ("gnorm", _Gnorm), ("rmsnorm", _Rmsnorm),
                 ("sgd", _Sgd), ("adam", _Adam), ("lamb", _Lamb), ("rmsprop", _Rmsprop), ("gelu", _Gelu), ("blas", _Blas), ("label_smoothing", _LabelSmoothing), ("reduce", _Reduce), ("transpose", _Transpose),
-                ("upsample", _Upsample), ("clamp", _Clamp), ("leaky_relu", _LeakyRelu), ("dropout", _Dropout), ("scaled_dot_product_attention", _Sdpa),
+                ("upsample", _Upsample), ("clamp", _Clamp), ("histogram", _Histogram), ("leaky_relu", _LeakyRelu), ("dropout", _Dropout), ("scaled_dot_product_attention", _Sdpa),
                 ("binary_crossentropy", _BinaryCrossentropy), ("smooth_l1", _SmoothL1), ("mse", _Mse), ("nms", _Nms), ("pad", _Pad), ("userdata", C.c_void_p)]
 
 

@@ -130,6 +130,7 @@ void ccv_nnc_init(void)
 		CCV_NNC_SM100_DETECTION_COMMANDS(CCV_SM100_CALL_REGISTER)
 		CCV_NNC_SM100_OPTIMIZER_COMMANDS(CCV_SM100_CALL_REGISTER)
 		CCV_NNC_SM100_COMPRESSION_COMMANDS(CCV_SM100_CALL_REGISTER)
+		CCV_NNC_SM100_STATISTICS_COMMANDS(CCV_SM100_CALL_REGISTER)
 #undef CCV_SM100_CALL_REGISTER
 	});
 }

@@ -1545,6 +1545,70 @@ int exec_ewsum_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const in
 	return CCV_NNC_EXEC_SUCCESS;
 }
 
+// EWPROD operands: one floating-point kind, packed, the dims of `like` (no broadcasting), at most 4-d (ew/ccv_nnc_ew_cpu_ref.c:262-264)
+bool ewprod_operand(const ccv_nnc_tensor_t* const t, const int kind, const TV& like)
+{
+	if (!t || kind_of(t) != kind)
+		return false;
+	const TV v = view_of(t);
+	return v.contiguous && v.nd <= 4 && same_shape(v, like);
+}
+
+// ew/ccv_nnc_ew_cpu_ref.c:235-334,1688-1694: c = a0 * a1 * ... in EWSUM's operand order (ewsum_order), every product rounded on its own
+int exec_ewprod_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
+{
+	if (input_size < 1 || output_size < 1 || !inputs || !outputs || !outputs[0])
+		return CCV_NNC_EXEC_INVALID;
+	const int kind = kind_of(outputs[0]);
+	if (kind < 0 || input_size > (kind == 0 ? 64 : 8))
+		return CCV_NNC_EXEC_INVALID;
+	const TV c = view_of(outputs[0]);
+	if (!ewprod_operand(outputs[0], kind, c))
+		return CCV_NNC_EXEC_INVALID;
+	for (int i = 0; i < input_size; i++)
+		if (!ewprod_operand(inputs[i], kind, c))
+			return CCV_NNC_EXEC_INVALID;
+	int order[64];
+	const void* ptrs[64];
+	ewsum_order(inputs, input_size, outputs[0]->data.u8, order);
+	for (int i = 0; i < input_size; i++)
+		ptrs[i] = inputs[order[i]]->data.u8;
+	cudaStream_t s = stream_of(stream_context);
+	if (input_size == 1)
+	{
+		if (ptrs[0] != outputs[0]->data.u8 && c.count && cudaMemcpyAsync(outputs[0]->data.u8, ptrs[0], c.count * kind_size(kind), cudaMemcpyDeviceToDevice, s) != cudaSuccess)
+			return CCV_NNC_EXEC_INVALID;
+		return CCV_NNC_EXEC_SUCCESS;
+	}
+	RC(ew_prod(s, kind, ptrs, input_size, outputs[0]->data.u8, c.count));
+	return CCV_NNC_EXEC_SUCCESS;
+}
+
+// ew/ccv_nnc_ew_cpu_ref.c:336-480: inputs (g, a_1 .. a_n, b), outputs (h_1 .. h_n), h_i = g * b / a_i (b / a_i without g).  Every a, b and h
+// is required; all outputs are written by one launch.
+int exec_ewprod_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
+{
+	if (output_size < 1 || input_size != output_size + 2 || !inputs || !outputs || !inputs[input_size - 1])
+		return CCV_NNC_EXEC_INVALID;
+	const ccv_nnc_tensor_t* const b = inputs[input_size - 1];
+	const int kind = kind_of(b);
+	if (kind < 0 || output_size > (kind == 0 ? 64 : 8))
+		return CCV_NNC_EXEC_INVALID;
+	const TV bv = view_of(b);
+	if (!ewprod_operand(b, kind, bv) || (inputs[0] && !ewprod_operand(inputs[0], kind, bv)))
+		return CCV_NNC_EXEC_INVALID;
+	const void* a[64];
+	void* h[64];
+	for (int z = 0; z < output_size; z++)
+	{
+		if (!ewprod_operand(inputs[z + 1], kind, bv) || !ewprod_operand(outputs[z], kind, bv))
+			return CCV_NNC_EXEC_INVALID;
+		a[z] = inputs[z + 1]->data.u8, h[z] = outputs[z]->data.u8;
+	}
+	RC(ew_prod_back(stream_of(stream_context), kind, inputs[0] ? inputs[0]->data.u8 : 0, b->data.u8, a, h, output_size, bv.count));
+	return CCV_NNC_EXEC_SUCCESS;
+}
+
 // broadcasting helper: c's 4-d shape drives the loop; an operand dimension of 1 broadcasts (stride 0)
 bool bcast_strides(const TV& c, const TV& x, int xs[4])
 {
@@ -2628,6 +2692,8 @@ REGISTER_SM100(CCV_NNC_RMSNORM_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | 
 REGISTER_SM100(CCV_NNC_RMSNORM_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, ccv_nnc_sm100_exec_rmsnorm_back); }
 REGISTER_SM100(CCV_NNC_EWSUM_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF | CCV_32S, 1, exec_ewsum_forw); }
 REGISTER_SM100(CCV_NNC_EWSUM_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_ewsum_back); }
+REGISTER_SM100(CCV_NNC_EWPROD_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_ewprod_forw); }
+REGISTER_SM100(CCV_NNC_EWPROD_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_ewprod_back); }
 REGISTER_SM100(CCV_NNC_ADD_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_via_f32<exec_add_forw>); }
 REGISTER_SM100(CCV_NNC_ADD_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_via_f32<exec_add_back>); }
 REGISTER_SM100(CCV_NNC_MUL_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_via_f32<exec_mul_forw>); }

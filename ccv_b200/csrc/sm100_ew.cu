@@ -1312,6 +1312,119 @@ int ew_sum_16(cudaStream_t s, int kind, const void* const* inputs, int k, void* 
 		sum16_kernel<__half><<<grid_for(vec ? (n >> 3) + 1 : n, 256), 256, 0, s>>>(a, (__half*)out, n, vec);
 	return check("ew_sum16");
 }
+
+// ew/ccv_nnc_ew_cpu_ref.c:235-334 (EWPROD): c = a0 * a1 * ..., every product rounded on its own, left to right.  fp32 in chunks of
+// 8 operands like EWSUM, each later chunk continuing from the output; 16-bit in one launch of <= 8 widened operands, rounded once.
+// The running product starts from 1, and 1 * a0 is a0 exactly (signed zeros and NaN payloads included).
+template <typename T, int VEC>
+__global__ void prod_kernel(const SumArgs16 a, T* __restrict__ out, const size_t n, const int accumulate)
+{
+	const size_t nv = VEC > 1 ? n / VEC : 0;
+	if constexpr (VEC > 1)
+	for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < nv; i += (size_t)gridDim.x * blockDim.x)
+	{
+		float acc[VEC];
+		if (accumulate)
+			ldv(out + i * VEC, acc);
+		else
+#pragma unroll
+			for (int k = 0; k < VEC; k++)
+				acc[k] = 1.f;
+#pragma unroll 8
+		for (int j = 0; j < a.k; j++)
+		{
+			float v[VEC];
+			ldv(reinterpret_cast<const T*>(a.in[j]) + i * VEC, v);
+#pragma unroll
+			for (int k = 0; k < VEC; k++)
+				acc[k] = __fmul_rn(acc[k], v[k]);
+		}
+		stv(out + i * VEC, acc);
+	}
+	for (size_t i = nv * VEC + blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+	{
+		float acc = accumulate ? ldf(out + i) : 1.f;
+		for (int j = 0; j < a.k; j++)
+			acc = __fmul_rn(acc, ldf(reinterpret_cast<const T*>(a.in[j]) + i));
+		stf(out + i, acc);
+	}
+}
+template <typename T>
+static int prod_t(cudaStream_t s, const void* const* inputs, int k, T* out, size_t n)
+{
+	constexpr int W = Vec16<T>::W;
+	for (int done = 0; done < k;)
+	{
+		SumArgs16 a;
+		a.k = (k - done) > 8 ? 8 : (k - done);
+		bool vec = aligned_v16(out);
+		for (int j = 0; j < a.k; j++)
+			a.in[j] = inputs[done + j], vec = vec && aligned_v16(a.in[j]);
+		if (vec)
+			prod_kernel<T, W><<<grid_for(n / W + 1, 256), 256, 0, s>>>(a, out, n, done > 0);
+		else
+			prod_kernel<T, 1><<<grid_for(n, 256), 256, 0, s>>>(a, out, n, done > 0);
+		if (check("ew_prod"))
+			return -1;
+		done += a.k;
+	}
+	return 0;
+}
+int ew_prod(cudaStream_t s, int kind, const void* const* inputs, int k, void* out, size_t n)
+{
+	if (n == 0 || k <= 0)
+		return 0;
+	if (k > (kind == 0 ? 64 : 8))
+		return 1;
+	return kind == 0 ? prod_t<float>(s, inputs, k, (float*)out, n) : kind == 1 ? prod_t<__nv_bfloat16>(s, inputs, k, (__nv_bfloat16*)out, n) : prod_t<__half>(s, inputs, k, (__half*)out, n);
+}
+
+// ew/ccv_nnc_ew_cpu_ref.c:336-480 (EWPROD backward): h_z = g * b / a_z, or b / a_z without g, each operation rounded on its own.  One
+// launch for every output; a thread reads all operands of its element before it writes any output, so outputs may alias inputs.
+template <int MAXK>
+struct ProdBackArgs {
+	const void* a[MAXK];
+	void* h[MAXK];
+	const void* g;
+	const void* b;
+	int k;
+};
+template <typename T, int MAXK>
+__global__ void prod_back_kernel(const ProdBackArgs<MAXK> p, const size_t n)
+{
+	for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+	{
+		const float bv = ldf(reinterpret_cast<const T*>(p.b) + i);
+		const float num = p.g ? __fmul_rn(ldf(reinterpret_cast<const T*>(p.g) + i), bv) : bv;
+		float r[MAXK];
+#pragma unroll
+		for (int z = 0; z < MAXK; z++)
+			if (z < p.k)
+				r[z] = __fdiv_rn(num, ldf(reinterpret_cast<const T*>(p.a[z]) + i));
+#pragma unroll
+		for (int z = 0; z < MAXK; z++)
+			if (z < p.k)
+				stf(reinterpret_cast<T*>(p.h[z]) + i, r[z]);
+	}
+}
+template <typename T, int MAXK>
+static int prod_back_t(cudaStream_t s, const void* g, const void* b, const void* const* a, void* const* h, int k, size_t n)
+{
+	ProdBackArgs<MAXK> p;
+	p.g = g, p.b = b, p.k = k;
+	for (int z = 0; z < k; z++)
+		p.a[z] = a[z], p.h[z] = h[z];
+	prod_back_kernel<T, MAXK><<<grid_for(n, 256), 256, 0, s>>>(p, n);
+	return check("ew_prod_back");
+}
+int ew_prod_back(cudaStream_t s, int kind, const void* g, const void* b, const void* const* a, void* const* h, int k, size_t n)
+{
+	if (n == 0 || k <= 0)
+		return 0;
+	if (k > (kind == 0 ? 64 : 8))
+		return 1;
+	return kind == 0 ? prod_back_t<float, 64>(s, g, b, a, h, k, n) : kind == 1 ? prod_back_t<__nv_bfloat16, 8>(s, g, b, a, h, k, n) : prod_back_t<__half, 8>(s, g, b, a, h, k, n);
+}
 // column sums with any input / output element kind: per-block partial rows (fp32) in the workspace, combined in a fixed order
 template <typename T>
 __global__ void __launch_bounds__(256) colsum_any_kernel(const T* __restrict__ g, const size_t rows, const int cols, const long long ld, float* __restrict__ part)

@@ -25,6 +25,10 @@ int ew_relu_bwd_f32(cudaStream_t s, const float* g, const float* b, float* h, si
 int ew_relu_fwd_16(cudaStream_t s, int kind, const void* a, void* b, size_t n);
 int ew_relu_bwd_16(cudaStream_t s, int kind, const void* g, const void* b, void* h, size_t n);
 int ew_sum_16(cudaStream_t s, int kind, const void* const* inputs, int k, void* out, size_t n); // k <= 8
+// EWPROD, kind 0 = fp32 (k <= 64), 1 = bf16, 2 = fp16 (k <= 8): out = in[0] * in[1] * ... left to right (out may alias in[0]);
+// backward h[z] = g * b / a[z] (b / a[z] without g) for every z in one launch (any output may alias any input)
+int ew_prod(cudaStream_t s, int kind, const void* const* inputs, int k, void* out, size_t n);
+int ew_prod_back(cudaStream_t s, int kind, const void* g, const void* b, const void* const* a, void* const* h, int k, size_t n);
 // out[c] (+)= sum over rows of g[row * ld + c]  (bias gradients of GEMM / convolution)
 // workspace (colsum_workspace_bytes(cols), may be NULL): per-block partial rows, combined in a fixed order instead of by atomics
 size_t colsum_workspace_bytes(int cols);

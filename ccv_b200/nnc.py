@@ -920,6 +920,58 @@ def lssc_compressed_dims(dims, fmt):
     return dims
 
 
+def _histogram(type_, bins=0, lo=0.0, hi=0.0, rate=0.0, **kw):
+    c = _simple(abi.CCV_NNC_HISTOGRAM_FORWARD, **kw)
+    h = c.info.histogram
+    h.type, h.bins, h.min, h.max, h.rate = type_, bins, lo, hi, rate
+    return c
+
+
+def CMD_HISTOGRAM_EVEN(bins, lo, hi, **kw):
+    """HISTOGRAM (cmd/histogram): inputs (a) -> outputs (b int32 of bins + 3 counts, [s fp32 >= 4: min, max, sum, sum of squares]);
+    b[0] below lo, b[1 .. bins] the even bins of [lo, hi), b[bins + 1] at or above hi, b[bins + 2] NaN"""
+    return _histogram(abi.CCV_NNC_HISTOGRAM_EVEN, bins, lo, hi, **kw)
+
+
+def CMD_HISTOGRAM_LOG(lo=1e-12, hi=1e20, rate=1.1, **kw):
+    """inputs (a) -> outputs (b of >= histogram_bin_count(cmd) counts, [s]): bins whose edges grow by `rate` from lo to hi, mirrored
+    for negative values around the bin of (-lo, lo); the defaults are the reference's CMD_HISTOGRAM_LOG()"""
+    return _histogram(abi.CCV_NNC_HISTOGRAM_LOGARITHMIC, 0, lo, hi, rate, **kw)
+
+
+def CMD_HISTOGRAM_BINS(**kw):
+    """inputs (a, bounds fp32 of n values) -> outputs (b of n + 2 counts, [s]); b[i] counts the values v with bounds[i - 1] <= v <
+    bounds[i] as CPU_REF's binary search finds them, b[n + 1] NaN"""
+    return _histogram(abi.CCV_NNC_HISTOGRAM_BINS, **kw)
+
+
+def histogram_bin_count(cmd, bounds_count=0):
+    """The count of b the reference's _ccv_nnc_histogram_tensor_auto_forw gives: EVEN bins + 3, BINS n + 2, LOG 2 u + 2 with
+    u = ceilf(logf(max / min) * (float)(1.0 / logf(rate))), computed with the host's logf in float as the reference does"""
+    h = cmd.info.histogram
+    if h.type == abi.CCV_NNC_HISTOGRAM_EVEN:
+        return h.bins + 3
+    if h.type == abi.CCV_NNC_HISTOGRAM_BINS:
+        return bounds_count + 2
+    logf = C.CDLL("libm.so.6").logf
+    logf.restype, logf.argtypes = C.c_float, [C.c_float]
+    f = np.float32
+    log_base = f(1.0 / float(f(logf(f(h.rate)))))
+    upper = int(np.ceil(f(f(logf(f(f(h.max) / f(h.min)))) * log_base)))
+    return 2 * upper + 2
+
+
+def CMD_EWPROD_FORWARD(**kw):
+    """EWPROD (cmd/ew): inputs (a_0 .. a_{n-1}) -> outputs (c), c = a_0 * a_1 * ..., each product rounded on its own; when c is the
+    storage of some a_k (k >= 1) the order is a_k * a_0 * a_1 ... (skipping k), as the reference's"""
+    return _simple(abi.CCV_NNC_EWPROD_FORWARD, **kw)
+
+
+def CMD_EWPROD_BACKWARD(**kw):
+    """inputs (g or None, a_1 .. a_n, b) -> outputs (h_1 .. h_n), h_i = g * b / a_i (b / a_i without g)"""
+    return _simple(abi.CCV_NNC_EWPROD_BACKWARD, **kw)
+
+
 def CMD_DROPOUT_FORWARD(p, entirety=0, **kw):
     c = _simple(abi.CCV_NNC_DROPOUT_FORWARD, **kw)
     c.info.dropout.p, c.info.dropout.entirety = p, entirety

@@ -280,6 +280,13 @@ typedef struct {
 			float max;
 		} clamp;
 		struct {
+			int type; /* CCV_NNC_HISTOGRAM_EVEN / _LOGARITHMIC / _BINS */
+			int bins; /* EVEN: the number of bins between min and max */
+			float min; /* EVEN, LOGARITHMIC */
+			float max; /* EVEN, LOGARITHMIC */
+			float rate; /* LOGARITHMIC: the ratio of one bin edge to the previous one */
+		} histogram;
+		struct {
 			float negative_slope;
 		} leaky_relu;
 		struct {
@@ -510,6 +517,18 @@ enum {
 	/* cmd/compression */
 	CCV_NNC_COMPRESSION_LSSC_FORWARD = 0x17ea8f72,
 	CCV_NNC_COMPRESSION_LSSC_BACKWARD = 0x17ea8f73,
+	/* cmd/histogram, cmd/ew */
+	CCV_NNC_HISTOGRAM_FORWARD = 0xc5473e44,
+	CCV_NNC_HISTOGRAM_BACKWARD = 0xc5473e45,
+	CCV_NNC_EWPROD_FORWARD = 0xee07e8fe,
+	CCV_NNC_EWPROD_BACKWARD = 0xee07e8ff,
+};
+
+/* lib/nnc/ccv_nnc.h:86-90 (cmd.info.histogram.type) */
+enum {
+	CCV_NNC_HISTOGRAM_EVEN = 0,
+	CCV_NNC_HISTOGRAM_LOGARITHMIC = 1,
+	CCV_NNC_HISTOGRAM_BINS = 2,
 };
 
 /* lib/nnc/ccv_nnc.h:97-100 (cmd.info.pad.type) */
@@ -603,6 +622,9 @@ CCV_NNC_SM100_OPTIMIZER_COMMANDS(CCV_SM100_DECLARE_REGISTER)
 #define CCV_NNC_SM100_COMPRESSION_COMMANDS(X) \
 	X(CCV_NNC_COMPRESSION_LSSC_FORWARD) X(CCV_NNC_COMPRESSION_LSSC_BACKWARD)
 CCV_NNC_SM100_COMPRESSION_COMMANDS(CCV_SM100_DECLARE_REGISTER)
+#define CCV_NNC_SM100_STATISTICS_COMMANDS(X) \
+	X(CCV_NNC_HISTOGRAM_FORWARD) X(CCV_NNC_HISTOGRAM_BACKWARD) X(CCV_NNC_EWPROD_FORWARD) X(CCV_NNC_EWPROD_BACKWARD)
+CCV_NNC_SM100_STATISTICS_COMMANDS(CCV_SM100_DECLARE_REGISTER)
 #undef CCV_SM100_DECLARE_REGISTER
 
 /* What the backend needs back from its host (ccv's own when linked into libccv: lib/nnc/gpu/ccv_nnc_compat.h:95-97,

@@ -191,6 +191,7 @@ def main():
     sm100_cmds += re.findall(r"X\((CCV_NNC_[A-Z0-9_]+)\)", header[header.index("#define CCV_NNC_SM100_DETECTION_COMMANDS(X)"):header.index("CCV_NNC_SM100_DETECTION_COMMANDS(CCV_SM100_DECLARE_REGISTER)")])
     sm100_cmds += re.findall(r"X\((CCV_NNC_[A-Z0-9_]+)\)", header[header.index("#define CCV_NNC_SM100_OPTIMIZER_COMMANDS(X)"):header.index("CCV_NNC_SM100_OPTIMIZER_COMMANDS(CCV_SM100_DECLARE_REGISTER)")])
     sm100_cmds += re.findall(r"X\((CCV_NNC_[A-Z0-9_]+)\)", header[header.index("#define CCV_NNC_SM100_COMPRESSION_COMMANDS(X)"):header.index("CCV_NNC_SM100_COMPRESSION_COMMANDS(CCV_SM100_DECLARE_REGISTER)")])
+    sm100_cmds += re.findall(r"X\((CCV_NNC_[A-Z0-9_]+)\)", header[header.index("#define CCV_NNC_SM100_STATISTICS_COMMANDS(X)"):header.index("CCV_NNC_SM100_STATISTICS_COMMANDS(CCV_SM100_DECLARE_REGISTER)")])
     ids = dict(cmds)
     lines = ["/* regenerated by tools/gen_backend_ph.py: what build-cmd.rb adds to ccv_nnc_cmd.inc for every (command, GPU_SM100) pair */"]
     for c in sm100_cmds:
