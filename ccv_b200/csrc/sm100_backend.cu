@@ -2492,9 +2492,10 @@ const int ALL_FORMATS = CCV_TENSOR_FORMAT_NCHW | CCV_TENSOR_FORMAT_NHWC | CCV_TE
 // scratch copies of the operands): every algorithm of this backend that accepts the shapes is timed on the device (CUDA
 // events on the caller's stream, best of 3 after a warm-up) and the index of the fastest one is returned.  The generic
 // fallback of the reference times the asynchronous *enqueue* with a host clock (ccv_nnc_cmd.c:549-555), which says nothing
-// about a GPU kernel -- hence a real autotune function.
-template <ccv_nnc_cmd_exec_f EXEC>
-int autotune_contraction(const ccv_nnc_cmd_t cmd, const size_t max_workspace_size, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
+// about a GPU kernel -- hence a real autotune function.  The attention commands use it too: algorithm 0 refuses some calls algorithm 1
+// runs (a 16-bit D = 160 forward that asks for the log-sum-exp), so the tuned command is the one that runs.
+template <ccv_nnc_cmd_exec_f EXEC, int COUNT>
+int autotune_algorithms(const ccv_nnc_cmd_t cmd, const size_t max_workspace_size, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
 {
 	cudaStream_t s = stream_of(stream_context);
 	cudaEvent_t e0, e1;
@@ -2502,11 +2503,10 @@ int autotune_contraction(const ccv_nnc_cmd_t cmd, const size_t max_workspace_siz
 		return 0;
 	int best = 0;
 	float best_ms = -1.f;
-	const int candidates[3] = { CCV_NNC_SM100_ALGO_TF32, CCV_NNC_SM100_ALGO_3XTF32, CCV_NNC_SM100_ALGO_FFMA };
-	for (int k = 0; k < 3; k++)
+	for (int k = 0; k < COUNT; k++) // the contractions: TF32, 3XTF32, FFMA; attention: COMPOSED, FLASH
 	{
 		ccv_nnc_cmd_t c = cmd;
-		c.algorithm = candidates[k];
+		c.algorithm = k;
 		if (EXEC(c, hint, flags, inputs, input_size, outputs, output_size, stream_context) != CCV_NNC_EXEC_SUCCESS) // warm-up + applicability
 			continue;
 		float ms = -1.f;
@@ -2522,7 +2522,7 @@ int autotune_contraction(const ccv_nnc_cmd_t cmd, const size_t max_workspace_siz
 				ms = t;
 		}
 		if (ms >= 0.f && (best_ms < 0.f || ms < best_ms))
-			best_ms = ms, best = candidates[k];
+			best_ms = ms, best = k;
 	}
 	cudaEventDestroy(e0);
 	cudaEventDestroy(e1);
@@ -2672,14 +2672,14 @@ int exec_via_f32_rt(ccv_nnc_cmd_exec_f f32, const ccv_nnc_cmd_t cmd, const ccv_n
 
 #define REGISTER_SM100(cmd) extern "C" void _register_command_ ## cmd ## _backend_CCV_NNC_BACKEND_GPU_SM100(ccv_nnc_cmd_backend_registry_t* const registry)
 
-REGISTER_SM100(CCV_NNC_GEMM_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_gemm_forw_any); registry->autotune = autotune_contraction<exec_gemm_forw_any>; }
-REGISTER_SM100(CCV_NNC_GEMM_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_gemm_back_any); registry->autotune = autotune_contraction<exec_gemm_back_any>; }
-REGISTER_SM100(CCV_NNC_CONVOLUTION_FORWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_conv_any<conv_forw_nhwc, conv_forw_workspace, 0>); registry->autotune = autotune_contraction<exec_conv_any<conv_forw_nhwc, conv_forw_workspace, 0> >; }
-REGISTER_SM100(CCV_NNC_CONVOLUTION_BACKWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_conv_any<conv_back_nhwc, conv_back_workspace, 1>); registry->autotune = autotune_contraction<exec_conv_any<conv_back_nhwc, conv_back_workspace, 1> >; }
-REGISTER_SM100(CCV_NNC_CONVOLUTION_TRANSPOSE_FORWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_conv_any<conv_transpose_forw_nhwc, conv_transpose_forw_workspace, 0>); registry->autotune = autotune_contraction<exec_conv_any<conv_transpose_forw_nhwc, conv_transpose_forw_workspace, 0> >; }
-REGISTER_SM100(CCV_NNC_CONVOLUTION_TRANSPOSE_BACKWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_conv_any<conv_transpose_back_nhwc, conv_transpose_back_workspace, 1>); registry->autotune = autotune_contraction<exec_conv_any<conv_transpose_back_nhwc, conv_transpose_back_workspace, 1> >; }
-REGISTER_SM100(CCV_NNC_SCALED_DOT_PRODUCT_ATTENTION_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, 1, ccv_nnc_sm100_exec_sdpa_forw); }
-REGISTER_SM100(CCV_NNC_SCALED_DOT_PRODUCT_ATTENTION_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, ccv_nnc_sm100_exec_sdpa_back); }
+REGISTER_SM100(CCV_NNC_GEMM_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_gemm_forw_any); registry->autotune = autotune_algorithms<exec_gemm_forw_any, CCV_NNC_SM100_ALGO_COUNT>; }
+REGISTER_SM100(CCV_NNC_GEMM_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_gemm_back_any); registry->autotune = autotune_algorithms<exec_gemm_back_any, CCV_NNC_SM100_ALGO_COUNT>; }
+REGISTER_SM100(CCV_NNC_CONVOLUTION_FORWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_conv_any<conv_forw_nhwc, conv_forw_workspace, 0>); registry->autotune = autotune_algorithms<exec_conv_any<conv_forw_nhwc, conv_forw_workspace, 0> , CCV_NNC_SM100_ALGO_COUNT>; }
+REGISTER_SM100(CCV_NNC_CONVOLUTION_BACKWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_conv_any<conv_back_nhwc, conv_back_workspace, 1>); registry->autotune = autotune_algorithms<exec_conv_any<conv_back_nhwc, conv_back_workspace, 1> , CCV_NNC_SM100_ALGO_COUNT>; }
+REGISTER_SM100(CCV_NNC_CONVOLUTION_TRANSPOSE_FORWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_conv_any<conv_transpose_forw_nhwc, conv_transpose_forw_workspace, 0>); registry->autotune = autotune_algorithms<exec_conv_any<conv_transpose_forw_nhwc, conv_transpose_forw_workspace, 0> , CCV_NNC_SM100_ALGO_COUNT>; }
+REGISTER_SM100(CCV_NNC_CONVOLUTION_TRANSPOSE_BACKWARD) { fill(registry, CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_conv_any<conv_transpose_back_nhwc, conv_transpose_back_workspace, 1>); registry->autotune = autotune_algorithms<exec_conv_any<conv_transpose_back_nhwc, conv_transpose_back_workspace, 1> , CCV_NNC_SM100_ALGO_COUNT>; }
+REGISTER_SM100(CCV_NNC_SCALED_DOT_PRODUCT_ATTENTION_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_SDPA_ALGO_COUNT, ccv_nnc_sm100_exec_sdpa_forw); registry->autotune = autotune_algorithms<ccv_nnc_sm100_exec_sdpa_forw, CCV_NNC_SM100_SDPA_ALGO_COUNT>; }
+REGISTER_SM100(CCV_NNC_SCALED_DOT_PRODUCT_ATTENTION_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, CCV_NNC_SM100_SDPA_ALGO_COUNT, ccv_nnc_sm100_exec_sdpa_back); registry->autotune = autotune_algorithms<ccv_nnc_sm100_exec_sdpa_back, CCV_NNC_SM100_SDPA_ALGO_COUNT>; }
 REGISTER_SM100(CCV_NNC_SOFTMAX_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_via_f32<exec_softmax_forw>); }
 REGISTER_SM100(CCV_NNC_SOFTMAX_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_via_f32<exec_softmax_back>); }
 REGISTER_SM100(CCV_NNC_BATCH_NORM_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_bnorm_forw); }

@@ -205,6 +205,9 @@ static int sdpa_forw_core(SM100_EXEC_ARGS)
 			lse = outputs[1]->data.f32;
 		}
 		int rc = mask ? 1 : sdpa_forward_f16(stream_of(stream_context), g, dt == CCV_16BF, inputs[0]->data.u8, inputs[1]->data.u8, inputs[2]->data.u8, outputs[0]->data.u8, lse);
+		// algorithm 1 also runs 128 < D <= 256 on the wide flash kernel (sm100_fmha_wide.cu); what it does not take goes on as algorithm 0
+		if (rc == 1 && !mask && cmd.algorithm == CCV_NNC_SM100_SDPA_ALGO_FLASH)
+			rc = sdpa_forward_f16_wide(stream_of(stream_context), g, dt == CCV_16BF, inputs[0]->data.u8, inputs[1]->data.u8, inputs[2]->data.u8, outputs[0]->data.u8, lse);
 		if (rc < 0)
 			return CCV_NNC_EXEC_INVALID;
 		if (rc == 0)
@@ -246,7 +249,8 @@ static int sdpa_forw_core(SM100_EXEC_ARGS)
 
 // The command's entry point.  With "unify head" weights (inputs[4] = w [H Dv, H Dv], inputs[5] = bias, :26-27,:184-255) the per-head
 // attention goes to outputs[2] and outputs[0] = that tensor seen as [B, Sq, H Dv], times w^T, plus bias: the attention above followed
-// by one dense projection on the tensor cores (fp32: the GEMM command's default 3xTF32; 16-bit: kind::f16).
+// by one dense projection on the tensor cores (fp32: the GEMM command's default 3xTF32; 16-bit: kind::f16).  cmd.algorithm selects the
+// attention's kernels (CCV_NNC_SM100_SDPA_ALGO_*) with or without the projection.
 int ccv_nnc_sm100_exec_sdpa_forw(SM100_EXEC_ARGS)
 {
 	ccv_nnc_tensor_t* const w = input_size > 4 ? inputs[4] : 0;
@@ -351,8 +355,12 @@ int ccv_nnc_sm100_exec_sdpa_back(SM100_EXEC_ARGS)
 			void* const fws = ccv_nnc_stream_context_get_workspace(stream_context, sdpa_backward_f16_workspace_bytes(g, need_forward), CCV_TENSOR_GPU_MEMORY);
 			if (!fws)
 				return CCV_NNC_EXEC_OOM;
-			const int rc = sdpa_backward_f16(stream_of(stream_context), g, dg, dt == CCV_16BF, inputs[0]->data.u8, inputs[3]->data.u8, inputs[4]->data.u8, inputs[5]->data.u8, o_ptr, oo_b, oo_s, oo_h, lse_ptr,
+			int rc = sdpa_backward_f16(stream_of(stream_context), g, dg, dt == CCV_16BF, inputs[0]->data.u8, inputs[3]->data.u8, inputs[4]->data.u8, inputs[5]->data.u8, o_ptr, oo_b, oo_s, oo_h, lse_ptr,
 				outputs[0]->data.u8, outputs[1]->data.u8, outputs[2]->data.u8, fws);
+			// algorithm 1: 128 < D <= 256 on the wide fused kernels, in the same workspace
+			if (rc == 1 && cmd.algorithm == CCV_NNC_SM100_SDPA_ALGO_FLASH)
+				rc = sdpa_backward_f16_wide(stream_of(stream_context), g, dg, dt == CCV_16BF, inputs[0]->data.u8, inputs[3]->data.u8, inputs[4]->data.u8, inputs[5]->data.u8, o_ptr, oo_b, oo_s, oo_h, lse_ptr,
+					outputs[0]->data.u8, outputs[1]->data.u8, outputs[2]->data.u8, fws);
 			if (rc < 0)
 				return CCV_NNC_EXEC_INVALID;
 			if (rc == 0)

@@ -132,6 +132,12 @@ int depalettize(cudaStream_t stream, const void* in, int palette_datatype, int q
 constexpr int PALETTIZED_GEMM_M_MAX = 1;
 int gemm_palettized_f16(cudaStream_t stream, int M, int N, int K, const void* a, long long lda, const void* wq, int qbits, int nib, void* c, long long ldc, const float* bias32, const void* bias16);
 
+// 16-bit flash attention with wide heads (sm100_fmha_wide.cu): 128 < D = Dv <= 256, a multiple of 8.  The arguments, workspace and
+// return convention of sdpa_forward_f16 / sdpa_backward_f16 (sdpa_backward_f16_workspace_bytes covers these kernels too).
+int sdpa_forward_f16_wide(cudaStream_t s, const SdpaGeom& g, int is_bf16, const void* q, const void* k, const void* v, void* o, float* lse);
+int sdpa_backward_f16_wide(cudaStream_t s, const SdpaGeom& g, const SdpaGeom& dg, int is_bf16, const void* dout, const void* q, const void* k, const void* v, const void* out, long long oo_b, long long oo_s, long long oo_h,
+	const float* lse, void* dq, void* dk, void* dv, void* workspace);
+
 // bookkeeping shared by every launcher in the backend
 void count_launch(int n = 1);
 unsigned long long launch_count();

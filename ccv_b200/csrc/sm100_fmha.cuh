@@ -21,6 +21,11 @@ __device__ __forceinline__ uint32_t pack2(const float a, const float b, const in
 	return *reinterpret_cast<const uint32_t*>(&v);
 }
 
+__device__ __forceinline__ float widen16(const uint16_t u, const int is_bf16)
+{
+	return is_bf16 ? __uint_as_float((uint32_t)u << 16) : __half2float(__ushort_as_half(u));
+}
+
 // the m16n8k16 A fragment of 16 key columns [16 kk, 16 kk + 16) of a wgmma accumulator (see sm100_ptx.cuh), rounded to 16 bits
 template <int R>
 __device__ __forceinline__ void acc_to_a(const float (&x)[R], const int kk, const int is_bf16, uint32_t (&a)[4])

@@ -66,11 +66,6 @@ struct FmhaBwdSmem {
 	static_assert(TOTAL <= 232448, "227 KB of shared memory per CTA");
 };
 
-__device__ __forceinline__ float widen16(const uint16_t u, const int is_bf16)
-{
-	return is_bf16 ? __uint_as_float((uint32_t)u << 16) : __half2float(__ushort_as_half(u));
-}
-
 // (-lse * log2 e, -delta) per query row: 16 lanes per row, 8 features each
 __global__ void __launch_bounds__(256) fmha_bwd_prep_kernel(const uint16_t* __restrict__ dout, const uint16_t* __restrict__ out, const float* __restrict__ lse, float* __restrict__ stat, int B, int H, int Sq, int Sq_r, int D, int is_bf16,
 	long long do_b, long long do_s, long long do_h, long long o_b, long long o_s, long long o_h)

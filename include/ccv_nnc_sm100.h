@@ -564,6 +564,13 @@ enum {
 	CCV_NNC_SM100_ALGO_COUNT = 3,
 };
 
+/* algorithm selectors of this backend for SCALED_DOT_PRODUCT_ATTENTION_FORWARD / _BACKWARD (cmd.algorithm; -1 = COMPOSED) */
+enum {
+	CCV_NNC_SM100_SDPA_ALGO_COMPOSED = 0, /* 16-bit D <= 128: the flash kernels; every other call: the fp32 path (16-bit widened) */
+	CCV_NNC_SM100_SDPA_ALGO_FLASH = 1,    /* as COMPOSED, plus 16-bit 128 < D = Dv <= 256 without a mask on the wide flash kernels */
+	CCV_NNC_SM100_SDPA_ALGO_COUNT = 2,
+};
+
 /* ------------------------------------------------------------------------------------------------------------ */
 /* (A) BACKEND registration surface.  One symbol per (command, backend) pair, spelled exactly as                */
 /* REGISTER_COMMAND_BACKEND(x, y) does (lib/nnc/ccv_nnc_internal.h:196-202); called by the generated            */
