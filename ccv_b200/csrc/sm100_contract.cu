@@ -304,17 +304,17 @@ void conv_stats_request(float* part, int max_rows, int* rows_out)
 		*rows_out = 0;
 }
 
-template <int AMODE, int BMODE, int BN, int X3 = 0, int K16 = 0, int OUT16 = 0>
+template <int AMODE, int BMODE, int BN, int X3 = 0, int K16 = 0, int OUT16 = 0, int BM = UMMA_BLOCK_M>
 static int launch_umma(cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB, const UmmaGemmParams& p)
 {
 	constexpr bool XF = GemmXform<AMODE, BMODE, K16, X3>::ANY, ARS = GemmXform<AMODE, BMODE, K16, X3>::A_RS;
-	constexpr int STAGES = GemmStages<BN, XF, X3, ARS>::value;
-	using S = UmmaSmem<BN, STAGES, XF, X3, ARS>;
-	auto kern = umma_gemm_kernel<AMODE, BMODE, BN, STAGES, X3, K16, OUT16>;
+	constexpr int STAGES = GemmStages<BN, XF, X3, ARS, BM, AMODE == OP_IM2COL_RS>::value;
+	using S = UmmaSmem<BN, STAGES, XF, X3, ARS, BM>;
+	auto kern = umma_gemm_kernel<AMODE, BMODE, BN, STAGES, X3, K16, OUT16, BM>;
 	static bool configured[MAX_DEVICES];
 	if (ensure_dynamic_smem(kern, S::TOTAL, configured, "cudaFuncSetAttribute(umma_gemm_kernel)"))
 		return -1;
-	const int tiles_m = (p.M + UMMA_BLOCK_M - 1) / UMMA_BLOCK_M, tiles_n = (p.N + BN - 1) / BN;
+	const int tiles_m = (p.M + BM - 1) / BM, tiles_n = (p.N + BN - 1) / BN;
 	dim3 grid(tiles_m, tiles_n, p.grid_taps * p.splits);
 	UmmaGemmParams q = p;
 	q.stats = 0, q.stats_rows = 0;
@@ -342,11 +342,11 @@ static int launch_umma(cudaStream_t stream, const CUtensorMap& tmA, const CUtens
 		}
 	}
 	const long long sms = num_sms(), columns = (long long)grid.y * grid.z, ctas = tiles_m * columns;
-	if (!q.stats && p.splits == 1 && p.grid_taps == 1 && BMODE != OP_IM2COL && ctas > sms)
+	if (!q.stats && p.splits == 1 && p.grid_taps == 1 && BMODE != OP_IM2COL && AMODE != OP_IM2COL_RS && ctas > sms)
 	{
 		// more tiles than one wave of one CTA per SM: gx CTAs per column walk the M tiles, so the producer loads the next tile while the
 		// consumers store this one.  Taken only when it costs no more rounds of tiles than one tile per CTA does.  Not for split-K or
-		// im2col-B launches (the weight gradients with filter taps): their few M tiles share one large B slice per column, which
+		// im2col launches of the weight gradient (the filter taps along a tile's columns or rows): their few M tiles share one large B slice per column, which
 		// side-by-side CTAs read from L2 once and walking CTAs read again from HBM (walked, ResNet-50's 1x1 weight gradients ran 12-19 %
 		// slower on an H100)
 		long long gx = sms / columns;
@@ -483,11 +483,19 @@ static int launch_kind16(cudaStream_t stream, const CUtensorMap& tmA, const CUte
 	return bn == 64 ? launch_umma<AMODE, BMODE, 64, 0, 2, 0>(stream, tmA, tmB, p) : launch_umma<AMODE, BMODE, 128, 0, 2, 0>(stream, tmA, tmB, p);
 }
 // AMODE = OP_MN2D_RS: TF32 reads A into registers (bn 64, 128 or 256); 3xTF32 and the 16-bit kinds read the same operand as OP_MN2D.
+// AMODE = OP_IM2COL_RS: TF32 only, bn 32 or 64, tiles of bm = 128 or 256 rows.
 template <int AMODE, int BMODE>
-static int launch_kind(cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB, const UmmaGemmParams& p, int bn, int kind, bool out16)
+static int launch_kind(cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB, const UmmaGemmParams& p, int bn, int kind, bool out16, int bm = UMMA_BLOCK_M)
 {
 	constexpr int A_SS = AMODE == OP_MN2D_RS ? OP_MN2D : AMODE;
-	if (kind == 0)
+	if constexpr (AMODE == OP_IM2COL_RS)
+	{
+		if (kind != 0 || t_x3)
+			return 1;
+		if (bm == 256)
+			return bn == 32 ? launch_umma<AMODE, BMODE, 32, 0, 0, 0, 256>(stream, tmA, tmB, p) : launch_umma<AMODE, BMODE, 64, 0, 0, 0, 256>(stream, tmA, tmB, p);
+		return bn == 32 ? launch_umma<AMODE, BMODE, 32>(stream, tmA, tmB, p) : launch_umma<AMODE, BMODE, 64>(stream, tmA, tmB, p);
+	} else if (kind == 0)
 	{
 		if (t_x3)
 			return bn == 64 ? launch_umma<A_SS, BMODE, 64, 1>(stream, tmA, tmB, p) : launch_umma<A_SS, BMODE, 128, 1>(stream, tmA, tmB, p);
@@ -496,20 +504,21 @@ static int launch_kind(cudaStream_t stream, const CUtensorMap& tmA, const CUtens
 		else
 			return bn == 64 ? launch_umma<AMODE, BMODE, 64>(stream, tmA, tmB, p) : launch_umma<AMODE, BMODE, 128>(stream, tmA, tmB, p);
 	}
-	return launch_kind16<A_SS, BMODE>(stream, tmA, tmB, p, bn, kind, out16);
+	else
+		return launch_kind16<A_SS, BMODE>(stream, tmA, tmB, p, bn, kind, out16);
 }
 
 // Launch with the split factor already chosen in p.splits.  One split: straight into `out` (pitch ldo, element kind `kind`).
 // Several: fp32 slices [rows, ldp] in the scratch, one per split, then the ordered combine into `out` (which also applies
 // CCV_NNC_ACCUMULATE_OUTPUT and rounds once for 16-bit outputs).
 template <int AMODE, int BMODE>
-static int launch_umma_split(cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB, UmmaGemmParams& p, int bn, int kind, const Scratch& scratch, int rows, int cols, void* out, long long ldo, int accumulate)
+static int launch_umma_split(cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB, UmmaGemmParams& p, int bn, int kind, const Scratch& scratch, int rows, int cols, void* out, long long ldo, int accumulate, int bm = UMMA_BLOCK_M)
 {
 	if (p.splits <= 1)
 	{
 		p.splits = 1, p.split_out_stride = 0, p.accumulate = accumulate;
 		p.out = (float*)out;
-		return launch_kind<AMODE, BMODE>(stream, tmA, tmB, p, bn, kind, kind != 0);
+		return launch_kind<AMODE, BMODE>(stream, tmA, tmB, p, bn, kind, kind != 0, bm);
 	}
 	// slices are dense [rows, cols] tiles of pitch cols rounded up to 4 floats (for a filter gradient cols = R * S * C is already
 	// a multiple of 4, so a slice has dW's own layout and tap-as-grid-dimension launches address it unchanged)
@@ -519,7 +528,7 @@ static int launch_umma_split(cudaStream_t stream, const CUtensorMap& tmA, const 
 	p.split_out_stride = (long long)rows * slice_ld;
 	p.accumulate = 0;
 	p.bias16 = 0; // a 16-bit bias is only read by the 16-bit epilogue: callers do not split when they pass one
-	const int rc = launch_kind<AMODE, BMODE>(stream, tmA, tmB, p, bn, kind, false);
+	const int rc = launch_kind<AMODE, BMODE>(stream, tmA, tmB, p, bn, kind, false, bm);
 	if (rc)
 		return rc;
 	return splitk_reduce(stream, (const float*)scratch.ptr, p.splits, p.split_out_stride, rows, cols, slice_ld, (float*)out, ldo, accumulate, kind);
@@ -842,14 +851,46 @@ int conv_wgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, const void*
 	const bool pointwise = conv_is_pointwise(g), rs = kind == 0 && !x3;
 	const long long sms = num_sms();
 	const auto rounds = [sms](long long ctas) { return (ctas + sms - 1) / sms; };
+	if (rs && !pointwise && g.C % bk == 0 && g.K <= 64)
+	{
+		// Swapped operands for the narrow layers (K below the 128-row MMA tile, where gradient rows would leave most of the tile zero):
+		// dW^T[R*S*C, K] = im2col(a)^T [R*S*C, NPQ] x grad_b [NPQ, K].  A row m = tap * C + c; each 32-row box of a tile is one tap's
+		// 32-channel span, read from the stage into registers; B = the [32 pixels][K] box of grad_b, transposed once per stage for all
+		// the tile's taps; N = K in one 32- or 64-column tile; the epilogue stores the tile transposed into dW (or its split slice).
+		// Tile height: the fewest rounds of CTAs over the SMs, then the shorter tile (128 rows, 64 per consumer warpgroup) over 256
+		const int bn_s = g.K <= 32 ? 32 : 64, bm = rounds((rsc + 255) / 256 * splits) < rounds((rsc + 127) / 128 * splits) ? 256 : 128;
+		CUtensorMap tmA, tmB;
+		// A: im2col(a) boxes of 32 pixels x 32 channels, 128-byte swizzled (see load_a_frags); B = grad_b [NPQ, K], MN-major
+		if (!map_im2col(&tmA, kind, a, g.N, g.H, g.W, g.C, g.an, g.ah, g.aw, -g.pad_h0, -g.pad_w0, g.pad_h1 - (g.R - 1) * g.dil_h, g.pad_w1 - (g.S - 1) * g.dil_w, g.stride_h, g.stride_w, bk, false) ||
+			!map_2d(&tmB, kind, grad_b, npq, g.K, g.K, bk, true))
+			return 1;
+		UmmaGemmParams p;
+		init_params_kind(p, kind);
+		p.M = (int)rsc, p.N = g.K;
+		p.k_iters = k_iters;
+		p.chunks_per_tap = k_iters;
+		p.rowmap.mode = 0, p.rowmap.ld = rsc;
+		p.splits = splits;
+		p.C_tap = g.C;
+		p.P = g.P, p.Q = g.Q;
+		p.stride_h = g.stride_h, p.stride_w = g.stride_w;
+		p.base_h = -g.pad_h0, p.base_w = -g.pad_w0;
+		for (int r = 0; r < g.R; r++)
+			for (int s = 0; s < g.S; s++)
+			{
+				p.tap_off_h[r * g.S + s] = (unsigned short)(r * g.dil_h);
+				p.tap_off_w[r * g.S + s] = (unsigned short)(s * g.dil_w);
+			}
+		return launch_umma_split<OP_IM2COL_RS, OP_MN2D>(stream, tmA, tmB, p, bn_s, kind, scratch, g.K, (int)rsc, grad_w, rsc, accumulate, bm);
+	}
 	int bn = 0;
 	bool tap_cols = false;
 	if (rs)
 	{
 		// TF32 (A from registers, tiles 64, 128 or 256 wide): the fewest rounds of CTAs over the SMs, then the narrower tile, then the
 		// fewer CTAs, the per-tap grid on a tie.  A wider tile runs nearer the tensor rate (its B transform and B reads serve more
-		// columns per A fragment), so it pays when it saves a round: ResNet-50's layer1 3 x 3 64 -> 64 goes from a per-tap grid of 261 CTAs
-		// (two rounds on 132 SMs) to 3 column tiles of 256 x 29 splits, most later layers from two rounds at 128 to one at 256.
+		// columns per A fragment), so it pays when it saves a round: most of ResNet-50's layers after layer1 go from two rounds at 128
+		// to one at 256.
 		long long best = 0, best_ctas = 0;
 		for (int w = 64; w <= 256; w *= 2)
 			for (int c = 0; c < 2; c++)

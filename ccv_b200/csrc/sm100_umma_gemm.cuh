@@ -15,7 +15,8 @@
 // K-major only, so the fp32 kernels whose operands arrive MN-major, and the 3xTF32 kernels, pass every stage through a transform
 // step first: the consumers copy the staged tiles into one of two K-major operand slots (transposing MN-major tiles, splitting
 // 3xTF32 operands into hi / lo) and release the stage to the producer before the MMAs run.  The TF32 weight gradient (A =
-// OP_MN2D_RS) transposes only B: its A = grad^T goes from the stage into registers, and its tiles are up to 256 columns wide.
+// OP_MN2D_RS) transposes only B: its A = grad^T goes from the stage into registers, and its tiles are up to 256 columns wide.  For
+// output-channel counts K <= 64 it swaps the operands (A = OP_IM2COL_RS, the filter taps along M, tiles of 128 or 256 rows, N = K).
 #pragma once
 #include "sm100_ptx.cuh"
 #include <cuda_bf16.h>
@@ -30,6 +31,9 @@ enum OperandMode {
 	               //                                       As B: pixels are K   (MN-major, channels = N).
 	OP_MN2D_RS = 3, // A only, TF32 only: an OP_MN2D tile staged 128-byte swizzled, which the consumers read straight into wgmma A
 	                // fragments (see load_a_frags): it never goes through the transform step
+	OP_IM2COL_RS = 4, // A only, TF32 only: the weight gradient's im2col(x)^T, rows = filter tap * C_tap + channel.  Each 32-row box of
+	                  // the tile is one tap's 32-channel span of 32 pixels (the reduction), staged 128-byte swizzled like OP_MN2D_RS and
+	                  // read into registers the same way; the epilogue stores the tile transposed (row m -> column m of the output)
 };
 
 constexpr int UMMA_BLOCK_M = 128;
@@ -106,15 +110,15 @@ __device__ __forceinline__ float cvt16(const uint16_t x, const int kind)
 // (the reference's fp32 GEMM is CUBLAS_COMPUTE_32F, lib/nnc/gpu/ccv_nnc_compat.cu:786-803) at a third of the tensor rate.
 template <int AMODE, int BMODE, int K16, int X3>
 struct GemmXform {
-	static constexpr bool A_RS = AMODE == OP_MN2D_RS;     // A from registers (TF32 only)
+	static constexpr bool A_RS = AMODE == OP_MN2D_RS || AMODE == OP_IM2COL_RS; // A from registers (TF32 only)
 	static constexpr bool A_T = !K16 && AMODE == OP_MN2D; // fp32 MN-major A: transposed into the K-major slot
 	static constexpr bool B_T = !K16 && BMODE != OP_K2D;  // fp32 MN-major B (2-D or im2col)
 	static constexpr bool ANY = A_T || B_T || X3;
 };
 
-template <int BN, int STAGES, bool XF, int X3, bool ARS = false>
+template <int BN, int STAGES, bool XF, int X3, bool ARS = false, int BM = UMMA_BLOCK_M>
 struct UmmaSmem {
-	static constexpr int A_BYTES = UMMA_BLOCK_M * 128;
+	static constexpr int A_BYTES = BM * 128;
 	static constexpr int B_BYTES = BN * 128;
 	static constexpr int RAW_BYTES = A_BYTES + B_BYTES;            // one TMA stage
 	static constexpr int SLOT_A_BYTES = ARS ? 0 : A_BYTES;          // where B starts in the operand the MMAs read (A from registers: B alone)
@@ -127,10 +131,12 @@ struct UmmaSmem {
 };
 
 // stages per kernel: as deep as 227 KB of shared memory allows with the transform slots (A from registers: 3 stages of 48 KB and
-// two 32 KB B slots at BN = 256; 4 at BN = 64 / 128, which ran ResNet-50's weight gradients no slower than 6)
-template <int BN, bool XF, int X3, bool ARS = false>
+// two 32 KB B slots at BN = 256; 4 at BN = 64 / 128, which ran ResNet-50's weight gradients no slower than 6).  The swapped weight
+// gradient (A = OP_IM2COL_RS, BN <= 64) does little MMA work per stage, so it keeps more stages in flight: 8 of up to 24 KB with
+// 128-row tiles, 5 of up to 40 KB with 256-row tiles.
+template <int BN, bool XF, int X3, bool ARS = false, int BM = UMMA_BLOCK_M, bool SWAP = false>
 struct GemmStages {
-	static constexpr int value = ARS ? (BN == 256 ? 3 : 4) : X3 ? (BN == 128 ? 3 : 4) : (XF ? 4 : (BN == 128 ? 5 : 6));
+	static constexpr int value = SWAP ? (BM == 256 ? 5 : 8) : ARS ? (BN == 256 ? 3 : 4) : X3 ? (BN == 128 ? 3 : 4) : (XF ? 4 : (BN == 128 ? 5 : 6));
 };
 
 // one staged fp32 operand tile (rows x 32 k) -> K-major 128-byte-swizzled slot (16-byte chunk c of row r at chunk c ^ (r & 7)).
@@ -196,11 +202,14 @@ __device__ __forceinline__ void load_a_frags(uint32_t (&af)[4][4], const float* 
 // K16 = 1 / 2: bf16 / fp16 operands (p.out_kind holds the same kind), 64 elements per 128-byte row, K = 16 per MMA; K16 = 0: fp32
 // operands (32 per row, K = 8 per MMA).  The element type is a template parameter so that every wgmma of a k-step sits in one basic
 // block (a runtime type branch makes ptxas fence each MMA on its own).  OUT16 = 1: the output tensor (and an optional 16-bit bias) is bf16 / fp16 (p.out_kind).
-template <int AMODE, int BMODE, int BN, int STAGES, int X3 = 0, int K16 = 0, int OUT16 = 0>
-__global__ void __launch_bounds__(AMODE == OP_MN2D_RS ? GEMM_THREADS_RS : GEMM_THREADS, 1) umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const UmmaGemmParams p)
+// BM: output rows per tile, 128 (64 per consumer warpgroup) or, for A = OP_IM2COL_RS only, 256 (two m64 blocks per warpgroup).
+template <int AMODE, int BMODE, int BN, int STAGES, int X3 = 0, int K16 = 0, int OUT16 = 0, int BM = UMMA_BLOCK_M>
+__global__ void __launch_bounds__(AMODE == OP_MN2D_RS || AMODE == OP_IM2COL_RS ? GEMM_THREADS_RS : GEMM_THREADS, 1) umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const UmmaGemmParams p)
 {
 	using XF = GemmXform<AMODE, BMODE, K16, X3>;
-	using S = UmmaSmem<BN, STAGES, XF::ANY, X3, XF::A_RS>;
+	using S = UmmaSmem<BN, STAGES, XF::ANY, X3, XF::A_RS, BM>;
+	constexpr bool SWAP = AMODE == OP_IM2COL_RS;
+	constexpr int MSUB = BM / UMMA_BLOCK_M; // m64 blocks per consumer warpgroup
 	extern __shared__ uint8_t smem_raw[];
 	uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
 	uint64_t* full_bar = (uint64_t*)(smem + S::BAR_OFFSET);
@@ -210,7 +219,7 @@ __global__ void __launch_bounds__(AMODE == OP_MN2D_RS ? GEMM_THREADS_RS : GEMM_T
 	constexpr int MN_BOX_BYTES = BK * 128;     // an MN-major box: BK k-rows of 128 bytes
 	const int warp = threadIdx.x >> 5;
 	const int lane = threadIdx.x & 31;
-	const int tiles_m = (p.M + UMMA_BLOCK_M - 1) / UMMA_BLOCK_M; // M tiles blockIdx.x, blockIdx.x + gridDim.x, ... (launch_umma picks gridDim.x)
+	const int tiles_m = (p.M + BM - 1) / BM; // M tiles blockIdx.x, blockIdx.x + gridDim.x, ... (launch_umma picks gridDim.x)
 	const int n0 = blockIdx.y * BN;
 	const int split = blockIdx.z % p.splits;
 	const int gtap = blockIdx.z / p.splits;
@@ -260,7 +269,20 @@ __global__ void __launch_bounds__(AMODE == OP_MN2D_RS ? GEMM_THREADS_RS : GEMM_T
 			uint32_t phase = 0;
 			for (int mt = blockIdx.x; mt < tiles_m; mt += gridDim.x)
 			{
-			const int m0 = mt * UMMA_BLOCK_M;
+			const int m0 = mt * BM;
+			// A = OP_IM2COL_RS: box j holds rows [m0 + 32 j, +32), one tap's channel span (C_tap is a multiple of 32); a box past the
+			// last row asks for channels beyond C, which the TMA unit fills with zeros
+			int a_ch[SWAP ? BM / 32 : 1], a_off_w[SWAP ? BM / 32 : 1], a_off_h[SWAP ? BM / 32 : 1];
+			if constexpr (SWAP)
+			{
+#pragma unroll
+				for (int j = 0; j < BM / 32; j++)
+				{
+					const int row = m0 + 32 * j;
+					const int t = row < p.M ? row / p.C_tap : 0;
+					a_ch[j] = row - t * p.C_tap, a_off_w[j] = p.tap_off_w[t], a_off_h[j] = p.tap_off_h[t];
+				}
+			}
 			int a_w = 0, a_h = 0, a_n = 0;
 			if (AMODE == OP_IM2COL)
 			{
@@ -280,7 +302,18 @@ __global__ void __launch_bounds__(AMODE == OP_MN2D_RS ? GEMM_THREADS_RS : GEMM_T
 				mbar_expect_tx(&full_bar[stage], S::RAW_BYTES);
 				if (AMODE == OP_K2D)
 					tma_load_2d(sA, &tmA, &full_bar[stage], chunk * BK, m0);
-				else if (AMODE == OP_MN2D || AMODE == OP_MN2D_RS) {
+				else if (AMODE == OP_IM2COL_RS) {
+					// pixels are the reduction: this iteration covers base pixels [it * BK, it * BK + BK)
+					const int pix = it * BK;
+					const int q = pix % p.Q;
+					const int t = pix / p.Q;
+					const int x_w = q * p.stride_w + p.base_w;
+					const int x_h = (t % p.P) * p.stride_h + p.base_h;
+					const int x_n = t / p.P;
+#pragma unroll
+					for (int j = 0; j < BM / 32; j++)
+						tma_load_im2col_4d(sA + j * MN_BOX_BYTES, &tmA, &full_bar[stage], a_ch[j], x_w, x_h, x_n, (uint16_t)a_off_w[j], (uint16_t)a_off_h[j]);
+				} else if (AMODE == OP_MN2D || AMODE == OP_MN2D_RS) {
 #pragma unroll
 					for (int j = 0; j < UMMA_BLOCK_M / BK; j++)
 						tma_load_2d(sA + j * MN_BOX_BYTES, &tmA, &full_bar[stage], m0 + BK * j, it * BK);
@@ -314,8 +347,8 @@ __global__ void __launch_bounds__(AMODE == OP_MN2D_RS ? GEMM_THREADS_RS : GEMM_T
 	// ------------------------------------------------------------------ consumers (warps 0..7)
 	if constexpr (XF::A_RS)
 		setmaxnreg_inc<224>();
-	const int wg = warp >> 2; // output rows [64 * wg, +64) of the tile
-	float acc[BN / 2];
+	const int wg = warp >> 2; // output rows [64 * MSUB * wg, +64 * MSUB) of the tile
+	float acc[MSUB * BN / 2];
 	constexpr bool A_MN16 = K16 && AMODE == OP_MN2D, B_MN16 = K16 && BMODE != OP_K2D;
 	constexpr uint32_t A_STEP = A_MN16 ? 2048 : 32, B_STEP = B_MN16 ? 2048 : 32; // bytes per MMA step along K
 	int stage = 0;
@@ -330,11 +363,11 @@ __global__ void __launch_bounds__(AMODE == OP_MN2D_RS ? GEMM_THREADS_RS : GEMM_T
 			st_run[i * 4] = 0.f;
 	for (int mt = blockIdx.x; mt < tiles_m; mt += gridDim.x)
 	{
-	const int m0 = mt * UMMA_BLOCK_M;
+	const int m0 = mt * BM;
 #pragma unroll
-	for (int i = 0; i < BN / 2; i++)
+	for (int i = 0; i < MSUB * BN / 2; i++)
 		acc[i] = 0.f;
-	uint32_t af[4][4]; // A from registers: this k-iteration's A fragments
+	uint32_t af[MSUB][4][4]; // A from registers: this k-iteration's A fragments
 	for (int it = 0; it < n_it; it++, gi++)
 	{
 		mbar_wait(&full_bar[stage], phase);
@@ -356,7 +389,9 @@ __global__ void __launch_bounds__(AMODE == OP_MN2D_RS ? GEMM_THREADS_RS : GEMM_T
 				// complete (overwritten in flight, ptxas would serialise every wgmma), so only now load this stage's; the stage is
 				// released below
 				wgmma_wait<0>();
-				load_a_frags(af, raw + wg * 2048, warp, lane);
+#pragma unroll
+				for (int u = 0; u < MSUB; u++)
+					load_a_frags(af[u], raw + (wg * MSUB + u) * 2048, warp, lane);
 			}
 			fence_proxy_async(); // the tensor core reads shared memory through the async proxy
 			named_bar_sync(1, 256);
@@ -387,12 +422,19 @@ __global__ void __launch_bounds__(AMODE == OP_MN2D_RS ? GEMM_THREADS_RS : GEMM_T
 						wgmma_f16_ss_n64<A_MN16, B_MN16>(*reinterpret_cast<float(*)[32]>(acc), da, db);
 				}
 			} else if constexpr (XF::A_RS) {
-				if constexpr (BN == 256)
-					wgmma_tf32_rs_n256(*reinterpret_cast<float(*)[128]>(acc), af[k], db);
-				else if constexpr (BN == 128)
-					wgmma_tf32_rs_n128(*reinterpret_cast<float(*)[64]>(acc), af[k], db);
-				else
-					wgmma_tf32_rs_n64(*reinterpret_cast<float(*)[32]>(acc), af[k], db);
+#pragma unroll
+				for (int u = 0; u < MSUB; u++)
+				{
+					float* const d = acc + u * (BN / 2);
+					if constexpr (BN == 256)
+						wgmma_tf32_rs_n256(*reinterpret_cast<float(*)[128]>(d), af[u][k], db);
+					else if constexpr (BN == 128)
+						wgmma_tf32_rs_n128(*reinterpret_cast<float(*)[64]>(d), af[u][k], db);
+					else if constexpr (BN == 64)
+						wgmma_tf32_rs_n64(*reinterpret_cast<float(*)[32]>(d), af[u][k], db);
+					else
+						wgmma_tf32_rs_n32(*reinterpret_cast<float(*)[16]>(d), af[u][k], db);
+				}
 			} else {
 				constexpr uint32_t LO = (uint32_t)(S::RAW_BYTES >> 4);
 				if constexpr (BN == 128)
@@ -430,6 +472,36 @@ __global__ void __launch_bounds__(AMODE == OP_MN2D_RS ? GEMM_THREADS_RS : GEMM_T
 		mbar_arrive(&empty_bar[prev_stage]); // the last stage of this tile
 
 	// ------------------------------------------------------------------ epilogue: accumulator i -> (row, column), see sm100_ptx.cuh
+	if constexpr (SWAP)
+	{
+		// the tile is the transpose of the output: row m (filter tap * C_tap + channel) -> output column m, column n -> output row n
+		// (dW[K, R*S*C], or this split's slice of it); no bias, no 16-bit output, no statistics
+		float* const out = p.out + (long long)split * p.split_out_stride;
+		const bool accumulate = p.accumulate != 0;
+#pragma unroll
+		for (int u = 0; u < MSUB; u++)
+#pragma unroll
+			for (int h = 0; h < 2; h++)
+			{
+				const int row = m0 + (wg * MSUB + u) * 64 + a_row(warp, lane, h);
+				if (row >= p.M)
+					continue;
+#pragma unroll
+				for (int j = 0; j < BN / 8; j++)
+#pragma unroll
+					for (int e = 0; e < 2; e++)
+					{
+						const int col = n0 + 8 * j + 2 * (lane & 3) + e;
+						if (col >= p.N)
+							continue;
+						float* const o = out + col * p.rowmap.ld + row;
+						// + 0.f: the other layouts' epilogue adds a zero bias, which turns a -0 sum into +0
+						const float v = acc[u * (BN / 2) + 4 * j + 2 * h + e] + 0.f;
+						*o = accumulate ? *o + v : v;
+					}
+			}
+		continue;
+	}
 	constexpr int OSZ = OUT16 ? 2 : 4;
 	const bool add_bias = split == 0;
 	const float* const bias = p.bias;

@@ -12,7 +12,7 @@ dgrad g + w + h, wgrad g + x + dw.  The bound is max(flops / tensor peak, bytes 
 (dense TF32 494.5 TFLOP/s, a third of it for 3xTF32; HBM3 3.35 TB/s); `frac` = bound / measured time.  The summary weighs each shape by
 how often the step runs it.  The card's name, power limit and SM clocks are printed with the numbers.
 
-usage: python tools/bench_resnet_convs.py [--3xtf32] [--reps R] [--json FILE]"""
+usage: python tools/bench_resnet_convs.py [--3xtf32] [--reps R] [--only fwd,dgrad,wgrad] [--json FILE]"""
 import argparse
 import json
 import os
@@ -94,6 +94,7 @@ def main():
     ap.add_argument("--3xtf32", dest="x3", action="store_true", help="algorithm 1 (3xTF32) instead of 0 (TF32)")
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--batch", type=int, default=256)
+    ap.add_argument("--only", default="fwd,dgrad,wgrad", help="comma-separated commands to time (the summary covers only these)")
     ap.add_argument("--json", default="", help="also write the rows and the summary to this file")
     args = ap.parse_args()
     nnc.init()
@@ -123,6 +124,8 @@ def main():
             cmds.append(("dgrad", lambda: nnc.cmd_exec(bwd, hint, 0, [g, x, w], [dx], stream), g.nbytes + w.nbytes + dx.nbytes))
         cmds.append(("wgrad", lambda: nnc.cmd_exec(bwd, hint, 0, [g, x, w], [None, dw], stream), g.nbytes + x.nbytes + dw.nbytes))
         for kind, fn, nbytes in cmds:
+            if kind not in args.only.split(","):
+                continue
             ms = time_ms(fn, stream, args.reps)
             bound = max(flops / (peak * 1e9), nbytes / (HBM_GBS * 1e6))
             rows.append(dict(kind=kind, name=name, count=count, shape="%dx%d %d->%d /%d @%d" % (k, k, cin, cout, st, h), ms=ms, flops=flops, bytes=nbytes, bound_ms=bound,
