@@ -24,7 +24,8 @@ CCV_NNC_BACKEND_CPU_OPT = 0x46deb194
 CCV_NNC_BACKEND_CPU_REF = 0x3d9883e5
 CCV_NNC_BACKEND_GPU_SM100 = 0xdbfb784c
 CCV_NNC_SM100_ALGO_TF32, CCV_NNC_SM100_ALGO_3XTF32, CCV_NNC_SM100_ALGO_FFMA = 0, 1, 2
-CCV_NNC_SM100_SDPA_ALGO_COMPOSED, CCV_NNC_SM100_SDPA_ALGO_FLASH, CCV_NNC_SM100_SDPA_ALGO_COUNT = 0, 1, 2  # SCALED_DOT_PRODUCT_ATTENTION
+CCV_NNC_SM100_SDPA_ALGO_COMPOSED, CCV_NNC_SM100_SDPA_ALGO_FLASH, CCV_NNC_SM100_SDPA_ALGO_FLASH_MASK = 0, 1, 2  # SCALED_DOT_PRODUCT_ATTENTION
+CCV_NNC_SM100_SDPA_ALGO_COUNT = 3
 CCV_NNC_GEMM_32F, CCV_NNC_GEMM_32TF, CCV_NNC_GEMM_16F = 0x1, 0x2, 0x4  # lib/nnc/ccv_nnc.h:102-106 (cmd.info.blas.flags)
 
 # commands (lib/nnc/cmd/ccv_nnc_cmd.h)

@@ -165,6 +165,55 @@ static bool sdpa_geom(const ccv_nnc_cmd_t& cmd, const ccv_nnc_tensor_t* const q,
 	return true;
 }
 
+// CCV_NNC_SM100_SDPA_ALGO_FLASH_MASK: a 16-bit forward with an additive mask on one flash launch (sm100_fmha.cu for D = Dv <= 128,
+// sm100_fmha_wide.cu up to 256), with or without the log-sum-exp, q / k / v / o as views.  The mask is [Sq, Sk], [X, Sq, Sk] (X = 1 | H) or
+// [1|B, 1|H, Sq, Sk] (the shapes CPU_REF reads, :82-86,:104), fp32 or of the activations' type, keys contiguous, any row / head / batch
+// pitch of a view (CPU_REF reads amstride).  Calls without a mask, fp32 calls, and shapes or mask pitches the kernels do not take
+// return NO_KERNEL: algorithms 0 and 1 run those, so autotuning never times one kernel twice.
+static int sdpa_forw_flash_mask(SM100_EXEC_ARGS, SdpaGeom& g)
+{
+	const ccv_nnc_tensor_t* const mask_t = input_size > 3 ? inputs[3] : 0;
+	const int dt = CCV_GET_DATA_TYPE(inputs[0]->info.datatype);
+	if (!mask_t || dt == CCV_32F)
+		return CCV_NNC_EXEC_NO_KERNEL;
+	const int mdt = CCV_GET_DATA_TYPE(mask_t->info.datatype);
+	const int nd = nd_of(mask_t);
+	if ((mdt != CCV_32F && mdt != dt) || nd < 2 || nd > 4 || mask_t->info.dim[nd - 1] != g.Sk || mask_t->info.dim[nd - 2] != g.Sq)
+		return CCV_NNC_EXEC_INVALID;
+	long long stride[4];
+	long long packed = 1;
+	for (int i = nd - 1; i >= 0; i--)
+	{
+		stride[i] = CCV_IS_TENSOR_VIEW(mask_t) ? ((const ccv_nnc_tensor_view_t*)mask_t)->stride[i] : packed;
+		packed *= mask_t->info.dim[i];
+	}
+	if (stride[nd - 1] != 1)
+		return CCV_NNC_EXEC_INVALID;
+	int md[4] = { 1, 1, g.Sq, g.Sk };
+	long long ms[4] = { 0, 0, stride[nd - 2], 1 };
+	for (int i = 0; i < nd - 2; i++)
+		md[2 - (nd - 2) + i] = mask_t->info.dim[i], ms[2 - (nd - 2) + i] = stride[i];
+	if ((md[0] != 1 && md[0] != g.B) || (md[1] != 1 && md[1] != g.H))
+		return CCV_NNC_EXEC_INVALID;
+	g.mask_c = 1, g.mask_s = ms[2];
+	g.mask_h = md[1] > 1 ? ms[1] : 0;
+	g.mask_b = md[0] > 1 ? ms[0] : 0;
+	float* lse = 0;
+	if (output_size > 1 && outputs[1])
+	{
+		if (!packed_f32(outputs[1]) || count_of(outputs[1]) != (size_t)g.B * g.H * g.Sq)
+			return CCV_NNC_EXEC_INVALID;
+		lse = outputs[1]->data.f32;
+	}
+	const int is_bf16 = dt == CCV_16BF, mask_f32 = mdt == CCV_32F;
+	int rc = sdpa_forward_f16(stream_of(stream_context), g, is_bf16, inputs[0]->data.u8, inputs[1]->data.u8, inputs[2]->data.u8, outputs[0]->data.u8, lse, mask_t->data.u8, mask_f32);
+	if (rc == 1)
+		rc = sdpa_forward_f16_wide(stream_of(stream_context), g, is_bf16, inputs[0]->data.u8, inputs[1]->data.u8, inputs[2]->data.u8, outputs[0]->data.u8, lse, mask_t->data.u8, mask_f32);
+	if (rc < 0)
+		return CCV_NNC_EXEC_INVALID;
+	return rc == 0 ? CCV_NNC_EXEC_SUCCESS : CCV_NNC_EXEC_NO_KERNEL;
+}
+
 // scaled_dot_product_attention/ccv_nnc_scaled_dot_product_attention_cpu_ref.c:16-183: inputs (q, k, v, [attn_mask]) ->
 // outputs (y, [softmax_lse]); `outputs` here already has the per-head attention tensor in slot 0 (see the entry point below)
 static int sdpa_forw_core(SM100_EXEC_ARGS)
@@ -174,6 +223,8 @@ static int sdpa_forw_core(SM100_EXEC_ARGS)
 	SdpaGeom g;
 	if (!sdpa_geom(cmd, inputs[0], inputs[1], inputs[2], outputs[0], g))
 		return CCV_NNC_EXEC_INVALID;
+	if (cmd.algorithm == CCV_NNC_SM100_SDPA_ALGO_FLASH_MASK)
+		return sdpa_forw_flash_mask(cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context, g);
 	const ccv_nnc_tensor_t* const mask_t = input_size > 3 ? inputs[3] : 0;
 	const int dt = CCV_GET_DATA_TYPE(inputs[0]->info.datatype);
 	const float* mask = 0;
@@ -320,6 +371,8 @@ int ccv_nnc_sm100_exec_sdpa_forw(SM100_EXEC_ARGS)
 // :259-479: inputs[0] = g, [3] = q, [4] = k, [5] = v -> outputs (dq, dk, dv); masks are not differentiable here either (:262)
 int ccv_nnc_sm100_exec_sdpa_back(SM100_EXEC_ARGS)
 {
+	if (cmd.algorithm == CCV_NNC_SM100_SDPA_ALGO_FLASH_MASK) // a forward-only algorithm: the mask is not differentiable (:262)
+		return CCV_NNC_EXEC_NO_KERNEL;
 	if (input_size < 6 || output_size < 3 || !inputs[0] || !inputs[3] || !inputs[4] || !inputs[5] || !outputs[0] || !outputs[1] || !outputs[2])
 		return CCV_NNC_EXEC_INVALID;
 	if ((input_size > 6 && inputs[6]) || (input_size > 7 && inputs[7]))

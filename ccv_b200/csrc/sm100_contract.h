@@ -98,9 +98,10 @@ int sdpa_forward_f32(cudaStream_t s, const SdpaGeom& g, const float* q, const fl
 // dg carries the strides of dq / dk / dv in its q_* / k_* / v_* fields
 int sdpa_backward_f32(cudaStream_t s, const SdpaGeom& g, const float* dout, const float* q, const float* k, const float* v, float* dq, float* dk, float* dv, const SdpaGeom& dg, void* workspace);
 
-// 16-bit (bf16 / fp16) flash attention forward on wgmma (sm100_fmha.cu): D = Dv <= 128; lse [B, H, Sq] fp32 or NULL.
+// 16-bit (bf16 / fp16) flash attention forward on wgmma (sm100_fmha.cu): D = Dv <= 128; lse [B, H, Sq] fp32 or NULL.  mask: an additive
+// mask [B|1, H|1, Sq, Sk] with g.mask_b / mask_h / mask_s (keys contiguous), fp32 (mask_f32) or of the q / k / v type, or NULL.
 // returns 0 on success, 1 when the shape is not covered, < 0 on CUDA errors
-int sdpa_forward_f16(cudaStream_t s, const SdpaGeom& g, int is_bf16, const void* q, const void* k, const void* v, void* o, float* lse);
+int sdpa_forward_f16(cudaStream_t s, const SdpaGeom& g, int is_bf16, const void* q, const void* k, const void* v, void* o, float* lse, const void* mask = 0, int mask_f32 = 1);
 
 // 16-bit flash attention backward on wgmma (sm100_fmha_bwd.cu), deterministic: D = Dv <= 128.  g carries the strides of q / k / v and, in
 // o_*, of dout; dg the strides of dq / dk / dv in q_* / k_* / v_*.  out (strides oo_*) / lse = the forward's saved outputs, or NULL:
@@ -134,7 +135,7 @@ int gemm_palettized_f16(cudaStream_t stream, int M, int N, int K, const void* a,
 
 // 16-bit flash attention with wide heads (sm100_fmha_wide.cu): 128 < D = Dv <= 256, a multiple of 8.  The arguments, workspace and
 // return convention of sdpa_forward_f16 / sdpa_backward_f16 (sdpa_backward_f16_workspace_bytes covers these kernels too).
-int sdpa_forward_f16_wide(cudaStream_t s, const SdpaGeom& g, int is_bf16, const void* q, const void* k, const void* v, void* o, float* lse);
+int sdpa_forward_f16_wide(cudaStream_t s, const SdpaGeom& g, int is_bf16, const void* q, const void* k, const void* v, void* o, float* lse, const void* mask = 0, int mask_f32 = 1);
 int sdpa_backward_f16_wide(cudaStream_t s, const SdpaGeom& g, const SdpaGeom& dg, int is_bf16, const void* dout, const void* q, const void* k, const void* v, const void* out, long long oo_b, long long oo_s, long long oo_h,
 	const float* lse, void* dq, void* dk, void* dv, void* workspace);
 

@@ -1,5 +1,6 @@
 // sm100_fmha.cuh -- helpers shared by the 16-bit flash-attention kernels (sm100_fmha.cu forward, sm100_fmha_bwd.cu backward):
-// 16-bit packing, the 4-D TMA tensor map over a [B, S, H, D] tensor, and the register form of P / dS as a wgmma A operand.
+// 16-bit packing, the 4-D TMA tensor map over a [B, S, H, D] tensor, and the register form of P / dS as a wgmma A operand; the tensor map
+// and the shared-memory reads of an additive mask (sm100_fmha.cu, sm100_fmha_wide.cu under CCV_NNC_SM100_SDPA_ALGO_FLASH_MASK).
 #pragma once
 #include "sm100_ptx.cuh"
 #include <cuda_bf16.h>
@@ -68,6 +69,68 @@ inline bool make_map_bshd(CUtensorMap* map, const void* ptr, int B, int S, int H
 	cuuint32_t box[4] = { 64, 1, (cuuint32_t)box_rows, 1 };
 	cuuint32_t estr[4] = { 1, 1, 1, 1 };
 	return encode_fn()(map, is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, (void*)ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+// Additive attention mask [B | 1, H | 1, Sq, Sk] with element strides (sb, sh, ss), 0 = broadcast, keys contiguous; esz = 4 (fp32) or 2
+// (the activations' 16-bit type).  box = {128 bytes of keys, 128 query rows, 1 head, 1 batch}, 128-byte swizzle; the TMA unit zero-fills
+// keys past Sk and rows past Sq, so a tile never reads outside the tensor.  false when a pitch or the base is not a multiple of 16 bytes.
+inline bool make_map_mask(CUtensorMap* map, const void* ptr, int B, int H, int Sq, int Sk, long long sb, long long sh, long long ss, int esz, int is_bf16)
+{
+	if ((((uintptr_t)ptr) & 15) || ss <= 0 || ((ss * esz) & 15) || ((sh * esz) & 15) || ((sb * esz) & 15))
+		return false;
+	const int Hm = sh ? H : 1, Bm = sb ? B : 1;
+	if (!sh)
+		sh = (long long)Sq * ss;
+	if (!sb)
+		sb = (long long)Hm * sh;
+	cuuint64_t dims[4] = { (cuuint64_t)Sk, (cuuint64_t)Sq, (cuuint64_t)Hm, (cuuint64_t)Bm };
+	cuuint64_t strides[3] = { (cuuint64_t)(ss * esz), (cuuint64_t)(sh * esz), (cuuint64_t)(sb * esz) };
+	cuuint32_t box[4] = { (cuuint32_t)(128 / esz), 128, 1, 1 };
+	cuuint32_t estr[4] = { 1, 1, 1, 1 };
+	const CUtensorMapDataType t = esz == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : (is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
+	return encode_fn()(map, t, 4, (void*)ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+constexpr int MASK_ATOM_BYTES = 128 * 128; // one make_map_mask box: 128 rows x 128 bytes
+
+// mask[r][8 c + 2 t4], mask[r][8 c + 2 t4 + 1] (r < 128, t4 < 4; c a constant after unrolling) from a stage of make_map_mask boxes,
+// one 16 KB atom per 128 bytes of keys, 16-byte chunks XOR-swizzled by r & 7 (the stage is 1024-byte aligned).  row = stage + 128 r,
+// x = r & 7.  MASK 1 = fp32, 2 = 16-bit (widened exactly).
+template <int MASK, int BF16>
+__device__ __forceinline__ float2 mask_pair(const uint8_t* row, const int x, const int c, const int t4)
+{
+	if constexpr (MASK == 1)
+		return *reinterpret_cast<const float2*>(row + (c >> 2) * MASK_ATOM_BYTES + (((2 * (c & 3) + (t4 >> 1)) ^ x) << 4) + 8 * (t4 & 1));
+	else {
+		const uint32_t u = *reinterpret_cast<const uint32_t*>(row + (c >> 3) * MASK_ATOM_BYTES + (((c & 7) ^ x) << 4) + 4 * t4);
+		return make_float2(widen16((uint16_t)(u & 0xffff), BF16), widen16((uint16_t)(u >> 16), BF16));
+	}
+}
+
+// S (a wgmma accumulator of R / 4 groups of 8 keys, rows r and r + 8) -> scale * S + mask, in CPU_REF's order; the loads four groups
+// at a time.
+template <int MASK, int BF16, int R>
+__device__ __forceinline__ void add_mask(float (&sacc)[R], const uint8_t* stage, const int r, const int t4, const float scale)
+{
+#pragma unroll
+	for (int c0 = 0; c0 < R / 4; c0 += 4)
+	{
+		float2 mk[4][2];
+#pragma unroll
+		for (int c = 0; c < 4; c++)
+#pragma unroll
+			for (int hh = 0; hh < 2; hh++)
+				mk[c][hh] = mask_pair<MASK, BF16>(stage + 128 * (r + 8 * hh), r & 7, c0 + c, t4);
+#pragma unroll
+		for (int c = 0; c < 4; c++)
+#pragma unroll
+			for (int hh = 0; hh < 2; hh++)
+			{
+				const int i = 4 * (c0 + c) + 2 * hh;
+				sacc[i] = fmaf(sacc[i], scale, mk[c][hh].x);
+				sacc[i + 1] = fmaf(sacc[i + 1], scale, mk[c][hh].y);
+			}
+	}
 }
 
 } // namespace

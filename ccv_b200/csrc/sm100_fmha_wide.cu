@@ -15,6 +15,8 @@
 //   warps 8-11  producer warpgroup: one thread issues the TMA loads (Q once, K_j / V_j through two-stage rings); setmaxnreg gives its
 //               registers to the consumers (24 / 240 instead of 168 each)
 //   smem: Q 64 KB + K 2 x 32 KB + V 2 x 32 KB = 192 KB.
+//   MASK (1 = fp32, 2 = 16-bit; CCV_NNC_SM100_SDPA_ALGO_FLASH_MASK): an additive mask, staged and applied as in sm100_fmha.cu.  Its tile
+//   per key block (128 query rows x 64 keys) takes one more buffer of 32 KB fp32 / 16 KB 16-bit: 224 / 208 KB in all.
 //
 // Backward (the equations of sm100_fmha_bwd.cu): prep (lse * log2 e, delta) + one dK/dV launch + one dQ launch, no atomics.  A CTA
 // holds 64 resident rows (MODE 0: keys of a key head, MODE 1: queries of a query head) and streams 64-row blocks of the other side.
@@ -50,21 +52,27 @@ struct WideFwdParams {
 	void* o;
 	long long o_b, o_s, o_h; // element strides
 	float* lse;              // [B, H, Sq] or NULL
+	// MASK only
+	float scale;
+	int mask_h, mask_b; // the mask has a head / batch axis (else broadcast)
 };
 
+template <int MASK>
 struct WideFwdSmem {
 	static constexpr int Q_OFF = 0;
 	static constexpr int K_OFF = Q_OFF + FW_Q_BYTES;
 	static constexpr int V_OFF = K_OFF + 2 * FW_TILE;
-	static constexpr int BAR_OFF = V_OFF + 2 * FW_TILE;
+	static constexpr int M_OFF = V_OFF + 2 * FW_TILE;
+	static constexpr int M_BYTES = MASK == 0 ? 0 : FW_Q * FW_K * (MASK == 1 ? 4 : 2);
+	static constexpr int BAR_OFF = M_OFF + M_BYTES;
 	static constexpr int TOTAL = BAR_OFF + 256 + 1024;
 	static_assert(TOTAL <= 232448, "227 KB of shared memory per CTA");
 };
 
-template <int BF16>
-__global__ void __launch_bounds__(FW_THREADS, 1) fmha_wide_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV, const WideFwdParams p)
+template <int BF16, int MASK>
+__global__ void __launch_bounds__(FW_THREADS, 1) fmha_wide_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV, const WideFwdParams p, const __grid_constant__ CUtensorMap tmM)
 {
-	using L = WideFwdSmem;
+	using L = WideFwdSmem<MASK>;
 	extern __shared__ uint8_t smem_raw[];
 	uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
 	uint64_t* bars = (uint64_t*)(smem + L::BAR_OFF);
@@ -73,6 +81,8 @@ __global__ void __launch_bounds__(FW_THREADS, 1) fmha_wide_fwd_kernel(const __gr
 	uint64_t* k_empty = bars + 3; // [2] one arrival per consumer warpgroup
 	uint64_t* v_full = bars + 5;  // [2]
 	uint64_t* v_empty = bars + 7; // [2]
+	uint64_t* m_full = bars + 9;
+	uint64_t* m_empty = bars + 10; // one arrival per consumer warp
 
 	const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 	// causal: the last query tiles see the most keys; issue them first so the tail of the launch is made of short tiles
@@ -94,6 +104,8 @@ __global__ void __launch_bounds__(FW_THREADS, 1) fmha_wide_fwd_kernel(const __gr
 			mbar_init(&k_full[s], 1), mbar_init(&k_empty[s], 2);
 			mbar_init(&v_full[s], 1), mbar_init(&v_empty[s], 2);
 		}
+		if constexpr (MASK != 0)
+			mbar_init(m_full, 1), mbar_init(m_empty, 8);
 		fence_mbar_init();
 	}
 	__syncthreads();
@@ -106,6 +118,8 @@ __global__ void __launch_bounds__(FW_THREADS, 1) fmha_wide_fwd_kernel(const __gr
 			tma_prefetch_desc(&tmQ);
 			tma_prefetch_desc(&tmK);
 			tma_prefetch_desc(&tmV);
+			if constexpr (MASK != 0)
+				tma_prefetch_desc(&tmM);
 			mbar_expect_tx(q_full, FW_Q_BYTES);
 			for (int a = 0; a < 4; a++)
 				tma_load_4d(smem + L::Q_OFF + a * FW_Q_ATOM, &tmQ, q_full, 64 * a, h, q0, b);
@@ -119,6 +133,13 @@ __global__ void __launch_bounds__(FW_THREADS, 1) fmha_wide_fwd_kernel(const __gr
 				mbar_expect_tx(&k_full[s], FW_TILE);
 				for (int a = 0; a < 4; a++)
 					tma_load_4d(sk + a * FW_ATOM, &tmK, &k_full[s], 64 * a, hk, j * FW_K, b);
+				if constexpr (MASK != 0)
+				{
+					mbar_wait(m_empty, ((uint32_t)j & 1) ^ 1);
+					mbar_expect_tx(m_full, L::M_BYTES);
+					for (int a = 0; a < L::M_BYTES / MASK_ATOM_BYTES; a++)
+						tma_load_4d(smem + L::M_OFF + a * MASK_ATOM_BYTES, &tmM, m_full, j * FW_K + a * (MASK == 1 ? 32 : 64), q0, p.mask_h ? h : 0, p.mask_b ? b : 0);
+				}
 				mbar_wait(&v_empty[s], ph ^ 1);
 				mbar_expect_tx(&v_full[s], FW_TILE);
 				for (int a = 0; a < 4; a++)
@@ -176,6 +197,17 @@ __global__ void __launch_bounds__(FW_THREADS, 1) fmha_wide_fwd_kernel(const __gr
 		// online softmax: key of accumulator i = j * 64 + 8 * (i >> 2) + 2 * t4 + (i & 1), row r0 + 8 * ((i >> 1) & 1)
 		const int kv0 = j * FW_K + 2 * t4;
 		const bool edge = j * FW_K + FW_K > min(kv_limit[0], kv_limit[1]);
+		if constexpr (MASK != 0)
+		{
+			// t = scale * s + mask in CPU_REF's order; keys past the row's horizon are overwritten with -inf below
+			mbar_wait(m_full, (uint32_t)j & 1);
+			add_mask<MASK, BF16>(sacc, smem + L::M_OFF, r0, t4, p.scale);
+			__syncwarp();
+			if (lane == 0)
+				mbar_arrive(m_empty);
+		}
+		// the running max and the exponents in log2 units: S scaled here, or the masked t = scale * S + mask
+		const float scale_log2 = MASK != 0 ? 1.4426950408889634f : p.scale_log2;
 		float mx[2] = { -INFINITY, -INFINITY };
 #pragma unroll
 		for (int i = 0; i < 32; i++)
@@ -191,7 +223,7 @@ __global__ void __launch_bounds__(FW_THREADS, 1) fmha_wide_fwd_kernel(const __gr
 		{
 			mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
 			mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
-			const float m_new = fmaxf(m[hh], mx[hh] * p.scale_log2);
+			const float m_new = fmaxf(m[hh], mx[hh] * scale_log2);
 			m_use[hh] = m_new == -INFINITY ? 0.f : m_new; // a fully masked row keeps p = 0 without NaN
 			alpha[hh] = exp2f(m[hh] - m_use[hh]);          // m = -inf -> 0
 			m[hh] = m_new;
@@ -201,7 +233,7 @@ __global__ void __launch_bounds__(FW_THREADS, 1) fmha_wide_fwd_kernel(const __gr
 		for (int i = 0; i < 32; i++)
 		{
 			const int hh = (i >> 1) & 1;
-			const float e = ex2_approx(fmaf(sacc[i], p.scale_log2, -m_use[hh])); // exp2(-inf) = 0 for the masked keys
+			const float e = ex2_approx(fmaf(sacc[i], scale_log2, -m_use[hh])); // exp2(-inf) = 0 for the masked keys
 			sacc[i] = e;
 			sum[hh] += e;
 		}
@@ -272,8 +304,8 @@ __global__ void __launch_bounds__(FW_THREADS, 1) fmha_wide_fwd_kernel(const __gr
 			if (d + 128 < p.D) // the padded feature columns are not part of the tensor
 				*reinterpret_cast<uint32_t*>(orow + d + 128) = pack2(o1[4 * jn + 2 * hh] * inv, o1[4 * jn + 2 * hh + 1] * inv, BF16);
 		}
-		if (p.lse && t4 == 0)
-			p.lse[((long long)b * p.H + h) * p.Sq + qi] = l[hh] > 0.f ? (m[hh] + log2f(l[hh])) * 0.6931471805599453f : -INFINITY;
+		if (p.lse && t4 == 0) // (a NaN in the mask makes l NaN: the masked kernels pass it on)
+			p.lse[((long long)b * p.H + h) * p.Sq + qi] = (MASK != 0 ? l[hh] != 0.f : l[hh] > 0.f) ? (m[hh] + log2f(l[hh])) * 0.6931471805599453f : -INFINITY;
 	}
 }
 
@@ -630,13 +662,13 @@ int launch_wide_bwd(cudaStream_t stream, const int is_bf16, const CUtensorMap& r
 	return is_bf16 ? launch_wide_bwd<MODE, 1>(stream, r1, r2, t1, t2, p, tiles, heads, B) : launch_wide_bwd<MODE, 0>(stream, r1, r2, t1, t2, p, tiles, heads, B);
 }
 
-template <int BF16>
-int launch_wide_fwd(cudaStream_t stream, const CUtensorMap& q, const CUtensorMap& k, const CUtensorMap& v, const WideFwdParams& p, const dim3 grid)
+template <int BF16, int MASK>
+int launch_wide_fwd(cudaStream_t stream, const CUtensorMap& q, const CUtensorMap& k, const CUtensorMap& v, const WideFwdParams& p, const CUtensorMap& m, const dim3 grid)
 {
 	static bool configured_on[64];
-	if (configure(fmha_wide_fwd_kernel<BF16>, WideFwdSmem::TOTAL, "cudaFuncSetAttribute(fmha_wide_fwd_kernel)", configured_on))
+	if (configure(fmha_wide_fwd_kernel<BF16, MASK>, WideFwdSmem<MASK>::TOTAL, "cudaFuncSetAttribute(fmha_wide_fwd_kernel)", configured_on))
 		return -1;
-	fmha_wide_fwd_kernel<BF16><<<grid, FW_THREADS, WideFwdSmem::TOTAL, stream>>>(q, k, v, p);
+	fmha_wide_fwd_kernel<BF16, MASK><<<grid, FW_THREADS, WideFwdSmem<MASK>::TOTAL, stream>>>(q, k, v, p, m);
 	return launched("fmha_wide_fwd_kernel launch");
 }
 
@@ -647,15 +679,18 @@ bool wide_shape(const SdpaGeom& g)
 
 } // namespace
 
-// returns 0 on success, 1 when the shape is outside this kernel (128 < D = Dv <= 256, a multiple of 8; 16-byte aligned strides), < 0 on
-// CUDA errors
-int sdpa_forward_f16_wide(cudaStream_t stream, const SdpaGeom& g, int is_bf16, const void* q, const void* k, const void* v, void* o, float* lse)
+// returns 0 on success, 1 when the shape is outside this kernel (128 < D = Dv <= 256, a multiple of 8; 16-byte aligned strides; a mask's
+// base and pitches 16-byte aligned), < 0 on CUDA errors
+int sdpa_forward_f16_wide(cudaStream_t stream, const SdpaGeom& g, int is_bf16, const void* q, const void* k, const void* v, void* o, float* lse, const void* mask, int mask_f32)
 {
 	if (!wide_shape(g))
 		return 1;
 	if ((((uintptr_t)o) & 15) || (g.o_b & 7) || (g.o_s & 7) || (g.o_h & 7))
 		return 1;
-	CUtensorMap tmQ, tmK, tmV;
+	CUtensorMap tmQ, tmK, tmV, tmM;
+	memset(&tmM, 0, sizeof(tmM));
+	if (mask && !make_map_mask(&tmM, mask, g.B, g.H, g.Sq, g.Sk, g.mask_b, g.mask_h, g.mask_s, mask_f32 ? 4 : 2, is_bf16))
+		return 1;
 	if (!make_map_bshd(&tmQ, q, g.B, g.Sq, g.H, g.D, g.q_b, g.q_s, g.q_h, is_bf16, FW_Q) || !make_map_bshd(&tmK, k, g.B, g.Sk, g.Hk, g.D, g.k_b, g.k_s, g.k_h, is_bf16, FW_K) ||
 		!make_map_bshd(&tmV, v, g.B, g.Sk, g.Hk, g.Dv, g.v_b, g.v_s, g.v_h, is_bf16, FW_K))
 		return 1;
@@ -666,8 +701,13 @@ int sdpa_forward_f16_wide(cudaStream_t stream, const SdpaGeom& g, int is_bf16, c
 	p.scale_log2 = g.scale * 1.4426950408889634f;
 	p.o = o, p.o_b = g.o_b, p.o_s = g.o_s, p.o_h = g.o_h;
 	p.lse = lse;
+	p.scale = g.scale;
+	p.mask_h = g.mask_h != 0, p.mask_b = g.mask_b != 0;
 	const dim3 grid((g.Sq + FW_Q - 1) / FW_Q, g.H, g.B);
-	return is_bf16 ? launch_wide_fwd<1>(stream, tmQ, tmK, tmV, p, grid) : launch_wide_fwd<0>(stream, tmQ, tmK, tmV, p, grid);
+	const int kind = mask ? (mask_f32 ? 1 : 2) : 0;
+	if (is_bf16)
+		return kind == 0 ? launch_wide_fwd<1, 0>(stream, tmQ, tmK, tmV, p, tmM, grid) : kind == 1 ? launch_wide_fwd<1, 1>(stream, tmQ, tmK, tmV, p, tmM, grid) : launch_wide_fwd<1, 2>(stream, tmQ, tmK, tmV, p, tmM, grid);
+	return kind == 0 ? launch_wide_fwd<0, 0>(stream, tmQ, tmK, tmV, p, tmM, grid) : kind == 1 ? launch_wide_fwd<0, 1>(stream, tmQ, tmK, tmV, p, tmM, grid) : launch_wide_fwd<0, 2>(stream, tmQ, tmK, tmV, p, tmM, grid);
 }
 
 // The arguments and the workspace of sdpa_backward_f16 (sdpa_backward_f16_workspace_bytes covers this path: the same statistics, and

@@ -568,7 +568,9 @@ enum {
 enum {
 	CCV_NNC_SM100_SDPA_ALGO_COMPOSED = 0, /* 16-bit D <= 128: the flash kernels; every other call: the fp32 path (16-bit widened) */
 	CCV_NNC_SM100_SDPA_ALGO_FLASH = 1,    /* as COMPOSED, plus 16-bit 128 < D = Dv <= 256 without a mask on the wide flash kernels */
-	CCV_NNC_SM100_SDPA_ALGO_COUNT = 2,
+	CCV_NNC_SM100_SDPA_ALGO_FLASH_MASK = 2, /* forward only: 16-bit calls WITH an additive mask (fp32 or 16-bit), D = Dv <= 256, on the
+	                                           flash kernels, log-sum-exp and views included; every other call: CCV_NNC_EXEC_NO_KERNEL */
+	CCV_NNC_SM100_SDPA_ALGO_COUNT = 3,
 };
 
 /* ------------------------------------------------------------------------------------------------------------ */
