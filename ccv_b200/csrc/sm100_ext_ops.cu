@@ -204,12 +204,12 @@ __global__ void index_select_lerp_kernel(const float* __restrict__ a, const floa
 	if (j0 < 0 || j0 >= a_rows)
 		return;
 	const int j1 = min(j0 + 1, a_rows - 1);
-	const float w1 = f - j0, w0 = 1.f - w1;
+	const float w1 = __fsub_rn(f, (float)j0), w0 = __fsub_rn(1.f, w1);
 	const float* const ap0 = a + (long long)j0 * a_inc;
 	const float* const ap1 = a + (long long)j1 * a_inc;
 	float* const bp = b + (long long)i * b_inc;
 	for (int j = threadIdx.x; j < cols; j += blockDim.x)
-		bp[j] = ap0[j] * w0 + ap1[j] * w1;
+		bp[j] = __fadd_rn(__fmul_rn(ap0[j], w0), __fmul_rn(ap1[j], w1)); // the reference's rounding: no FMA
 }
 // backward: h[r, :] = sum over i with indices[i] == r of g[i, :], added in increasing i (the reference's order: bit-reproducible,
 // no atomics).  One block per row of h; every block walks the index list (broadcast loads).

@@ -375,27 +375,32 @@ int rmsnorm_bwd(cudaStream_t s, const NormKinds& k, const void* g, const void* x
 }
 
 // ------------------------------------------------------------------------------------------------ upsample
+// Every result is the reference's bit for bit: the source indices and coefficients use its arithmetic (double where it computes in
+// double, each intermediate rounded where it rounds, nothing contracted into an FMA), the forward its association, and the
+// backward sums each input element's contributions in the reference's order.
 struct Coef {
 	int i0, i1;
 	float c0, c1;
 };
-// _ccv_nnc_init_bi_coeffs (upsample/ccv_nnc_upsample_cpu_ref.c:220-243), same float arithmetic
+// _ccv_nnc_init_bi_coeffs (upsample/ccv_nnc_upsample_cpu_ref.c:220-243): xs = i * s in float, or (i + 0.5) * s - 0.5 in double
+// rounded to float once
 __device__ __forceinline__ Coef bi_coef(const int i, const int ss, const float s, const int align_corners)
 {
-	const float xs = align_corners ? i * s : (i + 0.5f) * s - 0.5f;
+	const float xs = align_corners ? __fmul_rn((float)i, s) : (float)__dsub_rn(__dmul_rn(i + 0.5, (double)s), 0.5);
 	Coef c;
 	c.i0 = (int)xs;
-	c.i1 = min((int)(xs + 1), ss - 1);
-	c.c1 = xs - c.i0;
-	c.c0 = 1.0f - c.c1;
+	c.i1 = min((int)__fadd_rn(xs, 1.f), ss - 1);
+	c.c1 = __fsub_rn(xs, (float)c.i0);
+	c.c0 = __fsub_rn(1.f, c.c1);
 	return c;
 }
+// upsample_cpu_ref.c:48,62: (int)((i + 0.5) * s) in double, or (int)(i * s + 0.5) with i * s in float and the sum in double.  In float
+// alone (i + 0.5) * s can round up to an integer k that the double product stays below (6 -> 19 rows at i = 9).
 __device__ __forceinline__ int nearest_idx(const int i, const int ss, const float s, const int align_corners)
 {
-	return min(align_corners ? (int)(i * s + 0.5f) : (int)((i + 0.5f) * s), ss - 1);
+	return min(align_corners ? (int)((double)__fmul_rn((float)i, s) + 0.5) : (int)__dmul_rn(i + 0.5, (double)s), ss - 1);
 }
 // thread per output element; NHWC: channels fastest (coalesced); NCHW: width fastest
-template <int BWD>
 __global__ void upsample_kernel(const float* __restrict__ src, float* __restrict__ dst, const int N, const int H, const int W, const int C, const int OH, const int OW, const int type, const int align_corners, const int nchw, const float rh, const float rw)
 {
 	const size_t total = (size_t)N * OH * OW * C;
@@ -408,32 +413,110 @@ __global__ void upsample_kernel(const float* __restrict__ src, float* __restrict
 		else
 			c = r % C, r /= C, ox = r % OW, r /= OW, oy = r % OH, n = (int)(r / OH);
 		auto in_at = [&](int y, int x) -> size_t { return nchw ? (((size_t)n * C + c) * H + y) * W + x : (((size_t)n * H + y) * W + x) * C + c; };
-		// forward: dst = output (upsampled), src = input. backward: src = output gradient (upsampled), dst = input gradient
 		if (type == 0)
 		{
-			const int y = nearest_idx(oy, H, rh, align_corners), x = nearest_idx(ox, W, rw, align_corners);
-			if (BWD)
-				atomicAdd(dst + in_at(y, x), src[i]);
-			else
-				dst[i] = src[in_at(y, x)];
-		} else {
-			const Coef cy = bi_coef(oy, H, rh, align_corners), cx = bi_coef(ox, W, rw, align_corners);
-			if (BWD)
-			{
-				const float v = src[i];
-				atomicAdd(dst + in_at(cy.i0, cx.i0), v * cy.c0 * cx.c0);
-				atomicAdd(dst + in_at(cy.i0, cx.i1), v * cy.c0 * cx.c1);
-				atomicAdd(dst + in_at(cy.i1, cx.i0), v * cy.c1 * cx.c0);
-				atomicAdd(dst + in_at(cy.i1, cx.i1), v * cy.c1 * cx.c1);
-			} else
-				dst[i] = src[in_at(cy.i0, cx.i0)] * cx.c0 * cy.c0 + src[in_at(cy.i0, cx.i1)] * cx.c1 * cy.c0 + src[in_at(cy.i1, cx.i0)] * cx.c0 * cy.c1 + src[in_at(cy.i1, cx.i1)] * cx.c1 * cy.c1;
+			dst[i] = src[in_at(nearest_idx(oy, H, rh, align_corners), nearest_idx(ox, W, rw, align_corners))];
+			continue;
 		}
+		const Coef cy = bi_coef(oy, H, rh, align_corners), cx = bi_coef(ox, W, rw, align_corners);
+		const float a00 = src[in_at(cy.i0, cx.i0)], a01 = src[in_at(cy.i0, cx.i1)], a10 = src[in_at(cy.i1, cx.i0)], a11 = src[in_at(cy.i1, cx.i1)];
+		float t00, t01, t10, t11;
+		if (nchw) // ap1[si0] * sc0 * ysc0 + ... (upsample_cpu_ref.c:304-305)
+			t00 = __fmul_rn(__fmul_rn(a00, cx.c0), cy.c0), t01 = __fmul_rn(__fmul_rn(a01, cx.c1), cy.c0), t10 = __fmul_rn(__fmul_rn(a10, cx.c0), cy.c1), t11 = __fmul_rn(__fmul_rn(a11, cx.c1), cy.c1);
+		else // c00 = sc0 * ysc0, ap00[cd] * c00 + ... (:345-355)
+			t00 = __fmul_rn(a00, __fmul_rn(cx.c0, cy.c0)), t01 = __fmul_rn(a01, __fmul_rn(cx.c1, cy.c0)), t10 = __fmul_rn(a10, __fmul_rn(cx.c0, cy.c1)), t11 = __fmul_rn(a11, __fmul_rn(cx.c1, cy.c1));
+		dst[i] = __fadd_rn(__fadd_rn(__fadd_rn(t00, t01), t10), t11);
+	}
+}
+// The output rows (columns) that read input row y form one range: f, the source row of an output row, is non-decreasing.  From an
+// estimate o, the least o with f(o) >= y (O when there is none) and the greatest o with f(o) <= y (-1 when there is none).
+template <typename F>
+__device__ __forceinline__ int first_at_least(const F& f, const int y, int o, const int O)
+{
+	while (o > 0 && f(o - 1) >= y)
+		o--;
+	while (o < O && f(o) < y)
+		o++;
+	return o;
+}
+template <typename F>
+__device__ __forceinline__ int last_at_most(const F& f, const int y, int o, const int O)
+{
+	while (o < O - 1 && f(o + 1) <= y)
+		o++;
+	while (o >= 0 && f(o) > y)
+		o--;
+	return o;
+}
+// where output row y / s lies, clamped to [0, O]
+__device__ __forceinline__ int estimate(const double y, const float s, const int O)
+{
+	return s > 0 ? (int)fmin(fmax(y / s, 0.0), (double)O) : 0;
+}
+// thread per input element: the sum of the output gradients that read it, in output raster order and, within one output, over the
+// corners 00, 01, 10, 11 -- the order the reference adds them in (upsample_cpu_ref.c:168-169, 204-205, 425-428, 478-481).  No atomics:
+// the result is the same on every run.
+__global__ void upsample_back_kernel(const float* __restrict__ g, float* __restrict__ h, const int N, const int H, const int W, const int C, const int OH, const int OW, const int type, const int align_corners, const int nchw, const float rh, const float rw)
+{
+	const size_t total = (size_t)N * H * W * C;
+	for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x)
+	{
+		int n, c, y, x;
+		size_t r = i;
+		if (nchw)
+			x = r % W, r /= W, y = r % H, r /= H, c = r % C, n = (int)(r / C);
+		else
+			c = r % C, r /= C, x = r % W, r /= W, y = r % H, n = (int)(r / H);
+		auto out_at = [&](int oy, int ox) -> size_t { return nchw ? (((size_t)n * C + c) * OH + oy) * OW + ox : (((size_t)n * OH + oy) * OW + ox) * C + c; };
+		float acc = 0.f;
+		if (type == 0)
+		{
+			auto fy = [&](int o) { return nearest_idx(o, H, rh, align_corners); };
+			auto fx = [&](int o) { return nearest_idx(o, W, rw, align_corners); };
+			const int y0 = first_at_least(fy, y, estimate(y, rh, OH), OH), y1 = last_at_most(fy, y, estimate(y + 1, rh, OH) - 1, OH);
+			const int x0 = first_at_least(fx, x, estimate(x, rw, OW), OW), x1 = last_at_most(fx, x, estimate(x + 1, rw, OW) - 1, OW);
+			for (int oy = y0; oy <= y1; oy++)
+				for (int ox = x0; ox <= x1; ox++)
+					acc = __fadd_rn(acc, g[out_at(oy, ox)]);
+		} else {
+			// an output reads row y when its i1 >= y and its i0 <= y, and then through one or both of its corner rows
+			auto fy0 = [&](int o) { return bi_coef(o, H, rh, align_corners).i0; };
+			auto fy1 = [&](int o) { return bi_coef(o, H, rh, align_corners).i1; };
+			auto fx0 = [&](int o) { return bi_coef(o, W, rw, align_corners).i0; };
+			auto fx1 = [&](int o) { return bi_coef(o, W, rw, align_corners).i1; };
+			const int y0 = first_at_least(fy1, y, estimate(y - 1, rh, OH), OH), y1 = last_at_most(fy0, y, estimate(y + 1, rh, OH) - 1, OH);
+			const int x0 = first_at_least(fx1, x, estimate(x - 1, rw, OW), OW), x1 = last_at_most(fx0, x, estimate(x + 1, rw, OW) - 1, OW);
+			for (int oy = y0; oy <= y1; oy++)
+			{
+				const Coef cy = bi_coef(oy, H, rh, align_corners);
+				for (int ox = x0; ox <= x1; ox++)
+				{
+					const Coef cx = bi_coef(ox, W, rw, align_corners);
+					const float v = g[out_at(oy, ox)];
+					for (int ry = 0; ry < 2; ry++)
+						if ((ry ? cy.i1 : cy.i0) == y)
+							for (int rx = 0; rx < 2; rx++)
+								if ((rx ? cx.i1 : cx.i0) == x)
+								{
+									const float ysc = ry ? cy.c1 : cy.c0, xsc = rx ? cx.c1 : cx.c0;
+									// NCHW: bp1[xd] * ysc * sc; NHWC: bp1[cd] * (sc * ysc)
+									acc = __fadd_rn(acc, nchw ? __fmul_rn(__fmul_rn(v, ysc), xsc) : __fmul_rn(v, __fmul_rn(xsc, ysc)));
+								}
+				}
+			}
+		}
+		h[i] = acc;
 	}
 }
 static void ratios(int H, int W, int OH, int OW, int align_corners, float& rh, float& rw)
 {
 	rh = align_corners ? (float)(H - 1) / (OH - 1 > 1 ? OH - 1 : 1) : (float)H / OH;
 	rw = align_corners ? (float)(W - 1) / (OW - 1 > 1 ? OW - 1 : 1) : (float)W / OW;
+}
+static unsigned upsample_blocks(const size_t total)
+{
+	const size_t blocks = (total + 255) / 256;
+	return (unsigned)(blocks > 132 * 16 ? 132 * 16 : blocks);
 }
 int upsample_fwd_f32(cudaStream_t s, const float* a, float* b, int N, int H, int W, int C, int OH, int OW, int type, int align_corners, int nchw)
 {
@@ -442,25 +525,17 @@ int upsample_fwd_f32(cudaStream_t s, const float* a, float* b, int N, int H, int
 		return 0;
 	float rh, rw;
 	ratios(H, W, OH, OW, align_corners, rh, rw);
-	size_t blocks = (total + 255) / 256;
-	if (blocks > 132 * 16)
-		blocks = 132 * 16;
-	upsample_kernel<0><<<(unsigned)blocks, 256, 0, s>>>(a, b, N, H, W, C, OH, OW, type, align_corners, nchw, rh, rw);
+	upsample_kernel<<<upsample_blocks(total), 256, 0, s>>>(a, b, N, H, W, C, OH, OW, type, align_corners, nchw, rh, rw);
 	return check("upsample_fwd");
 }
 int upsample_bwd_f32(cudaStream_t s, const float* g, float* h, int N, int H, int W, int C, int OH, int OW, int type, int align_corners, int nchw)
 {
-	const size_t total = (size_t)N * OH * OW * C;
-	if (cudaMemsetAsync(h, 0, (size_t)N * H * W * C * 4, s) != cudaSuccess)
-		return -1;
+	const size_t total = (size_t)N * H * W * C;
 	if (total == 0)
 		return 0;
 	float rh, rw;
 	ratios(H, W, OH, OW, align_corners, rh, rw);
-	size_t blocks = (total + 255) / 256;
-	if (blocks > 132 * 16)
-		blocks = 132 * 16;
-	upsample_kernel<1><<<(unsigned)blocks, 256, 0, s>>>(g, h, N, H, W, C, OH, OW, type, align_corners, nchw, rh, rw);
+	upsample_back_kernel<<<upsample_blocks(total), 256, 0, s>>>(g, h, N, H, W, C, OH, OW, type, align_corners, nchw, rh, rw);
 	return check("upsample_bwd");
 }
 
