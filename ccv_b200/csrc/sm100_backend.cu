@@ -2547,6 +2547,30 @@ int backend_qx_decode(void* const stream_context, const void* const tensor, void
 {
 	return qx_decode(stream_of((ccv_nnc_stream_context_t*)stream_context), (const ccv_nnc_tensor_t*)tensor, out);
 }
+// GEMM_BACKWARD(NO_TRANSPOSE, TRANSPOSE(0, 1)) as ccv_nnc_cmd() makes it: algorithm -1, no blas flags
+static ccv_nnc_cmd_t gemm_back_nt_cmd()
+{
+	ccv_nnc_cmd_t cmd;
+	memset(&cmd, 0, sizeof(cmd));
+	cmd.cmd = CCV_NNC_GEMM_BACKWARD;
+	cmd.backend = CCV_NNC_BACKEND_GPU_SM100;
+	cmd.algorithm = -1;
+	cmd.info.blas.a[0] = 1, cmd.info.blas.a[1] = 1;
+	cmd.info.blas.transpose_b[0] = 0, cmd.info.blas.transpose_b[1] = 1;
+	return cmd;
+}
+size_t backend_gemm_back_workspace(void* const* const inputs, void* const* const outputs)
+{
+	ccv_nnc_hint_t hint;
+	memset(&hint, 0, sizeof(hint));
+	return gemm_back_workspace(gemm_back_nt_cmd(), hint, (ccv_nnc_tensor_t* const*)inputs, 3, (ccv_nnc_tensor_t* const*)outputs, 3);
+}
+int backend_gemm_back(void* const stream_context, const int flags, void* const* const inputs, void* const* const outputs)
+{
+	ccv_nnc_hint_t hint;
+	memset(&hint, 0, sizeof(hint));
+	return exec_gemm_back_any(gemm_back_nt_cmd(), hint, flags, (ccv_nnc_tensor_t* const*)inputs, 3, (ccv_nnc_tensor_t* const*)outputs, 3, (ccv_nnc_stream_context_t*)stream_context);
+}
 } // namespace sm100
 
 // implemented in sm100_backend_ext.cu (attention, layer / rms norm, upsample, allreduce)

@@ -4,6 +4,7 @@
 #include "sm100_ew.h"
 #include <cuda_runtime.h>
 #include <string.h>
+#include <algorithm>
 
 using namespace sm100;
 
@@ -368,14 +369,31 @@ int ccv_nnc_sm100_exec_sdpa_forw(SM100_EXEC_ARGS)
 	return CCV_NNC_EXEC_SUCCESS;
 }
 
-// :259-479: inputs[0] = g, [3] = q, [4] = k, [5] = v -> outputs (dq, dk, dv); masks are not differentiable here either (:262)
-int ccv_nnc_sm100_exec_sdpa_back(SM100_EXEC_ARGS)
+// The forward's saved output and log-sum-exp (inputs[9], inputs[10] of the backward without weights: ...flash_attn.cu:240-241), when both
+// are there and fit the call; otherwise the fused kernels recompute them
+static void sdpa_saved(const ccv_nnc_tensor_t* const o_t, const ccv_nnc_tensor_t* const lse_t, const int dt, const SdpaGeom& g, const void*& o_ptr, const float*& lse_ptr, long long& oo_b, long long& oo_s, long long& oo_h)
 {
-	if (cmd.algorithm == CCV_NNC_SM100_SDPA_ALGO_FLASH_MASK) // a forward-only algorithm: the mask is not differentiable (:262)
-		return CCV_NNC_EXEC_NO_KERNEL;
+	o_ptr = 0, lse_ptr = 0, oo_b = oo_s = oo_h = 0;
+	if (o_t && lse_t && packed_f32(lse_t) && count_of(lse_t) == (size_t)g.B * g.H * g.Sq)
+	{
+		int oB, oS, oH, oD;
+		if (sdpa_axes(o_t, dt, oB, oS, oH, oD, oo_b, oo_s, oo_h) && oB == g.B && oS == g.Sq && oH == g.H && oD == g.Dv)
+			o_ptr = o_t->data.u8, lse_ptr = lse_t->data.f32;
+	}
+}
+
+// the functional form's workspace: g, q, k, v widened, dq, dk, dv in fp32, the fp32 path's own
+static size_t sdpa_back_func_bytes(ccv_nnc_tensor_t* const* const inputs, const SdpaGeom& g)
+{
+	const size_t floats = count_of(inputs[0]) + 2 * (count_of(inputs[3]) + count_of(inputs[4]) + count_of(inputs[5]));
+	return floats * sizeof(float) + 256 + sdpa_workspace_bytes(g.Sq, g.Sk, 1);
+}
+
+// inputs (g, -, -, q, k, v, -, -, -, [o], [lse]) -> outputs (dq, dk, dv).  No workspace request is larger than ws_cap: a call that would need
+// more is refused (the unify-head backward holds its output gradient past that size).
+static int sdpa_back_core(SM100_EXEC_ARGS, const size_t ws_cap)
+{
 	if (input_size < 6 || output_size < 3 || !inputs[0] || !inputs[3] || !inputs[4] || !inputs[5] || !outputs[0] || !outputs[1] || !outputs[2])
-		return CCV_NNC_EXEC_INVALID;
-	if ((input_size > 6 && inputs[6]) || (input_size > 7 && inputs[7]))
 		return CCV_NNC_EXEC_INVALID;
 	SdpaGeom g, dg;
 	const int dt = CCV_GET_DATA_TYPE(inputs[3]->info.datatype);
@@ -390,22 +408,17 @@ int ccv_nnc_sm100_exec_sdpa_back(SM100_EXEC_ARGS)
 		if (dg.B != g.B || dg.H != g.H || dg.Hk != g.Hk || dg.Sq != g.Sq || dg.Sk != g.Sk || dg.D != g.D || dg.Dv != g.Dv)
 			return CCV_NNC_EXEC_INVALID;
 		// the fused wgmma backward (sm100_fmha_bwd.cu) when it covers the call: head dimension 128, 16-byte aligned rows.  It works
-		// from the forward's saved output and log-sum-exp (inputs[9], inputs[10]: ...flash_attn.cu:240-241) and recomputes both itself
-		// when the caller does not pass them.
+		// from the forward's saved output and log-sum-exp and recomputes both itself when the caller does not pass them.
 		{
-			const ccv_nnc_tensor_t* const o_t = input_size > 9 ? inputs[9] : 0;
-			const ccv_nnc_tensor_t* const lse_t = input_size > 10 ? inputs[10] : 0;
-			const void* o_ptr = 0;
-			const float* lse_ptr = 0;
-			long long oo_b = 0, oo_s = 0, oo_h = 0;
-			if (o_t && lse_t && packed_f32(lse_t) && count_of(lse_t) == (size_t)g.B * g.H * g.Sq)
-			{
-				int oB, oS, oH, oD;
-				if (sdpa_axes(o_t, dt, oB, oS, oH, oD, oo_b, oo_s, oo_h) && oB == g.B && oS == g.Sq && oH == g.H && oD == g.Dv)
-					o_ptr = o_t->data.u8, lse_ptr = lse_t->data.f32;
-			}
+			const void* o_ptr;
+			const float* lse_ptr;
+			long long oo_b, oo_s, oo_h;
+			sdpa_saved(input_size > 9 ? inputs[9] : 0, input_size > 10 ? inputs[10] : 0, dt, g, o_ptr, lse_ptr, oo_b, oo_s, oo_h);
 			const int need_forward = !o_ptr;
-			void* const fws = ccv_nnc_stream_context_get_workspace(stream_context, sdpa_backward_f16_workspace_bytes(g, need_forward), CCV_TENSOR_GPU_MEMORY);
+			const size_t fws_bytes = sdpa_backward_f16_workspace_bytes(g, need_forward);
+			if (fws_bytes > ws_cap)
+				return CCV_NNC_EXEC_INVALID;
+			void* const fws = ccv_nnc_stream_context_get_workspace(stream_context, fws_bytes, CCV_TENSOR_GPU_MEMORY);
 			if (!fws)
 				return CCV_NNC_EXEC_OOM;
 			int rc = sdpa_backward_f16(stream_of(stream_context), g, dg, dt == CCV_16BF, inputs[0]->data.u8, inputs[3]->data.u8, inputs[4]->data.u8, inputs[5]->data.u8, o_ptr, oo_b, oo_s, oo_h, lse_ptr,
@@ -426,8 +439,12 @@ int ccv_nnc_sm100_exec_sdpa_back(SM100_EXEC_ARGS)
 			if (CCV_IS_TENSOR_VIEW(outputs[i]))
 				return CCV_NNC_EXEC_INVALID;
 		const size_t nq = count_of(inputs[3]), nk = count_of(inputs[4]), nv = count_of(inputs[5]), no = count_of(inputs[0]);
-		const size_t floats = no + 2 * nq + 2 * nk + 2 * nv;
-		const size_t ws_bytes = floats * sizeof(float) + 256 + sdpa_workspace_bytes(g.Sq, g.Sk, 1);
+		const size_t ws_bytes = sdpa_back_func_bytes(inputs, g);
+		if (ws_bytes > ws_cap)
+		{
+			set_last_error("attention backward: the functional form's workspace exceeds the unify-head backward's request", cudaErrorInvalidValue);
+			return CCV_NNC_EXEC_INVALID;
+		}
 		float* const base = (float*)ccv_nnc_stream_context_get_workspace(stream_context, ws_bytes, CCV_TENSOR_GPU_MEMORY);
 		if (!base)
 			return CCV_NNC_EXEC_OOM;
@@ -455,12 +472,149 @@ int ccv_nnc_sm100_exec_sdpa_back(SM100_EXEC_ARGS)
 		return CCV_NNC_EXEC_INVALID;
 	if (dg.B != g.B || dg.H != g.H || dg.Hk != g.Hk || dg.Sq != g.Sq || dg.Sk != g.Sk || dg.D != g.D || dg.Dv != g.Dv)
 		return CCV_NNC_EXEC_INVALID;
+	if (sdpa_workspace_bytes(g.Sq, g.Sk, 1) > ws_cap)
+		return CCV_NNC_EXEC_INVALID;
 	void* const ws = ccv_nnc_stream_context_get_workspace(stream_context, sdpa_workspace_bytes(g.Sq, g.Sk, 1), CCV_TENSOR_GPU_MEMORY);
 	if (!ws)
 		return CCV_NNC_EXEC_OOM;
 	if (sdpa_backward_f32(stream_of(stream_context), g, inputs[0]->data.f32, inputs[3]->data.f32, inputs[4]->data.f32, inputs[5]->data.f32, outputs[0]->data.f32, outputs[1]->data.f32, outputs[2]->data.f32, dg, ws))
 		return CCV_NNC_EXEC_INVALID;
 	return CCV_NNC_EXEC_SUCCESS;
+}
+
+// The largest workspace request sdpa_back_core makes for these operands (whose data pointers it does not read), (size_t)-1 when it refuses
+// them.  16-bit: the fused kernels' statistics (and O / LSE when they recompute them), plus the functional form's when the fused kernels may
+// decline the call: sdpa_backward_f16_takes, the same test those kernels make (and the saved output's alignment, which they test later).
+static size_t sdpa_back_workspace(const ccv_nnc_cmd_t& cmd, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs)
+{
+	SdpaGeom g, dg;
+	if (!sdpa_geom(cmd, inputs[3], inputs[4], inputs[5], inputs[0], g) || !sdpa_geom(cmd, outputs[0], outputs[1], outputs[2], inputs[0], dg))
+		return (size_t)-1;
+	if (dg.B != g.B || dg.H != g.H || dg.Hk != g.Hk || dg.Sq != g.Sq || dg.Sk != g.Sk || dg.D != g.D || dg.Dv != g.Dv)
+		return (size_t)-1;
+	const int dt = CCV_GET_DATA_TYPE(inputs[3]->info.datatype);
+	if (dt == CCV_32F)
+		return sdpa_workspace_bytes(g.Sq, g.Sk, 1);
+	const void* o_ptr;
+	const float* lse_ptr;
+	long long oo_b, oo_s, oo_h;
+	sdpa_saved(input_size > 9 ? inputs[9] : 0, input_size > 10 ? inputs[10] : 0, dt, g, o_ptr, lse_ptr, oo_b, oo_s, oo_h);
+	const size_t fused = sdpa_backward_f16_workspace_bytes(g, !o_ptr);
+	const void* const ptrs[8] = { outputs[0]->data.u8, outputs[1]->data.u8, outputs[2]->data.u8, inputs[0]->data.u8, inputs[3]->data.u8, inputs[4]->data.u8, inputs[5]->data.u8, o_ptr };
+	bool takes = sdpa_backward_f16_takes(g, dg, 0, ptrs, 8) || (cmd.algorithm == CCV_NNC_SM100_SDPA_ALGO_FLASH && sdpa_backward_f16_takes(g, dg, 1, ptrs, 8));
+	for (const long long st : { oo_b, oo_s, oo_h })
+		takes = takes && !(st & 7);
+	if (takes)
+		return fused;
+	for (int i : { 0, 3, 4, 5 }) // the functional form refuses views
+		if (CCV_IS_TENSOR_VIEW(inputs[i]) || (i < 3 && CCV_IS_TENSOR_VIEW(outputs[i])))
+			return (size_t)-1;
+	return std::max(fused, sdpa_back_func_bytes(inputs, g));
+}
+
+// The backward through the unify-head projection y = c_flat w^T + bias, c_flat = c seen as [B S, n], n = H Dv:
+//   dc = g w, dw (+)= g^T c_flat, dbias (+)= the column sums of g
+// are GEMM_BACKWARD(transpose_b) on g, c_flat and w, bit for bit; dc goes to the stream workspace as a packed [B, S, H, Dv] tensor and the
+// attention backward runs on it with O = c.  One workspace request [the inner calls' largest | dc]: neither inner call asks for more than
+// the first part, so dc stays where it is.
+static int sdpa_back_unify(SM100_EXEC_ARGS)
+{
+	ccv_nnc_tensor_t* const gy = inputs[0];
+	ccv_nnc_tensor_t* const w = inputs[7];
+	ccv_nnc_tensor_t* const bias = input_size > 8 ? inputs[8] : 0;
+	ccv_nnc_tensor_t* const lse = input_size > 10 ? inputs[10] : 0;
+	ccv_nnc_tensor_t* const c = input_size > 11 ? inputs[11] : 0;
+	ccv_nnc_tensor_t* const dw = output_size > 4 ? outputs[4] : 0;
+	ccv_nnc_tensor_t* const dbias = output_size > 5 ? outputs[5] : 0;
+	if (input_size < 12 || output_size < 3 || !gy || !inputs[3] || !inputs[4] || !inputs[5] || !c || !outputs[0] || !outputs[1] || !outputs[2])
+		return CCV_NNC_EXEC_INVALID;
+	if ((output_size > 3 && outputs[3]) || (dbias && !bias))
+		return CCV_NNC_EXEC_INVALID;
+	// the weights are dense here: their gradient is asked for
+	const int dt = CCV_GET_DATA_TYPE(inputs[3]->info.datatype);
+	if (dt != CCV_32F && dt != CCV_16BF && dt != CCV_16F)
+		return CCV_NNC_EXEC_INVALID;
+	for (ccv_nnc_tensor_t* const t : { gy, c, w, dw, dbias })
+		if (t && CCV_IS_TENSOR_VIEW(t))
+			return CCV_NNC_EXEC_INVALID;
+	SdpaGeom g;
+	if (!sdpa_geom(cmd, inputs[3], inputs[4], inputs[5], c, g)) // c: [B, Sq, H, Dv] (3-d: one head) of the activations' type
+		return CCV_NNC_EXEC_INVALID;
+	const long long n = (long long)g.H * g.Dv, rows = (long long)g.B * g.Sq;
+	if (n > 0x7fffffff || rows > 0x7fffffff)
+		return CCV_NNC_EXEC_INVALID;
+	if (CCV_GET_DATA_TYPE(gy->info.datatype) != dt || nd_of(gy) != 3 || gy->info.dim[0] != g.B || gy->info.dim[1] != g.Sq || gy->info.dim[2] != n)
+		return CCV_NNC_EXEC_INVALID;
+	if (CCV_GET_DATA_TYPE(w->info.datatype) != dt || nd_of(w) != 2 || w->info.dim[0] != n || w->info.dim[1] != n)
+		return CCV_NNC_EXEC_INVALID;
+	if (dw && (CCV_GET_DATA_TYPE(dw->info.datatype) != dt || count_of(dw) != (size_t)(n * n)))
+		return CCV_NNC_EXEC_INVALID;
+	for (ccv_nnc_tensor_t* const b : { bias, dbias })
+		if (b && ((CCV_GET_DATA_TYPE(b->info.datatype) != dt && CCV_GET_DATA_TYPE(b->info.datatype) != CCV_32F) || count_of(b) != (size_t)n))
+			return CCV_NNC_EXEC_INVALID;
+	if (lse && (!packed_f32(lse) || count_of(lse) != (size_t)g.B * g.H * g.Sq))
+		return CCV_NNC_EXEC_INVALID;
+	// matrix headers of the same memory: g and dc as [B Sq, n], c_flat, w [n, n], dw [n, n], dbias [n]
+	const int esz = dt == CCV_32F ? 4 : 2;
+	ccv_nnc_tensor_t g2 = *gy, c2 = *c, dc2 = *gy, dc = *c, w2 = *w, dw2, db2;
+	for (ccv_nnc_tensor_t* const t : { &g2, &c2, &dc2, &w2 })
+	{
+		memset(t->info.dim, 0, sizeof(t->info.dim));
+		t->info.dim[0] = (int)(t == &w2 ? n : rows), t->info.dim[1] = (int)n;
+	}
+	if (dw)
+	{
+		dw2 = *dw, memset(dw2.info.dim, 0, sizeof(dw2.info.dim));
+		dw2.info.dim[0] = (int)n, dw2.info.dim[1] = (int)n;
+	}
+	if (dbias)
+	{
+		db2 = *dbias, memset(db2.info.dim, 0, sizeof(db2.info.dim));
+		db2.info.dim[0] = (int)n;
+	}
+	dc2.data.u8 = 0, dc.data.u8 = 0;
+	void* gemm_in[3] = { &g2, &c2, &w2 };
+	void* params_out[3] = { 0, dw ? &dw2 : 0, dbias ? &db2 : 0 };
+	void* dc_out[3] = { &dc2, 0, 0 };
+	void* all_out[3] = { &dc2, dw ? &dw2 : 0, dbias ? &db2 : 0 };
+	ccv_nnc_tensor_t* core_in[11] = { &dc, 0, 0, inputs[3], inputs[4], inputs[5], 0, 0, 0, c, lse };
+	const size_t attn = sdpa_back_workspace(cmd, core_in, 11, outputs);
+	if (attn == (size_t)-1)
+		return CCV_NNC_EXEC_INVALID;
+	const size_t inner = std::max(backend_gemm_back_workspace(gemm_in, all_out), attn);
+	const size_t at = (inner + 255) & ~(size_t)255;
+	unsigned char* const ws = (unsigned char*)ccv_nnc_stream_context_get_workspace(stream_context, at + (size_t)rows * n * esz, CCV_TENSOR_GPU_MEMORY);
+	if (!ws)
+		return CCV_NNC_EXEC_OOM;
+	dc2.data.u8 = dc.data.u8 = ws + at;
+	// dbias and dw accumulate as GEMM_BACKWARD's do; dc is the workspace's, written afresh
+	int rc = dw || dbias ? backend_gemm_back(stream_context, flags, gemm_in, params_out) : CCV_NNC_EXEC_SUCCESS;
+	if (rc == CCV_NNC_EXEC_SUCCESS)
+		rc = backend_gemm_back(stream_context, flags & ~CCV_NNC_ACCUMULATE_OUTPUT, gemm_in, dc_out);
+	if (rc == CCV_NNC_EXEC_SUCCESS)
+		rc = sdpa_back_core(cmd, hint, flags, core_in, 11, outputs, 3, stream_context, inner);
+	if (rc == CCV_NNC_EXEC_SUCCESS && ccv_nnc_stream_context_get_workspace(stream_context, 1, CCV_TENSOR_GPU_MEMORY) != (void*)ws)
+	{
+		set_last_error("attention backward: the workspace moved under the output gradient", cudaErrorInvalidValue);
+		return CCV_NNC_EXEC_INVALID;
+	}
+	return rc;
+}
+
+// :259-479: inputs (g, -, -, q, k, v, [attn_mask], [w], [bias], y, [lse], [c]) -> outputs (dq, dk, dv, -, [dw], [dbias]).  Without weights
+// inputs[9] is the attention's output O; with the unify-head weights (inputs[7]) y is the projection's output, c (inputs[11]) the attention's,
+// and the call is sdpa_back_unify above.  Masks are not differentiable here either (:262): a call with one is refused.
+int ccv_nnc_sm100_exec_sdpa_back(SM100_EXEC_ARGS)
+{
+	if (cmd.algorithm == CCV_NNC_SM100_SDPA_ALGO_FLASH_MASK) // a forward-only algorithm: the mask is not differentiable (:262)
+		return CCV_NNC_EXEC_NO_KERNEL;
+	if (input_size > 6 && inputs[6])
+		return CCV_NNC_EXEC_INVALID;
+	if (input_size > 7 && inputs[7])
+		return sdpa_back_unify(cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
+	if (input_size > 8 && inputs[8]) // a bias always requires a weight matrix (:27-28)
+		return CCV_NNC_EXEC_INVALID;
+	return sdpa_back_core(cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context, (size_t)-1);
 }
 // ---- layer norm / rms norm: statistics over the trailing axes (saved_mean dims [d0, .., 1, .., 1]) -----------------
 // norm/ccv_nnc_layer_norm_cpu_ref.c:16-190: inputs (x, [scale, bias]) -> outputs (y, [saved_mean, saved_inv_std])

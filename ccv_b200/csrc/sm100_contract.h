@@ -107,6 +107,10 @@ int sdpa_forward_f16(cudaStream_t s, const SdpaGeom& g, int is_bf16, const void*
 // o_*, of dout; dg the strides of dq / dk / dv in q_* / k_* / v_*.  out (strides oo_*) / lse = the forward's saved outputs, or NULL:
 // both are then recomputed into the workspace (sdpa_backward_f16_workspace_bytes(g, 1)).  Same return convention as the forward.
 size_t sdpa_backward_f16_workspace_bytes(const SdpaGeom& g, int need_forward);
+// The shape, stride and pointer tests of sdpa_backward_f16 (wide = 0) and sdpa_backward_f16_wide (wide = 1); ptrs are dq, dk, dv, dout, q,
+// k, v (and, for a caller that checks ahead, the saved output).  Those entry points decline what fails them; a call that passes is declined
+// only when a tensor map cannot be encoded, which these strides and pointers already rule out.
+bool sdpa_backward_f16_takes(const SdpaGeom& g, const SdpaGeom& dg, int wide, const void* const* ptrs, int ptr_count);
 int sdpa_backward_f16(cudaStream_t s, const SdpaGeom& g, const SdpaGeom& dg, int is_bf16, const void* dout, const void* q, const void* k, const void* v, const void* out, long long oo_b, long long oo_s, long long oo_h,
 	const float* lse, void* dq, void* dk, void* dv, void* workspace);
 
@@ -119,6 +123,12 @@ int backend_gemm_nt_bias(void* stream_context, int kind, int M, int N, int K, co
 // writes its decoded elements to out (device memory) and returns like depalettize.
 bool backend_qx_ok(const void* tensor, int dense);
 int backend_qx_decode(void* stream_context, const void* tensor, void* out);
+// GEMM_BACKWARD with transpose_b = (0, 1) at the GEMM command's default algorithm, for a command whose gradient ends in one (the attention's
+// unify-head projection): inputs (g, a, w) and outputs (h, dw, dbias) are three ccv_nnc_tensor_t* each, any of them NULL; flags as the
+// command's (CCV_NNC_ACCUMULATE_OUTPUT).  backend_gemm_back_workspace is the one workspace request the call makes for those operands, so a
+// caller that asks for more first keeps whatever it holds past that size.  Returns a CCV_NNC_EXEC_* status.
+size_t backend_gemm_back_workspace(void* const* inputs, void* const* outputs);
+int backend_gemm_back(void* stream_context, int flags, void* const* inputs, void* const* outputs);
 
 // palettized (CCV_QX) tensors (sm100_palettize.cu).  qbits 4..8; nib (elements per palette block) must make the block stride
 // nib * qbits / 8 a whole number of bytes.  palette_datatype is CCV_16F, CCV_32F or CCV_64F; out holds `count` decoded elements.

@@ -385,17 +385,26 @@ size_t sdpa_backward_f16_workspace_bytes(const SdpaGeom& g, int need_forward)
 // g: q / k / v strides, o_* = the strides of dout; dg: the strides of dq / dk / dv in its q_* / k_* / v_* fields.  `out` (strides oo_*)
 // and `lse` are the forward's saved outputs; when either is NULL both are recomputed into the workspace with the forward kernel.
 // returns 0 on success, 1 when the shape is outside these kernels (D = Dv <= 128 and a multiple of 8, 16-byte aligned strides), < 0 on CUDA errors
+bool sdpa_backward_f16_takes(const SdpaGeom& g, const SdpaGeom& dg, const int wide, const void* const* const ptrs, const int ptr_count)
+{
+	const bool d_ok = wide ? g.D > FB_D && g.D <= 256 : g.D >= 8 && g.D <= FB_D;
+	if (!d_ok || (g.D & 7) || g.Dv != g.D || g.B <= 0 || g.H <= 0 || g.Hk <= 0 || g.H % g.Hk != 0 || g.Sq <= 0 || g.Sk <= 0)
+		return false;
+	for (int i = 0; i < ptr_count; i++)
+		if (((uintptr_t)ptrs[i]) & 15)
+			return false;
+	for (const long long st : { g.q_b, g.q_s, g.q_h, g.k_b, g.k_s, g.k_h, g.v_b, g.v_s, g.v_h, dg.q_b, dg.q_s, dg.q_h, dg.k_b, dg.k_s, dg.k_h, dg.v_b, dg.v_s, dg.v_h, g.o_b, g.o_s, g.o_h })
+		if (st & 7)
+			return false;
+	return true;
+}
+
 int sdpa_backward_f16(cudaStream_t stream, const SdpaGeom& g, const SdpaGeom& dg, int is_bf16, const void* dout, const void* q, const void* k, const void* v, const void* out, long long oo_b, long long oo_s, long long oo_h,
 	const float* lse, void* dq, void* dk, void* dv, void* workspace)
 {
-	if (g.D > FB_D || g.D < 8 || (g.D & 7) || g.Dv != g.D || g.B <= 0 || g.H <= 0 || g.Hk <= 0 || g.H % g.Hk != 0 || g.Sq <= 0 || g.Sk <= 0 || !encode_init())
+	const void* const ptrs[7] = { dq, dk, dv, dout, q, k, v };
+	if (!sdpa_backward_f16_takes(g, dg, 0, ptrs, 7) || !encode_init())
 		return 1;
-	for (const void* ptr : { (const void*)dq, (const void*)dk, (const void*)dv, dout })
-		if (((uintptr_t)ptr) & 15)
-			return 1;
-	for (const long long st : { dg.q_b, dg.q_s, dg.q_h, dg.k_b, dg.k_s, dg.k_h, dg.v_b, dg.v_s, dg.v_h, g.o_b, g.o_s, g.o_h })
-		if (st & 7)
-			return 1;
 	CUtensorMap tmQr, tmQt, tmKr, tmKt, tmVr, tmVt, tmGr, tmGt;
 	if (!make_map_bshd(&tmQr, q, g.B, g.Sq, g.H, g.D, g.q_b, g.q_s, g.q_h, is_bf16, FB_R) || !make_map_bshd(&tmQt, q, g.B, g.Sq, g.H, g.D, g.q_b, g.q_s, g.q_h, is_bf16, FB_T) ||
 		!make_map_bshd(&tmKr, k, g.B, g.Sk, g.Hk, g.D, g.k_b, g.k_s, g.k_h, is_bf16, FB_R) || !make_map_bshd(&tmKt, k, g.B, g.Sk, g.Hk, g.D, g.k_b, g.k_s, g.k_h, is_bf16, FB_T) ||

@@ -715,14 +715,9 @@ int sdpa_forward_f16_wide(cudaStream_t stream, const SdpaGeom& g, int is_bf16, c
 int sdpa_backward_f16_wide(cudaStream_t stream, const SdpaGeom& g, const SdpaGeom& dg, int is_bf16, const void* dout, const void* q, const void* k, const void* v, const void* out, long long oo_b, long long oo_s, long long oo_h,
 	const float* lse, void* dq, void* dk, void* dv, void* workspace)
 {
-	if (!wide_shape(g))
+	const void* const ptrs[7] = { dq, dk, dv, dout, q, k, v };
+	if (!wide_shape(g) || !sdpa_backward_f16_takes(g, dg, 1, ptrs, 7))
 		return 1;
-	for (const void* ptr : { (const void*)dq, (const void*)dk, (const void*)dv, dout })
-		if (((uintptr_t)ptr) & 15)
-			return 1;
-	for (const long long st : { dg.q_b, dg.q_s, dg.q_h, dg.k_b, dg.k_s, dg.k_h, dg.v_b, dg.v_s, dg.v_h, g.o_b, g.o_s, g.o_h })
-		if (st & 7)
-			return 1;
 	CUtensorMap tmQ, tmK, tmV, tmG;
 	if (!make_map_bshd(&tmQ, q, g.B, g.Sq, g.H, g.D, g.q_b, g.q_s, g.q_h, is_bf16, FW_K) || !make_map_bshd(&tmK, k, g.B, g.Sk, g.Hk, g.D, g.k_b, g.k_s, g.k_h, is_bf16, FW_K) ||
 		!make_map_bshd(&tmV, v, g.B, g.Sk, g.Hk, g.Dv, g.v_b, g.v_s, g.v_h, is_bf16, FW_K) || !make_map_bshd(&tmG, dout, g.B, g.Sq, g.H, g.Dv, g.o_b, g.o_s, g.o_h, is_bf16, FW_K))

@@ -564,7 +564,9 @@ enum {
 	CCV_NNC_SM100_ALGO_COUNT = 3,
 };
 
-/* algorithm selectors of this backend for SCALED_DOT_PRODUCT_ATTENTION_FORWARD / _BACKWARD (cmd.algorithm; -1 = COMPOSED) */
+/* algorithm selectors of this backend for SCALED_DOT_PRODUCT_ATTENTION_FORWARD / _BACKWARD (cmd.algorithm; -1 = COMPOSED).  They pick
+ * the attention's kernels with or without the unify-head projection: its forward GEMM and, in the backward, the GEMM_BACKWARD that gives
+ * dweight, dbias and the attention's output gradient run the same whatever the algorithm. */
 enum {
 	CCV_NNC_SM100_SDPA_ALGO_COMPOSED = 0, /* 16-bit D <= 128: the flash kernels; every other call: the fp32 path (16-bit widened) */
 	CCV_NNC_SM100_SDPA_ALGO_FLASH = 1,    /* as COMPOSED, plus 16-bit 128 < D = Dv <= 256 without a mask on the wide flash kernels */
