@@ -540,8 +540,8 @@ int exec_masked_fill_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, co
 // the stream context's generator (ccv_nnc_stream_context_genrand_uint32) and fills the tensor from a counter-based Philox
 // 4x32-10 stream.  Same contract here: seed from the stream context, Philox 4x32-10 written out below (Salmon et al., SC'11:
 // public algorithm) with the element-quad index as the counter, so a fill is reproducible for a given seed and independent of
-// the launch shape.  What parameter initialisation (lib/nnc/ccv_cnnp_model_addons.c:996,1158) needs is the distribution, which the
-// tests check; the reference's own sample sequence (cuRAND's counter layout) is not part of its API.
+// the launch shape.  The tests restate the stream and hold the uniform to its bits, the normal to a per-element bound; the
+// reference's own sample sequence (cuRAND's counter layout) is not part of its API.
 __device__ __forceinline__ void philox_round(uint32_t (&c)[4], const uint32_t k0, const uint32_t k1)
 {
 	const uint32_t hi0 = __umulhi(0xD2511F53u, c[0]), lo0 = 0xD2511F53u * c[0];
@@ -587,7 +587,7 @@ __global__ void __launch_bounds__(256) random_kernel(T* __restrict__ a, const si
 			for (int j = 0; j < 4; j++)
 			{
 				const float u = u01(r[j]);
-				v[j] = u * p1 + (1.f - u) * p0;
+				v[j] = __fadd_rn(__fmul_rn(u, p1), __fmul_rn(1.f - u, p0)); // each product and the sum rounded on its own: no FMA
 			}
 		}
 #pragma unroll
@@ -625,9 +625,9 @@ int exec_random(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int fl
 // dropout/ccv_nnc_dropout_cpu_ref.c:16-215: b = mask ? 0 : a / (1 - p), mask[i] = (u_i <= p) as one byte per element in the reserved
 // second output (dropout/ccv_nnc_dropout.c:21-44 sizes it in 128-byte lines, never below one byte per element); `entirety` = one
 // decision for the whole tensor, kept as an int32 in mask[0].  Backward (g, -, -, -, mask): h = mask ? 0 : g / (1 - p).  The
-// uniforms are the Philox stream of the random-fill commands above, keyed by the stream context's seed: as for those, the contract
-// is the distribution and the forward / backward consistency of the mask (SURVEY.md 8f-4: there is no bit-level parity to define
-// against the reference's dSFMT / cuDNN generator states).
+// uniforms are the Philox stream of the random-fill commands above, keyed by the stream context's seed (the reference's dSFMT / cuDNN
+// generator states are not part of its API).  Given the mask, b and h are CPU_REF's arithmetic bit for bit: 1 / (1 - p) is taken in
+// double and rounded once, as CPU_REF does.
 template <typename T>
 __global__ void __launch_bounds__(256) dropout_fwd_kernel(const T* __restrict__ a, T* __restrict__ b, uint8_t* __restrict__ mask, const size_t n, const uint32_t seed, const float p, const float inv_p, const int entirety)
 {
@@ -684,7 +684,7 @@ int exec_dropout_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const 
 		return CCV_NNC_EXEC_INVALID;
 	if (n == 0)
 		return CCV_NNC_EXEC_SUCCESS;
-	const float p = cmd.info.dropout.p, inv_p = 1.f / (1.f - p);
+	const float p = cmd.info.dropout.p, inv_p = 1. / (1. - p); // in double, rounded once (dropout/ccv_nnc_dropout_cpu_ref.c:20)
 	const uint32_t seed = ccv_nnc_stream_context_genrand_uint32(stream_context);
 	cudaStream_t s = stream_of(stream_context);
 	const int grid = grid_for(entirety ? n : (n + 3) / 4, 256);
@@ -709,7 +709,7 @@ int exec_dropout_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const 
 		return CCV_NNC_EXEC_INVALID;
 	if (n == 0)
 		return CCV_NNC_EXEC_SUCCESS;
-	const float inv_p = 1.f / (1.f - cmd.info.dropout.p);
+	const float inv_p = 1. / (1. - cmd.info.dropout.p); // in double, rounded once (dropout/ccv_nnc_dropout_cpu_ref.c:153)
 	cudaStream_t s = stream_of(stream_context);
 	const int grid = grid_for(n, 256);
 	const uint8_t* const mask = inputs[4]->data.u8;

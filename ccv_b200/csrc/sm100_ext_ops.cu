@@ -300,28 +300,34 @@ int exec_index_select_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, c
 }
 
 // ------------------------------------------------------------------------------------------------ AdamW
-// inputs (g, a, m, v, [vm]) -> outputs (b, n, u, [um]); g fp32 / bf16 / fp16, everything else fp32; contiguous
+// inputs (g, a, m, v, [vm]) -> outputs (b, n, u, [um]); g fp32 / bf16 / fp16, everything else fp32; contiguous.  Every product and
+// sum is rounded on its own, in CPU_REF's association (adam/ccv_nnc_adam{,w}_cpu_ref.c), so b, n, u and um equal CPU_REF's bit for
+// bit; the amsgrad maximum is CPU_REF's ccv_max(vm, v_hat) = vm > v_hat ? vm : v_hat, which keeps a NaN v_hat.  No operand is
+// __restrict__: models call the command in place (b = a, n = m, u = v, um = vm).
 template <int L2>
-__global__ void __launch_bounds__(256) adamw_kernel(const void* __restrict__ g, const int g_kind, const float* __restrict__ a, const float* __restrict__ m, const float* __restrict__ v, const float* __restrict__ vm,
-	float* __restrict__ b, float* __restrict__ n, float* __restrict__ u, float* __restrict__ um, const size_t count, const float scale, const float beta1, const float beta2, const float rate_inv_bias_correction1,
+__global__ void __launch_bounds__(256) adamw_kernel(const void* g, const int g_kind, const float* a, const float* m, const float* v, const float* vm,
+	float* b, float* n, float* u, float* um, const size_t count, const float scale, const float beta1, const float beta2, const float rate_inv_bias_correction1,
 	const float inv_bias_correction2, const float rate_decay, const float epsilon)
 {
 	for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < count; i += (size_t)gridDim.x * blockDim.x)
 	{
-		float grad = scale * ld_kind(g, i, g_kind);
+		const float av = a[i];
+		float grad = __fmul_rn(scale, ld_kind(g, i, g_kind));
 		if (L2)
-			grad += rate_decay * a[i]; // ADAM: the decay is an L2 term of the gradient (adam/ccv_nnc_adam_cpu_ref.c:117-118); rate_decay carries `decay` itself
-		const float mom = beta1 * m[i] + (1.f - beta1) * grad;
-		const float vel = beta2 * v[i] + (1.f - beta2) * grad * grad;
-		n[i] = mom, u[i] = vel;
-		float vel_hat = vel * inv_bias_correction2;
+			grad = __fadd_rn(grad, __fmul_rn(rate_decay, av)); // ADAM: the decay is an L2 term of the gradient (adam/ccv_nnc_adam_cpu_ref.c:117-118); rate_decay carries `decay` itself
+		const float mom = __fadd_rn(__fmul_rn(beta1, m[i]), __fmul_rn(1.f - beta1, grad));
+		const float vel = __fadd_rn(__fmul_rn(beta2, v[i]), __fmul_rn(__fmul_rn(1.f - beta2, grad), grad));
+		float vel_hat = __fmul_rn(vel, inv_bias_correction2);
 		if (vm)
 		{
-			vel_hat = fmaxf(vm[i], vel_hat);
-			um[i] = vel_hat;
+			const float vmax = vm[i];
+			vel_hat = vmax > vel_hat ? vmax : vel_hat;
 		}
-		const float av = a[i];
-		b[i] = (L2 ? av : av - rate_decay * av) - (mom * rate_inv_bias_correction1) / (sqrtf(vel_hat) + epsilon);
+		n[i] = mom, u[i] = vel;
+		if (vm)
+			um[i] = vel_hat;
+		const float q = __fdiv_rn(__fmul_rn(mom, rate_inv_bias_correction1), __fadd_rn(__fsqrt_rn(vel_hat), epsilon));
+		b[i] = __fsub_rn(L2 ? av : __fsub_rn(av, __fmul_rn(rate_decay, av)), q);
 	}
 }
 template <int L2>
@@ -354,7 +360,7 @@ int exec_adam_f32(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int 
 		return CCV_NNC_EXEC_SUCCESS;
 	const float rate = cmd.info.adam.rate, beta1 = cmd.info.adam.beta1, beta2 = cmd.info.adam.beta2;
 	const float rate_inv_bias_correction1 = rate / (1 - powf(beta1, cmd.info.adam.step));
-	const float inv_bias_correction2 = 1.f / (1 - powf(beta2, cmd.info.adam.step));
+	const float inv_bias_correction2 = 1. / (1 - powf(beta2, cmd.info.adam.step)); // the quotient in double, rounded once, as CPU_REF
 	adamw_kernel<L2><<<grid_for(count, 256), 256, 0, stream_of(stream_context)>>>(inputs[0]->data.u8, g_kind, inputs[1]->data.f32, inputs[2]->data.f32, inputs[3]->data.f32, ams ? vm->data.f32 : 0,
 		outputs[0]->data.f32, outputs[1]->data.f32, outputs[2]->data.f32, ams ? um->data.f32 : 0, count, cmd.info.adam.scale, beta1, beta2, rate_inv_bias_correction1, inv_bias_correction2, L2 ? cmd.info.adam.decay : rate * cmd.info.adam.decay, cmd.info.adam.epsilon);
 	return check("adamw") ? CCV_NNC_EXEC_INVALID : CCV_NNC_EXEC_SUCCESS;

@@ -178,29 +178,3 @@ def test_random_uniform_and_normal(gpu, n):
     # bf16 tensors
     st, (ub,) = gpu_exec16(nnc, nnc.CMD_RANDOM_UNIFORM_FORWARD(0.0, 1.0), None, 0, [], [np.zeros((n,), np.float32)], abi.CCV_16BF)
     assert st == 0 and ub.min() >= 0.0 and ub.max() <= 1.0 and abs(ub.mean() - 0.5) <= 0.02
-
-
-@pytest.mark.xfail(strict=False, reason="DROPOUT was added after the builder's GPU budget was spent: first hardware run is the driver's")
-@pytest.mark.parametrize("entirety", [0, 1])
-def test_dropout_forward_backward(gpu, entirety):
-    """DROPOUT (dropout/ccv_nnc_dropout_cpu_ref.c:16-215): b = mask ? 0 : a / (1 - p) with a byte mask in the reserved second output
-    (dropout/ccv_nnc_dropout.c:21-44), backward h = mask ? 0 : g / (1 - p) with the same mask.  The random stream is this backend's
-    (Philox keyed by the stream context's seed), so what is checked is what the reference's own tests check: the drop rate and the
-    consistency of output, mask and gradient (test/int/nnc/cudnn.tests.c:3389-3464)."""
-    nnc = gpu
-    n, p = 20 * 50 * 100, 0.2
-    a, g = seeded((20, 50, 100), 1, 0.5, 1.5), seeded((20, 50, 100), 2, 0.5, 1.5)
-    mask_shape = (32, ((20 + 127) // 128) * 50 * 100) if not entirety else (1,)   # the reference's tensor_auto: 128-byte lines
-    st, (b, mask) = gpu_exec(nnc, nnc.CMD_DROPOUT_FORWARD(p, entirety), None, 0, [a], [np.zeros_like(a), np.zeros(mask_shape, np.float32)])
-    assert st == 0
-    if entirety:
-        dropped = bool(mask.view(np.int32)[0])
-        assert np.array_equal(b, np.zeros_like(a)) if dropped else np.allclose(b, a / (1 - p), rtol=1e-6)
-        m = np.full(a.shape, dropped)
-    else:
-        m = mask.view(np.uint8).reshape(-1)[:n].reshape(a.shape).astype(bool)
-        assert abs(m.mean() - p) < 0.01
-        assert np.array_equal(b == 0, m) and np.allclose(b[~m], (a / (1 - p))[~m], rtol=1e-6)
-    st, (h,) = gpu_exec(nnc, nnc.CMD_DROPOUT_BACKWARD(p, entirety), None, 0, [g, None, None, None, mask], [np.zeros_like(g)])
-    assert st == 0
-    assert np.array_equal(h == 0, m) and np.allclose(h[~m], (g / (1 - p))[~m], rtol=1e-6)
