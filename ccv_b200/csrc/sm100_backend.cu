@@ -5,8 +5,7 @@
 // REGISTER_COMMAND_BACKEND(cmd, CCV_NNC_BACKEND_GPU_SM100) would (lib/nnc/ccv_nnc_internal.h:196-202).  An exec only
 // validates shapes, pulls the CUDA stream / workspace from the stream context and enqueues kernels; it never
 // synchronises and there is no CPU path: anything it cannot run returns CCV_NNC_EXEC_INVALID.
-#include "../../include/ccv_nnc_sm100.h"
-#include "sm100_contract.h"
+#include "sm100_cmd.h"
 #include "sm100_ew.h"
 #include <cuda_runtime.h>
 #include <string.h>
@@ -28,22 +27,13 @@ struct TV {
 	size_t count;
 };
 
-int tensor_nd(const int* const dim)
-{
-	int i;
-	for (i = 0; i < CCV_NNC_MAX_DIM_ALLOC; i++)
-		if (dim[i] == 0)
-			return i;
-	return CCV_NNC_MAX_DIM_ALLOC;
-}
-
 // ccv_nnc_tensor_view_get_stride (lib/nnc/ccv_nnc_easy.h): a view carries its strides, a plain tensor is packed
 TV view_of(const ccv_nnc_tensor_t* const t)
 {
 	TV v;
 	memset(&v, 0, sizeof(v));
 	v.p = t->data.u8;
-	v.nd = tensor_nd(t->info.dim);
+	v.nd = nd_of(t);
 	v.datatype = CCV_GET_DATA_TYPE(t->info.datatype);
 	v.format = t->info.format;
 	v.count = 1;
@@ -85,11 +75,6 @@ void dims4(const TV& v, int dim[4], int stride[4])
 	}
 }
 
-inline cudaStream_t stream_of(ccv_nnc_stream_context_t* const stream_context)
-{
-	return (cudaStream_t)ccv_nnc_stream_context_get_stream(stream_context);
-}
-
 // split-K scratch of a command that no staging layer wraps: the stream workspace (grow-only, one buffer per stream:
 // lib/nnc/gpu/ccv_nnc_compat.cu:438-471).  The wrapped commands carve it out of their one workspace request (scratch_at).
 inline Scratch scratch_of(ccv_nnc_stream_context_t* const stream_context)
@@ -105,18 +90,6 @@ inline Scratch scratch_at(void* const p, const size_t bytes)
 }
 
 inline bool is_f32(const ccv_nnc_tensor_t* const t) { return CCV_GET_DATA_TYPE(t->info.datatype) == CCV_32F; }
-// element kind of the kernels that exist for three floating-point types: 0 = fp32, 1 = bf16, 2 = fp16; -1 otherwise
-inline int kind_of(const ccv_nnc_tensor_t* const t)
-{
-	switch (CCV_GET_DATA_TYPE(t->info.datatype))
-	{
-		case CCV_32F: return 0;
-		case CCV_16BF: return 1;
-		case CCV_16F: return 2;
-	}
-	return -1;
-}
-inline size_t kind_size(const int kind) { return kind == 0 ? 4 : 2; }
 inline uint16_t f32_to_16(const float v, const int kind); // host-side rounding of a fill value (defined with exec_via_f32)
 
 bool same_shape(const TV& a, const TV& b)
@@ -429,7 +402,7 @@ struct Slice4 {
 };
 inline void slice4_make(ccv_nnc_tensor_t* const t, Slice4& sl)
 {
-	sl.is4 = t && tensor_nd(t->info.dim) == 4;
+	sl.is4 = t && nd_of(t) == 4;
 	if (!sl.is4)
 		return;
 	const TV tv = view_of(t);
@@ -453,10 +426,10 @@ int exec_gemm_nd4(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int 
 	enum { MAXT = 4 };
 	int outer = 0;
 	for (int i = 0; i < input_size; i++)
-		if (inputs[i] && tensor_nd(inputs[i]->info.dim) == 4)
+		if (inputs[i] && nd_of(inputs[i]) == 4)
 			outer = std::max(outer, inputs[i]->info.dim[0]);
 	for (int i = 0; i < output_size; i++)
-		if (outputs[i] && tensor_nd(outputs[i]->info.dim) == 4)
+		if (outputs[i] && nd_of(outputs[i]) == 4)
 			outer = std::max(outer, outputs[i]->info.dim[0]);
 	if (outer == 0)
 		return F(cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
@@ -583,7 +556,7 @@ struct GroupPlan {
 bool group_plan(const ConvGeom& g, const int kind, const int groups, const int pass, GroupPlan& p)
 {
 	const int align = kind == 0 ? 4 : 8;
-	const size_t es = kind_size(kind);
+	const size_t es = elem_size(kind);
 	if (groups <= 1 || g.C % groups || g.K % groups)
 		return false;
 	const int Cg = g.C / groups, Kg = g.K / groups;
@@ -613,7 +586,7 @@ int conv_grouped_tc(cudaStream_t s, unsigned char* const ws, const int kind, con
 		return 1;
 	const ConvGeom& gg = p.gg;
 	const int Cg = gg.C, Kg = gg.K;
-	const size_t es = kind_size(kind);
+	const size_t es = elem_size(kind);
 	const Scratch scratch = scratch_at(ws, CONTRACT_SCRATCH_BYTES);
 	unsigned char* const xg = ws + p.inner;
 	unsigned char* const yg = xg + p.xb;
@@ -799,7 +772,7 @@ int conv_forw_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 			rc = conv_grouped_tc<0>(s, ws, kind, g, groups, x3, 0, a, w, bias32, bias16, 0, b);
 		else {
 			rc = conv_fprop_any(s, kind, g, a, w, bias32, bias16, b, scratch_at(ws, CONTRACT_SCRATCH_BYTES), x3);
-			if (rc > 0 && g.C % (16 / kind_size(kind)) != 0) // TMA cannot address pixels of other sizes (the 3-channel stem): explicit im2col + tensor-core GEMM
+			if (rc > 0 && g.C % (16 / elem_size(kind)) != 0) // TMA cannot address pixels of other sizes (the 3-channel stem): explicit im2col + tensor-core GEMM
 				rc = conv_fprop_im2col_any(s, kind, g, a, w, bias32, bias16, b, ws, x3);
 		}
 	}
@@ -862,7 +835,7 @@ int conv_back_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 				rc = conv_grouped_tc<1>(s, ws, kind, g, groups, x3, accumulate, a, 0, 0, 0, gb, dw_t->data.u8);
 			else {
 				rc = conv_wgrad_any(s, kind, g, gb, a, dw_t->data.u8, accumulate, scratch_at(ws, CONTRACT_SCRATCH_BYTES), x3);
-				if (rc > 0 && g.C % (16 / kind_size(kind)) != 0)
+				if (rc > 0 && g.C % (16 / elem_size(kind)) != 0)
 					rc = conv_wgrad_im2col_any(s, kind, g, gb, a, dw_t->data.u8, accumulate, ws, x3);
 			}
 		}
@@ -895,7 +868,7 @@ int conv_back_nhwc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 // workspace function is inner(shadows) + staging.
 enum { STAGE_NCHW, STAGE_F32, STAGE_QX };
 
-inline bool is_nchw(const ccv_nnc_tensor_t* const t) { return t && t->info.format == CCV_TENSOR_FORMAT_NCHW && tensor_nd(t->info.dim) >= 3; }
+inline bool is_nchw(const ccv_nnc_tensor_t* const t) { return t && t->info.format == CCV_TENSOR_FORMAT_NCHW && nd_of(t) >= 3; }
 inline bool is_qx(const ccv_nnc_tensor_t* const t) { return t && CCV_GET_DATA_TYPE(t->info.datatype) == CCV_QX; }
 inline int qx_palette(const ccv_nnc_tensor_t* const t) { return (t->info.datatype & 0xff) << 12; }
 inline int qx_bits(const ccv_nnc_tensor_t* const t) { return (t->info.datatype >> 8) & 0xf; }
@@ -1538,7 +1511,7 @@ int exec_ewsum_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const in
 			const TV g = view_of(inputs[0]);
 			if (!g.contiguous || g.count != h.count || kind_of(inputs[0]) != kind)
 				return CCV_NNC_EXEC_INVALID;
-			if (cudaMemcpyAsync(outputs[i]->data.u8, inputs[0]->data.u8, h.count * kind_size(kind), cudaMemcpyDeviceToDevice, s) != cudaSuccess)
+			if (cudaMemcpyAsync(outputs[i]->data.u8, inputs[0]->data.u8, h.count * elem_size(kind), cudaMemcpyDeviceToDevice, s) != cudaSuccess)
 				return CCV_NNC_EXEC_INVALID;
 		}
 	}
@@ -1576,7 +1549,7 @@ int exec_ewprod_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const i
 	cudaStream_t s = stream_of(stream_context);
 	if (input_size == 1)
 	{
-		if (ptrs[0] != outputs[0]->data.u8 && c.count && cudaMemcpyAsync(outputs[0]->data.u8, ptrs[0], c.count * kind_size(kind), cudaMemcpyDeviceToDevice, s) != cudaSuccess)
+		if (ptrs[0] != outputs[0]->data.u8 && c.count && cudaMemcpyAsync(outputs[0]->data.u8, ptrs[0], c.count * elem_size(kind), cudaMemcpyDeviceToDevice, s) != cudaSuccess)
 			return CCV_NNC_EXEC_INVALID;
 		return CCV_NNC_EXEC_SUCCESS;
 	}
@@ -2126,11 +2099,6 @@ int exec_sgd_multi(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 	return CCV_NNC_EXEC_SUCCESS;
 }
 
-int exec_invalid(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
-{
-	return CCV_NNC_EXEC_INVALID; // e.g. SGD backward (sgd/ccv_nnc_sgd_cpu_ref.c:128-131)
-}
-
 // ================================================================================================ SET / MOVES
 // util/ccv_nnc_util_cpu_ref.c:637-664
 int exec_set_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
@@ -2475,19 +2443,6 @@ int exec_data_transfer_any(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, c
 	return CCV_NNC_EXEC_SUCCESS;
 }
 
-void fill(ccv_nnc_cmd_backend_registry_t* const registry, const int formats, const int datatypes, const int algorithms, const ccv_nnc_cmd_exec_f exec)
-{
-	registry->tensor_formats = formats;
-	registry->tensor_datatypes = datatypes;
-	registry->tensor_memory = CCV_TENSOR_GPU_MEMORY;
-	registry->algorithms = algorithms;
-	registry->exec = exec;
-	registry->autotune = 0;
-	registry->aux = 0;
-}
-
-const int ALL_FORMATS = CCV_TENSOR_FORMAT_NCHW | CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_CHWN;
-
 // registry->autotune of the contraction commands (lib/nnc/ccv_nnc.h:323; called by ccv_nnc_cmd_autotune, ccv_nnc_cmd.c:519-531, on
 // scratch copies of the operands): every algorithm of this backend that accepts the shapes is timed on the device (CUDA
 // events on the caller's stream, best of 3 after a warm-up) and the index of the fastest one is returned.  The generic
@@ -2693,8 +2648,6 @@ int exec_via_f32_rt(ccv_nnc_cmd_exec_f f32, const ccv_nnc_cmd_t cmd, const ccv_n
 	return staged(STAGE_F32, 0, f32, no_workspace, cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
 }
 }
-
-#define REGISTER_SM100(cmd) extern "C" void _register_command_ ## cmd ## _backend_CCV_NNC_BACKEND_GPU_SM100(ccv_nnc_cmd_backend_registry_t* const registry)
 
 REGISTER_SM100(CCV_NNC_GEMM_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_gemm_forw_any); registry->autotune = autotune_algorithms<exec_gemm_forw_any, CCV_NNC_SM100_ALGO_COUNT>; }
 REGISTER_SM100(CCV_NNC_GEMM_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF | CCV_QX, CCV_NNC_SM100_ALGO_COUNT, exec_gemm_back_any); registry->autotune = autotune_algorithms<exec_gemm_back_any, CCV_NNC_SM100_ALGO_COUNT>; }

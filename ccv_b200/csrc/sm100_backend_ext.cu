@@ -1,6 +1,5 @@
 // sm100_backend_ext.cu -- command layer for attention, layer / rms norm, upsample and the gradient allreduce.
-#include "../../include/ccv_nnc_sm100.h"
-#include "sm100_contract.h"
+#include "sm100_cmd.h"
 #include "sm100_ew.h"
 #include <cuda_runtime.h>
 #include <string.h>
@@ -10,43 +9,9 @@ using namespace sm100;
 
 namespace {
 
-inline cudaStream_t stream_of(ccv_nnc_stream_context_t* const stream_context) { return (cudaStream_t)ccv_nnc_stream_context_get_stream(stream_context); }
-
-int nd_of(const ccv_nnc_tensor_t* const t)
-{
-	int i;
-	for (i = 0; i < CCV_NNC_MAX_DIM_ALLOC; i++)
-		if (t->info.dim[i] == 0)
-			return i;
-	return CCV_NNC_MAX_DIM_ALLOC;
-}
-
-size_t count_of(const ccv_nnc_tensor_t* const t)
-{
-	size_t c = 1;
-	for (int i = 0; i < nd_of(t); i++)
-		c *= (size_t)t->info.dim[i];
-	return c;
-}
-
 bool packed_f32(const ccv_nnc_tensor_t* const t)
 {
 	return CCV_GET_DATA_TYPE(t->info.datatype) == CCV_32F && CCV_IS_TENSOR_CONTIGUOUS(t);
-}
-
-// element kind of an fp32 / bf16 / fp16 tensor (ElemKind: 0, 1, 2); -1 for every other type, palettized ones included
-int kind_of(const ccv_nnc_tensor_t* const t)
-{
-	switch (CCV_GET_DATA_TYPE(t->info.datatype))
-	{
-		case CCV_32F:
-			return 0;
-		case CCV_16BF:
-			return 1;
-		case CCV_16F:
-			return 2;
-	}
-	return -1;
 }
 
 // The normalisations' datatype rule.  The activations (x and y; g, x and h) share one kind kx: fp32, bf16 or fp16.  Each parameter

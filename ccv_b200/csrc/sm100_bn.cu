@@ -8,51 +8,17 @@
 //
 // Workspace (bn_workspace_bytes): double s[2C] (cross-block sums) followed by float coef[4C] (per-channel a, b, p, q).
 #include "sm100_ew.h"
-#include "sm100_contract.h"
+#include "sm100_cmd.h"
 #include "sm100_elem.cuh"
 
 namespace sm100 {
 
-static int g_sms_bn = 0;
-static int sms()
-{
-	if (!g_sms_bn)
-	{
-		int dev = 0;
-		cudaGetDevice(&dev);
-		cudaDeviceGetAttribute(&g_sms_bn, cudaDevAttrMultiProcessorCount, dev);
-		if (g_sms_bn <= 0)
-			g_sms_bn = 132;
-	}
-	return g_sms_bn;
-}
-static int check(const char* what)
-{
-	count_launch();
-	const cudaError_t e = cudaGetLastError();
-	if (e != cudaSuccess)
-	{
-		set_last_error(what, e);
-		return -1;
-	}
-	return 0;
-}
-static int grid_for(size_t work_items, int threads, int max_waves = 8)
-{
-	size_t blocks = (work_items + threads - 1) / threads;
-	const size_t cap = (size_t)sms() * max_waves;
-	if (blocks > cap)
-		blocks = cap;
-	return blocks < 1 ? 1 : (int)blocks;
-}
-
 // workspace: double s[2C] (reduced sums), float coef[4C] (per-channel a, b, p, q), float part[gy_max][2C] (per-block partial sums)
-static inline size_t bn_part_rows() { return (size_t)sms() * 4 + 8; }
+static inline size_t bn_part_rows() { return (size_t)sm_count() * 4 + 8; }
 size_t bn_workspace_bytes(int C) { return (size_t)C * (2 * sizeof(double) + 4 * sizeof(float)) + bn_part_rows() * 2 * (size_t)C * sizeof(float) + 256; }
 static inline double* ws_sums(void* ws) { return (double*)ws; }
 static inline float* ws_coef(void* ws, int C) { return (float*)((double*)ws + 2 * (size_t)C); }
 static inline float* ws_part(void* ws, int C) { return (float*)(((uintptr_t)(ws_coef(ws, C) + 4 * (size_t)C) + 255) & ~(uintptr_t)255); }
-
 
 // ------------------------------------------------------------------------------------------------ reductions
 // NHWC: thread = (column-vector tx, row-lane ty); each thread walks rows with 4 independent 128-bit loads in flight.
@@ -631,7 +597,7 @@ static void reduce_config(size_t rows, int CV, int& cpb, dim3& grid)
 	const int rpi = 256 / cpb;
 	const int gx = (CV + cpb - 1) / cpb;
 	size_t gy = (rows + (size_t)rpi * 32 - 1) / ((size_t)rpi * 32);
-	const size_t cap = (size_t)(sms() * 4 + gx - 1) / gx;
+	const size_t cap = (size_t)(sm_count() * 4 + gx - 1) / gx;
 	if (gy > cap)
 		gy = cap;
 	if (gy < 1)
@@ -652,11 +618,11 @@ static int run_reduce(cudaStream_t s, const T* x, const T* g, const float* mean,
 		reduce_config(outer, C / W, cpb, grid);
 		bn_reduce_kernel<T, MODE, MASK><<<grid, 256, 0, s>>>(x, g, mean, coef, outer, C, part, cpb);
 		*part_rows = (int)grid.y;
-		return check("bn_reduce");
+		return launched("bn_reduce");
 	}
 	*part_rows = 0;
 	bn_reduce_generic_kernel<T, MODE, MASK><<<C, 512, 0, s>>>(x, g, mean, coef, outer, C, inner, ws);
-	return check("bn_reduce");
+	return launched("bn_reduce");
 }
 
 // colsum_out / colsum_kind: per-channel sums of the values written (backward only), stored in element kind colsum_kind
@@ -669,42 +635,42 @@ static int run_apply(cudaStream_t s, const T* x, const T* g, T* out, const float
 	if (inner == 1 && C % W == 0 && (256 % CW == 0 || CW % 256 == 0) && aligned_v16(x) && aligned_v16(out) && ((!BWD && RELU != 2) || aligned_v16(g)))
 	{
 		// channel-stationary threads: the grid stride is a multiple of the channel groups per pixel
-		int grid = grid_for(total / W / 4, 256);
+		int grid = grid_for(total / W / 4, 256, 8);
 		if (CW > 256)
 			grid = (grid + CW / 256 - 1) / (CW / 256) * (CW / 256);
 		if (BWD && part && colsum_out)
 		{
 			bn_apply_fixed_kernel<T, BWD, RELU, 1><<<grid, 256, 0, s>>>(x, g, out, coef, total / W, C, part);
-			if (check("bn_apply"))
+			if (launched("bn_apply"))
 				return -1;
 			const int rows = CW < 256 ? grid : (int)((size_t)grid * 256 / CW);
 			bn_colsum_rows_kernel<<<(C + 31) / 32, 1024, 0, s>>>(part, rows, C, colsum_out, colsum_kind);
 			*colsum_done = 1;
-			return check("bn_colsum_rows");
+			return launched("bn_colsum_rows");
 		}
 		bn_apply_fixed_kernel<T, BWD, RELU, 0><<<grid, 256, 0, s>>>(x, g, out, coef, total / W, C, 0);
-		return check("bn_apply");
+		return launched("bn_apply");
 	}
 	if (inner == 1 && C % 4 == 0 && aligned_v4(x) && aligned_v4(out) && ((!BWD && RELU != 2) || aligned_v4(g)))
 	{
-		int grid = grid_for(total / 8, 256);
+		int grid = grid_for(total / 8, 256, 8);
 		const int CV = C / 4;
 		if (BWD && part && colsum_out && (256 % CV == 0 || CV % 256 == 0))
 		{
 			if (CV > 256) // the grid stride must be a multiple of CV
 				grid = (grid + CV / 256 - 1) / (CV / 256) * (CV / 256);
 			bn_apply_vec_kernel<T, BWD, RELU, 1><<<grid, 256, 0, s>>>(x, g, out, coef, total / 4, C, part);
-			if (check("bn_apply"))
+			if (launched("bn_apply"))
 				return -1;
 			const int rows = CV < 256 ? grid : (int)((size_t)grid * 256 / CV);
 			bn_colsum_rows_kernel<<<(C + 31) / 32, 1024, 0, s>>>(part, rows, C, colsum_out, colsum_kind);
 			*colsum_done = 1;
-			return check("bn_colsum_rows");
+			return launched("bn_colsum_rows");
 		}
 		bn_apply_vec_kernel<T, BWD, RELU, 0><<<grid, 256, 0, s>>>(x, g, out, coef, total / 4, C, 0);
 	} else
-		bn_apply_generic_kernel<T, BWD, RELU><<<grid_for(total, 256), 256, 0, s>>>(x, g, out, coef, total, C, inner);
-	return check("bn_apply");
+		bn_apply_generic_kernel<T, BWD, RELU><<<grid_for(total, 256, 8), 256, 0, s>>>(x, g, out, coef, total, C, inner);
+	return launched("bn_apply");
 }
 
 template <typename T>
@@ -723,7 +689,7 @@ static int bn_fwd_train_t(cudaStream_t s, const T* x, T* y, const float* scale, 
 	{
 		// the producing convolution already folded its output into per-(CTA, warp quarter) shifted sums (four planes of ext_rows x C)
 		bn_finalize_ext_kernel<<<(C + 31) / 32, 1024, 0, s>>>(ext_part, ext_rows, C, epsilon, momentum, scale, bias, running_mean, running_var, saved_mean, saved_inv_std, coef);
-		if (check("bn_fwd_finalize(ext)"))
+		if (launched("bn_fwd_finalize(ext)"))
 			return -1;
 		return apply(coef);
 	}
@@ -733,7 +699,7 @@ static int bn_fwd_train_t(cudaStream_t s, const T* x, T* y, const float* scale, 
 		bn_finalize_partials_kernel<T, 0, 0><<<(C + 31) / 32, 1024, 0, s>>>(ws_part(workspace, C), part_rows, x, C, (double)outer * (double)inner, epsilon, momentum, scale, bias, running_mean, running_var, saved_mean, saved_inv_std, 0, 0, coef);
 	else
 		bn_fwd_finalize_kernel<T><<<(C + 127) / 128, 128, 0, s>>>(x, inner, ws, C, (double)outer * (double)inner, epsilon, momentum, scale, bias, running_mean, running_var, saved_mean, saved_inv_std, coef);
-	if (check("bn_fwd_finalize"))
+	if (launched("bn_fwd_finalize"))
 		return -1;
 	return apply(coef);
 }
@@ -745,7 +711,7 @@ static int bn_fwd_test_t(cudaStream_t s, const T* x, T* y, const float* scale, c
 		return 0;
 	float* coef = ws_coef(workspace, C);
 	bn_test_coef_kernel<<<(C + 127) / 128, 128, 0, s>>>(C, epsilon, scale, bias, mean, var, coef);
-	if (check("bn_test_coef"))
+	if (launched("bn_test_coef"))
 		return -1;
 	return run_apply<T, 0, 0>(s, x, (const T*)0, y, coef, outer, C, inner);
 }
@@ -763,12 +729,12 @@ static int bn_bwd_t(cudaStream_t s, const T* g, const T* x, const float* scale, 
 	if (mask)
 	{
 		bn_mask_coef_kernel<<<(C + 127) / 128, 128, 0, s>>>(C, scale, bias, saved_mean, saved_inv_std, coef);
-		if (check("bn_mask_coef"))
+		if (launched("bn_mask_coef"))
 			return -1;
 	} else if (!vec) {
 		// a is still needed by the apply pass (the vector path gets it from bn_finalize_partials_kernel<1, 1>)
 		bn_mask_coef_kernel<<<(C + 127) / 128, 128, 0, s>>>(C, scale, scale, saved_mean, saved_inv_std, coef);
-		if (check("bn_coef"))
+		if (launched("bn_coef"))
 			return -1;
 	}
 	int part_rows = 0;
@@ -781,7 +747,7 @@ static int bn_bwd_t(cudaStream_t s, const T* g, const T* x, const float* scale, 
 		bn_finalize_partials_kernel<T, 1, 1><<<(C + 31) / 32, 1024, 0, s>>>(ws_part(workspace, C), part_rows, (const T*)0, C, count, 0.f, 0.f, scale, 0, 0, 0, const_cast<float*>(saved_mean), const_cast<float*>(saved_inv_std), dscale, dbias, coef);
 	else
 		bn_bwd_finalize_kernel<<<(C + 127) / 128, 128, 0, s>>>(ws, C, (float)count, scale, saved_mean, saved_inv_std, dscale, dbias, coef);
-	if (check("bn_bwd_finalize"))
+	if (launched("bn_bwd_finalize"))
 		return -1;
 	if (!dx)
 		return 0;
@@ -865,8 +831,8 @@ static int add_relu_fwd_t(cudaStream_t s, const T* a, const T* b, T* out, size_t
 	if (n == 0)
 		return 0;
 	const int vec = aligned_v16(a) && aligned_v16(b) && aligned_v16(out);
-	add_relu_kernel<T, 0><<<grid_for(vec ? n / Vec16<T>::W + 1 : n, 256), 256, 0, s>>>(a, b, (const T*)0, out, n, vec);
-	return check("add_relu_fwd");
+	add_relu_kernel<T, 0><<<grid_for(vec ? n / Vec16<T>::W + 1 : n, 256, 8), 256, 0, s>>>(a, b, (const T*)0, out, n, vec);
+	return launched("add_relu_fwd");
 }
 template <typename T>
 static int add_relu_bwd_t(cudaStream_t s, const T* a, const T* b, const T* y, T* out, size_t n)
@@ -874,8 +840,8 @@ static int add_relu_bwd_t(cudaStream_t s, const T* a, const T* b, const T* y, T*
 	if (n == 0)
 		return 0;
 	const int vec = aligned_v16(a) && aligned_v16(b) && aligned_v16(out) && aligned_v16(y);
-	add_relu_kernel<T, 1><<<grid_for(vec ? n / Vec16<T>::W + 1 : n, 256), 256, 0, s>>>(a, b, y, out, n, vec);
-	return check("add_relu_bwd");
+	add_relu_kernel<T, 1><<<grid_for(vec ? n / Vec16<T>::W + 1 : n, 256, 8), 256, 0, s>>>(a, b, y, out, n, vec);
+	return launched("add_relu_bwd");
 }
 int ew_add_relu_fwd_f32(cudaStream_t s, const float* a, const float* b, float* out, size_t n) { return add_relu_fwd_t<float>(s, a, b, out, n); }
 int ew_add_relu_bwd_f32(cudaStream_t s, const float* a, const float* b, const float* y, float* out, size_t n) { return add_relu_bwd_t<float>(s, a, b, y, out, n); }

@@ -26,8 +26,7 @@
 //                                  reverse backward), coalesced along C.
 //   otherwise (NHWC, NCHW wider than LSSC_BAND_MAX_W)
 //                                  one thread per (block, channel), the same scan on scalar accesses, channel fastest.
-#include "../../include/ccv_nnc_sm100.h"
-#include "sm100_contract.h"
+#include "sm100_cmd.h"
 #include "sm100_elem.cuh"
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -41,18 +40,6 @@ constexpr int LSSC_THREADS = 256;
 constexpr long long LSSC_SPAN = 8192;     // halves of either side staged by one CTA of the band form (16 KB)
 constexpr int LSSC_BAND_MAX_W = 2048;     // LSSC_SPAN / 4: one 4-row band fits
 constexpr int LSSC_CTAS_PER_SM = 8;       // the band form spreads its bands over at least this many CTAs per SM when it can
-
-int check(const char* what)
-{
-	count_launch();
-	const cudaError_t e = cudaGetLastError();
-	if (e != cudaSuccess)
-	{
-		set_last_error(what, e);
-		return -1;
-	}
-	return 0;
-}
 
 // ------------------------------------------------------------------------------------------------ one block (CPU_REF's arithmetic)
 __device__ __forceinline__ float h2f(const uint16_t h) { return __half2float(__ushort_as_half(h)); }
@@ -390,25 +377,6 @@ __global__ void __launch_bounds__(LSSC_THREADS) lssc_back_vec_kernel(const uint1
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-int sms()
-{
-	static int n = 0;
-	if (!n)
-	{
-		int dev = 0;
-		cudaGetDevice(&dev);
-		cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-		if (n <= 0)
-			n = 132;
-	}
-	return n;
-}
-
-int grid_for(const long long items)
-{
-	const long long want = (items + LSSC_THREADS - 1) / LSSC_THREADS, cap = (long long)sms() * 16;
-	return (int)(want < cap ? want : cap);
-}
 
 // one (original, compressed) pair, checked: the original's geometry and layout
 struct Pair {
@@ -418,14 +386,6 @@ struct Pair {
 	long long outer; // NCHW: N x C planes; NHWC: N
 	int H, W, C;     // C: NHWC channels (1 for NCHW)
 };
-
-int nd_of(const ccv_nnc_tensor_t* const t)
-{
-	int nd = 0;
-	while (nd < CCV_NNC_MAX_DIM_ALLOC && t->info.dim[nd] > 0)
-		nd++;
-	return nd;
-}
 
 bool fp16_dense(const ccv_nnc_tensor_t* const t)
 {
@@ -475,7 +435,7 @@ int run_pair(const Pair& p, const bool forward, cudaStream_t s)
 		b.H = p.H, b.W = p.W, b.Hb = Hb, b.Wc = Wc, b.G = p.outer * Hb, b.HW = (long long)p.H * p.W;
 		// as many bands as fit (LSSC_SPAN halves of the original per CTA), but no fewer than LSSC_CTAS_PER_SM CTAs per SM when the
 		// tensor has that many bands
-		const long long fit = LSSC_SPAN / (4 * b.W), spread = (b.G + (long long)sms() * LSSC_CTAS_PER_SM - 1) / ((long long)sms() * LSSC_CTAS_PER_SM);
+		const long long fit = LSSC_SPAN / (4 * b.W), spread = (b.G + (long long)sm_count() * LSSC_CTAS_PER_SM - 1) / ((long long)sm_count() * LSSC_CTAS_PER_SM);
 		b.bands = (int)(spread < fit ? (spread > 0 ? spread : 1) : fit);
 		const long long ctas = (b.G + b.bands - 1) / b.bands;
 		// the original's span is at most 4 W bands halves, the compressed one's bands Wc <= LSSC_SPAN (W >= 1); 8 halves of slack
@@ -485,7 +445,7 @@ int run_pair(const Pair& p, const bool forward, cudaStream_t s)
 			lssc_forw_band_kernel<<<(unsigned)ctas, LSSC_THREADS, shm, s>>>(xp, yp, b);
 		else
 			lssc_back_band_kernel<<<(unsigned)ctas, LSSC_THREADS, shm, s>>>(yp, xp, b);
-		return check(forward ? "lssc_forw_band" : "lssc_back_band");
+		return launched(forward ? "lssc_forw_band" : "lssc_back_band");
 	}
 	BlockGeom b;
 	b.H = p.H, b.W = p.W, b.Hb = (int)Hb, b.Wb = (int)Wb, b.C = p.C;
@@ -499,20 +459,20 @@ int run_pair(const Pair& p, const bool forward, cudaStream_t s)
 	}
 	const bool vec = !p.nchw && p.C % 8 == 0 && aligned_v16(xp) && aligned_v16(yp);
 	b.blocks = p.outer * Hb * Wb * (vec ? p.C / 8 : p.C);
-	const int grid = grid_for(b.blocks);
+	const int grid = grid_for((size_t)b.blocks, LSSC_THREADS, 16);
 	if (vec)
 	{
 		if (forward)
 			lssc_forw_vec_kernel<<<grid, LSSC_THREADS, 0, s>>>(xp, yp, b);
 		else
 			lssc_back_vec_kernel<<<grid, LSSC_THREADS, 0, s>>>(yp, xp, b);
-		return check(forward ? "lssc_forw_vec" : "lssc_back_vec");
+		return launched(forward ? "lssc_forw_vec" : "lssc_back_vec");
 	}
 	if (forward)
 		lssc_forw_scalar_kernel<<<grid, LSSC_THREADS, 0, s>>>(xp, yp, b);
 	else
 		lssc_back_scalar_kernel<<<grid, LSSC_THREADS, 0, s>>>(yp, xp, b);
-	return check(forward ? "lssc_forw_scalar" : "lssc_back_scalar");
+	return launched(forward ? "lssc_forw_scalar" : "lssc_back_scalar");
 }
 
 // forward: inputs (x_1 .. x_n) -> outputs (y_1 .. y_n), input_size == output_size; backward: inputs (y_1 .. y_m) -> outputs (x_1 ..
@@ -537,19 +497,7 @@ int exec_lssc(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flag
 	return rc;
 }
 
-void fill(ccv_nnc_cmd_backend_registry_t* const registry, const ccv_nnc_cmd_exec_f exec)
-{
-	registry->tensor_formats = CCV_TENSOR_FORMAT_NCHW | CCV_TENSOR_FORMAT_NHWC;
-	registry->tensor_datatypes = CCV_16F;
-	registry->tensor_memory = CCV_TENSOR_GPU_MEMORY;
-	registry->algorithms = 1;
-	registry->exec = exec;
-	registry->autotune = 0;
-	registry->aux = 0;
-}
-
 } // namespace
 
-#define REGISTER_SM100(cmd) extern "C" void _register_command_ ## cmd ## _backend_CCV_NNC_BACKEND_GPU_SM100(ccv_nnc_cmd_backend_registry_t* const registry)
-REGISTER_SM100(CCV_NNC_COMPRESSION_LSSC_FORWARD) { fill(registry, exec_lssc<true>); }
-REGISTER_SM100(CCV_NNC_COMPRESSION_LSSC_BACKWARD) { fill(registry, exec_lssc<false>); }
+REGISTER_SM100(CCV_NNC_COMPRESSION_LSSC_FORWARD) { fill(registry, CCV_TENSOR_FORMAT_NCHW | CCV_TENSOR_FORMAT_NHWC, CCV_16F, 1, exec_lssc<true>); }
+REGISTER_SM100(CCV_NNC_COMPRESSION_LSSC_BACKWARD) { fill(registry, CCV_TENSOR_FORMAT_NCHW | CCV_TENSOR_FORMAT_NHWC, CCV_16F, 1, exec_lssc<false>); }

@@ -25,6 +25,30 @@ void set_last_error(const char* what, cudaError_t err)
 	fprintf(stderr, "[ccv_nnc_sm100] %s\n", g_last_error);
 }
 const char* last_error() { return g_last_error; }
+int launched(const char* what)
+{
+	count_launch();
+	const cudaError_t e = cudaGetLastError();
+	if (e != cudaSuccess)
+	{
+		set_last_error(what, e);
+		return -1;
+	}
+	return 0;
+}
+static int g_sm_count = 0;
+int sm_count()
+{
+	if (!g_sm_count)
+	{
+		int dev = 0;
+		cudaGetDevice(&dev);
+		cudaDeviceGetAttribute(&g_sm_count, cudaDevAttrMultiProcessorCount, dev);
+		if (g_sm_count <= 0)
+			g_sm_count = 132;
+	}
+	return g_sm_count;
+}
 
 // ------------------------------------------------------------------------------------------------ TMA descriptors
 typedef CUresult (*encode_tiled_f)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -147,20 +171,6 @@ static bool make_map_im2col(CUtensorMap* map, const float* ptr, int N, int H, in
 }
 
 // ------------------------------------------------------------------------------------------------ launch
-static int g_num_sms = 0;
-static int num_sms()
-{
-	if (!g_num_sms)
-	{
-		int dev = 0;
-		cudaGetDevice(&dev);
-		cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-		if (g_num_sms <= 0)
-			g_num_sms = 132;
-	}
-	return g_num_sms;
-}
-
 // cudaFuncAttributeMaxDynamicSharedMemorySize is a per-device attribute: each launcher keeps one flag per device (a single
 // process may drive several GPUs, comm/gpu/ccv_nnc_comm_gpu_nccl.cu:12-58)
 constexpr int MAX_DEVICES = 64;
@@ -246,34 +256,20 @@ int splitk_reduce(cudaStream_t stream, const float* part, int splits, long long 
 	if (out_kind)
 	{
 		long long blocks = ((long long)rows * cols + 255) / 256;
-		if (blocks > (long long)num_sms() * 8)
-			blocks = (long long)num_sms() * 8;
+		if (blocks > (long long)sm_count() * 8)
+			blocks = (long long)sm_count() * 8;
 		splitk_reduce16_kernel<<<(unsigned)(blocks < 1 ? 1 : blocks), 256, 0, stream>>>(part, splits, split_stride, rows, cols, ldp, (uint16_t*)out, ldo, accumulate, out_kind);
-		count_launch();
-		const cudaError_t e = cudaGetLastError();
-		if (e != cudaSuccess)
-		{
-			set_last_error("splitk_reduce16_kernel", e);
-			return -1;
-		}
-		return 0;
+		return launched("splitk_reduce16_kernel");
 	}
 	const int vec = cols % 4 == 0 && ldp % 4 == 0 && ldo % 4 == 0 && split_stride % 4 == 0 && ((((uintptr_t)part) | ((uintptr_t)out)) & 15) == 0;
 	const long long work = (long long)rows * (vec ? cols / 4 : cols);
 	long long blocks = (work + 255) / 256;
-	if (blocks > (long long)num_sms() * 8)
-		blocks = (long long)num_sms() * 8;
+	if (blocks > (long long)sm_count() * 8)
+		blocks = (long long)sm_count() * 8;
 	if (blocks < 1)
 		blocks = 1;
 	splitk_reduce_kernel<<<(unsigned)blocks, 256, 0, stream>>>(part, splits, split_stride, rows, cols, ldp, out, ldo, accumulate, vec);
-	count_launch();
-	const cudaError_t e = cudaGetLastError();
-	if (e != cudaSuccess)
-	{
-		set_last_error("splitk_reduce_kernel", e);
-		return -1;
-	}
-	return 0;
+	return launched("splitk_reduce_kernel");
 }
 // the largest split factor <= splits whose slices fit the scratch and none of which is empty
 static int fit_splits(int splits, int k_iters, size_t slice_bytes, const Scratch& scratch)
@@ -326,7 +322,7 @@ static int launch_umma(cudaStream_t stream, const CUtensorMap& tmA, const CUtens
 		// M tile, so the slots fit the statistics tensor and the launch still fills the SMs once
 		if (!XF && AMODE != OP_MN2D && BMODE == OP_K2D && p.splits == 1 && p.grid_taps == 1 && p.rowmap.mode == 0 && !p.accumulate && r.max_rows >= 4)
 		{
-			int gx = num_sms() / tiles_n;
+			int gx = sm_count() / tiles_n;
 			gx = gx < 1 ? 1 : gx;
 			gx = gx < r.max_rows / 4 ? gx : r.max_rows / 4;
 			gx = gx < tiles_m ? gx : tiles_m;
@@ -341,7 +337,7 @@ static int launch_umma(cudaStream_t stream, const CUtensorMap& tmA, const CUtens
 			*r.rows_out = gx * 4;
 		}
 	}
-	const long long sms = num_sms(), columns = (long long)grid.y * grid.z, ctas = tiles_m * columns;
+	const long long sms = sm_count(), columns = (long long)grid.y * grid.z, ctas = tiles_m * columns;
 	if (!q.stats && p.splits == 1 && p.grid_taps == 1 && BMODE != OP_IM2COL && AMODE != OP_IM2COL_RS && ctas > sms)
 	{
 		// more tiles than one wave of one CTA per SM: gx CTAs per column walk the M tiles, so the producer loads the next tile while the
@@ -355,14 +351,7 @@ static int launch_umma(cudaStream_t stream, const CUtensorMap& tmA, const CUtens
 			grid.x = (unsigned)gx;
 	}
 	kern<<<grid, ARS ? GEMM_THREADS_RS : GEMM_THREADS, S::TOTAL, stream>>>(tmA, tmB, q);
-	count_launch();
-	cudaError_t e = cudaGetLastError();
-	if (e != cudaSuccess)
-	{
-		set_last_error("umma_gemm_kernel launch", e);
-		return -1;
-	}
-	return 0;
+	return launched("umma_gemm_kernel launch");
 }
 
 // output tile width: 64 columns for narrow outputs, else 128 (wgmma m64n128 per consumer warpgroup: 64 fp32 accumulator registers)
@@ -390,7 +379,7 @@ static int pick_splits(long long tiles, int k_iters, int min_iters_per_split)
 	// -> s = 3 (588 items, 3.97 rounds of thirds instead of 2 rounds of which the second is 1/3 full).  When the tiles already fill
 	// the machine a split is only taken if it buys more than 20 % (partial tiles cost a zero-fill, red.add traffic and the fused
 	// batch-norm statistics of the epilogue), never finer than `min_iters_per_split`.
-	const long long sms = num_sms();
+	const long long sms = sm_count();
 	long long max_s = k_iters / min_iters_per_split;
 	if (max_s < 1)
 		max_s = 1;
@@ -744,16 +733,11 @@ int conv_dgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, const void*
 	{
 		const long long total = (long long)g.N * g.H * g.W * g.C;
 		long long blocks = (total + 255) / 256;
-		if (blocks > (long long)num_sms() * 8)
-			blocks = (long long)num_sms() * 8;
+		if (blocks > (long long)sm_count() * 8)
+			blocks = (long long)sm_count() * 8;
 		bias_fill_kernel<<<(unsigned)blocks, 256, 0, stream>>>(grad_a, bias, (const uint16_t*)bias16, kind, g.C, total);
-		count_launch();
-		const cudaError_t e = cudaGetLastError();
-		if (e != cudaSuccess)
-		{
-			set_last_error("bias_fill_kernel", e);
+		if (launched("bias_fill_kernel"))
 			return -1;
-		}
 	} else if (need_zero) {
 		cudaError_t e = cudaMemsetAsync(grad_a, 0, (size_t)g.N * g.H * g.W * g.C * esz, stream);
 		if (e != cudaSuccess)
@@ -849,7 +833,7 @@ int conv_wgrad_any(cudaStream_t stream, int kind, const ConvGeom& g, const void*
 	// multiple of bk (else two taps would share a box).  Otherwise one launch with the filter tap on gridDim.z writes the columns
 	// [tap * C, +C).  A tile of the column layout carries several taps' work, and the per-tap grid reads grad_b and a once per tap.
 	const bool pointwise = conv_is_pointwise(g), rs = kind == 0 && !x3;
-	const long long sms = num_sms();
+	const long long sms = sm_count();
 	const auto rounds = [sms](long long ctas) { return (ctas + sms - 1) / sms; };
 	if (rs && !pointwise && g.C % bk == 0 && g.K <= 64)
 	{
@@ -1021,17 +1005,10 @@ static int run_im2col(cudaStream_t stream, const ConvGeom& g, const T* a, T* pat
 {
 	const size_t rows = (size_t)g.N * g.P * g.Q;
 	size_t blocks = (rows * (kp / 4) + 255) / 256;
-	if (blocks > (size_t)num_sms() * 32)
-		blocks = (size_t)num_sms() * 32;
+	if (blocks > (size_t)sm_count() * 32)
+		blocks = (size_t)sm_count() * 32;
 	im2col_kernel<T><<<(unsigned)blocks, 256, 0, stream>>>(g, a, patches, kp, (unsigned)rows);
-	count_launch();
-	const cudaError_t e = cudaGetLastError();
-	if (e != cudaSuccess)
-	{
-		set_last_error("im2col_kernel", e);
-		return -1;
-	}
-	return 0;
+	return launched("im2col_kernel");
 }
 template <typename T>
 static int conv_fprop_im2col_t(cudaStream_t stream, const ConvGeom& g, const T* a, const T* w, const float* bias, const void* bias16, T* b, void* workspace, int x3)

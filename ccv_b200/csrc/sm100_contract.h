@@ -154,5 +154,9 @@ void count_launch(int n = 1);
 unsigned long long launch_count();
 void set_last_error(const char* what, cudaError_t err);
 const char* last_error();
+// multiprocessors of the current device (read once; 132 when the query fails)
+int sm_count();
+// after each kernel launch: counts it and returns 0, or records `what` with the launch error for last_error() and returns -1
+int launched(const char* what);
 
 } // namespace sm100

@@ -25,38 +25,12 @@ constexpr int THREADS = 256;
 constexpr int VEC = 8; // 16-bit elements per 16-byte vector
 constexpr int DW_MAX_SMEM = 48 << 10;
 
-int sm_count()
-{
-	static int n = 0;
-	if (!n)
-	{
-		int dev = 0;
-		cudaGetDevice(&dev);
-		cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-		if (n <= 0)
-			n = 132;
-	}
-	return n;
-}
-
 // grid-stride launches: enough CTAs to fill the machine several times over, the rest walks
 unsigned grid_for(long long work, int per_cta, int other_dims = 1)
 {
 	long long b = (work + per_cta - 1) / per_cta;
 	const long long cap = std::max(1ll, (long long)sm_count() * 32 / std::max(1, other_dims));
 	return (unsigned)std::max(1ll, std::min(b, cap));
-}
-
-int launched(const char* what)
-{
-	count_launch();
-	const cudaError_t e = cudaGetLastError();
-	if (e != cudaSuccess)
-	{
-		set_last_error(what, e);
-		return -1;
-	}
-	return 0;
 }
 
 // (n, y, x) of index m of an [N, Y, X] grid; `small` (the grid has fewer than 2^32 points) takes 32-bit divisions, several times

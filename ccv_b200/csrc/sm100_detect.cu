@@ -29,8 +29,7 @@
 //           waits on another CTA.
 // The workspace is (5 + 1) * 4 * m + 8 * m * ceil(m / 64) bytes per item; the batch runs in groups that fit NMS_WORKSPACE_CAP.
 // Backward: one CTA per item zeroes the output and scatters g's rows to c's indices up to the first negative one.
-#include "../../include/ccv_nnc_sm100.h"
-#include "sm100_contract.h"
+#include "sm100_cmd.h"
 #include "sm100_elem.cuh"
 #include <cuda_runtime.h>
 #include <float.h>
@@ -46,18 +45,6 @@ constexpr int RF_THREADS = 256;
 constexpr int RB_PIX = 4, RB_CPL = 8, RB_WARPS = 8, RB_CHUNK = 128;
 constexpr int NMS_THREADS = 256;
 constexpr size_t NMS_WORKSPACE_CAP = (size_t)1 << 30;
-
-int check(const char* what)
-{
-	count_launch();
-	const cudaError_t e = cudaGetLastError();
-	if (e != cudaSuccess)
-	{
-		set_last_error(what, e);
-		return -1;
-	}
-	return 0;
-}
 
 // ------------------------------------------------------------------------------------------------ ROI_ALIGN
 // one axis of one ROI: sample k sits at ay(k); live samples are [lo, hi); bins of `bin` samples, `pool` of them
@@ -507,23 +494,6 @@ __global__ void __launch_bounds__(NMS_THREADS) nms_bwd_kernel(const float* __res
 }
 
 // ------------------------------------------------------------------------------------------------ command layer
-inline cudaStream_t stream_of(ccv_nnc_stream_context_t* const sc) { return (cudaStream_t)ccv_nnc_stream_context_get_stream(sc); }
-inline int kind_of(const ccv_nnc_tensor_t* const t)
-{
-	switch (CCV_GET_DATA_TYPE(t->info.datatype))
-	{
-		case CCV_32F: return 0;
-		case CCV_16BF: return 1;
-		case CCV_16F: return 2;
-	}
-	return -1;
-}
-int nd_of(const ccv_nnc_tensor_t* const t)
-{
-	int i;
-	for (i = 0; i < CCV_NNC_MAX_DIM_ALLOC && t->info.dim[i] > 0; i++) {}
-	return i;
-}
 // element steps of every axis: a view's strides, else packed
 void steps_of(const ccv_nnc_tensor_t* const t, const int nd, long long* const s)
 {
@@ -581,7 +551,7 @@ template <typename T>
 int roi_fwd_t(cudaStream_t s, const void* a, const float* b, void* c, const RoiArg& p)
 {
 	roi_align_fwd_kernel<T><<<dim3((unsigned)p.n, (unsigned)p.pool_h), RF_THREADS, 0, s>>>((const T*)a, b, (T*)c, p);
-	return check("roi align forward");
+	return launched("roi align forward");
 }
 template <typename T>
 int roi_bwd_t(cudaStream_t s, const void* g, const float* b, void* o, const RoiArg& p, const int o_n)
@@ -589,7 +559,7 @@ int roi_bwd_t(cudaStream_t s, const void* g, const float* b, void* o, const RoiA
 	const long long hw = (long long)p.h * p.w, per = (long long)RB_WARPS * RB_PIX;
 	const dim3 grid((unsigned)((hw + per - 1) / per), (unsigned)o_n, (unsigned)((p.ch + 32 * RB_CPL - 1) / (32 * RB_CPL)));
 	roi_align_bwd_kernel<T><<<grid, RB_WARPS * 32, 0, s>>>((const T*)g, b, (T*)o, p, o_n);
-	return check("roi align backward");
+	return launched("roi align backward");
 }
 
 // (a, b) -> c
@@ -704,13 +674,13 @@ int exec_nms_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int 
 	{
 		const int items = n - item0 < group ? n - item0 : group;
 		nms_rank_kernel<<<dim3((unsigned)((m + NMS_THREADS - 1) / NMS_THREADS), (unsigned)items), NMS_THREADS, 0, s>>>(a->data.f32, sorted, idx, p, item0);
-		if (check("nms rank"))
+		if (launched("nms rank"))
 			return CCV_NNC_EXEC_INVALID;
 		nms_mask_kernel<<<dim3((unsigned)p.words, (unsigned)p.words, (unsigned)items), 64, 0, s>>>(sorted, mask, p);
-		if (check("nms mask"))
+		if (launched("nms mask"))
 			return CCV_NNC_EXEC_INVALID;
 		nms_sweep_kernel<<<(unsigned)items, NMS_THREADS, smem, s>>>(sorted, idx, mask, b->data.f32, c->data.i32, p, item0);
-		if (check("nms sweep"))
+		if (launched("nms sweep"))
 			return CCV_NNC_EXEC_INVALID;
 	}
 	return CCV_NNC_EXEC_SUCCESS;
@@ -730,24 +700,12 @@ int exec_nms_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int 
 		return CCV_NNC_EXEC_INVALID;
 	p.m = m, p.words = (m + 63) / 64, p.thr = 0;
 	nms_bwd_kernel<<<(unsigned)n, NMS_THREADS, 0, stream_of(stream_context)>>>(g->data.f32, c->data.i32, h->data.f32, p);
-	return check("nms backward") ? CCV_NNC_EXEC_INVALID : CCV_NNC_EXEC_SUCCESS;
-}
-
-void fill(ccv_nnc_cmd_backend_registry_t* const registry, const int datatypes, const ccv_nnc_cmd_exec_f exec)
-{
-	registry->tensor_formats = CCV_TENSOR_FORMAT_NCHW | CCV_TENSOR_FORMAT_NHWC;
-	registry->tensor_datatypes = datatypes;
-	registry->tensor_memory = CCV_TENSOR_GPU_MEMORY;
-	registry->algorithms = 1;
-	registry->exec = exec;
-	registry->autotune = 0;
-	registry->aux = 0;
+	return launched("nms backward") ? CCV_NNC_EXEC_INVALID : CCV_NNC_EXEC_SUCCESS;
 }
 
 } // namespace
 
-#define REGISTER_SM100(cmd) extern "C" void _register_command_ ## cmd ## _backend_CCV_NNC_BACKEND_GPU_SM100(ccv_nnc_cmd_backend_registry_t* const registry)
-REGISTER_SM100(CCV_NNC_ROI_ALIGN_FORWARD) { fill(registry, CCV_32F | CCV_16F | CCV_16BF, exec_roi_forw); }
-REGISTER_SM100(CCV_NNC_ROI_ALIGN_BACKWARD) { fill(registry, CCV_32F | CCV_16F | CCV_16BF, exec_roi_back); }
-REGISTER_SM100(CCV_NNC_NMS_FORWARD) { fill(registry, CCV_32F | CCV_32S, exec_nms_forw); }
-REGISTER_SM100(CCV_NNC_NMS_BACKWARD) { fill(registry, CCV_32F | CCV_32S, exec_nms_back); }
+REGISTER_SM100(CCV_NNC_ROI_ALIGN_FORWARD) { fill(registry, CCV_TENSOR_FORMAT_NCHW | CCV_TENSOR_FORMAT_NHWC, CCV_32F | CCV_16F | CCV_16BF, 1, exec_roi_forw); }
+REGISTER_SM100(CCV_NNC_ROI_ALIGN_BACKWARD) { fill(registry, CCV_TENSOR_FORMAT_NCHW | CCV_TENSOR_FORMAT_NHWC, CCV_32F | CCV_16F | CCV_16BF, 1, exec_roi_back); }
+REGISTER_SM100(CCV_NNC_NMS_FORWARD) { fill(registry, CCV_TENSOR_FORMAT_NCHW | CCV_TENSOR_FORMAT_NHWC, CCV_32F | CCV_32S, 1, exec_nms_forw); }
+REGISTER_SM100(CCV_NNC_NMS_BACKWARD) { fill(registry, CCV_TENSOR_FORMAT_NCHW | CCV_TENSOR_FORMAT_NHWC, CCV_32F | CCV_32S, 1, exec_nms_back); }

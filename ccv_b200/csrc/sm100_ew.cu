@@ -4,49 +4,12 @@
 // (file:line cited per kernel, relative to /root/reference/lib/nnc/cmd).
 #include "sm100_ew.h"
 #include "sm100_elem.cuh"
-#include "sm100_contract.h"
+#include "sm100_cmd.h"
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <float.h>
 
 namespace sm100 {
-
-static int g_sms = 0;
-static int sms()
-{
-	if (!g_sms)
-	{
-		int dev = 0;
-		cudaGetDevice(&dev);
-		cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, dev);
-		if (g_sms <= 0)
-			g_sms = 132;
-	}
-	return g_sms;
-}
-
-static int grid_for(size_t work_items, int threads, int max_waves = 8)
-{
-	size_t blocks = (work_items + threads - 1) / threads;
-	const size_t cap = (size_t)sms() * max_waves;
-	if (blocks > cap)
-		blocks = cap;
-	if (blocks < 1)
-		blocks = 1;
-	return (int)blocks;
-}
-
-static int check(const char* what)
-{
-	count_launch();
-	const cudaError_t e = cudaGetLastError();
-	if (e != cudaSuccess)
-	{
-		set_last_error(what, e);
-		return -1;
-	}
-	return 0;
-}
 
 __device__ __forceinline__ float warp_sum(float v)
 {
@@ -109,10 +72,10 @@ int ew_set_f32(cudaStream_t s, float* p, size_t n, float v)
 	if (n == 0)
 		return 0;
 	if (aligned16(p))
-		set_f32_kernel<<<grid_for((n >> 2) + 1, 256), 256, 0, s>>>(p, n, v);
+		set_f32_kernel<<<grid_for((n >> 2) + 1, 256, 8), 256, 0, s>>>(p, n, v);
 	else
-		set_f32_scalar_kernel<<<grid_for(n, 256), 256, 0, s>>>(p, n, v);
-	return check("set_f32");
+		set_f32_scalar_kernel<<<grid_for(n, 256, 8), 256, 0, s>>>(p, n, v);
+	return launched("set_f32");
 }
 __global__ void set_u16_kernel(uint16_t* __restrict__ p, const size_t n, const uint16_t v)
 {
@@ -123,8 +86,8 @@ int ew_set_u16(cudaStream_t s, uint16_t* p, size_t n, uint16_t v)
 {
 	if (n == 0)
 		return 0;
-	set_u16_kernel<<<grid_for(n, 256), 256, 0, s>>>(p, n, v);
-	return check("set_u16");
+	set_u16_kernel<<<grid_for(n, 256, 8), 256, 0, s>>>(p, n, v);
+	return launched("set_u16");
 }
 __global__ void set_u64_kernel(uint64_t* __restrict__ p, const size_t n, const uint64_t v)
 {
@@ -135,8 +98,8 @@ int ew_set_u64(cudaStream_t s, uint64_t* p, size_t n, uint64_t v)
 {
 	if (n == 0)
 		return 0;
-	set_u64_kernel<<<grid_for(n, 256), 256, 0, s>>>(p, n, v);
-	return check("set_u64");
+	set_u64_kernel<<<grid_for(n, 256, 8), 256, 0, s>>>(p, n, v);
+	return launched("set_u64");
 }
 // int32 n-ary sum (label / index arithmetic in graphs: small tensors, scalar accesses)
 struct SumArgsI32 {
@@ -163,8 +126,8 @@ int ew_sum_i32(cudaStream_t s, const int* const* inputs, int k, int* out, size_t
 	for (int j = 0; j < k; j++)
 		a.in[j] = inputs[j];
 	a.k = k;
-	sum_i32_kernel<<<grid_for(n, 256), 256, 0, s>>>(a, out, n);
-	return check("sum_i32");
+	sum_i32_kernel<<<grid_for(n, 256, 8), 256, 0, s>>>(a, out, n);
+	return launched("sum_i32");
 }
 
 struct SumArgs {
@@ -222,10 +185,10 @@ int ew_sum_f32(cudaStream_t s, const float* const* inputs, int k, float* out, si
 			vec = vec && aligned16(a.in[j]);
 		}
 		if (vec)
-			sum_kernel<4><<<grid_for((n >> 2) + 1, 256), 256, 0, s>>>(a, out, n, done > 0);
+			sum_kernel<4><<<grid_for((n >> 2) + 1, 256, 8), 256, 0, s>>>(a, out, n, done > 0);
 		else
-			sum_kernel<1><<<grid_for(n, 256), 256, 0, s>>>(a, out, n, done > 0);
-		if (check("ew_sum"))
+			sum_kernel<1><<<grid_for(n, 256, 8), 256, 0, s>>>(a, out, n, done > 0);
+		if (launched("ew_sum"))
 			return -1;
 		done += a.k;
 	}
@@ -260,8 +223,8 @@ int ew_axpby_f32(cudaStream_t s, float p, const float* a, float q, const float* 
 	if (n == 0)
 		return 0;
 	const int vec = aligned16(a) && aligned16(c) && (!b || aligned16(b));
-	axpby_kernel<<<grid_for(vec ? (n >> 2) + 1 : n, 256), 256, 0, s>>>(p, a, q, b, c, n, vec);
-	return check("ew_axpby");
+	axpby_kernel<<<grid_for(vec ? (n >> 2) + 1 : n, 256, 8), 256, 0, s>>>(p, a, q, b, c, n, vec);
+	return launched("ew_axpby");
 }
 
 struct Bcast4 {
@@ -301,8 +264,8 @@ int ew_axpby_bcast_f32(cudaStream_t s, float p, const float* a, const int* astri
 	const size_t n = (size_t)d.dim[0] * d.dim[1] * d.dim[2] * d.dim[3];
 	if (n == 0)
 		return 0;
-	bcast_kernel<0><<<grid_for(n, 256), 256, 0, s>>>(p, a, q, b, c, d, n);
-	return check("ew_axpby_bcast");
+	bcast_kernel<0><<<grid_for(n, 256, 8), 256, 0, s>>>(p, a, q, b, c, d, n);
+	return launched("ew_axpby_bcast");
 }
 int ew_mul_bcast_f32(cudaStream_t s, float p, const float* a, const int* astride, const float* b, const int* bstride, float* c, const int* cstride, const int* dim)
 {
@@ -310,8 +273,8 @@ int ew_mul_bcast_f32(cudaStream_t s, float p, const float* a, const int* astride
 	const size_t n = (size_t)d.dim[0] * d.dim[1] * d.dim[2] * d.dim[3];
 	if (n == 0)
 		return 0;
-	bcast_kernel<1><<<grid_for(n, 256), 256, 0, s>>>(p, a, 0.f, b, c, d, n);
-	return check("ew_mul_bcast");
+	bcast_kernel<1><<<grid_for(n, 256, 8), 256, 0, s>>>(p, a, 0.f, b, c, d, n);
+	return launched("ew_mul_bcast");
 }
 
 // =============================================================================================== relu
@@ -337,8 +300,8 @@ int ew_relu_fwd_f32(cudaStream_t s, const float* a, float* b, size_t n)
 	if (n == 0)
 		return 0;
 	const int vec = aligned16(a) && aligned16(b);
-	relu_fwd_kernel<<<grid_for(vec ? (n >> 2) + 1 : n, 256), 256, 0, s>>>(a, b, n, vec);
-	return check("relu_fwd");
+	relu_fwd_kernel<<<grid_for(vec ? (n >> 2) + 1 : n, 256, 8), 256, 0, s>>>(a, b, n, vec);
+	return launched("relu_fwd");
 }
 __global__ void relu_bwd_kernel(const float* __restrict__ g, const float* __restrict__ b, float* __restrict__ h, const size_t n, const int vec)
 {
@@ -363,8 +326,8 @@ int ew_relu_bwd_f32(cudaStream_t s, const float* g, const float* b, float* h, si
 	if (n == 0)
 		return 0;
 	const int vec = aligned16(g) && aligned16(b) && aligned16(h);
-	relu_bwd_kernel<<<grid_for(vec ? (n >> 2) + 1 : n, 256), 256, 0, s>>>(g, b, h, n, vec);
-	return check("relu_bwd");
+	relu_bwd_kernel<<<grid_for(vec ? (n >> 2) + 1 : n, 256, 8), 256, 0, s>>>(g, b, h, n, vec);
+	return launched("relu_bwd");
 }
 
 // =============================================================================================== column sums
@@ -462,7 +425,7 @@ __global__ void __launch_bounds__(1024) colsum_partials_kernel(const float* __re
 		out[col] = accumulate ? out[col] + t : t;
 	}
 }
-size_t colsum_workspace_bytes(int cols) { return ((size_t)sms() * 8 + 8) * (size_t)((cols + 3) / 4 * 4) * sizeof(float); }
+size_t colsum_workspace_bytes(int cols) { return ((size_t)sm_count() * 8 + 8) * (size_t)((cols + 3) / 4 * 4) * sizeof(float); }
 static int colsum_f32(cudaStream_t s, const float* g, size_t rows, int cols, long long ld, float* out, int accumulate, void* workspace)
 {
 	if (cols <= 0)
@@ -488,18 +451,18 @@ static int colsum_f32(cudaStream_t s, const float* g, size_t rows, int cols, lon
 		const int rpi = 256 / cpb;
 		const int gx = (cols4 + cpb - 1) / cpb;
 		size_t gy = (rows + (size_t)rpi * 16 - 1) / ((size_t)rpi * 16);
-		const size_t cap = (size_t)(sms() * 8 + gx - 1) / gx;
+		const size_t cap = (size_t)(sm_count() * 8 + gx - 1) / gx;
 		if (gy > cap)
 			gy = cap;
 		if (gy < 1)
 			gy = 1;
 		colsum_vec_kernel<<<dim3(gx, (unsigned)gy), 256, 0, s>>>((const float4*)g, rows, cols4, ld / 4, out, (float*)workspace, cpb);
-		if (check("colsum_vec"))
+		if (launched("colsum_vec"))
 			return -1;
 		if (workspace)
 		{
 			colsum_partials_kernel<<<(cols + 31) / 32, 1024, 0, s>>>((const float*)workspace, (int)gy, cols, out, accumulate);
-			return check("colsum_partials");
+			return launched("colsum_partials");
 		}
 		return 0;
 	}
@@ -507,13 +470,13 @@ static int colsum_f32(cudaStream_t s, const float* g, size_t rows, int cols, lon
 	const int rpi = 256 / cpb;
 	const int gx = (cols + cpb - 1) / cpb;
 	size_t gy = (rows + rpi * 8 - 1) / ((size_t)rpi * 8);
-	const size_t cap = (size_t)(sms() * 4 + gx - 1) / gx;
+	const size_t cap = (size_t)(sm_count() * 4 + gx - 1) / gx;
 	if (gy > cap)
 		gy = cap;
 	if (gy < 1)
 		gy = 1;
 	colsum_kernel<<<dim3(gx, (unsigned)gy), 256, 256 * sizeof(float), s>>>(g, rows, cols, ld, out, cpb);
-	return check("colsum");
+	return launched("colsum");
 }
 
 // generic <= 4-d reduction to a broadcast shape: one thread block per output element (small outputs only)
@@ -558,7 +521,7 @@ int reduce_sum_bcast_f32(cudaStream_t s, const float* a, const int* adim, const 
 	if (outs > 0x7fffffff)
 		return 1;
 	reduce_sum_kernel<<<(unsigned)outs, 256, 0, s>>>(a, out, d, scale, accumulate);
-	return check("reduce_sum");
+	return launched("reduce_sum");
 }
 
 // =============================================================================================== pooling (NHWC)
@@ -647,10 +610,10 @@ static int pool_fwd_t(cudaStream_t s, const PoolGeom& g, const T* a, T* b)
 	if (total == 0)
 		return 0;
 	if (pool_vec_ok(g, a, (const T*)b))
-		pool_fwd_kernel<T, Vec16<T>::W, IS_MAX><<<grid_for(total / Vec16<T>::W, 256), 256, 0, s>>>(g, a, b);
+		pool_fwd_kernel<T, Vec16<T>::W, IS_MAX><<<grid_for(total / Vec16<T>::W, 256, 8), 256, 0, s>>>(g, a, b);
 	else
-		pool_fwd_kernel<T, 1, IS_MAX><<<grid_for(total, 256), 256, 0, s>>>(g, a, b);
-	return check(IS_MAX ? "pool_max_fwd" : "pool_avg_fwd");
+		pool_fwd_kernel<T, 1, IS_MAX><<<grid_for(total, 256, 8), 256, 0, s>>>(g, a, b);
+	return launched(IS_MAX ? "pool_max_fwd" : "pool_avg_fwd");
 }
 int pool_max_fwd_f32(cudaStream_t s, const PoolGeom& g, const float* a, float* b) { return pool_fwd_t<float, 1>(s, g, a, b); }
 int pool_avg_fwd_f32(cudaStream_t s, const PoolGeom& g, const float* a, float* b) { return pool_fwd_t<float, 0>(s, g, a, b); }
@@ -761,10 +724,10 @@ static int pool_max_bwd_t(cudaStream_t s, const PoolGeom& g, const T* grad_b, co
 	if (total == 0)
 		return 0;
 	if (pool_vec_ok(g, a, b) && aligned_v16(grad_b) && aligned_v16(grad_a))
-		pool_bwd_kernel<T, Vec16<T>::W, 1><<<grid_for(total / Vec16<T>::W, 256), 256, 0, s>>>(g, grad_b, a, b, grad_a);
+		pool_bwd_kernel<T, Vec16<T>::W, 1><<<grid_for(total / Vec16<T>::W, 256, 8), 256, 0, s>>>(g, grad_b, a, b, grad_a);
 	else
-		pool_bwd_kernel<T, 1, 1><<<grid_for(total, 256), 256, 0, s>>>(g, grad_b, a, b, grad_a);
-	return check("pool_max_bwd");
+		pool_bwd_kernel<T, 1, 1><<<grid_for(total, 256, 8), 256, 0, s>>>(g, grad_b, a, b, grad_a);
+	return launched("pool_max_bwd");
 }
 // Average-pool backward when the windows tile the input exactly (window = stride, no padding, H = P * R, W = Q * S: the 2 x 2 / 2
 // shortcut pools and the global pool of a ResNet): one thread per OUTPUT gradient group -- one 16-byte load, one multiply per
@@ -830,14 +793,14 @@ static int pool_avg_bwd_t(cudaStream_t s, const PoolGeom& g, const T* grad_b, T*
 	constexpr int W = Vec16<T>::W;
 	if (avgpool_tiles_ok(g, grad_b, grad_a))
 	{
-		avgpool_bwd_tiles_kernel<T, 0><<<grid_for((size_t)g.N * g.P * g.Q * (g.C / W), 256), 256, 0, s>>>(g, grad_b, grad_a, (const T*)0, (const T*)0);
-		return check("pool_avg_bwd");
+		avgpool_bwd_tiles_kernel<T, 0><<<grid_for((size_t)g.N * g.P * g.Q * (g.C / W), 256, 8), 256, 0, s>>>(g, grad_b, grad_a, (const T*)0, (const T*)0);
+		return launched("pool_avg_bwd");
 	}
 	if (pool_vec_ok(g, (const T*)grad_a, grad_b))
-		pool_bwd_kernel<T, Vec16<T>::W, 0><<<grid_for(total / Vec16<T>::W, 256), 256, 0, s>>>(g, grad_b, (const T*)0, (const T*)0, grad_a);
+		pool_bwd_kernel<T, Vec16<T>::W, 0><<<grid_for(total / Vec16<T>::W, 256, 8), 256, 0, s>>>(g, grad_b, (const T*)0, (const T*)0, grad_a);
 	else
-		pool_bwd_kernel<T, 1, 0><<<grid_for(total, 256), 256, 0, s>>>(g, grad_b, (const T*)0, (const T*)0, grad_a);
-	return check("pool_avg_bwd");
+		pool_bwd_kernel<T, 1, 0><<<grid_for(total, 256, 8), 256, 0, s>>>(g, grad_b, (const T*)0, (const T*)0, grad_a);
+	return launched("pool_avg_bwd");
 }
 // grad_a = y > 0 ? r + avgpool_backward(grad_b) : 0 in one pass; r and y are addressed with grad_a's strides.  1 (nothing launched)
 // when the geometry is not the tiles kernel's
@@ -848,8 +811,8 @@ static int pool_avg_bwd_add_relu_t(cudaStream_t s, const PoolGeom& g, const T* g
 		return 1;
 	if ((size_t)g.N * g.H * g.W * g.C == 0)
 		return 0;
-	avgpool_bwd_tiles_kernel<T, 1><<<grid_for((size_t)g.N * g.P * g.Q * (g.C / Vec16<T>::W), 256), 256, 0, s>>>(g, grad_b, grad_a, r, y);
-	return check("pool_avg_bwd_add_relu") ? -1 : 0;
+	avgpool_bwd_tiles_kernel<T, 1><<<grid_for((size_t)g.N * g.P * g.Q * (g.C / Vec16<T>::W), 256, 8), 256, 0, s>>>(g, grad_b, grad_a, r, y);
+	return launched("pool_avg_bwd_add_relu") ? -1 : 0;
 }
 int pool_avg_bwd_add_relu(cudaStream_t s, int kind, const PoolGeom& g, const void* grad_b, const void* r, const void* y, void* grad_a)
 {
@@ -901,7 +864,7 @@ int softmax_fwd_f32(cudaStream_t s, const float* a, float* b, int batch, int cou
 	if (batch <= 0 || count <= 0)
 		return 0;
 	softmax_fwd_kernel<<<batch, softmax_threads(count), 0, s>>>(a, b, count);
-	return check("softmax_fwd");
+	return launched("softmax_fwd");
 }
 // softmax/ccv_nnc_softmax_cpu_ref.c:42-75: h = (g - sum(g * b)) * b; h may be g (in place)
 __global__ void softmax_bwd_kernel(const float* g, const float* __restrict__ b, float* h, const int count)
@@ -920,7 +883,7 @@ int softmax_bwd_f32(cudaStream_t s, const float* g, const float* b, float* h, in
 	if (batch <= 0 || count <= 0)
 		return 0;
 	softmax_bwd_kernel<<<batch, softmax_threads(count), 0, s>>>(g, b, h, count);
-	return check("softmax_bwd");
+	return launched("softmax_bwd");
 }
 __device__ __forceinline__ int label_of(const void* label, const int kind, const int i)
 {
@@ -958,7 +921,7 @@ int cce_fwd_f32(cudaStream_t s, const float* a, const void* label, int label_kin
 	if (batch <= 0 || count <= 0)
 		return 0;
 	cce_fwd_kernel<<<batch, softmax_threads(count), 0, s>>>(a, label, label_kind, c, count, trim0, trim1);
-	return check("cce_fwd");
+	return launched("cce_fwd");
 }
 // loss/ccv_nnc_categorical_crossentropy_cpu_ref.c:107-300: h = -g * t / a (g == NULL means 1)
 __global__ void cce_bwd_kernel(const float* __restrict__ g, const float* __restrict__ a, const void* __restrict__ label, const int kind, float* __restrict__ h, const int count, const float trim0, const float trim1)
@@ -989,7 +952,7 @@ int cce_bwd_f32(cudaStream_t s, const float* g, const float* a, const void* labe
 	if (batch <= 0 || count <= 0)
 		return 0;
 	cce_bwd_kernel<<<batch, softmax_threads(count), 0, s>>>(g, a, label, label_kind, h, count, trim0, trim1);
-	return check("cce_bwd");
+	return launched("cce_bwd");
 }
 // softmax_loss/ccv_nnc_softmax_crossentropy_cpu_ref.c:13-170: d = softmax(a); c = sum_j t_j * (max - a_j).
 // (The reference's "loss" deliberately leaves out log(sum exp): it is assigned before the exponentials, :46,:71,:98.)
@@ -1037,7 +1000,7 @@ int softmax_cce_fwd_f32(cudaStream_t s, const float* a, const void* label, int l
 	if (batch <= 0 || count <= 0)
 		return 0;
 	softmax_cce_fwd_kernel<<<batch, softmax_threads(count), 0, s>>>(a, label, label_kind, c, d, count, trim0, trim1);
-	return check("softmax_cce_fwd");
+	return launched("softmax_cce_fwd");
 }
 // softmax_loss/ccv_nnc_softmax_crossentropy_cpu_ref.c:172-340: h = g * (d - t); g == NULL means 1.  h may be d
 // (softmax_loss/ccv_nnc_softmax_crossentropy.c:31-40)
@@ -1063,7 +1026,7 @@ int softmax_cce_bwd_f32(cudaStream_t s, const float* g, const void* label, int l
 	if (batch <= 0 || count <= 0)
 		return 0;
 	softmax_cce_bwd_kernel<<<batch, softmax_threads(count), 0, s>>>(g, label, label_kind, d, h, count, trim0, trim1);
-	return check("softmax_cce_bwd");
+	return launched("softmax_cce_bwd");
 }
 
 // =============================================================================================== SGD
@@ -1115,10 +1078,10 @@ int sgd_any(cudaStream_t s, int g_kind, const void* g, const float* a, const flo
 		return 0;
 	const float inv_dampening = 1.f - dampening;
 	if (count % 4 == 0 && g_aligned(g, g_kind) && aligned16(a) && aligned16(m) && aligned16(b) && aligned16(n))
-		sgd_kernel<4><<<grid_for(count / 4, 256), 256, 0, s>>>(g, g_kind, a, m, b, n, count, nesterov, rate, scale, decay, momentum, inv_dampening);
+		sgd_kernel<4><<<grid_for(count / 4, 256, 8), 256, 0, s>>>(g, g_kind, a, m, b, n, count, nesterov, rate, scale, decay, momentum, inv_dampening);
 	else
-		sgd_kernel<1><<<grid_for(count, 256), 256, 0, s>>>(g, g_kind, a, m, b, n, count, nesterov, rate, scale, decay, momentum, inv_dampening);
-	return check("sgd");
+		sgd_kernel<1><<<grid_for(count, 256, 8), 256, 0, s>>>(g, g_kind, a, m, b, n, count, nesterov, rate, scale, decay, momentum, inv_dampening);
+	return launched("sgd");
 }
 
 // Many SGD commands with the same hyper-parameters in one launch (the per-parameter SGD nodes of a model are a run of ~200
@@ -1212,7 +1175,7 @@ int sgd_multi_any(cudaStream_t s, int tensors, int g_kind, const void* const* g,
 		{
 			t.block_start[t.tensors] = blocks;
 			sgd_multi_kernel<<<blocks, 256, 0, s>>>(t, nesterov, rate, scale, decay, momentum, inv_dampening);
-			if (check("sgd_multi"))
+			if (launched("sgd_multi"))
 				return -1;
 		}
 	}
@@ -1247,10 +1210,10 @@ static int relu16_t(cudaStream_t s, const T* g, const T* a, T* out, size_t n, in
 		return 0;
 	const int vec = aligned_v16(a) && aligned_v16(out) && (!bwd || aligned_v16(g));
 	if (bwd)
-		relu16_kernel<T, 1><<<grid_for(vec ? n / Vec16<T>::W + 1 : n, 256), 256, 0, s>>>(g, a, out, n, vec);
+		relu16_kernel<T, 1><<<grid_for(vec ? n / Vec16<T>::W + 1 : n, 256, 8), 256, 0, s>>>(g, a, out, n, vec);
 	else
-		relu16_kernel<T, 0><<<grid_for(vec ? n / Vec16<T>::W + 1 : n, 256), 256, 0, s>>>(g, a, out, n, vec);
-	return check("relu16");
+		relu16_kernel<T, 0><<<grid_for(vec ? n / Vec16<T>::W + 1 : n, 256, 8), 256, 0, s>>>(g, a, out, n, vec);
+	return launched("relu16");
 }
 int ew_relu_fwd_16(cudaStream_t s, int kind, const void* a, void* b, size_t n)
 {
@@ -1307,10 +1270,10 @@ int ew_sum_16(cudaStream_t s, int kind, const void* const* inputs, int k, void* 
 	for (int j = 0; j < k; j++)
 		a.in[j] = inputs[j], vec = vec && (((uintptr_t)inputs[j]) & 15) == 0;
 	if (kind == 1)
-		sum16_kernel<__nv_bfloat16><<<grid_for(vec ? (n >> 3) + 1 : n, 256), 256, 0, s>>>(a, (__nv_bfloat16*)out, n, vec);
+		sum16_kernel<__nv_bfloat16><<<grid_for(vec ? (n >> 3) + 1 : n, 256, 8), 256, 0, s>>>(a, (__nv_bfloat16*)out, n, vec);
 	else
-		sum16_kernel<__half><<<grid_for(vec ? (n >> 3) + 1 : n, 256), 256, 0, s>>>(a, (__half*)out, n, vec);
-	return check("ew_sum16");
+		sum16_kernel<__half><<<grid_for(vec ? (n >> 3) + 1 : n, 256, 8), 256, 0, s>>>(a, (__half*)out, n, vec);
+	return launched("ew_sum16");
 }
 
 // ew/ccv_nnc_ew_cpu_ref.c:235-334 (EWPROD): c = a0 * a1 * ..., every product rounded on its own, left to right.  fp32 in chunks of
@@ -1361,10 +1324,10 @@ static int prod_t(cudaStream_t s, const void* const* inputs, int k, T* out, size
 		for (int j = 0; j < a.k; j++)
 			a.in[j] = inputs[done + j], vec = vec && aligned_v16(a.in[j]);
 		if (vec)
-			prod_kernel<T, W><<<grid_for(n / W + 1, 256), 256, 0, s>>>(a, out, n, done > 0);
+			prod_kernel<T, W><<<grid_for(n / W + 1, 256, 8), 256, 0, s>>>(a, out, n, done > 0);
 		else
-			prod_kernel<T, 1><<<grid_for(n, 256), 256, 0, s>>>(a, out, n, done > 0);
-		if (check("ew_prod"))
+			prod_kernel<T, 1><<<grid_for(n, 256, 8), 256, 0, s>>>(a, out, n, done > 0);
+		if (launched("ew_prod"))
 			return -1;
 		done += a.k;
 	}
@@ -1414,8 +1377,8 @@ static int prod_back_t(cudaStream_t s, const void* g, const void* b, const void*
 	p.g = g, p.b = b, p.k = k;
 	for (int z = 0; z < k; z++)
 		p.a[z] = a[z], p.h[z] = h[z];
-	prod_back_kernel<T, MAXK><<<grid_for(n, 256), 256, 0, s>>>(p, n);
-	return check("ew_prod_back");
+	prod_back_kernel<T, MAXK><<<grid_for(n, 256, 8), 256, 0, s>>>(p, n);
+	return launched("ew_prod_back");
 }
 int ew_prod_back(cudaStream_t s, int kind, const void* g, const void* b, const void* const* a, void* const* h, int k, size_t n)
 {
@@ -1503,12 +1466,12 @@ int colsum_any(cudaStream_t s, int g_kind, const void* g, size_t rows, int cols,
 	if (cols % 4 || ld % 4 || !workspace || (((uintptr_t)g) & (g_kind == 0 ? 15 : 7)))
 	{
 		colsum_scalar_kernel<<<cols, 256, 0, s>>>(g, g_kind, rows, ld, out, out_kind, accumulate);
-		return check("colsum_scalar");
+		return launched("colsum_scalar");
 	}
 	const int cols4 = cols / 4, cpb = cols4 >= 256 ? 256 : cols4, rpi = 256 / cpb;
 	const int gx = (cols4 + cpb - 1) / cpb;
 	size_t gy = (rows + (size_t)rpi * 32 - 1) / ((size_t)rpi * 32);
-	const size_t cap = (size_t)(sms() * 8 + gx - 1) / gx;
+	const size_t cap = (size_t)(sm_count() * 8 + gx - 1) / gx;
 	if (gy > cap)
 		gy = cap;
 	if (gy < 1)
@@ -1520,10 +1483,10 @@ int colsum_any(cudaStream_t s, int g_kind, const void* g, size_t rows, int cols,
 		colsum_any_kernel<__nv_bfloat16><<<dim3(gx, (unsigned)gy), 256, 0, s>>>((const __nv_bfloat16*)g, rows, cols, ld, part);
 	else
 		colsum_any_kernel<__half><<<dim3(gx, (unsigned)gy), 256, 0, s>>>((const __half*)g, rows, cols, ld, part);
-	if (check("colsum_any"))
+	if (launched("colsum_any"))
 		return -1;
 	colsum_partials_any_kernel<<<(cols + 31) / 32, 1024, 0, s>>>(part, (int)gy, cols, out, out_kind, accumulate);
-	return check("colsum_partials_any");
+	return launched("colsum_partials_any");
 }
 
 // strided [rows, cols] matrix of element kind `kind` <-> dense fp32 [rows, cols]: the operands of 16-bit GEMMs whose strides the
@@ -1551,15 +1514,15 @@ int widen_matrix(cudaStream_t s, const void* src, int kind, long long rs, long l
 {
 	if (rows <= 0 || cols <= 0)
 		return 0;
-	widen_matrix_kernel<<<grid_for((size_t)rows * cols, 256), 256, 0, s>>>(src, kind, rs, cs, dst, rows, cols);
-	return check("widen_matrix");
+	widen_matrix_kernel<<<grid_for((size_t)rows * cols, 256, 8), 256, 0, s>>>(src, kind, rs, cs, dst, rows, cols);
+	return launched("widen_matrix");
 }
 int narrow_matrix(cudaStream_t s, const float* src, void* dst, int kind, long long rs, long long cs, int rows, int cols, int accumulate)
 {
 	if (rows <= 0 || cols <= 0)
 		return 0;
-	narrow_matrix_kernel<<<grid_for((size_t)rows * cols, 256), 256, 0, s>>>(src, dst, kind, rs, cs, rows, cols, accumulate);
-	return check("narrow_matrix");
+	narrow_matrix_kernel<<<grid_for((size_t)rows * cols, 256, 8), 256, 0, s>>>(src, dst, kind, rs, cs, rows, cols, accumulate);
+	return launched("narrow_matrix");
 }
 
 // =============================================================================================== dtype conversion
@@ -1591,8 +1554,8 @@ int convert_dtype(cudaStream_t s, const void* a, int ad, void* b, int bd, size_t
 {
 	if (n == 0)
 		return 0;
-	const int grid = grid_for(n, 256);
-#define CONV_CASE(A, B) if (ad == A && bd == B) { convert_kernel<A, B><<<grid, 256, 0, s>>>(a, b, n); return check("convert_dtype"); }
+	const int grid = grid_for(n, 256, 8);
+#define CONV_CASE(A, B) if (ad == A && bd == B) { convert_kernel<A, B><<<grid, 256, 0, s>>>(a, b, n); return launched("convert_dtype"); }
 	CONV_CASE(0, 1) CONV_CASE(1, 0) CONV_CASE(0, 2) CONV_CASE(2, 0) CONV_CASE(0, 3) CONV_CASE(3, 0) CONV_CASE(2, 1) CONV_CASE(1, 2)
 #undef CONV_CASE
 	return 1;
@@ -1635,7 +1598,7 @@ int copy_strided(cudaStream_t s, const void* a, const int* astride, void* b, con
 	const size_t n = (size_t)e.dim[0] * e.dim[1] * e.dim[2] * e.dim[3];
 	if (n == 0)
 		return 0;
-	const int grid = grid_for(n, 256);
+	const int grid = grid_for(n, 256, 8);
 	if (elem_size == 4)
 		copy_strided_kernel<uint32_t><<<grid, 256, 0, s>>>((const uint32_t*)a, (uint32_t*)b, e, n);
 	else if (elem_size == 2)
@@ -1646,7 +1609,7 @@ int copy_strided(cudaStream_t s, const void* a, const int* astride, void* b, con
 		copy_strided_kernel<uint8_t><<<grid, 256, 0, s>>>((const uint8_t*)a, (uint8_t*)b, e, n);
 	else
 		return 1;
-	return check("copy_strided");
+	return launched("copy_strided");
 }
 
 } // namespace sm100

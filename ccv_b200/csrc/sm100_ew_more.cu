@@ -13,8 +13,7 @@
 //   reduce/ccv_nnc_reduce_{sum,mean,max,min,norm2}_cpu_ref.c   the output's unit dimensions are the reduced axes
 //   util/ccv_nnc_util_cpu_ref.c:1300-1481     MASKED_FILL c = mask == p ? q : a (mask int32 or fp32, broadcast); backward q = 0
 // A missing gradient (inputs[0] == NULL) reads as all ones, as in the reference.
-#include "../../include/ccv_nnc_sm100.h"
-#include "sm100_contract.h"
+#include "sm100_cmd.h"
 #include "sm100_elem.cuh"
 #include "sm100_ew.h"
 #include <cuda_runtime.h>
@@ -26,73 +25,6 @@ using namespace sm100;
 
 namespace {
 
-int g_sms = 0;
-int sms()
-{
-	if (!g_sms)
-	{
-		int dev = 0;
-		cudaGetDevice(&dev);
-		cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, dev);
-		if (g_sms <= 0)
-			g_sms = 132;
-	}
-	return g_sms;
-}
-int grid_for(size_t work, int threads)
-{
-	size_t blocks = (work + threads - 1) / threads;
-	const size_t cap = (size_t)sms() * 8;
-	if (blocks > cap)
-		blocks = cap;
-	return blocks < 1 ? 1 : (int)blocks;
-}
-int check(const char* what)
-{
-	count_launch();
-	const cudaError_t e = cudaGetLastError();
-	if (e != cudaSuccess)
-	{
-		set_last_error(what, e);
-		return -1;
-	}
-	return 0;
-}
-inline cudaStream_t stream_of(ccv_nnc_stream_context_t* const sc) { return (cudaStream_t)ccv_nnc_stream_context_get_stream(sc); }
-inline int kind_of(const ccv_nnc_tensor_t* const t)
-{
-	switch (CCV_GET_DATA_TYPE(t->info.datatype))
-	{
-		case CCV_32F: return 0;
-		case CCV_16BF: return 1;
-		case CCV_16F: return 2;
-	}
-	return -1;
-}
-int nd_of(const ccv_nnc_tensor_t* const t)
-{
-	int i;
-	for (i = 0; i < CCV_NNC_MAX_DIM_ALLOC && t->info.dim[i] > 0; i++) {}
-	return i;
-}
-size_t count_of(const ccv_nnc_tensor_t* const t)
-{
-	size_t n = 1;
-	for (int i = 0; i < CCV_NNC_MAX_DIM_ALLOC && t->info.dim[i] > 0; i++)
-		n *= (size_t)t->info.dim[i];
-	return n;
-}
-bool same_dims(const ccv_nnc_tensor_t* const a, const ccv_nnc_tensor_t* const b)
-{
-	for (int i = 0; i < CCV_NNC_MAX_DIM_ALLOC; i++)
-	{
-		if (a->info.dim[i] != b->info.dim[i])
-			return false;
-		if (a->info.dim[i] == 0)
-			break;
-	}
-	return true;
-}
 // right-aligned 4-d shape and strides (ccv_nnc_tensor_view_get_dim / _get_stride); false when the tensor has more than 4 axes
 bool dims4(const ccv_nnc_tensor_t* const t, int dim[4], int stride[4])
 {
@@ -182,8 +114,8 @@ int run_ew_t(cudaStream_t s, const void* x, const void* y, const void* z, void* 
 	if (n == 0)
 		return 0;
 	const int vec = aligned_v16((const T*)out) && (!x || aligned_v16((const T*)x)) && (!y || aligned_v16((const T*)y)) && (!z || aligned_v16((const T*)z));
-	ew_kernel<T, OP><<<grid_for(vec ? n / Vec16<T>::W + 1 : n, 256), 256, 0, s>>>((const T*)x, (const T*)y, (const T*)z, (T*)out, n, vec, k);
-	return check("element-wise");
+	ew_kernel<T, OP><<<grid_for(vec ? n / Vec16<T>::W + 1 : n, 256, 8), 256, 0, s>>>((const T*)x, (const T*)y, (const T*)z, (T*)out, n, vec, k);
+	return launched("element-wise");
 }
 template <int OP>
 int run_ew(cudaStream_t s, const int kind, const void* x, const void* y, const void* z, void* out, const size_t n, const EwArg& k)
@@ -366,10 +298,10 @@ template <typename T, int MODE>
 int run_reduce_t(cudaStream_t s, const void* a, void* b, const Red4& r, const size_t outputs, const float scale)
 {
 	if (r.rcount <= 64)
-		reduce_kernel<T, MODE, 32><<<grid_for(outputs * 32, 256), 256, 0, s>>>((const T*)a, (T*)b, r, outputs, scale);
+		reduce_kernel<T, MODE, 32><<<grid_for(outputs * 32, 256, 8), 256, 0, s>>>((const T*)a, (T*)b, r, outputs, scale);
 	else
-		reduce_kernel<T, MODE, 256><<<(int)(outputs < (size_t)sms() * 8 ? outputs : (size_t)sms() * 8), 256, 0, s>>>((const T*)a, (T*)b, r, outputs, scale);
-	return check("reduce");
+		reduce_kernel<T, MODE, 256><<<(int)(outputs < (size_t)sm_count() * 8 ? outputs : (size_t)sm_count() * 8), 256, 0, s>>>((const T*)a, (T*)b, r, outputs, scale);
+	return launched("reduce");
 }
 // does `small` broadcast onto `big` (every axis equal or 1)?
 bool broadcast_onto(const int small[4], const int big[4])
@@ -460,7 +392,7 @@ int exec_reduce_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const i
 		}
 	}
 	cudaStream_t s = stream_of(stream_context);
-	const int grid = grid_for(n, 256);
+	const int grid = grid_for(n, 256, 8);
 #define LAUNCH_RB(T) reduce_back_kernel<T, MODE><<<grid, 256, 0, s>>>(g ? (const T*)g->data.u8 : 0, a ? (const T*)a->data.u8 : 0, b ? (const T*)b->data.u8 : 0, (T*)h->data.u8, hd[1], hd[2], hd[3], n, \
 		hs[0], hs[1], hs[2], hs[3], as[0], as[1], as[2], as[3], gs[0], gs[1], gs[2], gs[3], bs[0], bs[1], bs[2], bs[3], scale)
 	if (kind == 0)
@@ -470,7 +402,7 @@ int exec_reduce_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const i
 	else
 		LAUNCH_RB(__half);
 #undef LAUNCH_RB
-	return check("reduce backward") ? CCV_NNC_EXEC_INVALID : CCV_NNC_EXEC_SUCCESS;
+	return launched("reduce backward") ? CCV_NNC_EXEC_INVALID : CCV_NNC_EXEC_SUCCESS;
 }
 
 // ------------------------------------------------------------------------------------------------ masked fill
@@ -508,7 +440,7 @@ int masked_fill(cudaStream_t s, const float p, const float q, const ccv_nnc_tens
 	const size_t n = (size_t)cd[0] * cd[1] * cd[2] * cd[3];
 	if (n == 0)
 		return CCV_NNC_EXEC_SUCCESS;
-	const int grid = grid_for(n, 256);
+	const int grid = grid_for(n, 256, 8);
 #define LAUNCH_MF(T, M, pv) masked_fill_kernel<T, M><<<grid, 256, 0, s>>>((const T*)a->data.u8, (const M*)mask->data.u8, (T*)c->data.u8, cd[1], cd[2], cd[3], n, \
 		as[0], as[1], as[2], as[3], ms[0], ms[1], ms[2], ms[3], cs[0], cs[1], cs[2], cs[3], pv, q)
 	if (mtype == CCV_32S)
@@ -519,7 +451,7 @@ int masked_fill(cudaStream_t s, const float p, const float q, const ccv_nnc_tens
 		if (kind == 0) LAUNCH_MF(float, float, p); else if (kind == 1) LAUNCH_MF(__nv_bfloat16, float, p); else LAUNCH_MF(__half, float, p);
 	}
 #undef LAUNCH_MF
-	return check("masked fill") ? CCV_NNC_EXEC_INVALID : CCV_NNC_EXEC_SUCCESS;
+	return launched("masked fill") ? CCV_NNC_EXEC_INVALID : CCV_NNC_EXEC_SUCCESS;
 }
 int exec_masked_fill_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
 {
@@ -610,7 +542,7 @@ int exec_random(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int fl
 		return CCV_NNC_EXEC_SUCCESS;
 	const uint32_t seed = ccv_nnc_stream_context_genrand_uint32(stream_context);
 	cudaStream_t s = stream_of(stream_context);
-	const int grid = grid_for((n + 3) / 4, 256);
+	const int grid = grid_for((n + 3) / 4, 256, 8);
 	const float p0 = cmd.info.blas.a[0], p1 = cmd.info.blas.a[1];
 	if (kind == 0)
 		random_kernel<float, NORMAL><<<grid, 256, 0, s>>>((float*)a->data.u8, n, seed, p0, p1);
@@ -618,7 +550,7 @@ int exec_random(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int fl
 		random_kernel<__nv_bfloat16, NORMAL><<<grid, 256, 0, s>>>((__nv_bfloat16*)a->data.u8, n, seed, p0, p1);
 	else
 		random_kernel<__half, NORMAL><<<grid, 256, 0, s>>>((__half*)a->data.u8, n, seed, p0, p1);
-	return check("random fill") ? CCV_NNC_EXEC_INVALID : CCV_NNC_EXEC_SUCCESS;
+	return launched("random fill") ? CCV_NNC_EXEC_INVALID : CCV_NNC_EXEC_SUCCESS;
 }
 
 // ------------------------------------------------------------------------------------------------ dropout
@@ -687,7 +619,7 @@ int exec_dropout_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const 
 	const float p = cmd.info.dropout.p, inv_p = 1. / (1. - p); // in double, rounded once (dropout/ccv_nnc_dropout_cpu_ref.c:20)
 	const uint32_t seed = ccv_nnc_stream_context_genrand_uint32(stream_context);
 	cudaStream_t s = stream_of(stream_context);
-	const int grid = grid_for(entirety ? n : (n + 3) / 4, 256);
+	const int grid = grid_for(entirety ? n : (n + 3) / 4, 256, 8);
 	uint8_t* const mask = outputs[1]->data.u8;
 	if (kind == 0)
 		dropout_fwd_kernel<float><<<grid, 256, 0, s>>>((const float*)inputs[0]->data.u8, (float*)outputs[0]->data.u8, mask, n, seed, p, inv_p, entirety);
@@ -695,7 +627,7 @@ int exec_dropout_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const 
 		dropout_fwd_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>((const __nv_bfloat16*)inputs[0]->data.u8, (__nv_bfloat16*)outputs[0]->data.u8, mask, n, seed, p, inv_p, entirety);
 	else
 		dropout_fwd_kernel<__half><<<grid, 256, 0, s>>>((const __half*)inputs[0]->data.u8, (__half*)outputs[0]->data.u8, mask, n, seed, p, inv_p, entirety);
-	return check("dropout") ? CCV_NNC_EXEC_INVALID : CCV_NNC_EXEC_SUCCESS;
+	return launched("dropout") ? CCV_NNC_EXEC_INVALID : CCV_NNC_EXEC_SUCCESS;
 }
 int exec_dropout_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
 {
@@ -711,7 +643,7 @@ int exec_dropout_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const 
 		return CCV_NNC_EXEC_SUCCESS;
 	const float inv_p = 1. / (1. - cmd.info.dropout.p); // in double, rounded once (dropout/ccv_nnc_dropout_cpu_ref.c:153)
 	cudaStream_t s = stream_of(stream_context);
-	const int grid = grid_for(n, 256);
+	const int grid = grid_for(n, 256, 8);
 	const uint8_t* const mask = inputs[4]->data.u8;
 	if (kind == 0)
 		dropout_bwd_kernel<float><<<grid, 256, 0, s>>>((const float*)inputs[0]->data.u8, mask, (float*)outputs[0]->data.u8, n, inv_p, entirety);
@@ -719,7 +651,7 @@ int exec_dropout_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const 
 		dropout_bwd_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>((const __nv_bfloat16*)inputs[0]->data.u8, mask, (__nv_bfloat16*)outputs[0]->data.u8, n, inv_p, entirety);
 	else
 		dropout_bwd_kernel<__half><<<grid, 256, 0, s>>>((const __half*)inputs[0]->data.u8, mask, (__half*)outputs[0]->data.u8, n, inv_p, entirety);
-	return check("dropout backward") ? CCV_NNC_EXEC_INVALID : CCV_NNC_EXEC_SUCCESS;
+	return launched("dropout backward") ? CCV_NNC_EXEC_INVALID : CCV_NNC_EXEC_SUCCESS;
 }
 
 // ------------------------------------------------------------------------------------------------ complex multiplication
@@ -824,9 +756,9 @@ void launch_cmul(cudaStream_t s, const T* x, const T* y, T* out, const CmulArg& 
 {
 	// 32-bit index arithmetic whenever the grid-stride loop cannot overflow it
 	if (n < (1ull << 31))
-		cmul_kernel<T, CONJ, VEC, unsigned><<<grid_for(n, 256), 256, 0, s>>>(x, y, out, p, (unsigned)n, null_conj);
+		cmul_kernel<T, CONJ, VEC, unsigned><<<grid_for(n, 256, 8), 256, 0, s>>>(x, y, out, p, (unsigned)n, null_conj);
 	else
-		cmul_kernel<T, CONJ, VEC, size_t><<<grid_for(n, 256), 256, 0, s>>>(x, y, out, p, n, null_conj);
+		cmul_kernel<T, CONJ, VEC, size_t><<<grid_for(n, 256, 8), 256, 0, s>>>(x, y, out, p, n, null_conj);
 }
 // reduce = 0: cmul_kernel over p.d; 1: cmul_reduce_kernel onto p.d over the extents p.r
 template <typename T>
@@ -840,10 +772,10 @@ int run_cmul_t(cudaStream_t s, const int conj, const int reduce, const void* xp,
 	{
 		const size_t n = rows * (p.d[3] / 2);
 		if (n < (1ull << 31))
-			cmul_reduce_kernel<T, unsigned><<<grid_for(n, 256), 256, 0, s>>>(x, y, out, p, (unsigned)n);
+			cmul_reduce_kernel<T, unsigned><<<grid_for(n, 256, 8), 256, 0, s>>>(x, y, out, p, (unsigned)n);
 		else
-			cmul_reduce_kernel<T, size_t><<<grid_for(n, 256), 256, 0, s>>>(x, y, out, p, n);
-		return check("cmul reduce");
+			cmul_reduce_kernel<T, size_t><<<grid_for(n, 256, 8), 256, 0, s>>>(x, y, out, p, n);
+		return launched("cmul reduce");
 	}
 	constexpr int W = Vec16<T>::W;
 	bool vec = p.d[3] % W == 0 && aligned_v16(y) && aligned_v16(out) && (!x || aligned_v16(x));
@@ -854,7 +786,7 @@ int run_cmul_t(cudaStream_t s, const int conj, const int reduce, const void* xp,
 		conj ? launch_cmul<T, 1, true>(s, x, y, out, p, n, null_conj) : launch_cmul<T, 0, true>(s, x, y, out, p, n, null_conj);
 	else
 		conj ? launch_cmul<T, 1, false>(s, x, y, out, p, n, null_conj) : launch_cmul<T, 0, false>(s, x, y, out, p, n, null_conj);
-	return check("cmul");
+	return launched("cmul");
 }
 int run_cmul(cudaStream_t s, const int kind, const int conj, const int reduce, const void* x, const void* y, void* out, const CmulArg& p, const int null_conj)
 {
@@ -997,7 +929,6 @@ bool packed4(const int d[4], const int s[4])
 // refuse anything but a plain int32 tensor (palettized int32 included)
 bool is_i32(const ccv_nnc_tensor_t* const t) { return t && t->info.datatype == CCV_32S; }
 bool is_kind(const ccv_nnc_tensor_t* const t, const int kind) { return t && kind_of(t) == kind && t->info.datatype == (kind == 0 ? CCV_32F : kind == 1 ? CCV_16BF : CCV_16F); }
-int elem_size(const int kind) { return kind == 0 ? 4 : 2; }
 
 // PAD forward (pad/ccv_nnc_pad_cpu_ref.c:13-84): output-stationary; each output element reads a at i - begin (zero outside a) or at
 // min(adim - 1, max(0, i - begin)) (replicate).  VEC: the innermost axis is not padded and every row is whole aligned 16-byte vectors,
@@ -1043,9 +974,9 @@ void launch_pad(cudaStream_t s, const void* a, void* b, const PadArg& p)
 {
 	const size_t n = (size_t)p.d[0] * p.d[1] * p.d[2] * p.d[3];
 	if (n < (1ull << 31))
-		pad_kernel<R, VEC, unsigned><<<grid_for(n, 256), 256, 0, s>>>((const R*)a, (R*)b, p, (unsigned)n);
+		pad_kernel<R, VEC, unsigned><<<grid_for(n, 256, 8), 256, 0, s>>>((const R*)a, (R*)b, p, (unsigned)n);
 	else
-		pad_kernel<R, VEC, size_t><<<grid_for(n, 256), 256, 0, s>>>((const R*)a, (R*)b, p, n);
+		pad_kernel<R, VEC, size_t><<<grid_for(n, 256, 8), 256, 0, s>>>((const R*)a, (R*)b, p, n);
 }
 // begin / end of the command, right-aligned onto 4 axes as CPU_REF does; false when one is negative
 bool pad_sides(const ccv_nnc_cmd_t& cmd, const int nd, int begin[4], int end[4])
@@ -1097,7 +1028,7 @@ int exec_pad_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int 
 		kind == 0 ? launch_pad<uint32_t, true>(s, a->data.u8, b->data.u8, p) : launch_pad<uint16_t, true>(s, a->data.u8, b->data.u8, p);
 	} else
 		kind == 0 ? launch_pad<uint32_t, false>(s, a->data.u8, b->data.u8, p) : launch_pad<uint16_t, false>(s, a->data.u8, b->data.u8, p);
-	return check("pad") ? CCV_NNC_EXEC_INVALID : CCV_NNC_EXEC_SUCCESS;
+	return launched("pad") ? CCV_NNC_EXEC_INVALID : CCV_NNC_EXEC_SUCCESS;
 }
 // inputs (g) -> outputs (h): h = g[begin : begin + hdim] for both pad types (pad_cpu_ref.c:87-137: the replicated border is not
 // accumulated into the edge, so this is not the true gradient of replicate padding).  One strided copy.
@@ -1234,9 +1165,9 @@ int run_cmp(cudaStream_t s, const int bwd, const void* const* ptr, const CmpArg&
 	const size_t n = v ? count / W : count;
 #define LAUNCH_CMP(V, I) do { \
 		if (bwd) \
-			cmp_bwd_kernel<T, MIN, V, I><<<grid_for(n, 256), 256, 0, s>>>((const R*)ptr[0], (const R*)ptr[1], (const R*)ptr[2], (R*)ptr[3], (R*)ptr[4], p, (I)n); \
+			cmp_bwd_kernel<T, MIN, V, I><<<grid_for(n, 256, 8), 256, 0, s>>>((const R*)ptr[0], (const R*)ptr[1], (const R*)ptr[2], (R*)ptr[3], (R*)ptr[4], p, (I)n); \
 		else \
-			cmp_fwd_kernel<T, MIN, V, I><<<grid_for(n, 256), 256, 0, s>>>((const R*)ptr[0], (const R*)ptr[1], (R*)ptr[2], p, (I)n); \
+			cmp_fwd_kernel<T, MIN, V, I><<<grid_for(n, 256, 8), 256, 0, s>>>((const R*)ptr[0], (const R*)ptr[1], (R*)ptr[2], p, (I)n); \
 	} while (0)
 	if (v)
 		LAUNCH_CMP(true, size_t);
@@ -1245,7 +1176,7 @@ int run_cmp(cudaStream_t s, const int bwd, const void* const* ptr, const CmpArg&
 	else
 		LAUNCH_CMP(false, size_t);
 #undef LAUNCH_CMP
-	return check(bwd ? "min / max backward" : "min / max");
+	return launched(bwd ? "min / max backward" : "min / max");
 }
 template <int MIN>
 int run_cmp_kind(cudaStream_t s, const int kind, const int bwd, const void* const* ptr, const CmpArg& p, const bool vec)
@@ -1416,14 +1347,14 @@ int run_arg(cudaStream_t s, const void* a, void* b, const size_t before, const i
 		constexpr int W = 16 / sizeof(typename Bits<T>::R);
 		const int vec = axis % W == 0 && aligned_v16((const T*)a);
 		if (axis <= 2048)
-			argrow_kernel<T, MIN, O, 32><<<grid_for(before * 32, 256), 256, 0, s>>>((const T*)a, (O*)b, before, axis, vec);
+			argrow_kernel<T, MIN, O, 32><<<grid_for(before * 32, 256, 8), 256, 0, s>>>((const T*)a, (O*)b, before, axis, vec);
 		else
-			argrow_kernel<T, MIN, O, 256><<<(int)(before < (size_t)sms() * 8 ? before : (size_t)sms() * 8), 256, 0, s>>>((const T*)a, (O*)b, before, axis, vec);
+			argrow_kernel<T, MIN, O, 256><<<(int)(before < (size_t)sm_count() * 8 ? before : (size_t)sm_count() * 8), 256, 0, s>>>((const T*)a, (O*)b, before, axis, vec);
 	} else {
 		const size_t work = before * ((after + 31) / 32);
-		argcol_kernel<T, MIN, O><<<(int)(work < (size_t)sms() * 8 ? work : (size_t)sms() * 8), 256, 0, s>>>((const T*)a, (O*)b, before, axis, after);
+		argcol_kernel<T, MIN, O><<<(int)(work < (size_t)sm_count() * 8 ? work : (size_t)sm_count() * 8), 256, 0, s>>>((const T*)a, (O*)b, before, axis, after);
 	}
-	return check("argmax / argmin");
+	return launched("argmax / argmin");
 }
 // inputs (a) -> outputs (b: int32, or fp32 holding the index); cmd.info.reduce.axis[0], reduce.count == 1; a contiguous
 template <int MIN>
@@ -1468,12 +1399,6 @@ int exec_arg_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int 
 #undef RUN_ARG
 	return rc ? CCV_NNC_EXEC_INVALID : CCV_NNC_EXEC_SUCCESS;
 }
-// ARGMAX / ARGMIN / REDUCE_ISNAN backward: the reference registers it and returns INVALID
-int exec_invalid(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
-{
-	return CCV_NNC_EXEC_INVALID;
-}
-
 // REDUCE_ISNAN (isnan/ccv_nnc_reduce_isnan_cpu_ref.c:16-64): b (int32, broadcast onto a; its unit axes are the reduced ones) is
 // zeroed, then set to 1 wherever an element mapping to it is NaN.  Two launches: the zero fill, then one read of a in which a thread
 // that meets a NaN stores 1 into its b slot.  Every such store writes the same value, so their order does not matter.
@@ -1533,11 +1458,11 @@ void launch_isnan(cudaStream_t s, const void* a, int* b, const NanArg& p, const 
 	constexpr int W = 16 / sizeof(typename Bits<T>::R);
 	const size_t n = vec ? count / W : count;
 	if (vec)
-		isnan_kernel<T, true, size_t><<<grid_for(n, 256), 256, 0, s>>>((const T*)a, b, p, n);
+		isnan_kernel<T, true, size_t><<<grid_for(n, 256, 8), 256, 0, s>>>((const T*)a, b, p, n);
 	else if (n < (1ull << 31))
-		isnan_kernel<T, false, unsigned><<<grid_for(n, 256), 256, 0, s>>>((const T*)a, b, p, (unsigned)n);
+		isnan_kernel<T, false, unsigned><<<grid_for(n, 256, 8), 256, 0, s>>>((const T*)a, b, p, (unsigned)n);
 	else
-		isnan_kernel<T, false, size_t><<<grid_for(n, 256), 256, 0, s>>>((const T*)a, b, p, n);
+		isnan_kernel<T, false, size_t><<<grid_for(n, 256, 8), 256, 0, s>>>((const T*)a, b, p, n);
 }
 // inputs (a) -> outputs (b)
 int exec_isnan_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
@@ -1561,8 +1486,8 @@ int exec_isnan_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const in
 	if (bcount == 0)
 		return CCV_NNC_EXEC_SUCCESS;
 	cudaStream_t s = stream_of(stream_context);
-	fill_i32_kernel<<<grid_for(bcount, 256), 256, 0, s>>>(b->data.i32, z, bcount, packed4(bd, bs));
-	if (check("reduce isnan (zero)"))
+	fill_i32_kernel<<<grid_for(bcount, 256, 8), 256, 0, s>>>(b->data.i32, z, bcount, packed4(bd, bs));
+	if (launched("reduce isnan (zero)"))
 		return CCV_NNC_EXEC_INVALID;
 	if (count == 0)
 		return CCV_NNC_EXEC_SUCCESS;
@@ -1574,69 +1499,58 @@ int exec_isnan_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const in
 		launch_isnan<__nv_bfloat16>(s, a->data.u8, b->data.i32, p, count, vec);
 	else
 		launch_isnan<__half>(s, a->data.u8, b->data.i32, p, count, vec);
-	return check("reduce isnan") ? CCV_NNC_EXEC_INVALID : CCV_NNC_EXEC_SUCCESS;
-}
-
-void fill(ccv_nnc_cmd_backend_registry_t* const registry, const int datatypes, const ccv_nnc_cmd_exec_f exec)
-{
-	registry->tensor_formats = CCV_TENSOR_FORMAT_NCHW | CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_CHWN;
-	registry->tensor_datatypes = datatypes;
-	registry->tensor_memory = CCV_TENSOR_GPU_MEMORY;
-	registry->algorithms = 1;
-	registry->exec = exec;
-	registry->autotune = 0;
-	registry->aux = 0;
+	return launched("reduce isnan") ? CCV_NNC_EXEC_INVALID : CCV_NNC_EXEC_SUCCESS;
 }
 
 } // namespace
 
 #define F3 (CCV_32F | CCV_16F | CCV_16BF)
-#define REGISTER_SM100(cmd) extern "C" void _register_command_ ## cmd ## _backend_CCV_NNC_BACKEND_GPU_SM100(ccv_nnc_cmd_backend_registry_t* const registry)
-REGISTER_SM100(CCV_NNC_SIGMOID_FORWARD) { fill(registry, F3, exec_unary_forw<OP_SIGMOID>); }
-REGISTER_SM100(CCV_NNC_SIGMOID_BACKWARD) { fill(registry, F3, exec_unary_back<OP_SIGMOID_B, 2>); }
-REGISTER_SM100(CCV_NNC_TANH_FORWARD) { fill(registry, F3, exec_unary_forw<OP_TANH>); }
-REGISTER_SM100(CCV_NNC_TANH_BACKWARD) { fill(registry, F3, exec_unary_back<OP_TANH_B, 2>); }
-REGISTER_SM100(CCV_NNC_LEAKY_RELU_FORWARD) { fill(registry, F3, exec_unary_forw<OP_LEAKY>); }
-REGISTER_SM100(CCV_NNC_LEAKY_RELU_BACKWARD) { fill(registry, F3, exec_unary_back<OP_LEAKY_B, 2>); }
-REGISTER_SM100(CCV_NNC_EWEXP_FORWARD) { fill(registry, F3, exec_unary_forw<OP_EXP>); }
-REGISTER_SM100(CCV_NNC_EWEXP_BACKWARD) { fill(registry, F3, exec_unary_back<OP_EXP_B, 2>); }
-REGISTER_SM100(CCV_NNC_EWLOG_FORWARD) { fill(registry, F3, exec_unary_forw<OP_LOG>); }
-REGISTER_SM100(CCV_NNC_EWLOG_BACKWARD) { fill(registry, F3, exec_unary_back<OP_LOG_B, 1>); }
-REGISTER_SM100(CCV_NNC_EWSQRT_FORWARD) { fill(registry, F3, exec_unary_forw<OP_SQRT>); }
-REGISTER_SM100(CCV_NNC_EWSQRT_BACKWARD) { fill(registry, F3, exec_unary_back<OP_SQRT_B, 2>); }
-REGISTER_SM100(CCV_NNC_CLAMP_FORWARD) { fill(registry, F3, exec_unary_forw<OP_CLAMP>); }
-REGISTER_SM100(CCV_NNC_CLAMP_BACKWARD) { fill(registry, F3, exec_unary_back<OP_CLAMP_B, 2>); }
-REGISTER_SM100(CCV_NNC_EWDIV_FORWARD) { fill(registry, F3, exec_ewdiv_forw); }
-REGISTER_SM100(CCV_NNC_EWDIV_BACKWARD) { fill(registry, F3, exec_ewdiv_back); }
-REGISTER_SM100(CCV_NNC_REDUCE_SUM_FORWARD) { fill(registry, F3, exec_reduce_forw<RED_SUM>); }
-REGISTER_SM100(CCV_NNC_REDUCE_SUM_BACKWARD) { fill(registry, F3, exec_reduce_back<RED_SUM>); }
-REGISTER_SM100(CCV_NNC_REDUCE_MEAN_FORWARD) { fill(registry, F3, exec_reduce_forw<RED_MEAN>); }
-REGISTER_SM100(CCV_NNC_REDUCE_MEAN_BACKWARD) { fill(registry, F3, exec_reduce_back<RED_MEAN>); }
-REGISTER_SM100(CCV_NNC_REDUCE_MAX_FORWARD) { fill(registry, F3, exec_reduce_forw<RED_MAX>); }
-REGISTER_SM100(CCV_NNC_REDUCE_MAX_BACKWARD) { fill(registry, F3, exec_reduce_back<RED_MAX>); }
-REGISTER_SM100(CCV_NNC_REDUCE_MIN_FORWARD) { fill(registry, F3, exec_reduce_forw<RED_MIN>); }
-REGISTER_SM100(CCV_NNC_REDUCE_MIN_BACKWARD) { fill(registry, F3, exec_reduce_back<RED_MIN>); }
-REGISTER_SM100(CCV_NNC_REDUCE_NORM2_FORWARD) { fill(registry, F3, exec_reduce_forw<RED_NORM2>); }
-REGISTER_SM100(CCV_NNC_REDUCE_NORM2_BACKWARD) { fill(registry, F3, exec_reduce_back<RED_NORM2>); }
-REGISTER_SM100(CCV_NNC_MASKED_FILL_FORWARD) { fill(registry, F3 | CCV_32S, exec_masked_fill_forw); }
-REGISTER_SM100(CCV_NNC_MASKED_FILL_BACKWARD) { fill(registry, F3 | CCV_32S, exec_masked_fill_back); }
-REGISTER_SM100(CCV_NNC_RANDOM_UNIFORM_FORWARD) { fill(registry, F3, exec_random<0>); }
-REGISTER_SM100(CCV_NNC_RANDOM_UNIFORM_BACKWARD) { fill(registry, F3, exec_random<0>); }
-REGISTER_SM100(CCV_NNC_RANDOM_NORMAL_FORWARD) { fill(registry, F3, exec_random<1>); }
-REGISTER_SM100(CCV_NNC_RANDOM_NORMAL_BACKWARD) { fill(registry, F3, exec_random<1>); }
-REGISTER_SM100(CCV_NNC_DROPOUT_FORWARD) { fill(registry, F3, exec_dropout_forw); }
-REGISTER_SM100(CCV_NNC_DROPOUT_BACKWARD) { fill(registry, F3, exec_dropout_back); }
-REGISTER_SM100(CCV_NNC_CMUL_FORWARD) { fill(registry, F3, exec_cmul_forw); }
-REGISTER_SM100(CCV_NNC_CMUL_BACKWARD) { fill(registry, F3, exec_cmul_back); }
-REGISTER_SM100(CCV_NNC_PAD_FORWARD) { fill(registry, F3, exec_pad_forw); }
-REGISTER_SM100(CCV_NNC_PAD_BACKWARD) { fill(registry, F3, exec_pad_back); }
-REGISTER_SM100(CCV_NNC_MIN_FORWARD) { fill(registry, F3, exec_cmp_forw<1>); }
-REGISTER_SM100(CCV_NNC_MIN_BACKWARD) { fill(registry, F3, exec_cmp_back<1>); }
-REGISTER_SM100(CCV_NNC_MAX_FORWARD) { fill(registry, F3, exec_cmp_forw<0>); }
-REGISTER_SM100(CCV_NNC_MAX_BACKWARD) { fill(registry, F3, exec_cmp_back<0>); }
-REGISTER_SM100(CCV_NNC_ARGMAX_FORWARD) { fill(registry, F3 | CCV_32S, exec_arg_forw<0>); }
-REGISTER_SM100(CCV_NNC_ARGMAX_BACKWARD) { fill(registry, F3 | CCV_32S, exec_invalid); }
-REGISTER_SM100(CCV_NNC_ARGMIN_FORWARD) { fill(registry, F3 | CCV_32S, exec_arg_forw<1>); }
-REGISTER_SM100(CCV_NNC_ARGMIN_BACKWARD) { fill(registry, F3 | CCV_32S, exec_invalid); }
-REGISTER_SM100(CCV_NNC_REDUCE_ISNAN_FORWARD) { fill(registry, F3 | CCV_32S, exec_isnan_forw); }
-REGISTER_SM100(CCV_NNC_REDUCE_ISNAN_BACKWARD) { fill(registry, F3 | CCV_32S, exec_invalid); }
+REGISTER_SM100(CCV_NNC_SIGMOID_FORWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_unary_forw<OP_SIGMOID>); }
+REGISTER_SM100(CCV_NNC_SIGMOID_BACKWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_unary_back<OP_SIGMOID_B, 2>); }
+REGISTER_SM100(CCV_NNC_TANH_FORWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_unary_forw<OP_TANH>); }
+REGISTER_SM100(CCV_NNC_TANH_BACKWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_unary_back<OP_TANH_B, 2>); }
+REGISTER_SM100(CCV_NNC_LEAKY_RELU_FORWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_unary_forw<OP_LEAKY>); }
+REGISTER_SM100(CCV_NNC_LEAKY_RELU_BACKWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_unary_back<OP_LEAKY_B, 2>); }
+REGISTER_SM100(CCV_NNC_EWEXP_FORWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_unary_forw<OP_EXP>); }
+REGISTER_SM100(CCV_NNC_EWEXP_BACKWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_unary_back<OP_EXP_B, 2>); }
+REGISTER_SM100(CCV_NNC_EWLOG_FORWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_unary_forw<OP_LOG>); }
+REGISTER_SM100(CCV_NNC_EWLOG_BACKWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_unary_back<OP_LOG_B, 1>); }
+REGISTER_SM100(CCV_NNC_EWSQRT_FORWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_unary_forw<OP_SQRT>); }
+REGISTER_SM100(CCV_NNC_EWSQRT_BACKWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_unary_back<OP_SQRT_B, 2>); }
+REGISTER_SM100(CCV_NNC_CLAMP_FORWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_unary_forw<OP_CLAMP>); }
+REGISTER_SM100(CCV_NNC_CLAMP_BACKWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_unary_back<OP_CLAMP_B, 2>); }
+REGISTER_SM100(CCV_NNC_EWDIV_FORWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_ewdiv_forw); }
+REGISTER_SM100(CCV_NNC_EWDIV_BACKWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_ewdiv_back); }
+REGISTER_SM100(CCV_NNC_REDUCE_SUM_FORWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_reduce_forw<RED_SUM>); }
+REGISTER_SM100(CCV_NNC_REDUCE_SUM_BACKWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_reduce_back<RED_SUM>); }
+REGISTER_SM100(CCV_NNC_REDUCE_MEAN_FORWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_reduce_forw<RED_MEAN>); }
+REGISTER_SM100(CCV_NNC_REDUCE_MEAN_BACKWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_reduce_back<RED_MEAN>); }
+REGISTER_SM100(CCV_NNC_REDUCE_MAX_FORWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_reduce_forw<RED_MAX>); }
+REGISTER_SM100(CCV_NNC_REDUCE_MAX_BACKWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_reduce_back<RED_MAX>); }
+REGISTER_SM100(CCV_NNC_REDUCE_MIN_FORWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_reduce_forw<RED_MIN>); }
+REGISTER_SM100(CCV_NNC_REDUCE_MIN_BACKWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_reduce_back<RED_MIN>); }
+REGISTER_SM100(CCV_NNC_REDUCE_NORM2_FORWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_reduce_forw<RED_NORM2>); }
+REGISTER_SM100(CCV_NNC_REDUCE_NORM2_BACKWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_reduce_back<RED_NORM2>); }
+REGISTER_SM100(CCV_NNC_MASKED_FILL_FORWARD) { fill(registry, ALL_FORMATS, F3 | CCV_32S, 1, exec_masked_fill_forw); }
+REGISTER_SM100(CCV_NNC_MASKED_FILL_BACKWARD) { fill(registry, ALL_FORMATS, F3 | CCV_32S, 1, exec_masked_fill_back); }
+REGISTER_SM100(CCV_NNC_RANDOM_UNIFORM_FORWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_random<0>); }
+REGISTER_SM100(CCV_NNC_RANDOM_UNIFORM_BACKWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_random<0>); }
+REGISTER_SM100(CCV_NNC_RANDOM_NORMAL_FORWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_random<1>); }
+REGISTER_SM100(CCV_NNC_RANDOM_NORMAL_BACKWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_random<1>); }
+REGISTER_SM100(CCV_NNC_DROPOUT_FORWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_dropout_forw); }
+REGISTER_SM100(CCV_NNC_DROPOUT_BACKWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_dropout_back); }
+REGISTER_SM100(CCV_NNC_CMUL_FORWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_cmul_forw); }
+REGISTER_SM100(CCV_NNC_CMUL_BACKWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_cmul_back); }
+REGISTER_SM100(CCV_NNC_PAD_FORWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_pad_forw); }
+REGISTER_SM100(CCV_NNC_PAD_BACKWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_pad_back); }
+REGISTER_SM100(CCV_NNC_MIN_FORWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_cmp_forw<1>); }
+REGISTER_SM100(CCV_NNC_MIN_BACKWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_cmp_back<1>); }
+REGISTER_SM100(CCV_NNC_MAX_FORWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_cmp_forw<0>); }
+REGISTER_SM100(CCV_NNC_MAX_BACKWARD) { fill(registry, ALL_FORMATS, F3, 1, exec_cmp_back<0>); }
+REGISTER_SM100(CCV_NNC_ARGMAX_FORWARD) { fill(registry, ALL_FORMATS, F3 | CCV_32S, 1, exec_arg_forw<0>); }
+// ARGMAX / ARGMIN / REDUCE_ISNAN backward: the reference registers it and returns INVALID
+REGISTER_SM100(CCV_NNC_ARGMAX_BACKWARD) { fill(registry, ALL_FORMATS, F3 | CCV_32S, 1, exec_invalid); }
+REGISTER_SM100(CCV_NNC_ARGMIN_FORWARD) { fill(registry, ALL_FORMATS, F3 | CCV_32S, 1, exec_arg_forw<1>); }
+REGISTER_SM100(CCV_NNC_ARGMIN_BACKWARD) { fill(registry, ALL_FORMATS, F3 | CCV_32S, 1, exec_invalid); }
+REGISTER_SM100(CCV_NNC_REDUCE_ISNAN_FORWARD) { fill(registry, ALL_FORMATS, F3 | CCV_32S, 1, exec_isnan_forw); }
+REGISTER_SM100(CCV_NNC_REDUCE_ISNAN_BACKWARD) { fill(registry, ALL_FORMATS, F3 | CCV_32S, 1, exec_invalid); }

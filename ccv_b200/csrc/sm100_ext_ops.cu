@@ -8,8 +8,7 @@
 //                                          rows j0 and min(j0 + 1, rows - 1)); backward zeroes h and adds g rows in index order
 //   adam/ccv_nnc_adamw_cpu_ref.c:13-250    decoupled weight decay: b = a - rate decay a - (m' rate / (1 - beta1^t)) / (sqrt(v' / (1 - beta2^t)) + eps)
 //                                          (amsgrad: running maximum of the bias-corrected second moment)
-#include "../../include/ccv_nnc_sm100.h"
-#include "sm100_contract.h"
+#include "sm100_cmd.h"
 #include "sm100_elem.cuh"
 #include <cuda_runtime.h>
 #include <math.h>
@@ -21,68 +20,6 @@ int exec_via_f32_rt(ccv_nnc_cmd_exec_f f32, const ccv_nnc_cmd_t cmd, const ccv_n
 using namespace sm100;
 
 namespace {
-
-int g_sms = 0;
-int sms()
-{
-	if (!g_sms)
-	{
-		int dev = 0;
-		cudaGetDevice(&dev);
-		cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, dev);
-		if (g_sms <= 0)
-			g_sms = 132;
-	}
-	return g_sms;
-}
-int grid_for(size_t work, int threads)
-{
-	size_t blocks = (work + threads - 1) / threads;
-	const size_t cap = (size_t)sms() * 8;
-	if (blocks > cap)
-		blocks = cap;
-	return blocks < 1 ? 1 : (int)blocks;
-}
-int check(const char* what)
-{
-	count_launch();
-	const cudaError_t e = cudaGetLastError();
-	if (e != cudaSuccess)
-	{
-		set_last_error(what, e);
-		return -1;
-	}
-	return 0;
-}
-inline cudaStream_t stream_of(ccv_nnc_stream_context_t* const sc) { return (cudaStream_t)ccv_nnc_stream_context_get_stream(sc); }
-inline int kind_of(const ccv_nnc_tensor_t* const t)
-{
-	switch (CCV_GET_DATA_TYPE(t->info.datatype))
-	{
-		case CCV_32F: return 0;
-		case CCV_16BF: return 1;
-		case CCV_16F: return 2;
-	}
-	return -1;
-}
-size_t count_of(const ccv_nnc_tensor_t* const t)
-{
-	size_t n = 1;
-	for (int i = 0; i < CCV_NNC_MAX_DIM_ALLOC && t->info.dim[i] > 0; i++)
-		n *= (size_t)t->info.dim[i];
-	return n;
-}
-bool same_dims(const ccv_nnc_tensor_t* const a, const ccv_nnc_tensor_t* const b)
-{
-	for (int i = 0; i < CCV_NNC_MAX_DIM_ALLOC; i++)
-	{
-		if (a->info.dim[i] != b->info.dim[i])
-			return false;
-		if (a->info.dim[i] == 0)
-			break;
-	}
-	return true;
-}
 
 // ------------------------------------------------------------------------------------------------ activations
 // OP 0: gelu (erf), 1: gelu (tanh), 2: swish
@@ -140,12 +77,12 @@ int run_act(cudaStream_t s, const void* g, const void* a, void* out, size_t n)
 	if (n == 0)
 		return 0;
 	const int vec = aligned_v16((const T*)a) && aligned_v16((const T*)out) && (!g || aligned_v16((const T*)g));
-	const int grid = grid_for(vec ? n / Vec16<T>::W + 1 : n, 256);
+	const int grid = grid_for(vec ? n / Vec16<T>::W + 1 : n, 256, 8);
 	if (g)
 		act_kernel<T, OP, 1><<<grid, 256, 0, s>>>((const T*)g, (const T*)a, (T*)out, n, vec);
 	else
 		act_kernel<T, OP, 0><<<grid, 256, 0, s>>>((const T*)0, (const T*)a, (T*)out, n, vec);
-	return check("activation");
+	return launched("activation");
 }
 template <int OP>
 int run_act_kind(cudaStream_t s, int kind, const void* g, const void* a, void* out, size_t n)
@@ -268,7 +205,7 @@ int exec_index_select_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, c
 		index_select_lerp_kernel<<<b_rows, threads, 0, s>>>(inputs[0]->data.f32, idx->data.f32, outputs[0]->data.f32, a_rows, a_cols, a_inc, b_inc);
 	else
 		return CCV_NNC_EXEC_INVALID;
-	return check("index_select") ? CCV_NNC_EXEC_INVALID : CCV_NNC_EXEC_SUCCESS;
+	return launched("index_select") ? CCV_NNC_EXEC_INVALID : CCV_NNC_EXEC_SUCCESS;
 }
 // inputs (g, a, indices) -> outputs (h, [zeroed gradient of the indices])
 int exec_index_select_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
@@ -296,7 +233,7 @@ int exec_index_select_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, c
 		index_select_back_kernel<__nv_bfloat16><<<h_rows, threads, 0, s>>>((const __nv_bfloat16*)inputs[0]->data.u8, idx->data.i32, (__nv_bfloat16*)outputs[0]->data.u8, g_rows, g_cols, g_inc, h_inc);
 	else
 		index_select_back_kernel<__half><<<h_rows, threads, 0, s>>>((const __half*)inputs[0]->data.u8, idx->data.i32, (__half*)outputs[0]->data.u8, g_rows, g_cols, g_inc, h_inc);
-	return check("index_select_back") ? CCV_NNC_EXEC_INVALID : CCV_NNC_EXEC_SUCCESS;
+	return launched("index_select_back") ? CCV_NNC_EXEC_INVALID : CCV_NNC_EXEC_SUCCESS;
 }
 
 // ------------------------------------------------------------------------------------------------ AdamW
@@ -361,9 +298,9 @@ int exec_adam_f32(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int 
 	const float rate = cmd.info.adam.rate, beta1 = cmd.info.adam.beta1, beta2 = cmd.info.adam.beta2;
 	const float rate_inv_bias_correction1 = rate / (1 - powf(beta1, cmd.info.adam.step));
 	const float inv_bias_correction2 = 1. / (1 - powf(beta2, cmd.info.adam.step)); // the quotient in double, rounded once, as CPU_REF
-	adamw_kernel<L2><<<grid_for(count, 256), 256, 0, stream_of(stream_context)>>>(inputs[0]->data.u8, g_kind, inputs[1]->data.f32, inputs[2]->data.f32, inputs[3]->data.f32, ams ? vm->data.f32 : 0,
+	adamw_kernel<L2><<<grid_for(count, 256, 8), 256, 0, stream_of(stream_context)>>>(inputs[0]->data.u8, g_kind, inputs[1]->data.f32, inputs[2]->data.f32, inputs[3]->data.f32, ams ? vm->data.f32 : 0,
 		outputs[0]->data.f32, outputs[1]->data.f32, outputs[2]->data.f32, ams ? um->data.f32 : 0, count, cmd.info.adam.scale, beta1, beta2, rate_inv_bias_correction1, inv_bias_correction2, L2 ? cmd.info.adam.decay : rate * cmd.info.adam.decay, cmd.info.adam.epsilon);
-	return check("adamw") ? CCV_NNC_EXEC_INVALID : CCV_NNC_EXEC_SUCCESS;
+	return launched("adamw") ? CCV_NNC_EXEC_INVALID : CCV_NNC_EXEC_SUCCESS;
 }
 // parameters / moments in half precision (adam/gpu/ccv_nnc_adamw_gpu_ref.cu registers CCV_16F; test/int/nnc/adam.tests.c:300-360): functional form
 template <int L2>
@@ -373,35 +310,17 @@ int exec_adam_any(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int 
 		return exec_via_f32_rt(exec_adam_f32<L2>, cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
 	return exec_adam_f32<L2>(cmd, hint, flags, inputs, input_size, outputs, output_size, stream_context);
 }
-void fill(ccv_nnc_cmd_backend_registry_t* const registry, const int datatypes, const ccv_nnc_cmd_exec_f exec)
-{
-	registry->tensor_formats = CCV_TENSOR_FORMAT_NCHW | CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_CHWN;
-	registry->tensor_datatypes = datatypes;
-	registry->tensor_memory = CCV_TENSOR_GPU_MEMORY;
-	registry->algorithms = 1;
-	registry->exec = exec;
-	registry->autotune = 0;
-	registry->aux = 0;
-}
 
 } // namespace
 
-namespace sm100 {
-// an optimizer has no backward (adam/ccv_nnc_adamw_cpu_ref.c: _ccv_nnc_adamw_back); also LAMB's and RMSPROP's (sm100_optim.cu)
-int exec_no_backward(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
-{
-	return CCV_NNC_EXEC_INVALID;
-}
-}
-
-#define REGISTER_SM100(cmd) extern "C" void _register_command_ ## cmd ## _backend_CCV_NNC_BACKEND_GPU_SM100(ccv_nnc_cmd_backend_registry_t* const registry)
-REGISTER_SM100(CCV_NNC_GELU_FORWARD) { fill(registry, CCV_32F | CCV_16F | CCV_16BF, exec_act<0, 0>); }
-REGISTER_SM100(CCV_NNC_GELU_BACKWARD) { fill(registry, CCV_32F | CCV_16F | CCV_16BF, exec_act<0, 1>); }
-REGISTER_SM100(CCV_NNC_SWISH_FORWARD) { fill(registry, CCV_32F | CCV_16F | CCV_16BF, exec_act<1, 0>); }
-REGISTER_SM100(CCV_NNC_SWISH_BACKWARD) { fill(registry, CCV_32F | CCV_16F | CCV_16BF, exec_act<1, 1>); }
-REGISTER_SM100(CCV_NNC_INDEX_SELECT_FORWARD) { fill(registry, CCV_32F | CCV_16F | CCV_16BF | CCV_32S, exec_index_select_forw); }
-REGISTER_SM100(CCV_NNC_INDEX_SELECT_BACKWARD) { fill(registry, CCV_32F | CCV_16F | CCV_16BF | CCV_32S, exec_index_select_back); }
-REGISTER_SM100(CCV_NNC_ADAMW_FORWARD) { fill(registry, CCV_32F | CCV_16F | CCV_16BF, exec_adam_any<0>); }
-REGISTER_SM100(CCV_NNC_ADAM_FORWARD) { fill(registry, CCV_32F | CCV_16F | CCV_16BF, exec_adam_any<1>); }
-REGISTER_SM100(CCV_NNC_ADAM_BACKWARD) { fill(registry, CCV_32F | CCV_16F | CCV_16BF, exec_no_backward); }
-REGISTER_SM100(CCV_NNC_ADAMW_BACKWARD) { fill(registry, CCV_32F | CCV_16F | CCV_16BF, exec_no_backward); }
+REGISTER_SM100(CCV_NNC_GELU_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_act<0, 0>); }
+REGISTER_SM100(CCV_NNC_GELU_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_act<0, 1>); }
+REGISTER_SM100(CCV_NNC_SWISH_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_act<1, 0>); }
+REGISTER_SM100(CCV_NNC_SWISH_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_act<1, 1>); }
+REGISTER_SM100(CCV_NNC_INDEX_SELECT_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF | CCV_32S, 1, exec_index_select_forw); }
+REGISTER_SM100(CCV_NNC_INDEX_SELECT_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF | CCV_32S, 1, exec_index_select_back); }
+REGISTER_SM100(CCV_NNC_ADAMW_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_adam_any<0>); }
+REGISTER_SM100(CCV_NNC_ADAM_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_adam_any<1>); }
+// an optimizer has no backward (adam/ccv_nnc_adamw_cpu_ref.c: _ccv_nnc_adamw_back)
+REGISTER_SM100(CCV_NNC_ADAM_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_invalid); }
+REGISTER_SM100(CCV_NNC_ADAMW_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_invalid); }

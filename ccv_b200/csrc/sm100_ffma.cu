@@ -174,13 +174,8 @@ static int launch_ffma(cudaStream_t stream, const AV& A, const BV& B, float* C, 
 		ffma_gemm_kernel<AV, BV><<<grid, 256, 0, stream>>>(A, B, (float*)scratch.ptr, ldp, bias, M, N, K, k_per, 0, (long long)M * ldp);
 	else
 		ffma_gemm_kernel<AV, BV><<<grid, 256, 0, stream>>>(A, B, C, ldc, bias, M, N, K, k_per, accumulate, 0);
-	count_launch();
-	cudaError_t e = cudaGetLastError();
-	if (e != cudaSuccess)
-	{
-		set_last_error("ffma_gemm_kernel launch", e);
+	if (launched("ffma_gemm_kernel launch"))
 		return -1;
-	}
 	return splits > 1 ? splitk_reduce(stream, (const float*)scratch.ptr, splits, (long long)M * ldp, M, N, ldp, C, ldc, accumulate) : 0;
 }
 

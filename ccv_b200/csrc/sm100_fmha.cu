@@ -308,14 +308,7 @@ int launch_fwd(cudaStream_t stream, const CUtensorMap& q, const CUtensorMap& k, 
 		configured = true;
 	}
 	fmha_fwd_kernel<BF16, MASK><<<grid, fm_threads(MASK), FmhaSmem<MASK>::TOTAL, stream>>>(q, k, v, p, m);
-	count_launch();
-	const cudaError_t e = cudaGetLastError();
-	if (e != cudaSuccess)
-	{
-		set_last_error("fmha_fwd_kernel launch", e);
-		return -1;
-	}
-	return 0;
+	return launched("fmha_fwd_kernel launch");
 }
 
 } // namespace

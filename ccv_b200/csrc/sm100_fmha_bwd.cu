@@ -355,14 +355,7 @@ int launch_bwd_t(cudaStream_t stream, const CUtensorMap& r1, const CUtensorMap& 
 		configured = true;
 	}
 	fmha_bwd_kernel<MODE, BF16><<<dim3(tiles, heads, B), FB_THREADS, FmhaBwdSmem::TOTAL, stream>>>(r1, r2, t1, t2, p);
-	count_launch();
-	const cudaError_t e = cudaGetLastError();
-	if (e != cudaSuccess)
-	{
-		set_last_error("fmha_bwd_kernel launch", e);
-		return -1;
-	}
-	return 0;
+	return launched("fmha_bwd_kernel launch");
 }
 
 template <int MODE>

@@ -634,18 +634,6 @@ int configure(K* kernel, const int bytes, const char* what, bool (&configured_on
 	return 0;
 }
 
-int launched(const char* what)
-{
-	count_launch();
-	const cudaError_t e = cudaGetLastError();
-	if (e != cudaSuccess)
-	{
-		set_last_error(what, e);
-		return -1;
-	}
-	return 0;
-}
-
 template <int MODE, int BF16>
 int launch_wide_bwd(cudaStream_t stream, const CUtensorMap& r1, const CUtensorMap& r2, const CUtensorMap& t1, const CUtensorMap& t2, const WideBwdParams& p, int tiles, int heads, int B)
 {

@@ -25,8 +25,7 @@
 // memory when the bins fit (HIST_SHARED_WORDS), with increments aggregated per warp over lanes of the same bin (__match_any_sync), and
 // are added to b at the end; otherwise straight to b with the same aggregated integer atomics.  Integer counts are exact in any order.
 // The per-CTA statistic slots are one workspace request made before the first launch.
-#include "../../include/ccv_nnc_sm100.h"
-#include "sm100_contract.h"
+#include "sm100_cmd.h"
 #include "sm100_elem.cuh"
 #include <climits>
 #include <cmath>
@@ -47,32 +46,6 @@ constexpr int HIST_CTAS_PER_SM = 4;
 constexpr int HIST_STATIC_BYTES = 1024;
 constexpr int HIST_SHARED_WORDS = (48 * 1024 - HIST_STATIC_BYTES) / 4;
 constexpr int FINAL_THREADS = 1024;
-
-int check(const char* what)
-{
-	count_launch();
-	const cudaError_t e = cudaGetLastError();
-	if (e != cudaSuccess)
-	{
-		set_last_error(what, e);
-		return -1;
-	}
-	return 0;
-}
-
-int sms()
-{
-	static int n = 0;
-	if (!n)
-	{
-		int dev = 0;
-		cudaGetDevice(&dev);
-		cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-		if (n <= 0)
-			n = 132;
-	}
-	return n;
-}
 
 struct HistParams {
 	int nbins; // counts the rule addresses: EVEN bins + 3, LOG 2u + 2, BINS n + 2 (the last one is NaN's)
@@ -397,26 +370,7 @@ __global__ void __launch_bounds__(FINAL_THREADS) histogram_stats_kernel(const St
 // ------------------------------------------------------------------------------------------------ host side
 bool packed(const ccv_nnc_tensor_t* const t) { return t && CCV_IS_TENSOR_CONTIGUOUS(t) && t->data.u8; }
 
-long long count_of(const ccv_nnc_tensor_t* const t)
-{
-	long long n = 1;
-	int nd = 0;
-	for (; nd < CCV_NNC_MAX_DIM_ALLOC && t->info.dim[nd] > 0; nd++)
-		n *= t->info.dim[nd];
-	return nd ? n : 0;
-}
-
 // element kind of a: 0 fp32, 1 bf16, 2 fp16; -1 otherwise (CCV_GET_DATA_TYPE keeps the CCV_QX bit, so palettized tensors are refused)
-int kind_of(const ccv_nnc_tensor_t* const t)
-{
-	switch (CCV_GET_DATA_TYPE(t->info.datatype))
-	{
-		case CCV_32F: return 0;
-		case CCV_16BF: return 1;
-		case CCV_16F: return 2;
-	}
-	return -1;
-}
 
 HistView view_of(const ccv_nnc_tensor_t* const t)
 {
@@ -461,7 +415,7 @@ int launch(const T* a, const HistView& v, const HistParams& p, int* b, StatSlot*
 		histogram_kernel<T, TYPE, 1><<<grid, HIST_THREADS, shm, s>>>(a, v, p, b, shared_bins, shared_bounds, slots, chunk);
 	else
 		histogram_kernel<T, TYPE, 2><<<grid, HIST_THREADS, shm, s>>>(a, v, p, b, shared_bins, shared_bounds, slots, chunk);
-	return check("histogram");
+	return launched("histogram");
 }
 
 template <typename T>
@@ -484,12 +438,12 @@ int exec_histogram_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, cons
 	ccv_nnc_tensor_t* const b = outputs[0];
 	ccv_nnc_tensor_t* const st = output_size > 1 ? outputs[1] : 0;
 	const int kind = kind_of(a);
-	const long long count = count_of(a);
+	const long long count = nd_of(a) ? (long long)count_of(a) : 0;
 	if (kind < 0 || count < 1 || count > INT_MAX)
 		return CCV_NNC_EXEC_INVALID;
 	if (!packed(b) || b->info.datatype != CCV_32S)
 		return CCV_NNC_EXEC_INVALID;
-	const long long bcount = count_of(b);
+	const long long bcount = (long long)count_of(b);
 	if (st && (!packed(st) || st->info.datatype != CCV_32F || count_of(st) < 4))
 		return CCV_NNC_EXEC_INVALID;
 	const ccv_nnc_cmd_param_t& info = cmd.info;
@@ -524,7 +478,7 @@ int exec_histogram_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, cons
 		const ccv_nnc_tensor_t* const h = input_size > 1 ? inputs[1] : 0;
 		if (!packed(h) || h->info.datatype != CCV_32F || CCV_TENSOR_GET_MEMORY(h->info.type) != CCV_TENSOR_GPU_MEMORY)
 			return CCV_NNC_EXEC_INVALID;
-		const long long n = count_of(h);
+		const long long n = nd_of(h) ? (long long)count_of(h) : 0;
 		if (n < 1 || n > INT_MAX - 2 || bcount != n + 2)
 			return CCV_NNC_EXEC_INVALID;
 		p.bounds = h->data.f32, p.nbounds = (int)n, p.nbins = (int)n + 2;
@@ -537,8 +491,8 @@ int exec_histogram_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, cons
 	// consecutive chunks of whole vectors, at most HIST_CTAS_PER_SM CTAs per SM
 	const long long tile = (long long)HIST_THREADS * W;
 	long long grid = (count + tile - 1) / tile;
-	if (grid > (long long)sms() * HIST_CTAS_PER_SM)
-		grid = (long long)sms() * HIST_CTAS_PER_SM;
+	if (grid > (long long)sm_count() * HIST_CTAS_PER_SM)
+		grid = (long long)sm_count() * HIST_CTAS_PER_SM;
 	long long chunk = (count + grid - 1) / grid;
 	chunk = (chunk + W - 1) / W * W;
 	grid = (count + chunk - 1) / chunk;
@@ -553,7 +507,7 @@ int exec_histogram_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, cons
 	}
 	cudaStream_t s = (cudaStream_t)ccv_nnc_stream_context_get_stream(stream_context);
 	cudaMemsetAsync(b->data.i32, 0, bcount * sizeof(int), s);
-	if (check("histogram_zero"))
+	if (launched("histogram_zero"))
 		return CCV_NNC_EXEC_INVALID;
 	int rc;
 	if (kind == 0)
@@ -567,31 +521,14 @@ int exec_histogram_forw(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, cons
 	if (st)
 	{
 		histogram_stats_kernel<<<1, FINAL_THREADS, 0, s>>>(slots, (int)grid, count, st->data.f32);
-		if (check("histogram_stats"))
+		if (launched("histogram_stats"))
 			return CCV_NNC_EXEC_INVALID;
 	}
 	return CCV_NNC_EXEC_SUCCESS;
 }
 
-// the reference has no histogram gradient (_ccv_nnc_histogram_back returns CCV_NNC_EXEC_INVALID)
-int exec_histogram_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
-{
-	return CCV_NNC_EXEC_INVALID;
-}
-
-void fill(ccv_nnc_cmd_backend_registry_t* const registry, const ccv_nnc_cmd_exec_f exec)
-{
-	registry->tensor_formats = CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_NCHW | CCV_TENSOR_FORMAT_CHWN;
-	registry->tensor_datatypes = CCV_32F | CCV_16F | CCV_16BF | CCV_32S;
-	registry->tensor_memory = CCV_TENSOR_GPU_MEMORY;
-	registry->algorithms = 1;
-	registry->exec = exec;
-	registry->autotune = 0;
-	registry->aux = 0;
-}
-
 } // namespace
 
-#define REGISTER_SM100(cmd) extern "C" void _register_command_ ## cmd ## _backend_CCV_NNC_BACKEND_GPU_SM100(ccv_nnc_cmd_backend_registry_t* const registry)
-REGISTER_SM100(CCV_NNC_HISTOGRAM_FORWARD) { fill(registry, exec_histogram_forw); }
-REGISTER_SM100(CCV_NNC_HISTOGRAM_BACKWARD) { fill(registry, exec_histogram_back); }
+REGISTER_SM100(CCV_NNC_HISTOGRAM_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF | CCV_32S, 1, exec_histogram_forw); }
+// the reference has no histogram gradient (_ccv_nnc_histogram_back returns CCV_NNC_EXEC_INVALID)
+REGISTER_SM100(CCV_NNC_HISTOGRAM_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF | CCV_32S, 1, exec_invalid); }

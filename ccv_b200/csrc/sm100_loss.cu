@@ -17,8 +17,7 @@
 // Backward: one element-wise pass (16-byte vectors on aligned rows, one element per thread otherwise) in CPU_REF's operations and
 // order, each product / sum rounded on its own (no FMA contraction): fp32 gradients equal CPU_REF's bit for bit, 16-bit ones CPU_REF's
 // on the widened inputs, rounded once.  BCE divides by the clamped denominator in double as CPU_REF does.
-#include "../../include/ccv_nnc_sm100.h"
-#include "sm100_contract.h"
+#include "sm100_cmd.h"
 #include "sm100_elem.cuh"
 #include <cuda_runtime.h>
 #include <string.h>
@@ -30,31 +29,6 @@ namespace {
 enum { L_BCE, L_SBCE, L_MSE, L_SL1 };
 constexpr int THREADS = 256;
 constexpr int LOSS_CHUNK_UNITS = 2048; // units per chunk of a split row: 8 per thread of a 256-thread CTA
-
-int sms()
-{
-	static int n = 0;
-	if (!n)
-	{
-		int dev = 0;
-		cudaGetDevice(&dev);
-		cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-		if (n <= 0)
-			n = 132;
-	}
-	return n;
-}
-int check(const char* what)
-{
-	count_launch();
-	const cudaError_t e = cudaGetLastError();
-	if (e != cudaSuccess)
-	{
-		set_last_error(what, e);
-		return -1;
-	}
-	return 0;
-}
 
 struct LossArg {
 	int batch, count;
@@ -355,22 +329,22 @@ int launch_fwd(cudaStream_t s, const LossCall& k, const LossArg& p, const LossPl
 {
 	const unsigned blocks = (unsigned)(plan.blocks < (1u << 30) ? plan.blocks : (1u << 30));
 	loss_fwd_kernel<OP, T, TB, MODE><<<blocks, THREADS, 0, s>>>((const T*)k.x, (const TB*)k.y, (T*)k.out, (T*)k.out2, (float*)k.part, p);
-	if (check("loss forward"))
+	if (launched("loss forward"))
 		return -1;
 	if (plan.launches == 1)
 		return 0;
 	loss_combine_kernel<OP, T><<<(unsigned)(((size_t)p.batch * 32 + THREADS - 1) / THREADS), THREADS, 0, s>>>((const float*)k.part, (T*)k.out, p);
-	return check("loss combine");
+	return launched("loss combine");
 }
 template <int OP, typename T, typename TB, int MODE>
 int launch_bwd(cudaStream_t s, const LossCall& k, const LossArg& p)
 {
 	const size_t n = MODE == B_FLAT ? (size_t)p.batch * p.count / Vec16<T>::W : (size_t)p.batch * (p.count / (MODE == B_ROWVEC ? Vec16<T>::W : 1));
 	size_t blocks = (n + THREADS - 1) / THREADS;
-	if (blocks > (size_t)sms() * 16)
-		blocks = (size_t)sms() * 16;
+	if (blocks > (size_t)sm_count() * 16)
+		blocks = (size_t)sm_count() * 16;
 	loss_bwd_kernel<OP, T, TB, MODE><<<(unsigned)blocks, THREADS, 0, s>>>((const T*)k.g, (const T*)k.x, (const TB*)k.y, (const T*)k.c, (T*)k.out, (T*)k.out2, p, n);
-	return check("loss backward");
+	return launched("loss backward");
 }
 template <int OP, typename T, typename TB>
 int run_t(cudaStream_t s, const int forward, const LossCall& k, const LossArg& p, const LossPlan& plan)
@@ -400,23 +374,6 @@ int run_loss(cudaStream_t s, const int kind, const int bkind, const int forward,
 }
 
 // ------------------------------------------------------------------------------------------------ command layer
-inline cudaStream_t stream_of(ccv_nnc_stream_context_t* const sc) { return (cudaStream_t)ccv_nnc_stream_context_get_stream(sc); }
-inline int kind_of(const ccv_nnc_tensor_t* const t)
-{
-	switch (CCV_GET_DATA_TYPE(t->info.datatype))
-	{
-		case CCV_32F: return 0;
-		case CCV_16BF: return 1;
-		case CCV_16F: return 2;
-	}
-	return -1;
-}
-int nd_of(const ccv_nnc_tensor_t* const t)
-{
-	int i;
-	for (i = 0; i < CCV_NNC_MAX_DIM_ALLOC && t->info.dim[i] > 0; i++) {}
-	return i;
-}
 // a [batch, count] operand (1-d: one row) whose inner axis is contiguous; its row pitch in elements
 struct Rows {
 	int batch, count;
@@ -546,25 +503,13 @@ int exec_loss_back(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int
 	return run_loss<OP>(stream_of(stream_context), kind, kind_of(y), 0, k, p, plan) ? CCV_NNC_EXEC_INVALID : CCV_NNC_EXEC_SUCCESS;
 }
 
-void fill(ccv_nnc_cmd_backend_registry_t* const registry, const ccv_nnc_cmd_exec_f exec)
-{
-	registry->tensor_formats = CCV_TENSOR_FORMAT_NCHW | CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_CHWN;
-	registry->tensor_datatypes = CCV_32F | CCV_16F | CCV_16BF;
-	registry->tensor_memory = CCV_TENSOR_GPU_MEMORY;
-	registry->algorithms = 1;
-	registry->exec = exec;
-	registry->autotune = 0;
-	registry->aux = 0;
-}
-
 } // namespace
 
-#define REGISTER_SM100(cmd) extern "C" void _register_command_ ## cmd ## _backend_CCV_NNC_BACKEND_GPU_SM100(ccv_nnc_cmd_backend_registry_t* const registry)
-REGISTER_SM100(CCV_NNC_BINARY_CROSSENTROPY_FORWARD) { fill(registry, exec_loss_forw<L_BCE>); }
-REGISTER_SM100(CCV_NNC_BINARY_CROSSENTROPY_BACKWARD) { fill(registry, exec_loss_back<L_BCE>); }
-REGISTER_SM100(CCV_NNC_SIGMOID_BINARY_CROSSENTROPY_FORWARD) { fill(registry, exec_loss_forw<L_SBCE>); }
-REGISTER_SM100(CCV_NNC_SIGMOID_BINARY_CROSSENTROPY_BACKWARD) { fill(registry, exec_loss_back<L_SBCE>); }
-REGISTER_SM100(CCV_NNC_MSE_FORWARD) { fill(registry, exec_loss_forw<L_MSE>); }
-REGISTER_SM100(CCV_NNC_MSE_BACKWARD) { fill(registry, exec_loss_back<L_MSE>); }
-REGISTER_SM100(CCV_NNC_SMOOTH_L1_FORWARD) { fill(registry, exec_loss_forw<L_SL1>); }
-REGISTER_SM100(CCV_NNC_SMOOTH_L1_BACKWARD) { fill(registry, exec_loss_back<L_SL1>); }
+REGISTER_SM100(CCV_NNC_BINARY_CROSSENTROPY_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_loss_forw<L_BCE>); }
+REGISTER_SM100(CCV_NNC_BINARY_CROSSENTROPY_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_loss_back<L_BCE>); }
+REGISTER_SM100(CCV_NNC_SIGMOID_BINARY_CROSSENTROPY_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_loss_forw<L_SBCE>); }
+REGISTER_SM100(CCV_NNC_SIGMOID_BINARY_CROSSENTROPY_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_loss_back<L_SBCE>); }
+REGISTER_SM100(CCV_NNC_MSE_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_loss_forw<L_MSE>); }
+REGISTER_SM100(CCV_NNC_MSE_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_loss_back<L_MSE>); }
+REGISTER_SM100(CCV_NNC_SMOOTH_L1_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_loss_forw<L_SL1>); }
+REGISTER_SM100(CCV_NNC_SMOOTH_L1_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_loss_back<L_SL1>); }

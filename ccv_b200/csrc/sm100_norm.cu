@@ -9,18 +9,6 @@
 
 namespace sm100 {
 
-static int check(const char* what)
-{
-	count_launch();
-	const cudaError_t e = cudaGetLastError();
-	if (e != cudaSuccess)
-	{
-		set_last_error(what, e);
-		return -1;
-	}
-	return 0;
-}
-
 __device__ __forceinline__ float wsum(float v)
 {
 #pragma unroll
@@ -185,7 +173,7 @@ template <int RMS, typename TX, typename TP, typename TB, typename TS>
 static int norm_fwd(cudaStream_t s, const void* x, const void* scale, const void* bias, void* y, void* saved_mean, void* saved_inv_std, int rows, int inner, float epsilon)
 {
 	norm_fwd_kernel<RMS, TX, TP, TB, TS><<<rows, row_threads(inner), 0, s>>>((const TX*)x, (const TP*)scale, (const TB*)bias, (TX*)y, (TS*)saved_mean, (TS*)saved_inv_std, inner, epsilon);
-	return check(RMS ? "rmsnorm_fwd" : "layer_norm_fwd");
+	return launched(RMS ? "rmsnorm_fwd" : "layer_norm_fwd");
 }
 int layer_norm_fwd(cudaStream_t s, const NormKinds& k, const void* x, const void* scale, const void* bias, void* y, void* saved_mean, void* saved_inv_std, int rows, int inner, float epsilon)
 {
@@ -330,17 +318,17 @@ static int norm_bwd(cudaStream_t s, const void* g, const void* x, const void* sc
 	if (dx)
 	{
 		norm_bwd_dx_kernel<RMS, TX, TP, TS><<<rows, row_threads(inner), 0, s>>>((const TX*)g, (const TX*)x, (const TP*)scale, (const TS*)saved_mean, (const TS*)saved_inv_std, (TX*)dx, inner);
-		if (check("norm_bwd_dx"))
+		if (launched("norm_bwd_dx"))
 			return -1;
 	}
 	if (dscale || dbias)
 	{
 		const int gy = dparam_row_blocks(rows);
 		norm_bwd_dparam_kernel<RMS, TX, TS><<<dim3((inner + 127) / 128, gy), 128, 0, s>>>((const TX*)g, (const TX*)x, (const TS*)saved_mean, (const TS*)saved_inv_std, (float*)workspace, rows, inner);
-		if (check("norm_bwd_dparam"))
+		if (launched("norm_bwd_dparam"))
 			return -1;
 		norm_bwd_dparam_rows_kernel<TDS, TDB><<<(inner + 31) / 32, 1024, 0, s>>>((const float*)workspace, gy, inner, (TDS*)dscale, (TDB*)dbias);
-		if (check("norm_bwd_dparam_rows"))
+		if (launched("norm_bwd_dparam_rows"))
 			return -1;
 	}
 	return 0;
@@ -526,7 +514,7 @@ int upsample_fwd_f32(cudaStream_t s, const float* a, float* b, int N, int H, int
 	float rh, rw;
 	ratios(H, W, OH, OW, align_corners, rh, rw);
 	upsample_kernel<<<upsample_blocks(total), 256, 0, s>>>(a, b, N, H, W, C, OH, OW, type, align_corners, nchw, rh, rw);
-	return check("upsample_fwd");
+	return launched("upsample_fwd");
 }
 int upsample_bwd_f32(cudaStream_t s, const float* g, float* h, int N, int H, int W, int C, int OH, int OW, int type, int align_corners, int nchw)
 {
@@ -536,7 +524,7 @@ int upsample_bwd_f32(cudaStream_t s, const float* g, float* h, int N, int H, int
 	float rh, rw;
 	ratios(H, W, OH, OW, align_corners, rh, rw);
 	upsample_back_kernel<<<upsample_blocks(total), 256, 0, s>>>(g, h, N, H, W, C, OH, OW, type, align_corners, nchw, rh, rw);
-	return check("upsample_bwd");
+	return launched("upsample_bwd");
 }
 
 
@@ -723,7 +711,7 @@ static int gn_fwd(cudaStream_t s, const GroupNormGeom& g, const void* x, const v
 	if (blocks > 132 * 16)
 		blocks = 132 * 16;
 	gn_apply_kernel<TX, TP, TB, TS><<<(unsigned)blocks, 256, 0, s>>>(g, (const TX*)x, (const TP*)scale, (const TB*)bias, (const TS*)saved_mean, (const TS*)saved_inv_std, (TX*)y, total);
-	return check("group_norm_fwd");
+	return launched("group_norm_fwd");
 }
 
 int group_norm_fwd(cudaStream_t s, const NormKinds& k, const GroupNormGeom& g, const void* x, const void* scale, const void* bias, void* y, void* saved_mean, void* saved_inv_std, float epsilon)
@@ -752,19 +740,19 @@ static int gn_bwd(cudaStream_t s, const GroupNormGeom& g, const void* grad, cons
 	{
 		float* const sums = (float*)workspace;
 		gn_bwd_stats_kernel<TX, TP, TS><<<(unsigned)slots, 512, 0, s>>>(g, (const TX*)grad, (const TX*)x, (const TP*)scale, (const TS*)saved_mean, (const TS*)saved_inv_std, sums);
-		if (check("group_norm_bwd_stats"))
+		if (launched("group_norm_bwd_stats"))
 			return -1;
 		long long blocks = (total + 255) / 256;
 		if (blocks > 132 * 16)
 			blocks = 132 * 16;
 		gn_bwd_apply_kernel<TX, TP, TS><<<(unsigned)blocks, 256, 0, s>>>(g, (const TX*)grad, (const TX*)x, (const TP*)scale, (const TS*)saved_mean, (const TS*)saved_inv_std, sums, (TX*)h, total, (float)slots / (float)total);
-		if (check("group_norm_bwd_apply"))
+		if (launched("group_norm_bwd_apply"))
 			return -1;
 	}
 	if (dscale || dbias)
 	{
 		gn_bwd_dparam_kernel<TX, TS, TDS, TDB><<<(unsigned)gn_count(g.sdim), 256, 0, s>>>(g, (const TX*)grad, (const TX*)x, (const TS*)saved_mean, (const TS*)saved_inv_std, (TDS*)dscale, (TDB*)dbias);
-		if (check("group_norm_bwd_dparam"))
+		if (launched("group_norm_bwd_dparam"))
 			return -1;
 	}
 	return 0;

@@ -24,17 +24,13 @@
 //            Every sum is a fixed tree (per thread in element order, warp butterfly, warps in order, partials per thread then the same
 //            tree): the same inputs give the same bits on every run.  Traffic: pass 1 reads g, a, m, v; pass 3 reads them again and
 //            writes b, n, u (44 B per element with fp32 state and gradient).
-#include "../../include/ccv_nnc_sm100.h"
-#include "sm100_contract.h"
+#include "sm100_cmd.h"
 #include "sm100_elem.cuh"
 #include <cuda_runtime.h>
 #include <limits.h>
 #include <math.h>
 #include <vector>
 
-namespace sm100 {
-int exec_no_backward(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context);
-}
 using namespace sm100;
 
 namespace {
@@ -63,18 +59,6 @@ struct LambArgs {
 struct RmspropArgs {
 	float rate, scale, decay, alpha, one_minus_alpha, momentum, epsilon;
 };
-
-int check(const char* what)
-{
-	count_launch();
-	const cudaError_t e = cudaGetLastError();
-	if (e != cudaSuccess)
-	{
-		set_last_error(what, e);
-		return -1;
-	}
-	return 0;
-}
 
 // ------------------------------------------------------------------------------------------------ arithmetic (CPU_REF's order)
 __device__ __forceinline__ float lamb_update(const LambArgs& p, const float g, const float a, const float m, const float v, float& n, float& u)
@@ -261,24 +245,6 @@ __global__ void __launch_bounds__(OPTIM_THREADS) rmsprop_kernel(const __grid_con
 }
 
 // ------------------------------------------------------------------------------------------------ host
-inline int kind_of(const ccv_nnc_tensor_t* const t)
-{
-	switch (CCV_GET_DATA_TYPE(t->info.datatype))
-	{
-		case CCV_32F: return 0;
-		case CCV_16BF: return 1;
-		case CCV_16F: return 2;
-	}
-	return -1;
-}
-inline size_t elem_size(const int kind) { return kind == 0 ? 4 : 2; }
-size_t count_of(const ccv_nnc_tensor_t* const t)
-{
-	size_t n = 1;
-	for (int i = 0; i < CCV_NNC_MAX_DIM_ALLOC && t->info.dim[i] > 0; i++)
-		n *= (size_t)t->info.dim[i];
-	return n;
-}
 
 // f(TG(), TS()) with the element types of the gradient and of the state
 template <typename F>
@@ -383,13 +349,13 @@ int run_lamb(const ccv_nnc_cmd_t cmd, ccv_nnc_tensor_t* const* const inputs, ccv
 			using TG = decltype(tg);
 			using TS = decltype(ts);
 			lamb_norm_kernel<TG, TS><<<blocks, OPTIM_THREADS, 0, s>>>(t, p, partial);
-			if (check("lamb_norm"))
+			if (launched("lamb_norm"))
 				return -1;
 			lamb_trust_kernel<<<t.tensors, OPTIM_THREADS, 0, s>>>(t, p.rate, partial, r);
-			if (check("lamb_trust"))
+			if (launched("lamb_trust"))
 				return -1;
 			lamb_apply_kernel<TG, TS><<<blocks, OPTIM_THREADS, 0, s>>>(t, p, r);
-			return check("lamb_apply");
+			return launched("lamb_apply");
 		});
 		if (rc)
 			return CCV_NNC_EXEC_INVALID;
@@ -413,7 +379,7 @@ int run_rmsprop(const ccv_nnc_cmd_t cmd, ccv_nnc_tensor_t* const* const inputs, 
 	{
 		const int rc = with_types(g_kind, s_kind, [&](auto tg, auto ts) {
 			rmsprop_kernel<decltype(tg), decltype(ts)><<<t.block_start[t.tensors], OPTIM_THREADS, 0, s>>>(t, p);
-			return check("rmsprop");
+			return launched("rmsprop");
 		});
 		if (rc)
 			return CCV_NNC_EXEC_INVALID;
@@ -439,17 +405,6 @@ int exec_optim_multi(const ccv_nnc_cmd_t cmd, ccv_nnc_tensor_t* const* const inp
 	return IS_LAMB ? run_lamb(cmd, inputs, outputs, T, stream_context) : run_rmsprop(cmd, inputs, outputs, T, stream_context);
 }
 
-void fill(ccv_nnc_cmd_backend_registry_t* const registry, const ccv_nnc_cmd_exec_f exec)
-{
-	registry->tensor_formats = CCV_TENSOR_FORMAT_NCHW | CCV_TENSOR_FORMAT_NHWC | CCV_TENSOR_FORMAT_CHWN;
-	registry->tensor_datatypes = CCV_32F | CCV_16F | CCV_16BF;
-	registry->tensor_memory = CCV_TENSOR_GPU_MEMORY;
-	registry->algorithms = 1;
-	registry->exec = exec;
-	registry->autotune = 0;
-	registry->aux = 0;
-}
-
 } // namespace
 
 extern "C" int ccv_nnc_sm100_fused_lamb_multi(const ccv_nnc_cmd_t cmd, const ccv_nnc_hint_t hint, const int flags, ccv_nnc_tensor_t* const* const inputs, const int input_size, ccv_nnc_tensor_t* const* const outputs, const int output_size, ccv_nnc_stream_context_t* const stream_context)
@@ -461,8 +416,7 @@ extern "C" int ccv_nnc_sm100_fused_rmsprop_multi(const ccv_nnc_cmd_t cmd, const 
 	return exec_optim_multi<0>(cmd, inputs, input_size, outputs, output_size, stream_context);
 }
 
-#define REGISTER_SM100(cmd) extern "C" void _register_command_ ## cmd ## _backend_CCV_NNC_BACKEND_GPU_SM100(ccv_nnc_cmd_backend_registry_t* const registry)
-REGISTER_SM100(CCV_NNC_LAMB_FORWARD) { fill(registry, exec_optim<1>); }
-REGISTER_SM100(CCV_NNC_LAMB_BACKWARD) { fill(registry, exec_no_backward); }
-REGISTER_SM100(CCV_NNC_RMSPROP_FORWARD) { fill(registry, exec_optim<0>); }
-REGISTER_SM100(CCV_NNC_RMSPROP_BACKWARD) { fill(registry, exec_no_backward); }
+REGISTER_SM100(CCV_NNC_LAMB_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_optim<1>); }
+REGISTER_SM100(CCV_NNC_LAMB_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_invalid); }
+REGISTER_SM100(CCV_NNC_RMSPROP_FORWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_optim<0>); }
+REGISTER_SM100(CCV_NNC_RMSPROP_BACKWARD) { fill(registry, ALL_FORMATS, CCV_32F | CCV_16F | CCV_16BF, 1, exec_invalid); }

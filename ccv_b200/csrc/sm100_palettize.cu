@@ -132,14 +132,7 @@ int launch_depalettize(cudaStream_t stream, const uint8_t* in, int q, int nib, s
 	const unsigned g = (unsigned)(grid < (size_t)132 * 64 ? grid : (size_t)132 * 64);
 	const size_t smem = (size_t)warps * ((size_t)1 << q) * sizeof(T);
 	depalettize_kernel<T><<<g, warps * 32, smem, stream>>>(in, q, nib, count, out);
-	count_launch();
-	const cudaError_t e = cudaGetLastError();
-	if (e != cudaSuccess)
-	{
-		set_last_error("depalettize_kernel launch", e);
-		return -1;
-	}
-	return 0;
+	return launched("depalettize_kernel launch");
 }
 
 // palette entry i of a block whose palette starts at `pal` (2-byte aligned when `aligned`; else read as two bytes)
@@ -274,14 +267,7 @@ int gemm_palettized_f16(cudaStream_t stream, const int M, const int N, const int
 	const int warps = 8;
 	const dim3 grid((N + warps - 1) / warps);
 	palettized_gemm_f16_kernel<PALETTIZED_GEMM_M_MAX><<<grid, warps * 32, 0, stream>>>((const __half*)a, lda, (const uint8_t*)wq, qbits, nib, M, N, K, (__half*)c, ldc, bias32, (const __half*)bias16);
-	count_launch();
-	const cudaError_t e = cudaGetLastError();
-	if (e != cudaSuccess)
-	{
-		set_last_error("palettized_gemm_f16_kernel launch", e);
-		return -1;
-	}
-	return 0;
+	return launched("palettized_gemm_f16_kernel launch");
 }
 
 } // namespace sm100

@@ -14,17 +14,6 @@ namespace sm100 {
 // the attention scores already occupy the command's workspace: these products run without split-K slices
 static const Scratch no_scratch = { 0, 0 };
 
-static int check(const char* what)
-{
-	count_launch();
-	const cudaError_t e = cudaGetLastError();
-	if (e != cudaSuccess)
-	{
-		set_last_error(what, e);
-		return -1;
-	}
-	return 0;
-}
 __device__ __forceinline__ float wsum_(float v)
 {
 #pragma unroll
@@ -126,7 +115,7 @@ int sdpa_forward_f32(cudaStream_t s, const SdpaGeom& g, const float* q, const fl
 				return rc;
 			const float* mp = mask ? mask + (g.mask_b ? b * g.mask_b : 0) + (g.mask_h ? h * g.mask_h : 0) : 0;
 			sdpa_softmax_kernel<<<g.Sq, row_threads(g.Sk), 0, s>>>(S, g.Sq, g.Sk, g.scale, mp, g.mask_s, g.mask_c, g.is_causal);
-			if (check("sdpa_softmax"))
+			if (launched("sdpa_softmax"))
 				return -1;
 			// O = P V
 			rc = gemm_any(s, 0, g.Sq, g.Dv, g.Sk, S, g.Sk, 0, vp, g.v_s, 0, op, g.o_s, 0, 0, 0, no_scratch);
@@ -168,7 +157,7 @@ int sdpa_backward_f32(cudaStream_t s, const SdpaGeom& g, const float* dout, cons
 			if (rc)
 				return rc;
 			sdpa_softmax_kernel<<<g.Sq, row_threads(g.Sk), 0, s>>>(P, g.Sq, g.Sk, g.scale, 0, 0, 0, g.is_causal);
-			if (check("sdpa_softmax(bwd)"))
+			if (launched("sdpa_softmax(bwd)"))
 				return -1;
 			rc = mm(s, g.Sk, g.Dv, g.Sq, P, g.Sk, 1, gp, g.o_s, 0, dvp, dg.v_s, !first); // dV (+)= P^T dO
 			if (rc)
@@ -177,7 +166,7 @@ int sdpa_backward_f32(cudaStream_t s, const SdpaGeom& g, const float* dout, cons
 			if (rc)
 				return rc;
 			sdpa_dsoftmax_kernel<<<g.Sq, row_threads(g.Sk), 0, s>>>(P, dP, g.Sk, g.scale);
-			if (check("sdpa_dsoftmax"))
+			if (launched("sdpa_dsoftmax"))
 				return -1;
 			rc = mm(s, g.Sq, g.D, g.Sk, dP, g.Sk, 0, kp, g.k_s, 0, dqp, dg.q_s, 0); // dQ = dS K
 			if (rc)

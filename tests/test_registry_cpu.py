@@ -1,8 +1,10 @@
 """The registry plumbing of an 8th backend (SURVEY.md 8b): tools/gen_backend_ph.py re-derives the reference's perfect hashes
 (lib/nnc/cmd/build-cmd.rb:303-386, lib/nnc/cmd/ccv_nnc_cmd.inc:152-190) and the stand-alone host dispatches through
 init_map[_ccv_nnc_cmd_ph(cmd)].backends[_ccv_nnc_cmd_backend_ph(backend)] exactly as lib/nnc/ccv_nnc_cmd.c does."""
+import ctypes as C
 import json
 import os
+import re
 import subprocess
 import sys
 
@@ -13,6 +15,8 @@ from ccv_b200 import abi, nnc
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 # the reference's generated registry tables (lib/nnc/cmd/ccv_nnc_cmd.inc), extracted by tests/golden/make_golden.py
 REGISTRY = os.path.join(ROOT, "tests", "golden", "reference_cmd_registry.json")
+# what every GPU_SM100 registration function writes, recorded by tests/golden/make_registry_golden.py
+SM100_REGISTRY = os.path.join(ROOT, "tests", "golden", "sm100_registry.json")
 REFERENCE_BACKENDS = {"CPU_OPT": 0x46deb194, "CPU_REF": 0x3d9883e5, "GPU_CUBLAS": 0x9b8cfed, "GPU_CUDNN": 0x854b679a, "GPU_NCCL": 0x7afed9c7, "GPU_REF": 0x5f19790a, "MPS": 0xb2f325e2}
 
 
@@ -94,3 +98,44 @@ def test_patched_cmd_inc_reslots_every_registration_call(tmp_path):
     cmd_slot = {c: i for c, _, i, _ in old_calls}
     sm100 = [(c, i) for c, b, i, _ in new_calls if b == "CCV_NNC_BACKEND_GPU_SM100"]
     assert len(sm100) == n_sm100 and all(cmd_slot[c] == i for c, i in sm100)
+
+
+class BackendRegistry(C.Structure):  # ccv_nnc_cmd_backend_registry_t
+    _fields_ = [("tensor_formats", C.c_int), ("tensor_datatypes", C.c_int), ("tensor_memory", C.c_int), ("algorithms", C.c_int),
+                ("exec", C.c_void_p), ("autotune", C.c_void_p), ("aux", C.c_void_p)]
+
+
+def registry_snapshot():
+    """Calls the registration function of every command include/ccv_nnc_sm100.h lists (no device needed: it only fills a record) and
+    returns what each one wrote, plus the commands that share one exec function.  The grouping does not depend on addresses, so it
+    tells a registration pointed at another command's exec apart from the same table."""
+    lib = nnc.lib()
+    cmds = re.findall(r"X\((CCV_NNC_[A-Z0-9_]+)\)", open(os.path.join(ROOT, "include", "ccv_nnc_sm100.h")).read())
+    entries, by_exec = {}, {}
+    for cmd in cmds:
+        r = BackendRegistry()
+        C.memset(C.byref(r), 0xa5, C.sizeof(r))
+        getattr(lib, "_register_command_%s_backend_CCV_NNC_BACKEND_GPU_SM100" % cmd)(C.byref(r))
+        entries[cmd] = {"tensor_formats": r.tensor_formats, "tensor_datatypes": r.tensor_datatypes, "tensor_memory": r.tensor_memory,
+                        "algorithms": r.algorithms, "exec": bool(r.exec), "autotune": bool(r.autotune), "aux": bool(r.aux)}
+        by_exec.setdefault(r.exec, []).append(cmd)
+    return {"commands": entries, "exec_groups": sorted(sorted(g) for g in by_exec.values() if len(g) > 1)}
+
+
+def test_every_sm100_registration_fills_the_recorded_entry():
+    want = json.load(open(SM100_REGISTRY))
+    got = registry_snapshot()
+    assert len(got["commands"]) == len(want["commands"]) == 132
+    for cmd, entry in want["commands"].items():
+        assert got["commands"].get(cmd) == entry, cmd
+    # The commands without a gradient register an exec that only returns CCV_NNC_EXEC_INVALID; whether they share one such function
+    # or each family has its own is not part of the table.  Every other command keeps its exec grouping.
+    invalid = set(want["invalid_exec"])
+
+    def split(groups, singles):
+        merged = [g for g in groups if invalid & set(g)] + [[c] for c in singles if c in invalid]
+        return sorted(c for g in merged for c in g), [g for g in groups if not invalid & set(g)]
+    singles = set(got["commands"]) - {c for g in got["exec_groups"] for c in g}
+    got_invalid, got_groups = split(got["exec_groups"], singles)
+    assert got_invalid == sorted(invalid)
+    assert got_groups == [g for g in want["exec_groups"] if not invalid & set(g)]
